@@ -353,6 +353,14 @@ extern "C" int h2_test_last_msm_flags(uint32_t *out) {
     *out = (f[0] ? 1u : 0u) | (f[1] ? 2u : 0u);
     return 0;
 }
+// test hook: what the most recent MSM pass ran (recorded on the host by msm_run; layout in include/halo2_b200.h)
+extern "C" int h2_test_last_msm_plan(uint32_t out[8]) {
+    std::lock_guard<std::mutex> lk(g_mu);
+    if (require_ready()) return 1;
+    if (!g_ctx.have_plan) return fail("h2_test_last_msm_plan: no MSM has run");
+    memcpy(out, g_ctx.last_plan, sizeof g_ctx.last_plan);
+    return 0;
+}
 // test / A-B hook: fixed-base passes first run without their fallback kernels (1, default) or always run the full pass (0)
 extern "C" int h2_test_set_fast_fixed(int on) {
     std::lock_guard<std::mutex> lk(g_mu);

@@ -110,9 +110,17 @@ static int msm_run(const fe *d_scalars, int scalars_mont, const affine *d_bases,
         return 0;
     }
     std::function<int()> issue;
+    // h2_test_last_msm_plan: mode, c, W, sets, accumulation, natural, fast, re-run of a fast pass -- recorded here on the host,
+    // so a pass replayed from a captured graph reports the same
+    auto record = [&X](uint32_t mode, uint32_t c_, uint32_t W, uint32_t sets_, uint32_t accum, uint32_t natural, uint32_t fast) {
+        const uint32_t v[8] = {mode, c_, W, sets_, accum, natural, fast, X.fast_retry ? 1u : 0u};
+        memcpy(X.last_plan, v, sizeof v);
+        X.have_plan = true;
+    };
     if (fixed == 2) {   // direct sum over the digit-multiples table (fixedbase.cuh): accumulate + reduce tree
         FbPlan fp;
         fp.total = n; fp.sets = sets ? sets : 1u; fp.split = fb_split(n, fp.sets); fp.scalars_mont = scalars_mont ? 1u : 0u;
+        record(2, H2_FB_BITS, H2_FB_WINDOWS, fp.sets, 2, 0, 0);
         const uint64_t count0 = n * fp.split;
         if (X.fb_a.ensure(fp.sets * count0 * sizeof(xyzz)) || X.fb_b.ensure(fp.sets * fb_ctas(count0, fb_fan(count0)) * sizeof(xyzz))) return 1;
         issue = [&X, fp, count0, d_scalars, d_bases, d_out, out_canonical, s]() -> int {
@@ -165,6 +173,9 @@ static int msm_run(const fe *d_scalars, int scalars_mont, const affine *d_bases,
         part_total = pk[j].part_total > part_total ? pk[j].part_total : part_total;
         t_max = pk[j].T > t_max ? pk[j].T : t_max;
     }
+    bool thread_per_item = false;   // the accumulation's branch below, for any chunk
+    for (uint32_t j = 0; j < K; j++) thread_per_item |= pk[j].max_refs > (pk[j].fixed ? 2 : 1) * H2_MSM_QUAD_ACCUM_REFS;
+    record(fixed, c, p.W, p.sets, thread_per_item ? 1u : 0u, p.natural, p.fast);
     // batched-affine rounds ahead of the XYZZ chain (msm.cuh K4a) for the throughput-bound sizes: every chunk plans its own
     // chunk's rounds; their level arrays (56 B per reference over the rounds, per chunk) may take at most half of the free
     // device memory -- a larger problem runs without them
@@ -467,9 +478,10 @@ static int msm_host_common(int curve, const void *scalars, size_t n_scalars, con
     }
     for (int attempt = 0; attempt < 2; attempt++) {   // fixed-base: the fast pass first, the full one if its flags came back set
         X.fast_now = attempt == 0 && fixed == 1 && X.fast_on && !bc.k;
+        X.fast_retry = attempt == 1;
         int rc = msm_dispatch(curve, X.scal_in.as<fe>(), repr == H2_REPR_MONTGOMERY, d_bases, n_total, c, X.result.as<jacobian>(),
                               repr == H2_REPR_CANONICAL, s, fixed, stride, bc.k ? &bc : nullptr);
-        X.fast_now = false;
+        X.fast_now = X.fast_retry = false;
         if (uploader.joinable()) uploader.join();
         if (up_failed.load()) { cudaStreamSynchronize(s); cudaStreamSynchronize(X.copy_stream); return fail(up_err); }
         if (rc) return rc;
@@ -594,9 +606,10 @@ static int msm_registered_batch_impl(uint64_t handle, const void *scalars, size_
     if (affine_out && X.ec_out.ensure(batch * sizeof(affine))) return 1;
     for (int attempt = 0; attempt < 2; attempt++) {   // the fast pass first, the full one if its flags came back set
         X.fast_now = attempt == 0 && tmode == 1 && X.fast_on;
+        X.fast_retry = attempt == 1;
         int rc = msm_dispatch(b->curve, d, repr == H2_REPR_MONTGOMERY, tbl, total, tc, X.result.as<jacobian>(),
                               affine_out ? 0 : canon, s, tmode, b->n, nullptr, (uint32_t)batch);
-        X.fast_now = false;
+        X.fast_now = X.fast_retry = false;
         if (rc) return rc;
         if (affine_out) {
             const uint32_t nb = blocks_for((batch + H2_NORM_CHUNK - 1) / H2_NORM_CHUNK, 64);
@@ -897,8 +910,9 @@ static int ipa_round_common(uint64_t session, const void *z, const void *l_rand,
     fixed_table(b, &tc0, &tmode0);
     for (int attempt = 0; attempt < 2; attempt++) {   // the fast pass first, the full one if its flags came back set (the prep / inner kernels are idempotent)
         g_ctx.fast_now = attempt == 0 && tmode0 == 1 && g_ctx.fast_on;
+        g_ctx.fast_retry = attempt == 1;
         int rc = b->curve == H2_CURVE_PALLAS ? ipa_round_impl<FqParams>(q, b, z, l_rand, r_rand, repr, oc, s) : ipa_round_impl<FpParams>(q, b, z, l_rand, r_rand, repr, oc, s);
-        g_ctx.fast_now = false;
+        g_ctx.fast_now = g_ctx.fast_retry = false;
         if (rc) return rc;
         if (affine_out) {
             const int canon = repr == H2_REPR_CANONICAL;
@@ -1013,10 +1027,11 @@ static int msm_registered_polys_impl(uint64_t bases_handle, const uint64_t *poly
     for (int attempt = 0; attempt < 2; attempt++) {   // the fast pass first, the full one if its flags came back set
         int rc;
         X.fast_now = attempt == 0 && tbl && tmode == 1 && X.fast_on;
+        X.fast_retry = attempt == 1;
         if (tbl) rc = msm_dispatch(b->curve, d, 1, tbl, total, tc, X.result.as<jacobian>(), affine_out ? 0 : canon, s, tmode, b->n,
                                    nullptr, (uint32_t)batch);
         else rc = msm_dispatch(b->curve, d, 1, b->buf.as<affine>(), total, 0, X.result.as<jacobian>(), affine_out ? 0 : canon, s);
-        X.fast_now = false;
+        X.fast_now = X.fast_retry = false;
         if (rc) return rc;
         if (affine_out) {
             const uint32_t nb = blocks_for((batch + H2_NORM_CHUNK - 1) / H2_NORM_CHUNK, 64);

@@ -116,6 +116,9 @@ struct Context {
                                              // batched commits: only a pass that is resident at once gains
     bool fast_now = false;                   // ... the pass being issued is such a fast one
     bool last_fast = false;                  // ... the most recent pass was
+    bool fast_retry = false;                 // the pass being issued re-runs, in full, a fast pass whose flags came back set
+    uint32_t last_plan[8] = {};              // what the most recent MSM pass ran, recorded on the host (h2_test_last_msm_plan)
+    bool have_plan = false;
     uint32_t *h_flags = nullptr;             // pinned host copy of the two flags
     uint32_t sort_bins = 1;                  // single-pass binned sort (0: always the exact two-pass sort)
     uint32_t glv_on = 1;                     // GLV endomorphism split for one-shot / table-less MSMs

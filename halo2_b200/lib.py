@@ -26,7 +26,7 @@ SYMBOLS = [
     "h2_poly_coeff_to_extended", "h2_poly_extended_to_coeff", "h2_msm_registered_polys", "h2_msm_registered_polys_affine", "h2_ipa_begin_poly", "h2_ipa_round_affine", "h2_poly_add_at", "h2_poly_copy", "h2_poly_eval", "h2_poly_inner_product", "h2_poly_kate_division", "h2_poly_divide_by_vanishing", "h2_poly_eval_ast", "h2_poly_batch_invert", "h2_poly_lookup_permute", "h2_poly_running_product", "h2_poly_compute_s", "h2_poly_scale_add", "h2_set_window_bits", "h2_set_glv", "h2_set_sort_mode", "h2_msm_dev", "h2_point_sum", "h2_point_sum_dev", "h2_multi_init", "h2_multi_count", "h2_msm_multi_gpu", "h2_multi_bases_register", "h2_multi_bases_release", "h2_msm_multi_registered", "h2_test_set_staging", "h2_test_set_copy_threads", "h2_test_set_batched_affine", "h2_test_set_ntt_tma", "h2_ntt",
     "h2_intt_scaled", "h2_coeff_to_extended", "h2_extended_to_coeff", "h2_ntt_dev", "h2_ntt_clear_cache",
     "h2_ec_fft", "h2_batch_normalize", "h2_params_lagrange", "h2_hash_to_curve", "h2_params_new", "h2_points_compress", "h2_points_decompress",
-    "h2_dev_gen_points", "h2_dev_convert", "h2_test_last_msm_flags", "h2_test_set_chunk_threshold", "h2_test_set_chunk_cuts", "h2_test_set_graphs", "h2_test_set_poly_cta", "h2_test_set_fast_fixed", "h2_test_set_ecfft_quad", "h2_test_set_accum_ways", "h2_test_field_op", "h2_test_curve_op", "h2_bench_field_mul", "h2_bench_latency",
+    "h2_dev_gen_points", "h2_dev_convert", "h2_test_last_msm_flags", "h2_test_last_msm_plan", "h2_test_set_chunk_threshold", "h2_test_set_chunk_cuts", "h2_test_set_graphs", "h2_test_set_poly_cta", "h2_test_set_fast_fixed", "h2_test_set_ecfft_quad", "h2_test_set_accum_ways", "h2_test_field_op", "h2_test_curve_op", "h2_bench_field_mul", "h2_bench_latency",
     "h2_launch_count", "h2_profile_enable", "h2_profile_read",
 ]
 

@@ -300,6 +300,15 @@ int h2_dev_convert(int field, void *d_a, size_t n, int to_montgomery, void *stre
 /* Test hook: bit 0 = the most recent MSM split some bucket over several work items, bit 1 = it used the exact
  * (two-pass) sort.  Synchronises the device. */
 int h2_test_last_msm_flags(uint32_t *out);
+/* Test hook: what the most recent MSM pass over at least one term ran, recorded on the host (graph replays included):
+ *   out[0] mode: 0 one-shot (no table), 1 window table, 2 digit-multiples table (direct sum)
+ *   out[1] window bits c   out[2] windows W   out[3] scalar vectors in the pass (sets)
+ *   out[4] accumulation: 0 cooperating lanes per work item, 1 a thread per work item (msm_accum0_kernel and the partial-merge
+ *          levels), 2 the direct sum of mode 2
+ *   out[5] natural (work items = the buckets in index order)   out[6] fast (fixed-base pass without the fallback kernels)
+ *   out[7] 1 if this pass re-ran, in full, a fast pass whose device flags came back set
+ * Fails if no MSM has run. */
+int h2_test_last_msm_plan(uint32_t out[8]);
 /* Test hook: h2_msm uploads the bases of inputs with >= 2^log2_n points in chunks that are sorted and accumulated
  * separately while the next chunk is on the PCIe link (default 19). */
 int h2_test_set_chunk_threshold(uint32_t log2_n);

@@ -1,7 +1,9 @@
 """GPU test: the proof-shaped replay of create_proof's hot path (tests/prover_replay.py) produces THE SAME PROOF BYTES through
 the engine (device-resident polynomials, fixed-base MSMs over the resident generators, fold-free IPA rounds) and through the
 C restatement of the reference algorithm, with the reference's Blake2b transcript (transcript.rs:160-219) in both arms and
-the challenges fed back into the computation.  BASELINE.json's north star: "bit-identical proof transcripts"."""
+the challenges fed back into the computation.  BASELINE.json's north star: "bit-identical proof transcripts".
+k = 14 and 16 are the sizes bench.py replays; from k = 16 the opening's rounds accumulate with a thread per work item and the
+evaluations run 4-level reduction trees."""
 import numpy as np
 import pytest
 
@@ -21,7 +23,7 @@ def eng():
     return halo2_b200
 
 
-@pytest.mark.parametrize("k,real_params", [(5, True), (8, False), (10, False)])
+@pytest.mark.parametrize("k,real_params", [(5, True), (8, False), (10, False), (14, False), (16, False), (17, False)])
 def test_replay_transcript_identical(eng, k, real_params):
     n = 1 << k
     c = pasta.VESTA

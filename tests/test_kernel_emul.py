@@ -186,27 +186,30 @@ def test_emul_msm_fixed_base_table(emu, curve):
             pts[7] = (g[0], c.p - g[1])
         pb = cref.affines_to_bytes(pts)
         want = cref.bytes_to_affine(cref.best_multiexp(curve, kb, pb))
-        for cb, t, kn in ((0, 0, 0), (4, 2, 4), (7, 0, 0), (13, 3, 8), (16, 0, 0)):
+        # 15 / 16 / 17 / 20: the default table windows from k = 14 on; 24 (2^23 buckets, seconds on the host) at one size only
+        for cb, t, kn in ((0, 0, 0), (4, 2, 4), (7, 0, 0), (13, 3, 8), (15, 0, 0), (16, 0, 0), (17, 0, 0), (20, 0, 0)) + (((24, 0, 0),) if n == 130 else ()):
             assert _msm_fixed(emu, curve, kb, pb, cb, t, kn) == want, (n, cb, t, kn)
     n = 64
     pb = cref.gen_points(curve, 9, n)
     for ks in ([0] * n, [1] * n, [c.r - 1] * n, [i & 1 for i in range(n)], [(1 << (i * 4 % 255)) % c.r for i in range(n)]):
         kb = cref.ints_to_bytes(ks)
         want = cref.bytes_to_affine(cref.best_multiexp(curve, kb, pb))
-        for cb in (5, 16):
-            assert _msm_fixed(emu, curve, kb, pb, cb) == want
+        for cb in (5, 15, 16, 17, 20):
+            assert _msm_fixed(emu, curve, kb, pb, cb) == want, cb
 
 
 @pytest.mark.parametrize("curve", ["pallas", "vesta"])
 def test_emul_msm_fixed_batch(emu, curve):
-    """Several scalar vectors against one table in a single pass (bucket set = vector index)."""
+    """Several scalar vectors against one table in a single pass (bucket set = vector index): a uniform, a 0/1 and an r - 1
+    column, at small windows and at the default table windows of production sizes (15, 17, 20) and the largest (24)."""
     c = pasta.CURVES[curve]
     n, sets = 70, 3
     pb = cref.gen_points(curve, 77, n)
     kbs = [cref.gen_scalars(c.scalar, 80 + k, n) for k in range(sets)]
     kbs[1] = cref.ints_to_bytes([i & 1 for i in range(n)])
+    kbs[2] = cref.ints_to_bytes([c.r - 1] * n)
     out = np.zeros(96 * sets, dtype=np.uint8)
-    for cb in (5, 13):
+    for cb in (5, 13, 15, 17, 20, 24):
         r = emu.emu_msm_fixed_batch(cref.CURVE_ID[curve], cref._p(np.ascontiguousarray(np.concatenate(kbs))), cref._p(pb),
                                     ctypes.c_size_t(n), sets, cb, cref._p(out))
         assert r > 0
