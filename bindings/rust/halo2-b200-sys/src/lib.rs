@@ -96,6 +96,10 @@ extern "C" {
     pub fn h2_multi_bases_register(curve: c_int, bases_xy: *const c_void, n: usize, repr: c_int, handle: *mut u64) -> c_int;
     pub fn h2_multi_bases_release(handle: u64) -> c_int;
     pub fn h2_msm_multi_registered(handle: u64, scalars: *const c_void, n: usize, repr: c_int, out_xyz: *mut c_void) -> c_int;
+    // prover lanes: one context per prover thread on the primary device
+    pub fn h2_lane_create(lane: *mut u64) -> c_int;
+    pub fn h2_lane_bind(lane: u64) -> c_int;
+    pub fn h2_lane_destroy(lane: u64) -> c_int;
 }
 
 fn check(rc: c_int) {
@@ -413,6 +417,33 @@ impl<C: B200Curve> Drop for ResidentBases<C> {
 /// Call once per process (one process per GPU).
 pub fn init(device: i32) {
     check(unsafe { h2_init(device) });
+}
+
+/// A prover lane bound to the current thread: every engine call this thread makes while the guard lives runs on a context
+/// of its own (streams, scratch, caches, settings, resident polynomials and IPA sessions), concurrently with threads on other
+/// lanes.  `ResidentBases` are shared by all lanes; resident polynomials (`h2_poly_*`) and IPA sessions belong to the lane
+/// they were created on and are freed with it.  Dropping the guard destroys the lane and puts the thread back on the primary context.
+/// Binding is per thread, so the guard is `!Send`.
+pub struct Lane {
+    handle: u64,
+    _not_send: std::marker::PhantomData<*const ()>,
+}
+impl Lane {
+    /// Creates a lane and binds the calling thread to it (after `init`; at most 16 lanes).
+    pub fn new() -> Self {
+        let mut handle = 0u64;
+        check(unsafe { h2_lane_create(&mut handle) });
+        if unsafe { h2_lane_bind(handle) } != 0 {
+            unsafe { h2_lane_destroy(handle) };
+            check(1);
+        }
+        Self { handle, _not_send: Default::default() }
+    }
+}
+impl Drop for Lane {
+    fn drop(&mut self) {
+        unsafe { h2_lane_destroy(self.handle) };
+    }
 }
 
 /// One process, several GPUs: after `init(primary)`, bind `ngpu` devices; `best_multiexp_multi_gpu` then shards every call

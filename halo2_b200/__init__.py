@@ -5,7 +5,7 @@ The compute path is the sm_90a CUDA library `_lib/libhalo2_b200.so` (C ABI:
 include/halo2_b200.h).  There is no CPU fallback: importing works anywhere, but every
 operation raises `H2Error` unless the library is built and an H100 is visible.
 """
-from .lib import H2Error, lib_path, load, init, launch_count  # noqa: F401
+from .lib import H2Error, Lane, lib_path, load, init, launch_count  # noqa: F401
 from .arithmetic import (best_multiexp, small_multiexp, best_fft, best_fft_curve, batch_normalize, multiexp_window_bits,  # noqa: F401
                          eval_polynomial, compute_inner_product, kate_division)
 from .poly import (Params, EvaluationDomain, Blind, ResidentPoly, lagrange_generators, compress_points, decompress_points, hash_to_curve,  # noqa: F401
@@ -16,7 +16,7 @@ from .evaluator import Ast, AstLeaf, Evaluator  # noqa: F401
 from .verifier import MSM, Guard, VerifyError, verify_proof, compute_b  # noqa: F401
 from . import multiopen, opening  # noqa: F401
 
-__all__ = ["Ast", "AstLeaf", "Evaluator", "MSM", "Guard", "VerifyError", "verify_proof", "compute_b", "multiopen", "opening", "H2Error", "lib_path", "load", "init", "launch_count", "best_multiexp", "small_multiexp", "best_fft",
+__all__ = ["Ast", "AstLeaf", "Evaluator", "MSM", "Guard", "VerifyError", "verify_proof", "compute_b", "multiopen", "opening", "H2Error", "Lane", "lib_path", "load", "init", "launch_count", "best_multiexp", "small_multiexp", "best_fft",
            "best_fft_curve", "batch_normalize", "multiexp_window_bits", "Params", "EvaluationDomain", "Blind", "ResidentPoly",
            "lagrange_generators", "compress_points", "decompress_points", "hash_to_curve",
            "eval_polynomial", "compute_inner_product", "kate_division", "eval_polynomial_resident", "inner_product_resident",

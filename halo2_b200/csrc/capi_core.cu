@@ -4,23 +4,91 @@
 static thread_local std::string g_err;
 int fail(const std::string &m) { g_err = m; return 1; }
 const std::string &last_error_string() { return g_err; }
+// Global because a release of a shared window table must invalidate the graphs of every lane; a lane that grows its own
+// scratch invalidates the others' graphs too, which costs one re-capture each and nothing else.
 std::atomic<uint64_t> g_alloc_gen{0};
 Context g_ctxs[H2_MAX_DEVICES];
+Context g_lanes[H2_MAX_LANES];
+Context g_dead;
 Context *g_primary = &g_ctxs[0];
 thread_local Context *g_cur = nullptr;
+thread_local uint64_t g_cur_epoch = 0;
+std::atomic<uint64_t> g_epoch{0};
 std::vector<int> g_multi;                // devices of the multi-GPU entry points (h2_multi_init), primary first
-std::mutex g_mu;
-bool g_prof_on = false;
+std::mutex g_life_mu, g_reg_mu;
+static std::atomic<uint64_t> g_next_handle{1};
+uint64_t new_handle() { return g_next_handle.fetch_add(1); }
+
+// ---- lanes ----------------------------------------------------------------------------------------------------------
+// Slot i of the table is g_lanes[i]: handle 0 = free.  binds counts the host threads bound to the lane.  Both under g_reg_mu.
+struct LaneSlot { uint64_t handle = 0; uint32_t binds = 0; };
+static LaneSlot g_lane_slots[H2_MAX_LANES];
+// The calling thread's binding; a thread that exits while bound gives its binding back.
+struct LaneBinding {
+    int slot = -1; uint64_t handle = 0, epoch = 0;
+    void drop() {   // under g_reg_mu
+        if (slot >= 0 && epoch == g_epoch.load() && g_lane_slots[slot].handle == handle) g_lane_slots[slot].binds--;
+        slot = -1; handle = 0;
+    }
+    ~LaneBinding() {
+        if (slot < 0) return;
+        std::lock_guard<std::mutex> lk(g_reg_mu);
+        drop();
+    }
+};
+static thread_local LaneBinding g_binding;
+bool on_lane() { return g_binding.slot >= 0; }
+
+std::map<uint64_t, BaseSet *> g_bases;
+static std::condition_variable g_bases_cv;   // a set's users dropped to 0
+BasesRef::BasesRef(uint64_t handle, bool open_session) {
+    std::lock_guard<std::mutex> lk(g_reg_mu);
+    auto it = g_bases.find(handle);
+    if (it == g_bases.end()) return;
+    b = it->second;
+    b->users++;
+    if (open_session) b->sessions++;
+}
+BasesRef::~BasesRef() {
+    if (!b) return;
+    std::lock_guard<std::mutex> lk(g_reg_mu);
+    if (--b->users == 0) g_bases_cv.notify_all();
+}
+void bases_session_end(uint64_t handle) {
+    std::lock_guard<std::mutex> lk(g_reg_mu);
+    auto it = g_bases.find(handle);
+    if (it != g_bases.end() && it->second->sessions) it->second->sessions--;
+}
+static void bases_free(BaseSet *b) { b->buf.release(); b->table.release(); b->dtable.release(); delete b; }
+// Waits for the calls on any lane that are reading the set; refuses while an open IPA session on any lane refers to it.
+extern "C" int h2_bases_release(uint64_t handle) {
+    std::unique_lock<std::mutex> lk(g_reg_mu);
+    auto it = g_bases.find(handle);
+    if (it == g_bases.end()) return fail("h2_bases_release: unknown handle");
+    BaseSet *b = it->second;
+    if (b->sessions) return fail("h2_bases_release: an open IPA session uses the base set (h2_ipa_finish it first)");
+    g_bases.erase(it);                   // no new user finds it
+    g_bases_cv.wait(lk, [b] { return b->users == 0; });
+    const int dev = g_primary->device;
+    lk.unlock();
+    cudaSetDevice(dev);
+    cudaDeviceSynchronize();
+    bases_free(b);
+    return 0;
+}
+
+std::atomic<bool> g_prof_on{false};
 std::vector<ProfSpan> g_prof;
+// primary-context work only: lanes (and the secondary devices of a multi-GPU call) run on other threads
 void prof_begin(int kind, cudaStream_t s) {
-    if (!g_prof_on) return;
+    if (!g_prof_on || &g_ctx != g_primary) return;
     ProfSpan sp; sp.kind = kind;
     cudaEventCreate(&sp.e0); cudaEventCreate(&sp.e1);
     cudaEventRecord(sp.e0, s);
     g_prof.push_back(sp);
 }
 void prof_end(cudaStream_t s) {
-    if (!g_prof_on || g_prof.empty()) return;
+    if (!g_prof_on || g_prof.empty() || &g_ctx != g_primary) return;
     cudaEventRecord(g_prof.back().e1, s);
 }
 std::atomic<uint64_t> g_launches{0};
@@ -211,6 +279,7 @@ int download_sync(void *h_dst, const void *d_src, size_t bytes, cudaStream_t s) 
 }
 
 int require_ready() {
+    if (&g_ctx == &g_dead) return fail("the lane this thread was bound to was destroyed by h2_shutdown: bind another (h2_lane_bind, 0 = the primary context)");
     if (!g_ctx.ready) return fail("h2_init has not been called (or failed): no CUDA device bound; there is no CPU fallback");
     CU(cudaSetDevice(g_ctx.device));
     return 0;
@@ -262,9 +331,13 @@ static void ctx_destroy(Context &C) {
     for (DevBuf *b : all) b->release();
     for (auto *t : C.twiddles) { t->buf.release(); delete t; }
     C.twiddles.clear();
-    for (auto &kv : C.bases) { kv.second->buf.release(); kv.second->table.release(); kv.second->dtable.release(); delete kv.second; }
-    C.bases.clear();
-    for (auto &kv : C.ipa) { IpaSession *q = kv.second; q->p.release(); q->b.release(); q->s.release(); q->scal.release(); q->out.release(); delete q; }
+    for (auto &kv : C.shards) bases_free(kv.second);
+    C.shards.clear();
+    for (auto &kv : C.ipa) {
+        IpaSession *q = kv.second;
+        bases_session_end(q->bases);
+        q->p.release(); q->b.release(); q->s.release(); q->scal.release(); q->out.release(); delete q;
+    }
     C.ipa.clear();
     for (auto &kv : C.polys) { kv.second->buf.release(); delete kv.second; }
     C.polys.clear();
@@ -284,21 +357,28 @@ static void ctx_destroy(Context &C) {
     C = Context();
 }
 extern "C" int h2_init(int device) {
-    std::lock_guard<std::mutex> lk(g_mu);
+    std::lock_guard<std::mutex> life(g_life_mu);
     if (g_primary->ready && g_primary->device == device) return 0;
     if (g_primary->ready) return fail("h2_init: already bound to another device (one process per GPU; h2_multi_init adds devices)");
     int n = 0;
     cudaError_t e = cudaGetDeviceCount(&n);
     if (e != cudaSuccess || n == 0) return fail(std::string("h2_init: no CUDA device: ") + cudaGetErrorString(e));
     if (device < 0 || device >= n || device >= H2_MAX_DEVICES) return fail("h2_init: device index out of range");
-    if (ctx_create(g_ctxs[device], device)) { ctx_destroy(g_ctxs[device]); return 1; }
+    {
+        std::lock_guard<std::mutex> lk(g_ctxs[device].mu.m);
+        if (ctx_create(g_ctxs[device], device)) { ctx_destroy(g_ctxs[device]); return 1; }
+    }
+    std::lock_guard<std::mutex> reg(g_reg_mu);
     g_primary = &g_ctxs[device];
     return 0;
 }
 // Single-process multi-GPU (SURVEY.md section 8(b): a Rust caller of best_multiexp is ONE process): binds contexts to
 // `ngpu` devices -- the primary one first, then the others in index order -- and enables peer access to the primary.
+// The h2_multi_* calls run on the primary context only: a thread bound to a lane is refused.
 extern "C" int h2_multi_init(int ngpu) {
-    std::lock_guard<std::mutex> lk(g_mu);
+    if (on_lane()) return fail("h2_multi_init: the multi-GPU entry points run on the primary context, not on a lane (h2_lane_bind(0))");
+    std::lock_guard<std::mutex> life(g_life_mu);
+    CtxLock lk;
     if (require_ready()) return 1;
     int n = 0;
     CU(cudaGetDeviceCount(&n));
@@ -317,73 +397,160 @@ extern "C" int h2_multi_init(int ngpu) {
         if (cudaDeviceCanAccessPeer(&can, prim, d) == cudaSuccess && can) { cudaSetDevice(prim); if (cudaDeviceEnablePeerAccess(d, 0) != cudaSuccess) cudaGetLastError(); }
     }
     CU(cudaSetDevice(prim));
+    std::lock_guard<std::mutex> reg(g_reg_mu);
     g_multi = devs;
     return 0;
 }
 extern "C" int h2_multi_count(void) {
-    std::lock_guard<std::mutex> lk(g_mu);
+    std::lock_guard<std::mutex> reg(g_reg_mu);
     return (int)g_multi.size();
 }
+void multi_bases_clear();   // capi_msm.cu
 extern "C" int h2_shutdown(void) {
-    std::lock_guard<std::mutex> lk(g_mu);
+    std::lock_guard<std::mutex> life(g_life_mu);
+    // every context's mutex: calls in flight on any lane finish first
+    std::vector<std::unique_lock<std::mutex>> held;
+    held.emplace_back(g_primary->mu.m);
+    std::vector<int> live;
+    {
+        std::lock_guard<std::mutex> reg(g_reg_mu);
+        for (int i = 0; i < H2_MAX_LANES; i++) if (g_lane_slots[i].handle) live.push_back(i);
+    }
+    for (int i : live) held.emplace_back(g_lanes[i].mu.m);
+    {   // from here on no lane handle is known and every thread bound to one finds its lane gone
+        std::lock_guard<std::mutex> reg(g_reg_mu);
+        for (auto &s : g_lane_slots) s = LaneSlot();
+        g_binding.slot = -1; g_binding.handle = 0;
+        g_epoch++;
+    }
+    for (int i : live) ctx_destroy(g_lanes[i]);
     for (int d = 0; d < H2_MAX_DEVICES; d++) ctx_destroy(g_ctxs[d]);
+    set_cur(nullptr);
+    std::lock_guard<std::mutex> reg(g_reg_mu);
+    for (auto &kv : g_bases) bases_free(kv.second);
+    g_bases.clear();
+    multi_bases_clear();
     g_multi.clear();
     g_primary = &g_ctxs[0];
     return 0;
 }
+
+// A lane: one more Context on the primary device (ctx.cuh), for one prover thread.  It starts with the library's default
+// settings and owns what is created on it.
+extern "C" int h2_lane_create(uint64_t *lane) {
+    std::lock_guard<std::mutex> life(g_life_mu);
+    if (!g_primary->ready) return fail("h2_lane_create: h2_init has not been called (or failed)");
+    int slot = -1;
+    {
+        std::lock_guard<std::mutex> reg(g_reg_mu);
+        for (int i = 0; i < H2_MAX_LANES && slot < 0; i++) if (!g_lane_slots[i].handle) slot = i;
+    }
+    if (slot < 0) return fail("h2_lane_create: all " + std::to_string(H2_MAX_LANES) + " lanes are in use (h2_lane_destroy one)");
+    Context &L = g_lanes[slot];
+    {
+        std::lock_guard<std::mutex> lk(L.mu.m);
+        if (ctx_create(L, g_primary->device)) { ctx_destroy(L); return 1; }
+    }
+    std::lock_guard<std::mutex> reg(g_reg_mu);
+    g_lane_slots[slot].handle = new_handle();
+    g_lane_slots[slot].binds = 0;
+    *lane = g_lane_slots[slot].handle;
+    return 0;
+}
+// Binds the calling host thread to `lane` (0: the primary context): every later call from this thread runs there.
+extern "C" int h2_lane_bind(uint64_t lane) {
+    std::lock_guard<std::mutex> reg(g_reg_mu);
+    int slot = -1;
+    if (lane) {
+        for (int i = 0; i < H2_MAX_LANES && slot < 0; i++) if (g_lane_slots[i].handle == lane) slot = i;
+        if (slot < 0) return fail("h2_lane_bind: unknown lane handle");
+    }
+    g_binding.drop();
+    if (slot < 0) { set_cur(nullptr); return 0; }
+    g_lane_slots[slot].binds++;
+    g_binding.slot = slot; g_binding.handle = lane; g_binding.epoch = g_epoch.load();
+    set_cur(&g_lanes[slot]);
+    return 0;
+}
+// Frees the lane's polynomials, IPA sessions, pools and streams.  Refused while another thread is bound to it; the calling
+// thread, if bound to it, goes back to the primary context.
+extern "C" int h2_lane_destroy(uint64_t lane) {
+    std::lock_guard<std::mutex> life(g_life_mu);
+    int slot = -1;
+    {
+        std::lock_guard<std::mutex> reg(g_reg_mu);
+        for (int i = 0; i < H2_MAX_LANES && slot < 0; i++) if (lane && g_lane_slots[i].handle == lane) slot = i;
+        if (slot < 0) return fail("h2_lane_destroy: unknown lane handle");
+        const bool mine = g_binding.slot == slot;
+        if (g_lane_slots[slot].binds > (mine ? 1u : 0u)) return fail("h2_lane_destroy: another thread is bound to the lane");
+        if (mine) { g_binding.drop(); set_cur(nullptr); }
+        g_lane_slots[slot] = LaneSlot();   // unknown from here on: nobody can bind it
+    }
+    std::lock_guard<std::mutex> lk(g_lanes[slot].mu.m);
+    ctx_destroy(g_lanes[slot]);
+    return 0;
+}
+
 extern "C" int h2_set_glv(int on) {
-    std::lock_guard<std::mutex> lk(g_mu);
+    CtxLock lk;
     g_ctx.glv_on = on ? 1u : 0u;
     return 0;
 }
 extern "C" int h2_set_sort_mode(int exact_only) {
-    std::lock_guard<std::mutex> lk(g_mu);
+    CtxLock lk;
     g_ctx.sort_bins = exact_only ? 0u : 1u;
     return 0;
 }
 // test hook: flags of the most recent MSM -- bit 0: some bucket was split into several work items, bit 1: the exact
 // sort ran (bin overflow, or no bins).  Synchronises the device.
 extern "C" int h2_test_last_msm_flags(uint32_t *out) {
-    std::lock_guard<std::mutex> lk(g_mu);
+    CtxLock lk;
     if (require_ready()) return 1;
     if (!g_ctx.last_flags) return fail("h2_test_last_msm_flags: no MSM has run");
     uint32_t f[2];
     CU(cudaDeviceSynchronize());
-    CU(cudaMemcpy(f, g_ctx.last_flags, sizeof f, cudaMemcpyDeviceToHost));
+    CU(cudaMemcpyAsync(f, g_ctx.last_flags, sizeof f, cudaMemcpyDeviceToHost, g_ctx.stream));   // not on the legacy default stream
+    CU(cudaStreamSynchronize(g_ctx.stream));
     *out = (f[0] ? 1u : 0u) | (f[1] ? 2u : 0u);
     return 0;
 }
 // test hook: what the most recent MSM pass ran (recorded on the host by msm_run; layout in include/halo2_b200.h)
 extern "C" int h2_test_last_msm_plan(uint32_t out[8]) {
-    std::lock_guard<std::mutex> lk(g_mu);
+    CtxLock lk;
     if (require_ready()) return 1;
     if (!g_ctx.have_plan) return fail("h2_test_last_msm_plan: no MSM has run");
     memcpy(out, g_ctx.last_plan, sizeof g_ctx.last_plan);
     return 0;
 }
+// The settings hooks below act on the calling thread's lane; on the primary context they act on every device's context,
+// so that the multi-GPU workers follow.
+static void for_settings(const std::function<void(Context &)> &f) {
+    if (on_lane()) { f(g_ctx); return; }
+    for (int d = 0; d < H2_MAX_DEVICES; d++) f(g_ctxs[d]);
+}
 // test / A-B hook: fixed-base passes first run without their fallback kernels (1, default) or always run the full pass (0)
 extern "C" int h2_test_set_fast_fixed(int on) {
-    std::lock_guard<std::mutex> lk(g_mu);
+    CtxLock lk;
     // on > 1 (tuning): log2 of the bucket count up to which a fast pass takes its buckets in index order (on = 2: never)
-    for (int d = 0; d < H2_MAX_DEVICES; d++) { g_ctxs[d].fast_on = on ? 1u : 0u; if (on > 1) g_ctxs[d].natural_max_buckets = on == 2 ? 0 : 1ull << on; }
+    for_settings([on](Context &C) { C.fast_on = on ? 1u : 0u; if (on > 1) C.natural_max_buckets = on == 2 ? 0 : 1ull << on; });
     return 0;
 }
 // test hook: small polynomials reduce in one CTA each (1, default) or through the level tree like large ones (0)
 extern "C" int h2_test_set_poly_cta(int on) {
-    std::lock_guard<std::mutex> lk(g_mu);
-    for (int d = 0; d < H2_MAX_DEVICES; d++) g_ctxs[d].poly_cta = on ? 1u : 0u;
+    CtxLock lk;
+    for_settings([on](Context &C) { C.poly_cta = on ? 1u : 0u; });
     return 0;
 }
 // test hook: CUDA-graph replay of fixed-base MSMs on / off
 extern "C" int h2_test_set_graphs(int on) {
-    std::lock_guard<std::mutex> lk(g_mu);
+    CtxLock lk;
     g_ctx.graphs_on = on ? 1u : 0u;
     return 0;
 }
 // test hook: quads per work item of the small-problem accumulation (1, 2 or 4).  Invalidates nothing: graphs are keyed by
 // their parameters only, so flip it before the first fixed-base MSM of a base set or with graphs off.
 extern "C" int h2_test_set_accum_ways(uint32_t ways) {
-    std::lock_guard<std::mutex> lk(g_mu);
+    CtxLock lk;
     if (ways >> 8) { g_ctx.small_accum_refs = 1ull << (ways >> 8); ways &= 0xffu; }   // tuning: bits 8.. = log2 of the reference count up to which lanes cooperate
     if (ways != 0 && ways != 1 && ways != 2 && ways != 4 && ways != 12 && ways != 14)
         return fail("h2_test_set_accum_ways: 0 (a pair of lanes), 1, 2 or 4 (quads), 12 / 14 (2 / 4 independent lanes per item)");
@@ -394,19 +561,19 @@ extern "C" int h2_test_set_accum_ways(uint32_t ways) {
 // test / tuning hook: batched-affine halving rounds ahead of the XYZZ accumulation of large one-shot MSMs (0 = classic
 // accumulation only, at most 3) and the pairs per thread that share one inversion (0 keeps the current value)
 extern "C" int h2_test_set_batched_affine(uint32_t rounds, uint32_t pairs_per_thread) {
-    std::lock_guard<std::mutex> lk(g_mu);
+    CtxLock lk;
     const uint32_t variant = rounds >> 8;     // bits 8..: kernel variant + 1 (tuning; 0 = the default variant)
     rounds &= 0xffu;
     if (rounds > H2_BA_MAX_ROUNDS) return fail("h2_test_set_batched_affine: at most 3 rounds");
-    for (int d = 0; d < H2_MAX_DEVICES; d++) {
-        g_ctxs[d].ba_rounds = rounds; g_ctxs[d].ba_variant = variant ? variant - 1 : 3;
-        if (pairs_per_thread) g_ctxs[d].ba_target = pairs_per_thread;
-    }
+    for_settings([=](Context &C) {
+        C.ba_rounds = rounds; C.ba_variant = variant ? variant - 1 : 3;
+        if (pairs_per_thread) C.ba_target = pairs_per_thread;
+    });
     return 0;
 }
 // test hook: EC-FFT butterfly form -- 1: quads of lanes, 0: one thread each, -1: by size (the default)
 extern "C" int h2_test_set_ecfft_quad(int on) {
-    std::lock_guard<std::mutex> lk(g_mu);
+    CtxLock lk;
     g_ctx.ecfft_quad = on < 0 ? 1u : on ? 2u : 0u;   // -1: by size (default), 0: thread form, 1: quad form
     return 0;
 }
@@ -414,7 +581,7 @@ extern "C" int h2_test_set_ecfft_quad(int on) {
 // tuning hook: where a k-chunk upload cuts its points, in sixteenths (k = 2 .. 4; c1 < c2 < c3 < 16, unused ones ignored)
 extern uint32_t g_chunk_cut[H2_MAX_UPLOAD_CHUNKS + 1][H2_MAX_UPLOAD_CHUNKS + 1];
 extern "C" int h2_test_set_chunk_cuts(uint32_t k, uint32_t c1, uint32_t c2, uint32_t c3) {
-    std::lock_guard<std::mutex> lk(g_mu);
+    CtxLock lk;
     if (k < 2 || k > H2_MAX_UPLOAD_CHUNKS) return fail("h2_test_set_chunk_cuts: k must be 2, 3 or 4");
     const uint32_t c[5] = {0, c1, k > 2 ? c2 : 16, k > 3 ? c3 : 16, 16};
     for (uint32_t j = 1; j <= 4; j++) if (c[j] < c[j - 1] || c[j] > 16 || (j < k && c[j] == c[j - 1])) return fail("h2_test_set_chunk_cuts: cuts must increase, below 16");
@@ -422,20 +589,20 @@ extern "C" int h2_test_set_chunk_cuts(uint32_t k, uint32_t c1, uint32_t c2, uint
     return 0;
 }
 extern "C" int h2_test_set_chunk_threshold(uint32_t log2_n) {
-    std::lock_guard<std::mutex> lk(g_mu);
+    CtxLock lk;
     if (log2_n > 40) return fail("h2_test_set_chunk_threshold: log2_n > 40");
     g_ctx.chunk_min_log = log2_n;
     return 0;
 }
 extern "C" int h2_set_window_bits(uint32_t c) {
     if (c > 24) return fail("h2_set_window_bits: c must be <= 24");
-    std::lock_guard<std::mutex> lk(g_mu);
+    CtxLock lk;
     g_ctx.window_override = c;
     return 0;
 }
 
 extern "C" int h2_dev_gen_points(int curve, uint64_t seed, uint64_t first, size_t n, void *d_out, void *stream) {
-    std::lock_guard<std::mutex> lk(g_mu);
+    CtxLock lk;
     if (require_ready()) return 1;
     cudaStream_t s = (cudaStream_t)stream;
     if (n == 0) return 0;
@@ -445,7 +612,7 @@ extern "C" int h2_dev_gen_points(int curve, uint64_t seed, uint64_t first, size_
     return 0;
 }
 extern "C" int h2_dev_convert(int field, void *d_a, size_t n, int to_montgomery, void *stream) {
-    std::lock_guard<std::mutex> lk(g_mu);
+    CtxLock lk;
     if (require_ready()) return 1;
     cudaStream_t s = (cudaStream_t)stream;
     if (n == 0) return 0;
@@ -455,7 +622,7 @@ extern "C" int h2_dev_convert(int field, void *d_a, size_t n, int to_montgomery,
     return 0;
 }
 extern "C" int h2_test_field_op(int field, int op, const void *a, const void *b, size_t n, void *out) {
-    std::lock_guard<std::mutex> lk(g_mu);
+    CtxLock lk;
     if (require_ready()) return 1;
     Context &X = g_ctx;
     cudaStream_t s = X.stream;
@@ -472,7 +639,7 @@ extern "C" int h2_test_field_op(int field, int op, const void *a, const void *b,
     return 0;
 }
 extern "C" int h2_test_curve_op(int curve, int op, const void *a_xy, const void *b_xy, size_t n, void *out_xy) {
-    std::lock_guard<std::mutex> lk(g_mu);
+    CtxLock lk;
     if (require_ready()) return 1;
     Context &X = g_ctx;
     cudaStream_t s = X.stream;
@@ -489,7 +656,7 @@ extern "C" int h2_test_curve_op(int curve, int op, const void *a_xy, const void 
     return 0;
 }
 extern "C" int h2_bench_field_mul(int field, uint32_t threads_per_block, uint32_t blocks, uint32_t iters, float *ms) {
-    std::lock_guard<std::mutex> lk(g_mu);
+    CtxLock lk;
     if (require_ready()) return 1;
     Context &X = g_ctx;
     cudaStream_t s = X.stream;
@@ -517,7 +684,7 @@ extern "C" int h2_bench_field_mul(int field, uint32_t threads_per_block, uint32_
 // mode: 0 dependent mul chain, 1 two chains, 2 four chains, 3 xyzz_double, 4 xyzz_add, 5 xyzz_add_mixed;
 // one warp, `iters` iterations; *ms = elapsed.
 extern "C" int h2_bench_latency(int mode, uint32_t iters, float *ms) {
-    std::lock_guard<std::mutex> lk(g_mu);
+    CtxLock lk;
     if (require_ready()) return 1;
     Context &X = g_ctx;
     cudaStream_t s = X.stream;
@@ -540,8 +707,9 @@ extern "C" int h2_bench_latency(int mode, uint32_t iters, float *ms) {
 // ------------------------------------------------------------------------------------------------
 // per-kernel timing for the roofline leg of bench.py
 // ------------------------------------------------------------------------------------------------
+// The records (g_prof) are of primary-context work and guarded by the primary's mutex, whichever thread asks.
 extern "C" int h2_profile_enable(int on) {
-    std::lock_guard<std::mutex> lk(g_mu);
+    std::lock_guard<std::mutex> lk(g_primary->mu.m);
     if (require_ready()) return 1;
     cudaDeviceSynchronize();
     for (auto &sp : g_prof) { cudaEventDestroy(sp.e0); cudaEventDestroy(sp.e1); }
@@ -551,7 +719,7 @@ extern "C" int h2_profile_enable(int on) {
 }
 // kind 0 = msm_accum0_kernel, 1 = ntt_pass_kernel.  Returns summed device time and launch count.
 extern "C" int h2_profile_read(int kind, float *total_ms, uint32_t *launches) {
-    std::lock_guard<std::mutex> lk(g_mu);
+    std::lock_guard<std::mutex> lk(g_primary->mu.m);
     if (require_ready()) return 1;
     CU(cudaDeviceSynchronize());
     float tot = 0; uint32_t cnt = 0;

@@ -73,7 +73,7 @@ static int ecfft_host(int scalar_field, int mode, const void *in, uint32_t log_n
     return 0;
 }
 static int ecfft_host_dispatch(int curve, int mode, const void *in, uint32_t log_n, const void *omega, const void *scale, int repr, void *out) {
-    std::lock_guard<std::mutex> lk(g_mu);
+    CtxLock lk;
     if (require_ready()) return 1;
     if (log_n > 26) return fail("ec_fft: log_n > 26 not supported");
     if (curve == H2_CURVE_PALLAS) return ecfft_host<FpParams, FqParams>(H2_FIELD_FQ, mode, in, log_n, omega, scale, repr, out);
@@ -121,7 +121,7 @@ static int hash_to_curve_host(const char *domain_prefix, const void *msgs, size_
     return 0;
 }
 extern "C" int h2_hash_to_curve(int curve, const char *domain_prefix, const void *messages, size_t msg_len, size_t n, int repr, void *out_xy) {
-    std::lock_guard<std::mutex> lk(g_mu);
+    CtxLock lk;
     if (require_ready()) return 1;
     if (curve != H2_CURVE_PALLAS && curve != H2_CURVE_VESTA) return fail("unknown curve id");
     if (!domain_prefix) return fail("h2_hash_to_curve: domain_prefix is NULL");
@@ -161,7 +161,7 @@ static int params_new_host(int scalar_field, uint32_t k, int repr, void *g_xy, v
     return ecfft_host<P, PS>(scalar_field, 1, nullptr, k, alpha_inv.v, minv.v, repr, gl_xy);   // releases the scratch, synchronises
 }
 extern "C" int h2_params_new(int curve, uint32_t k, int repr, void *out_g_xy, void *out_g_lagrange_xy, void *out_w_xy, void *out_u_xy) {
-    std::lock_guard<std::mutex> lk(g_mu);
+    CtxLock lk;
     if (require_ready()) return 1;
     if (k > 26) return fail("h2_params_new: k > 26 not supported");
     if (!out_g_xy || !out_g_lagrange_xy || !out_w_xy || !out_u_xy) return fail("h2_params_new: NULL output");
@@ -170,7 +170,7 @@ extern "C" int h2_params_new(int curve, uint32_t k, int repr, void *out_g_xy, vo
     return fail("unknown curve id");
 }
 extern "C" int h2_batch_normalize(int curve, const void *points_xyz, size_t n, int repr, void *out_xy) {
-    std::lock_guard<std::mutex> lk(g_mu);
+    CtxLock lk;
     if (require_ready()) return 1;
     if (curve != H2_CURVE_PALLAS && curve != H2_CURVE_VESTA) return fail("unknown curve id");
     if (n == 0) return 0;
@@ -220,7 +220,7 @@ template <class P> static int points_codec(int decompress, const void *in, size_
     return 0;
 }
 static int points_codec_dispatch(int curve, int decompress, const void *in, size_t n, int repr, void *out) {
-    std::lock_guard<std::mutex> lk(g_mu);
+    CtxLock lk;
     if (require_ready()) return 1;
     if (curve != H2_CURVE_PALLAS && curve != H2_CURVE_VESTA) return fail("unknown curve id");
     if (n >= (1ull << 32)) return fail("points codec: n >= 2^32");

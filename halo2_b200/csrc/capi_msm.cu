@@ -409,7 +409,7 @@ int convert_points(int curve, affine *d, size_t n, int to_mont, cudaStream_t s) 
 
 extern "C" int h2_msm_dev(int curve, const void *d_scalars, int scalars_repr, const void *d_bases, size_t n, uint32_t window_bits,
                           void *d_out_xyz, void *stream) {
-    std::lock_guard<std::mutex> lk(g_mu);
+    CtxLock lk;
     if (require_ready()) return 1;
     cudaStream_t s = (cudaStream_t)stream;
     if (scratch_acquire(s)) return 1;
@@ -453,7 +453,7 @@ static int msm_host_common(int curve, const void *scalars, size_t n_scalars, con
         // The uploads run on their own host thread: from pageable caller memory they are staged through the pinned ring
         // (upload_async blocks while it copies), and the kernels of chunk j must be issued while chunk j + 1 is staged.
         auto upload = [=, &recorded, &up_failed, &up_err]() {
-            g_cur = ctx;
+            set_cur(ctx);
             auto run = [&]() -> int {
                 CU(cudaSetDevice(ctx->device));
                 for (uint32_t j = 0; j < k; j++) {
@@ -497,7 +497,7 @@ static int msm_host_common(int curve, const void *scalars, size_t n_scalars, con
 }
 
 extern "C" int h2_msm(int curve, const void *scalars, const void *bases_xy, size_t n, int repr, void *out_xyz) {
-    std::lock_guard<std::mutex> lk(g_mu);
+    CtxLock lk;
     if (require_ready()) return 1;
     if (curve != H2_CURVE_PALLAS && curve != H2_CURVE_VESTA) return fail("unknown curve id");
     Context &X = g_ctx;
@@ -515,7 +515,7 @@ extern "C" int h2_bases_register_ex(int curve, const void *bases_xy, size_t n, i
     return bases_register_impl(curve, bases_xy, n, repr, window_bits, flags, handle);
 }
 static int bases_register_impl(int curve, const void *bases_xy, size_t n, int repr, uint32_t window_bits, uint32_t flags, uint64_t *handle) {
-    std::lock_guard<std::mutex> lk(g_mu);
+    CtxLock lk;
     if (require_ready()) return 1;
     if (curve != H2_CURVE_PALLAS && curve != H2_CURVE_VESTA) return fail("unknown curve id");
     BaseSet *b = new BaseSet();
@@ -529,30 +529,20 @@ static int bases_register_impl(int curve, const void *bases_xy, size_t n, int re
     if ((flags & H2_BASES_PRECOMPUTE) && n > 0 && build_table(b, direct ? H2_FB_BITS : window_bits, s)) return drop();
     if (direct && build_direct(b, s)) return drop();
     if (cudaStreamSynchronize(s) != cudaSuccess) { fail("h2_bases_register: device error while building the tables"); return drop(); }
-    uint64_t h = g_ctx.next_handle++;
-    g_ctx.bases[h] = b;
+    const uint64_t h = new_handle();
+    {   // shared by every lane from here on (h2_bases_release: capi_core.cu)
+        std::lock_guard<std::mutex> reg(g_reg_mu);
+        g_bases[h] = b;
+    }
     *handle = h;
     return 0;
 }
-extern "C" int h2_bases_release(uint64_t handle) {
-    std::lock_guard<std::mutex> lk(g_mu);
-    auto it = g_ctx.bases.find(handle);
-    if (it == g_ctx.bases.end()) return fail("h2_bases_release: unknown handle");
-    cudaSetDevice(g_ctx.device);
-    cudaDeviceSynchronize();
-    it->second->buf.release();
-    it->second->table.release();
-    it->second->dtable.release();
-    delete it->second;
-    g_ctx.bases.erase(it);
-    return 0;
-}
 extern "C" int h2_msm_registered(uint64_t handle, const void *scalars, size_t n, const void *extra_scalar, int repr, void *out_xyz) {
-    std::lock_guard<std::mutex> lk(g_mu);
+    CtxLock lk;
     if (require_ready()) return 1;
-    auto it = g_ctx.bases.find(handle);
-    if (it == g_ctx.bases.end()) return fail("h2_msm_registered: unknown handle");
-    BaseSet *b = it->second;
+    BasesRef ref(handle);
+    if (!ref.b) return fail("h2_msm_registered: unknown handle");
+    BaseSet *b = ref.b;
     size_t total = n + (extra_scalar ? 1 : 0);
     if (total > b->n) return fail("h2_msm_registered: more scalars than registered bases");
     if (b->table.p) {   // fixed-base path: digit-multiples table (direct sum) or window table (one shared bucket set)
@@ -579,11 +569,11 @@ extern "C" int h2_msm_registered_batch_affine(uint64_t handle, const void *scala
 }
 static int msm_registered_batch_impl(uint64_t handle, const void *scalars, size_t n, const void *extra_scalars, size_t batch, int repr,
                                      void *out_xyz, int affine_out) {
-    std::lock_guard<std::mutex> lk(g_mu);
+    CtxLock lk;
     if (require_ready()) return 1;
-    auto it = g_ctx.bases.find(handle);
-    if (it == g_ctx.bases.end()) return fail("h2_msm_registered_batch: unknown handle");
-    BaseSet *b = it->second;
+    BasesRef ref(handle);
+    if (!ref.b) return fail("h2_msm_registered_batch: unknown handle");
+    BaseSet *b = ref.b;
     if (!b->table.p) return fail("h2_msm_registered_batch: the base set has no window table (register with H2_BASES_PRECOMPUTE)");
     if (batch == 0) return 0;
     if (batch > 64) return fail("h2_msm_registered_batch: batch > 64");
@@ -631,7 +621,7 @@ static int msm_registered_batch_impl(uint64_t handle, const void *scalars, size_
 }
 
 extern "C" int h2_point_sum(int curve, const void *points_xyz, size_t g, int repr, void *out_xyz) {
-    std::lock_guard<std::mutex> lk(g_mu);
+    CtxLock lk;
     if (require_ready()) return 1;
     Context &X = g_ctx;
     cudaStream_t s = X.stream;
@@ -651,7 +641,7 @@ extern "C" int h2_point_sum(int curve, const void *points_xyz, size_t g, int rep
 
 // device-pointer form (the partial results of an NCCL all-gather stay on the device): Montgomery in, Montgomery out
 extern "C" int h2_point_sum_dev(int curve, const void *d_points_xyz, size_t g, void *d_out_xyz, void *stream) {
-    std::lock_guard<std::mutex> lk(g_mu);
+    CtxLock lk;
     if (require_ready()) return 1;
     cudaStream_t s = (cudaStream_t)stream;
     if (curve == H2_CURVE_PALLAS) LAUNCH(point_sum_kernel<FpParams>, 1, 32, 0, s, (const jacobian *)d_points_xyz, (uint32_t)g, 0, (jacobian *)d_out_xyz);
@@ -680,7 +670,7 @@ static int multi_run(const std::function<int(size_t)> &fn) {
     std::vector<std::thread> th;
     for (size_t g = 0; g < G; g++)
         th.emplace_back([&, g]() {
-            g_cur = &g_ctxs[g_multi[g]];
+            set_cur(&g_ctxs[g_multi[g]]);
             if (cudaSetDevice(g_multi[g]) != cudaSuccess) { rcs[g] = 1; errs[g] = "cudaSetDevice failed"; return; }
             rcs[g] = fn(g);
             if (rcs[g]) errs[g] = last_error_string();
@@ -702,8 +692,15 @@ static int multi_finish(int curve, int repr, void *out_xyz) {     // the G-term 
     CU(cudaStreamSynchronize(s));
     return 0;
 }
+// The h2_multi_* calls run on the primary context: they hold its mutex for the whole call, and g_multi, g_multi_bases and
+// the secondary devices' contexts change only under it (and g_reg_mu).  A thread bound to a lane is refused.
+static int multi_refuse_lane(const char *who) {
+    if (on_lane()) return fail(std::string(who) + ": the multi-GPU entry points run on the primary context, not on a lane (h2_lane_bind(0))");
+    return 0;
+}
 extern "C" int h2_msm_multi_gpu(int curve, const void *scalars, const void *bases_xy, size_t n, int repr, void *out_xyz) {
-    std::lock_guard<std::mutex> lk(g_mu);
+    if (multi_refuse_lane("h2_msm_multi_gpu")) return 1;
+    CtxLock lk;
     if (require_ready()) return 1;
     if (curve != H2_CURVE_PALLAS && curve != H2_CURVE_VESTA) return fail("unknown curve id");
     if (g_multi.empty()) return fail("h2_msm_multi_gpu: call h2_multi_init first");
@@ -724,21 +721,20 @@ extern "C" int h2_msm_multi_gpu(int curve, const void *scalars, const void *base
     if (rc) return rc;
     return multi_finish(curve, repr, out_xyz);
 }
-// resident shards: bases[lo_g, hi_g) live on device g (handle valid for h2_msm_multi_registered only)
+// resident shards: bases[lo_g, hi_g) live on device g, in that device context's `shards` (handle valid for
+// h2_msm_multi_registered only).  Handles come from new_handle(), so one from before an h2_shutdown is unknown after it.
 struct MultiBases { int curve; size_t n; std::vector<uint64_t> handles; };
 static std::map<uint64_t, MultiBases> g_multi_bases;
-static uint64_t g_multi_next = 1;
+void multi_bases_clear() { g_multi_bases.clear(); }   // h2_shutdown (the shards go with their contexts)
 extern "C" int h2_multi_bases_register(int curve, const void *bases_xy, size_t n, int repr, uint64_t *handle) {
-    {
-        std::lock_guard<std::mutex> lk(g_mu);
-        if (require_ready()) return 1;
-        if (curve != H2_CURVE_PALLAS && curve != H2_CURVE_VESTA) return fail("unknown curve id");
-        if (g_multi.empty()) return fail("h2_multi_bases_register: call h2_multi_init first");
-    }
+    if (multi_refuse_lane("h2_multi_bases_register")) return 1;
+    CtxLock lk;
+    if (require_ready()) return 1;
+    if (curve != H2_CURVE_PALLAS && curve != H2_CURVE_VESTA) return fail("unknown curve id");
+    if (g_multi.empty()) return fail("h2_multi_bases_register: call h2_multi_init first");
     const size_t G = g_multi.size();
     MultiBases mb;
     mb.curve = curve; mb.n = n; mb.handles.assign(G, 0);
-    std::lock_guard<std::mutex> lk(g_mu);
     int rc = multi_run([&](size_t g) -> int {
         Context &X = g_ctx;
         size_t lo, hi;
@@ -753,34 +749,41 @@ extern "C" int h2_multi_bases_register(int curve, const void *bases_xy, size_t n
             cudaStreamSynchronize(s); b->buf.release(); delete b;
             return fail("h2_multi_bases_register: upload failed");
         }
-        mb.handles[g] = X.next_handle++;
-        X.bases[mb.handles[g]] = b;
+        mb.handles[g] = new_handle();
+        X.shards[mb.handles[g]] = b;
         return 0;
     });
     if (rc) return rc;
-    *handle = g_multi_next++;
+    *handle = new_handle();
+    std::lock_guard<std::mutex> reg(g_reg_mu);
     g_multi_bases[*handle] = mb;
     return 0;
 }
 extern "C" int h2_multi_bases_release(uint64_t handle) {
-    std::lock_guard<std::mutex> lk(g_mu);
-    auto it = g_multi_bases.find(handle);
-    if (it == g_multi_bases.end()) return fail("h2_multi_bases_release: unknown handle");
-    MultiBases mb = it->second;
-    g_multi_bases.erase(it);
+    if (multi_refuse_lane("h2_multi_bases_release")) return 1;
+    CtxLock lk;
+    MultiBases mb;
+    {
+        std::lock_guard<std::mutex> reg(g_reg_mu);
+        auto it = g_multi_bases.find(handle);
+        if (it == g_multi_bases.end()) return fail("h2_multi_bases_release: unknown handle");
+        mb = it->second;
+        g_multi_bases.erase(it);
+    }
     return multi_run([&](size_t g) -> int {
         Context &X = g_ctx;
-        auto ib = X.bases.find(mb.handles[g]);
-        if (ib == X.bases.end()) return 0;
+        auto ib = X.shards.find(mb.handles[g]);
+        if (ib == X.shards.end()) return 0;
         cudaDeviceSynchronize();
         ib->second->buf.release(); ib->second->table.release(); ib->second->dtable.release();
         delete ib->second;
-        X.bases.erase(ib);
+        X.shards.erase(ib);
         return 0;
     });
 }
 extern "C" int h2_msm_multi_registered(uint64_t handle, const void *scalars, size_t n, int repr, void *out_xyz) {
-    std::lock_guard<std::mutex> lk(g_mu);
+    if (multi_refuse_lane("h2_msm_multi_registered")) return 1;
+    CtxLock lk;
     if (require_ready()) return 1;
     auto it = g_multi_bases.find(handle);
     if (it == g_multi_bases.end()) return fail("h2_msm_multi_registered: unknown handle");
@@ -796,8 +799,8 @@ extern "C" int h2_msm_multi_registered(uint64_t handle, const void *scalars, siz
         Context &X = g_ctx;
         size_t lo, hi;
         shard_range(n, g, G, &lo, &hi);
-        auto ib = X.bases.find(mb.handles[g]);
-        if (ib == X.bases.end()) return fail("h2_msm_multi_registered: a shard was released");
+        auto ib = X.shards.find(mb.handles[g]);
+        if (ib == X.shards.end()) return fail("h2_msm_multi_registered: a shard was released");
         return msm_host_common(mb.curve, (const fe *)scalars + lo, hi - lo, nullptr, ib->second->buf.as<affine>(), hi - lo, repr, nullptr, 0, 0, 0,
                                nullptr, parts + g, prim);
     });
@@ -831,28 +834,34 @@ template <class PS> static int ipa_begin_impl(IpaSession *q, const void *p_prime
     LAUNCH(twiddle_fill_kernel<PS>, blocks_for((n + 31) / 32, 128), 128, 0, s, S.b, X.pow2.as<fe>(), n);
     return 0;
 }
-static int ipa_begin_common(uint64_t bases_handle, uint32_t k, const void *p_prime, PolyBuf *p_poly, const void *x3, int repr, uint64_t *session);
+static int ipa_begin_common(uint64_t bases_handle, uint32_t k, const void *p_prime, const uint64_t *p_poly_handle, const void *x3, int repr,
+                            uint64_t *session);
 extern "C" int h2_ipa_begin(uint64_t bases_handle, uint32_t k, const void *p_prime, const void *x3, int repr, uint64_t *session) {
     return ipa_begin_common(bases_handle, k, p_prime, nullptr, x3, repr, session);
 }
 // p' taken from a device-resident polynomial (Montgomery form): nothing but x3 goes up
 extern "C" int h2_ipa_begin_poly(uint64_t bases_handle, uint32_t k, uint64_t p_prime_poly, const void *x3, int repr, uint64_t *session) {
-    PolyBuf *pp;
-    {
-        std::lock_guard<std::mutex> lk(g_mu);
-        if (require_ready()) return 1;
-        pp = find_poly(p_prime_poly);
-        if (!pp) return fail("h2_ipa_begin_poly: unknown polynomial handle");
-        if (k > 28 || pp->len < ((size_t)1 << k)) return fail("h2_ipa_begin_poly: the polynomial holds fewer than 2^k coefficients");
-    }
-    return ipa_begin_common(bases_handle, k, nullptr, pp, x3, repr, session);
+    return ipa_begin_common(bases_handle, k, nullptr, &p_prime_poly, x3, repr, session);
 }
-static int ipa_begin_common(uint64_t bases_handle, uint32_t k, const void *p_prime, PolyBuf *p_poly, const void *x3, int repr, uint64_t *session) {
-    std::lock_guard<std::mutex> lk(g_mu);
+// The session counts as a user of its base set until h2_ipa_finish: h2_bases_release refuses the set meanwhile.
+static int ipa_begin_common(uint64_t bases_handle, uint32_t k, const void *p_prime, const uint64_t *p_poly_handle, const void *x3, int repr,
+                            uint64_t *session) {
+    CtxLock lk;
     if (require_ready()) return 1;
-    auto it = g_ctx.bases.find(bases_handle);
-    if (it == g_ctx.bases.end()) return fail("h2_ipa_begin: unknown bases handle");
-    BaseSet *b = it->second;
+    PolyBuf *p_poly = nullptr;
+    if (p_poly_handle) {   // looked up and used under the one lock
+        p_poly = find_poly(*p_poly_handle);
+        if (!p_poly) return fail("h2_ipa_begin_poly: unknown polynomial handle");
+        if (k > 28 || p_poly->len < ((size_t)1 << k)) return fail("h2_ipa_begin_poly: the polynomial holds fewer than 2^k coefficients");
+    }
+    BasesRef ref(bases_handle, true);
+    if (!ref.b) return fail("h2_ipa_begin: unknown bases handle");
+    BaseSet *b = ref.b;
+    bool opened = false;
+    struct SessionGuard {   // the session count goes back unless the session opens
+        const uint64_t h; const bool &opened;
+        ~SessionGuard() { if (!opened) bases_session_end(h); }
+    } guard{bases_handle, opened};
     if (k == 0 || k > 28) return fail("h2_ipa_begin: k out of range");
     if (b->n != (1ull << k) + 2) return fail("h2_ipa_begin: the base set must hold g[0..2^k) || w || u");
     if (!b->table.p) return fail("h2_ipa_begin: the base set has no window table (register with H2_BASES_PRECOMPUTE)");
@@ -868,9 +877,10 @@ static int ipa_begin_common(uint64_t bases_handle, uint32_t k, const void *p_pri
     if (scratch_release(s)) { ipa_free(q); return 1; }
     cudaError_t e = cudaStreamSynchronize(s);   // p_prime may be pageable host memory
     if (e != cudaSuccess) { ipa_free(q); return fail(std::string("h2_ipa_begin: ") + cudaGetErrorString(e)); }
-    uint64_t h = g_ctx.next_handle++;
+    uint64_t h = new_handle();
     g_ctx.ipa[h] = q;
     *session = h;
+    opened = true;
     return 0;
 }
 template <class PS> static int ipa_round_impl(IpaSession *q, BaseSet *b, const void *z, const void *l_rand, const void *r_rand, int repr, int out_canonical, cudaStream_t s) {
@@ -892,16 +902,16 @@ extern "C" int h2_ipa_round_affine(uint64_t session, const void *z, const void *
     return ipa_round_common(session, z, l_rand, r_rand, repr, out_lr_xy, 1);
 }
 static int ipa_round_common(uint64_t session, const void *z, const void *l_rand, const void *r_rand, int repr, void *out_lr_xyz, int affine_out) {
-    std::lock_guard<std::mutex> lk(g_mu);
+    CtxLock lk;
     if (require_ready()) return 1;
     auto it = g_ctx.ipa.find(session);
     if (it == g_ctx.ipa.end()) return fail("h2_ipa_round: unknown session");
     IpaSession *q = it->second;
-    auto ib = g_ctx.bases.find(q->bases);
-    if (ib == g_ctx.bases.end()) return fail("h2_ipa_round: the session's base set was released");
+    BasesRef ref(q->bases);
+    if (!ref.b) return fail("h2_ipa_round: the session's base set was released");
     if (q->round >= q->k) return fail("h2_ipa_round: all k rounds are done");
     if (!q->folded) return fail("h2_ipa_round: h2_ipa_fold must follow each round");
-    BaseSet *b = ib->second;
+    BaseSet *b = ref.b;
     cudaStream_t s = g_ctx.stream;
     if (scratch_acquire(s)) return 1;
     const int oc = affine_out ? 0 : repr == H2_REPR_CANONICAL;
@@ -931,39 +941,39 @@ static int ipa_round_common(uint64_t session, const void *z, const void *l_rand,
     return 0;
 }
 extern "C" int h2_ipa_fold(uint64_t session, const void *u, const void *u_inv, int repr) {
-    std::lock_guard<std::mutex> lk(g_mu);
+    CtxLock lk;
     if (require_ready()) return 1;
     auto it = g_ctx.ipa.find(session);
     if (it == g_ctx.ipa.end()) return fail("h2_ipa_fold: unknown session");
     IpaSession *q = it->second;
-    auto ib = g_ctx.bases.find(q->bases);
-    if (ib == g_ctx.bases.end()) return fail("h2_ipa_fold: the session's base set was released");
+    BasesRef ref(q->bases);
+    if (!ref.b) return fail("h2_ipa_fold: the session's base set was released");
     if (q->folded) return fail("h2_ipa_fold: no round to fold");
     const uint64_t n = 1ull << q->k;
     const uint32_t bit = q->k - 1 - q->round;
     cudaStream_t s = g_ctx.stream;
     IpaState S = ipa_state(q);
-    if (ib->second->curve == H2_CURVE_PALLAS) LAUNCH(ipa_fold_kernel<FqParams>, blocks_for(n, 256), 256, 0, s, S, bit, host_to_mont<FqParams>(u, repr), host_to_mont<FqParams>(u_inv, repr));
+    if (ref.b->curve == H2_CURVE_PALLAS) LAUNCH(ipa_fold_kernel<FqParams>, blocks_for(n, 256), 256, 0, s, S, bit, host_to_mont<FqParams>(u, repr), host_to_mont<FqParams>(u_inv, repr));
     else LAUNCH(ipa_fold_kernel<FpParams>, blocks_for(n, 256), 256, 0, s, S, bit, host_to_mont<FpParams>(u, repr), host_to_mont<FpParams>(u_inv, repr));
     q->round++; q->folded = 1;   // asynchronous: the next round (or finish) is ordered behind it on the stream
     return 0;
 }
 extern "C" int h2_ipa_finish(uint64_t session, int repr, void *out_c_b) {
-    std::lock_guard<std::mutex> lk(g_mu);
+    CtxLock lk;
     if (require_ready()) return 1;
     auto it = g_ctx.ipa.find(session);
     if (it == g_ctx.ipa.end()) return fail("h2_ipa_finish: unknown session");
     IpaSession *q = it->second;
-    auto ib = g_ctx.bases.find(q->bases);
     int rc = 0;
     cudaStream_t s = g_ctx.stream;
+    BasesRef ref(q->bases);
     if (out_c_b) {
-        if (ib == g_ctx.bases.end()) rc = fail("h2_ipa_finish: the session's base set was released");
+        if (!ref.b) rc = fail("h2_ipa_finish: the session's base set was released");
         else if (q->round != q->k || !q->folded) rc = fail("h2_ipa_finish: the k rounds are not complete");
         else {
             IpaState S = ipa_state(q);
             fe *out = q->scal.as<fe>();
-            if (ib->second->curve == H2_CURVE_PALLAS) ipa_result_kernel<FqParams><<<1, 32, 0, s>>>(S, repr == H2_REPR_CANONICAL, out);
+            if (ref.b->curve == H2_CURVE_PALLAS) ipa_result_kernel<FqParams><<<1, 32, 0, s>>>(S, repr == H2_REPR_CANONICAL, out);
             else ipa_result_kernel<FpParams><<<1, 32, 0, s>>>(S, repr == H2_REPR_CANONICAL, out);
             g_launches.fetch_add(1, std::memory_order_relaxed);
             cudaError_t e = cudaMemcpyAsync(out_c_b, out, 2 * sizeof(fe), cudaMemcpyDeviceToHost, s);
@@ -972,6 +982,7 @@ extern "C" int h2_ipa_finish(uint64_t session, int repr, void *out_c_b) {
     }
     cudaError_t e = cudaStreamSynchronize(s);
     if (e != cudaSuccess && !rc) rc = fail(std::string("h2_ipa_finish: ") + cudaGetErrorString(e));
+    bases_session_end(q->bases);
     ipa_free(q);
     g_ctx.ipa.erase(it);
     return rc;
@@ -992,11 +1003,11 @@ extern "C" int h2_msm_registered_polys_affine(uint64_t bases_handle, const uint6
 }
 static int msm_registered_polys_impl(uint64_t bases_handle, const uint64_t *polys, size_t batch, size_t n, const void *extra_scalars, int repr,
                                      void *out_xyz, int affine_out) {
-    std::lock_guard<std::mutex> lk(g_mu);
+    CtxLock lk;
     if (require_ready()) return 1;
-    auto it = g_ctx.bases.find(bases_handle);
-    if (it == g_ctx.bases.end()) return fail("h2_msm_registered_polys: unknown bases handle");
-    BaseSet *b = it->second;
+    BasesRef ref(bases_handle);
+    if (!ref.b) return fail("h2_msm_registered_polys: unknown bases handle");
+    BaseSet *b = ref.b;
     if (batch == 0) return 0;
     if (batch > 64) return fail("h2_msm_registered_polys: batch > 64");
     if (batch > 1 && !b->table.p) return fail("h2_msm_registered_polys: a batch needs a base set with a window table (H2_BASES_PRECOMPUTE)");

@@ -66,8 +66,8 @@ static int ntt_run(int field, const fe *d_in, uint32_t in_log_n, fe *d_out, uint
         for (int k = 0; k < 3; k++) { A.in_scale[k] = sc.in_s[k]; A.out_scale[k] = sc.out_s[k]; }
         uint32_t tiles = (uint32_t)(n >> (sp[i] + logc[i]));
         uint32_t smem = ntt_smem_bytes(sp[i], logc[i]) + ntt_twc_bytes(sp[i], logc[i], i == passes - 1);
-        static bool smem_optin = false;      // per instantiation <P>: a single-CTA transform of 2^10 elements wants 64 KiB
-        if (!smem_optin) {
+        static std::atomic<bool> smem_optin{false};   // per instantiation <P>: a single-CTA transform of 2^10 elements wants 64 KiB
+        if (!smem_optin.load()) {
             CU(cudaFuncSetAttribute(ntt_pass_kernel<P>, cudaFuncAttributeMaxDynamicSharedMemorySize, 100 * 1024));
             CU(cudaFuncSetAttribute(ntt_pass_tma_kernel<P>, cudaFuncAttributeMaxDynamicSharedMemorySize, 100 * 1024));
             smem_optin = true;
@@ -134,7 +134,7 @@ static int ntt_host(int field, int mode, const void *a_in, uint32_t in_log_n, ui
 }
 static int ntt_host_dispatch(int field, int mode, const void *a_in, uint32_t in_log_n, uint32_t log_n, const void *omega, const void *zeta,
                              const void *divisor, size_t out_len, void *out, int repr) {
-    std::lock_guard<std::mutex> lk(g_mu);
+    CtxLock lk;
     if (require_ready()) return 1;
     if (log_n > 30 || in_log_n > log_n) return fail("ntt: bad sizes");
     if (field == H2_FIELD_FP) return ntt_host<FpParams>(field, mode, a_in, in_log_n, log_n, omega, zeta, divisor, out_len, out, repr);
@@ -156,7 +156,7 @@ extern "C" int h2_extended_to_coeff(int field, const void *a, uint32_t ext_k, co
     return ntt_host_dispatch(field, 3, a, ext_k, ext_k, ext_omega_inv, zeta, ext_divisor, out_len, out, repr);
 }
 extern "C" int h2_ntt_dev(int field, const void *d_in, void *d_out, const void *omega, int omega_repr, uint32_t log_n, void *stream) {
-    std::lock_guard<std::mutex> lk(g_mu);
+    CtxLock lk;
     if (require_ready()) return 1;
     cudaStream_t s = (cudaStream_t)stream;
     if (scratch_acquire(s)) return 1;
@@ -170,12 +170,12 @@ extern "C" int h2_ntt_dev(int field, const void *d_in, void *d_out, const void *
 }
 // test / bench hook: 1 = the bulk-copy (TMA) persistent pass kernel where it applies, 0 = the classic kernel (default; ctx.cuh)
 extern "C" int h2_test_set_ntt_tma(int on) {
-    std::lock_guard<std::mutex> lk(g_mu);
+    CtxLock lk;
     g_ctx.ntt_tma = on ? 1u : 0u;
     return 0;
 }
 extern "C" int h2_ntt_clear_cache(void) {
-    std::lock_guard<std::mutex> lk(g_mu);
+    CtxLock lk;
     if (require_ready()) return 1;
     cudaDeviceSynchronize();
     for (auto *t : g_ctx.twiddles) { t->buf.release(); delete t; }
@@ -195,7 +195,7 @@ int get_twiddles_any(int field, const fe &omega_mont, uint32_t log_n, cudaStream
 // slot so that a commit can append the blind.
 // ------------------------------------------------------------------------------------------------
 extern "C" int h2_poly_alloc(int field, size_t len, uint64_t *poly) {
-    std::lock_guard<std::mutex> lk(g_mu);
+    CtxLock lk;
     if (require_ready()) return 1;
     if (field != H2_FIELD_FP && field != H2_FIELD_FQ) return fail("unknown field id");
     // A prover allocates and frees the same few sizes proof after proof: freed polynomials keep their device buffer in a small
@@ -216,13 +216,13 @@ extern "C" int h2_poly_alloc(int field, size_t len, uint64_t *poly) {
     if (b->buf.ensure((len + 1) * sizeof(fe))) { delete b; return 1; }
     // zero-filled: a commit after a partial upload, or of a quotient shorter than the buffer, must not read stale memory
     if (cudaMemsetAsync(b->buf.p, 0, (len + 1) * sizeof(fe), X.stream) != cudaSuccess) { b->buf.release(); delete b; return fail("h2_poly_alloc: memset failed"); }
-    uint64_t h = X.next_handle++;
+    uint64_t h = new_handle();
     X.polys[h] = b;
     *poly = h;
     return 0;
 }
 extern "C" int h2_poly_free(uint64_t poly) {
-    std::lock_guard<std::mutex> lk(g_mu);
+    CtxLock lk;
     Context &X = g_ctx;
     auto it = X.polys.find(poly);
     if (it == X.polys.end()) return fail("h2_poly_free: unknown handle");
@@ -259,7 +259,7 @@ int convert_field(int field, fe *d, size_t n, int to_mont, cudaStream_t s) {
     return 0;
 }
 extern "C" int h2_poly_upload(uint64_t poly, const void *src, size_t len, int repr) {
-    std::lock_guard<std::mutex> lk(g_mu);
+    CtxLock lk;
     if (require_ready()) return 1;
     PolyBuf *b = find_poly(poly);
     if (!b) return fail("h2_poly_upload: unknown handle");
@@ -274,7 +274,7 @@ extern "C" int h2_poly_upload(uint64_t poly, const void *src, size_t len, int re
 // :78 `p_prime_poly[0] -= v`) on a resident polynomial
 template <class P> __global__ void poly_add_at_kernel(fe *a, fe delta_mont) { fe_store(a, fe_add<P>(fe_load(a), delta_mont)); }
 extern "C" int h2_poly_add_at(uint64_t poly, size_t index, const void *delta, int repr) {
-    std::lock_guard<std::mutex> lk(g_mu);
+    CtxLock lk;
     if (require_ready()) return 1;
     PolyBuf *b = find_poly(poly);
     if (!b) return fail("h2_poly_add_at: unknown handle");
@@ -287,7 +287,7 @@ extern "C" int h2_poly_add_at(uint64_t poly, size_t index, const void *delta, in
 // dst[dst_off .. dst_off + len) = src[src_off .. src_off + len) on the device: the h(X) pieces (plonk/vanishing/prover.rs:95-100
 // `h_poly.chunks_exact(n)`), or a copy of a column that an in-place step is about to overwrite
 extern "C" int h2_poly_copy(uint64_t dst, size_t dst_off, uint64_t src, size_t src_off, size_t len) {
-    std::lock_guard<std::mutex> lk(g_mu);
+    CtxLock lk;
     if (require_ready()) return 1;
     PolyBuf *d = find_poly(dst), *a = find_poly(src);
     if (!d || !a) return fail("h2_poly_copy: unknown handle");
@@ -298,7 +298,7 @@ extern "C" int h2_poly_copy(uint64_t dst, size_t dst_off, uint64_t src, size_t s
     return 0;
 }
 extern "C" int h2_poly_download(uint64_t poly, void *dst, size_t len, int repr) {
-    std::lock_guard<std::mutex> lk(g_mu);
+    CtxLock lk;
     if (require_ready()) return 1;
     PolyBuf *b = find_poly(poly);
     if (!b) return fail("h2_poly_download: unknown handle");
@@ -332,7 +332,7 @@ static int poly_transform(PolyBuf *dst, PolyBuf *src, int mode, uint32_t in_log_
 }
 static int poly_transform_dispatch(uint64_t dst, uint64_t src, int mode, uint32_t in_log_n, uint32_t log_n, const void *omega, const void *zeta,
                                    const void *divisor, size_t out_len, int repr) {
-    std::lock_guard<std::mutex> lk(g_mu);
+    CtxLock lk;
     if (require_ready()) return 1;
     PolyBuf *d = find_poly(dst), *a = find_poly(src);
     if (!d || !a) return fail("resident transform: unknown polynomial handle");

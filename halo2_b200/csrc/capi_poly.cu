@@ -93,7 +93,7 @@ static int polyops_run(int mode, const std::vector<PolyBuf *> &a, const std::vec
 }
 static int polyops_dispatch(int mode, const uint64_t *ah, const uint64_t *ch, size_t batch, size_t n, const void *points, int repr, void *out,
                             const char *who) {
-    std::lock_guard<std::mutex> lk(g_mu);
+    CtxLock lk;
     if (require_ready()) return 1;
     if (batch == 0) return 0;
     if (batch > 256) return fail(std::string(who) + ": batch > 256");
@@ -152,7 +152,7 @@ static int ast_run(PolyBuf *out, const std::vector<PolyBuf *> &polys, uint32_t l
 }
 extern "C" int h2_poly_eval_ast(uint64_t out, const uint64_t *polys, size_t n_polys, uint32_t log_n, const uint32_t *code, size_t n_code,
                                 const void *consts, size_t n_consts, const void *omega, const void *lin_base, int repr) {
-    std::lock_guard<std::mutex> lk(g_mu);
+    CtxLock lk;
     if (require_ready()) return 1;
     PolyBuf *o = find_poly(out);
     if (!o) return fail("h2_poly_eval_ast: unknown output handle");
@@ -189,7 +189,7 @@ extern "C" int h2_poly_eval_ast(uint64_t out, const uint64_t *polys, size_t n_po
 }
 // ff::BatchInvert on the first n elements of a resident polynomial, in place (zeros stay zero)
 extern "C" int h2_poly_batch_invert(uint64_t poly, size_t n) {
-    std::lock_guard<std::mutex> lk(g_mu);
+    CtxLock lk;
     if (require_ready()) return 1;
     PolyBuf *a = find_poly(poly);
     if (!a) return fail("h2_poly_batch_invert: unknown polynomial handle");
@@ -226,7 +226,7 @@ template <class P> static int grand_product_run(PolyBuf *d, PolyBuf *a, size_t n
     return scratch_release(s);
 }
 extern "C" int h2_poly_running_product(uint64_t dst, uint64_t src, size_t n, const void *init, int repr) {
-    std::lock_guard<std::mutex> lk(g_mu);
+    CtxLock lk;
     if (require_ready()) return 1;
     PolyBuf *d = find_poly(dst), *a = find_poly(src);
     if (!d || !a) return fail("h2_poly_running_product: unknown polynomial handle");
@@ -239,7 +239,7 @@ extern "C" int h2_poly_running_product(uint64_t dst, uint64_t src, size_t n, con
 }
 // divide_by_vanishing_poly on a resident extended-domain polynomial; t_evals: t_len = 2^(ext_k - k) host elements
 extern "C" int h2_poly_divide_by_vanishing(uint64_t poly, uint32_t ext_k, const void *t_evals, uint32_t t_len, int repr) {
-    std::lock_guard<std::mutex> lk(g_mu);
+    CtxLock lk;
     if (require_ready()) return 1;
     PolyBuf *a = find_poly(poly);
     if (!a) return fail("h2_poly_divide_by_vanishing: unknown polynomial handle");
@@ -328,7 +328,7 @@ template <class P> static int lookup_permute_run(PolyBuf *in, PolyBuf *tab, size
     return 0;
 }
 extern "C" int h2_poly_lookup_permute(uint64_t input, uint64_t table, size_t usable_rows, uint64_t out_input, uint64_t out_table) {
-    std::lock_guard<std::mutex> lk(g_mu);
+    CtxLock lk;
     if (require_ready()) return 1;
     PolyBuf *a = find_poly(input), *t = find_poly(table), *oa = find_poly(out_input), *ot = find_poly(out_table);
     if (!a || !t || !oa || !ot) return fail("h2_poly_lookup_permute: unknown polynomial handle");
@@ -361,7 +361,7 @@ template <class P> static int compute_s_run(PolyBuf *d, const void *u, uint32_t 
     return scratch_release(s);
 }
 extern "C" int h2_poly_compute_s(uint64_t dst, const void *u, uint32_t k, const void *init, int accumulate, int repr) {
-    std::lock_guard<std::mutex> lk(g_mu);
+    CtxLock lk;
     if (require_ready()) return 1;
     PolyBuf *d = find_poly(dst);
     if (!d) return fail("h2_poly_compute_s: unknown polynomial handle");
@@ -374,7 +374,7 @@ extern "C" int h2_poly_compute_s(uint64_t dst, const void *u, uint32_t k, const 
 // dst[i] = a * dst[i] + b * src[i], i < n (src == 0: dst[i] *= a): MSM::scale and the g_scalars part of MSM::add_msm
 // (poly/commitment/msm.rs:126-139, :37-62); BatchVerifier's accumulate_msm (plonk/verifier/batch.rs:83-93) is one call
 extern "C" int h2_poly_scale_add(uint64_t dst, const void *a, uint64_t src, const void *b, size_t n, int repr) {
-    std::lock_guard<std::mutex> lk(g_mu);
+    CtxLock lk;
     if (require_ready()) return 1;
     PolyBuf *d = find_poly(dst), *x = src ? find_poly(src) : nullptr;
     if (!d || (src && !x)) return fail("h2_poly_scale_add: unknown polynomial handle");

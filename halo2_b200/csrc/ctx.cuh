@@ -6,6 +6,7 @@
 #include <cuda_runtime.h>
 
 #include <atomic>
+#include <condition_variable>
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
@@ -63,6 +64,8 @@ struct BaseSet {
     int curve; size_t n; DevBuf buf;
     DevBuf table; uint32_t c = 0, W = 0;   // W x n window shifts 2^(c w) G_i (bucket method over one shared bucket set)
     DevBuf dtable;                         // 32 x 128 x n digit multiples m 2^(8 w) G_i (fixedbase.cuh: direct sum, small sets)
+    uint32_t users = 0;                    // registered sets (g_bases): calls in flight on any lane that read the set (BasesRef)
+    uint32_t sessions = 0;                 // ... and open IPA sessions on any lane that refer to it; both under g_reg_mu
 };
 
 struct PolyBuf { int field; size_t len; DevBuf buf; PolyBuf() { buf.tracked = false; } };   // device-resident polynomial, Montgomery form, len + 1 slots
@@ -97,7 +100,16 @@ struct StageRing {
     void destroy();
 };
 
+// The mutex of a Context.  Copying or assigning a Context (ctx_destroy resets one with `C = Context()`) leaves it alone.
+struct CtxMutex {
+    std::mutex m;
+    CtxMutex() {}
+    CtxMutex(const CtxMutex &) {}
+    CtxMutex &operator=(const CtxMutex &) { return *this; }
+};
+
 struct Context {
+    CtxMutex mu;                             // held for a whole call on this context (CtxLock)
     bool ready = false;
     int device = -1;
     cudaStream_t stream = nullptr;
@@ -156,7 +168,7 @@ struct Context {
     DevBuf lk_keys, lk_left, lk_u32;         // lookup.cuh: sorted canonical keys (input | table), leftover table values, flag / scan arrays
     std::vector<TwiddleEntry *> twiddles;
     uint64_t tw_stamp = 0;
-    std::map<uint64_t, BaseSet *> bases;
+    std::map<uint64_t, BaseSet *> shards;    // this device's shards of multi-GPU base sets (h2_multi_bases_register)
     std::map<uint64_t, IpaSession *> ipa;
     std::map<uint64_t, PolyBuf *> polys;
     std::vector<MsmGraph> graphs;
@@ -165,21 +177,61 @@ struct Context {
     std::vector<PolyBuf *> poly_pool;        // freed resident polynomials keep their buffers for the next h2_poly_alloc of that size
     size_t poly_pool_bytes = 0;
     std::vector<IpaSession *> ipa_pool;      // finished sessions keep their buffers for the next proof (no cudaMalloc per opening)
-    uint64_t next_handle = 1;
 };
-// One Context per CUDA device.  API functions work on the PRIMARY context (the device h2_init bound); the multi-GPU
-// entry points (h2_multi_*) run one worker thread per device, each of which points its thread-local g_cur at its device's
-// context while the calling thread holds g_mu -- so all the single-GPU code below runs unchanged, concurrently, on every
-// device.
+// One Context per CUDA device, plus up to H2_MAX_LANES lanes: extra contexts on the primary device, each with its own
+// streams, scratch, caches, settings, resident polynomials and IPA sessions, so that independent provers on different host
+// threads run concurrently (h2_lane_create / h2_lane_bind).  API functions work on the context the calling thread's
+// g_cur points at: its bound lane, or the PRIMARY context (the device h2_init bound) when it never bound one.  The multi-GPU
+// entry points (h2_multi_*) run one worker thread per device, each of which points its g_cur at its device's context
+// while the calling thread holds the primary's mutex -- so all the single-GPU code below runs unchanged, concurrently, on
+// every device and every lane.
+//
+// Locks, outermost first; a thread never takes one while holding a later one:
+//   1. g_life_mu      h2_init, h2_shutdown, h2_multi_init, h2_lane_create, h2_lane_destroy
+//   2. Context::mu    a call on that context, for the whole call.  A thread holds one at a time, except h2_shutdown, which
+//                     takes the primary's and then every live lane's in slot order (every other holder finishes its call
+//                     without waiting for a second context)
+//   3. g_reg_mu       the lane table and bindings, the shared base sets (g_bases) and their counts, g_multi, g_multi_bases;
+//                     held for map lookups only.  h2_bases_release waits on g_bases_cv under it for the set's users
+// Handles of base sets, polynomials, IPA sessions, multi-GPU base sets and lanes come from one process-wide counter
+// (new_handle) that h2_shutdown does not reset: a handle names one object of one kind on one lane, and any other use of it
+// -- a foreign lane, a stale handle from before a shutdown -- finds nothing and is reported as unknown.
+#define H2_MAX_LANES 16
 extern Context g_ctxs[H2_MAX_DEVICES];
+extern Context g_lanes[H2_MAX_LANES];
 extern Context *g_primary;
 extern thread_local Context *g_cur;
-static inline Context &cur_ctx() { return *(g_cur ? g_cur : g_primary); }
+extern thread_local uint64_t g_cur_epoch;    // g_epoch when g_cur was set
+extern std::atomic<uint64_t> g_epoch;        // bumped by h2_shutdown: a lane bound before it is gone
+extern Context g_dead;                       // never ready: what a thread whose lane h2_shutdown destroyed works on
+static inline Context &cur_ctx() {
+    if (!g_cur) return *g_primary;
+    if (g_cur_epoch != g_epoch.load(std::memory_order_relaxed)) return g_dead;
+    return *g_cur;
+}
+static inline void set_cur(Context *c) { g_cur = c; g_cur_epoch = g_epoch.load(); }
 #define g_ctx (cur_ctx())
-extern std::mutex g_mu;
+extern std::mutex g_life_mu, g_reg_mu;
+struct CtxLock {                             // the calling thread's context, for the whole call
+    std::lock_guard<std::mutex> g;
+    CtxLock() : g(cur_ctx().mu.m) {}
+};
+uint64_t new_handle();
+bool on_lane();                              // the calling thread is bound to a lane (not the primary context)
+// Shared base sets (h2_bases_register*): registered once, read by every lane.  A BasesRef holds the set for one call; the
+// set cannot be released before it is dropped.
+extern std::map<uint64_t, BaseSet *> g_bases;
+struct BasesRef {
+    BaseSet *b = nullptr;
+    explicit BasesRef(uint64_t handle, bool open_session = false);   // b == nullptr: unknown handle
+    ~BasesRef();
+    BasesRef(const BasesRef &) = delete;
+    BasesRef &operator=(const BasesRef &) = delete;
+};
+void bases_session_end(uint64_t handle);     // an IPA session on the set finished (or its lane was destroyed)
 // optional per-kernel timing (bench.py's roofline leg): event pairs recorded on the launch stream
 struct ProfSpan { int kind; cudaEvent_t e0, e1; };
-extern bool g_prof_on;
+extern std::atomic<bool> g_prof_on;
 extern std::vector<ProfSpan> g_prof;
 enum { PROF_MSM_ACCUM0 = 0, PROF_NTT_PASS = 1, PROF_KINDS = 2 };
 void prof_begin(int kind, cudaStream_t s);

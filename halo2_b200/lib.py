@@ -27,7 +27,7 @@ SYMBOLS = [
     "h2_intt_scaled", "h2_coeff_to_extended", "h2_extended_to_coeff", "h2_ntt_dev", "h2_ntt_clear_cache",
     "h2_ec_fft", "h2_batch_normalize", "h2_params_lagrange", "h2_hash_to_curve", "h2_params_new", "h2_points_compress", "h2_points_decompress",
     "h2_dev_gen_points", "h2_dev_convert", "h2_test_last_msm_flags", "h2_test_last_msm_plan", "h2_test_set_chunk_threshold", "h2_test_set_chunk_cuts", "h2_test_set_graphs", "h2_test_set_poly_cta", "h2_test_set_fast_fixed", "h2_test_set_ecfft_quad", "h2_test_set_accum_ways", "h2_test_field_op", "h2_test_curve_op", "h2_bench_field_mul", "h2_bench_latency",
-    "h2_launch_count", "h2_profile_enable", "h2_profile_read",
+    "h2_launch_count", "h2_profile_enable", "h2_profile_read", "h2_lane_create", "h2_lane_bind", "h2_lane_destroy",
 ]
 
 
@@ -77,6 +77,46 @@ def init(device: Optional[int] = None) -> ctypes.CDLL:
     elif _inited_device != int(device):
         raise H2Error(f"engine already bound to device {_inited_device} (one process per GPU)")
     return lib
+
+
+class Lane:
+    """An independent prover context on the GPU: its own streams, scratch, caches, settings, resident polynomials and IPA
+    sessions (include/halo2_b200.h, "lanes").  Every call from a thread bound to it runs there, concurrently with threads
+    on other lanes; base sets (Params) are shared by all lanes.  Binding is per host thread.
+
+        with Lane():          # created, bound to this thread; unbound and destroyed on exit
+            prove(...)
+    """
+
+    def __init__(self, device: Optional[int] = None):
+        lib = init(device)
+        h = ctypes.c_uint64(0)
+        check(lib.h2_lane_create(ctypes.byref(h)))
+        self.handle = int(h.value)
+
+    def bind(self) -> "Lane":
+        """Binds the calling thread: its later calls run on this lane."""
+        if not self.handle:
+            raise H2Error("the lane is closed")
+        check(load().h2_lane_bind(ctypes.c_uint64(self.handle)))
+        return self
+
+    def close(self) -> None:
+        """Destroys the lane and everything created on it; the calling thread, if bound to it, goes back to the primary
+        context.  Fails while another thread is bound to it."""
+        if self.handle:
+            check(load().h2_lane_destroy(ctypes.c_uint64(self.handle)))
+            self.handle = 0
+
+    def __enter__(self) -> "Lane":
+        try:
+            return self.bind()
+        except BaseException:
+            self.close()
+            raise
+
+    def __exit__(self, *exc) -> None:
+        self.close()
 
 
 def launch_count() -> int:

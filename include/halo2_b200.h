@@ -20,7 +20,9 @@
  *   - curve: H2_CURVE_PALLAS = EpAffine (coordinates Fp, scalars Fq),
  *            H2_CURVE_VESTA  = EqAffine (coordinates Fq, scalars Fp).
  *   - Thread-safe and re-entrant (BatchVerifier calls commit_lagrange from many rayon
- *     workers, plonk/verifier/batch.rs:97-110): calls are serialised on an internal lock.
+ *     workers, plonk/verifier/batch.rs:97-110): calls on one context are serialised on its
+ *     lock.  A thread that binds a lane (h2_lane_bind) gets a context of its own, so calls
+ *     from threads on different lanes run concurrently on the GPU.
  *   - There is NO CPU fallback: every function fails if no CUDA device is usable.
  *   - Functions suffixed _dev take CUDA device pointers (Montgomery form) and a cudaStream_t
  *     (passed as void*); they do not synchronise.  The others take host pointers, copy in
@@ -49,6 +51,24 @@ int h2_device_count(void);
 /* ABI version of this header (bumped on incompatible change). */
 uint32_t h2_abi_version(void);
 
+/* ---- lanes: independent provers on one GPU ------------------------------------------------------------------------
+ * A lane is one more context on the primary device: its own streams, scratch pools, staging ring, twiddle and graph
+ * caches and settings, and its own resident polynomials and IPA sessions.  A host thread bound to a lane runs every call
+ * there, concurrently with the threads on other lanes; a thread that never binds uses the primary context.
+ *   - h2_lane_create fails before h2_init and when all 16 lanes exist.  A new lane starts with the library's default
+ *     settings; h2_set_window_bits / h2_set_glv / h2_set_sort_mode, the h2_test_set_* hooks except the process-wide
+ *     staging, copy-thread and chunk-cut ones, and h2_test_last_msm_plan act on the calling thread's lane.
+ *   - h2_lane_bind(0) goes back to the primary context.  Binding an unknown lane fails.
+ *   - Polynomial and IPA-session handles belong to the lane that created them; from any other lane (the primary
+ *     included) they are unknown.  Base sets (h2_bases_register*) are shared by every lane.
+ *   - h2_lane_destroy frees the lane's polynomials, IPA sessions and pools; it fails while another thread is bound to
+ *     the lane.  h2_shutdown destroys every lane; lane handles from before it are unknown afterwards, and a thread that
+ *     was bound must bind again.
+ *   - The h2_multi_* entry points fail on a thread bound to a lane. */
+int h2_lane_create(uint64_t *lane);
+int h2_lane_bind(uint64_t lane);
+int h2_lane_destroy(uint64_t lane);
+
 /* ---- MSM: replaces best_multiexp, arithmetic.rs:143-180 ------------------------------------ */
 /* out = sum_i scalars[i] * bases[i].  Caller guarantees both arrays hold n entries
  * (the shim asserts coeffs.len() == bases.len() like arithmetic.rs:144). */
@@ -69,6 +89,8 @@ enum { H2_BASES_PRECOMPUTE = 1, H2_BASES_DIRECT = 2 };
  * select (three launches, no buckets): halo2_b200/csrc/fixedbase.cuh.  Same group element either way. */
 int h2_bases_register_ex(int curve, const void *bases_xy, size_t n, int repr, uint32_t window_bits, uint32_t flags,
                          uint64_t *handle);
+/* Base sets are shared by every lane.  Waits for calls on other lanes that are reading the set; fails while an open IPA
+ * session on any lane refers to it (h2_ipa_finish first). */
 int h2_bases_release(uint64_t handle);
 /* sum_{i<n} scalars[i] * bases[i]  (+ extra_scalar[0] * bases[n] when extra_scalar != NULL):
  * commit(poly, r) = h2_msm_registered(h(g ++ [w]), poly, n, &r, ...). */
