@@ -67,6 +67,9 @@ extern "C" {
     // the verifier's MSM with resident g_scalars: compute_s (poly/commitment/verifier.rs:156-171) and MSM::scale / add_msm (msm.rs:37-139)
     pub fn h2_poly_compute_s(dst: u64, u: *const c_void, k: u32, init: *const c_void, accumulate: c_int, repr: c_int) -> c_int;
     pub fn h2_poly_scale_add(dst: u64, a: *const c_void, src: u64, b: *const c_void, n: usize, repr: c_int) -> c_int;
+    // keygen: the permutation polynomials from the copy-constraint mapping (plonk/permutation/keygen.rs:102-211)
+    pub fn h2_poly_permutation_sigma(dst: *const u64, cols: usize, k: u32, mapping: *const u32, omega: *const c_void, delta: *const c_void,
+                                     repr: c_int) -> c_int;
     pub fn h2_poly_divide_by_vanishing(poly: u64, ext_k: u32, t_evals: *const c_void, t_len: u32, repr: c_int) -> c_int;
     pub fn h2_poly_eval(polys: *const u64, batch: usize, n: usize, points: *const c_void, repr: c_int, out: *mut c_void) -> c_int;
     pub fn h2_poly_inner_product(a: *const u64, b: *const u64, batch: usize, n: usize, repr: c_int, out: *mut c_void) -> c_int;
@@ -468,6 +471,43 @@ pub fn best_multiexp_multi_gpu<C: B200Curve>(coeffs: &[C::Scalar], bases: &[C]) 
 /// Returns false where the reference returns `Error::ConstraintSystemFailure` (:605-608).
 pub fn lookup_permute_resident(input: u64, table: u64, usable_rows: usize, out_input: u64, out_table: u64) -> bool {
     unsafe { h2_poly_lookup_permute(input, table, usable_rows, out_input, out_table) == 0 }
+}
+
+/// The permutation polynomials of `Assembly::build_vk` / `build_pk` (plonk/permutation/keygen.rs:108-143, :161-198) as
+/// resident Lagrange columns, built on the device without the n-element `omega_powers` / `deltaomega` tables.  `mapping` is
+/// the reference's `Assembly::mapping` (one `Vec` of n = 2^k (column, row) pairs per permutation column), `omega` =
+/// `domain.get_omega()`, `delta` = `F::DELTA`.  Returns one polynomial handle per column, owned by the caller's lane: commit
+/// them (`h2_msm_registered_polys_affine`), transform them, and free them with `h2_poly_free`.  Panics on an out-of-range entry.
+pub fn permutation_polys<F: PrimeField>(field_id: c_int, k: u32, mapping: &[Vec<(usize, usize)>], omega: F, delta: F) -> Vec<u64> {
+    let n = 1usize << k;
+    let mut flat = Vec::with_capacity(2 * n * mapping.len());
+    for col in mapping {
+        assert_eq!(col.len(), n);
+        for &(c, r) in col {
+            flat.push(u32::try_from(c).expect("column index >= 2^32"));
+            flat.push(u32::try_from(r).expect("row index >= 2^32"));
+        }
+    }
+    let mut handles = Vec::with_capacity(mapping.len());
+    for _ in mapping {
+        let mut h = 0u64;
+        let rc = unsafe { h2_poly_alloc(field_id, n, &mut h) };
+        if rc != 0 {
+            for h in handles { unsafe { h2_poly_free(h) }; }
+            check(rc);
+        }
+        handles.push(h);
+    }
+    let (w, d) = (omega.to_repr(), delta.to_repr());
+    let rc = unsafe {
+        h2_poly_permutation_sigma(handles.as_ptr(), handles.len(), k, flat.as_ptr(), w.as_ref().as_ptr() as *const c_void,
+                                  d.as_ref().as_ptr() as *const c_void, REPR_CANONICAL)
+    };
+    if rc != 0 {
+        for &h in &handles { unsafe { h2_poly_free(h) }; }
+        check(rc);
+    }
+    handles
 }
 
 /// The verifier's `g_scalars` (poly/commitment/msm.rs:12) kept in HBM: what `MSM<C>` holds under the `b200` feature instead of

@@ -1,9 +1,13 @@
-// C ABI of the engine, part 5 of 5: reductions and elementwise programs on resident polynomials (polyops.cuh, asteval.cuh).
+// C ABI of the engine, part 5 of 5: reductions and elementwise programs on resident polynomials (polyops.cuh, asteval.cuh),
+// the lookup permutation (lookup.cuh), the verifier's MSM scalars (verifier.cuh) and the permutation polynomials (keygen.cuh).
 #include "util_kernels.cuh"
 #include "polyops.cuh"
 #include "asteval.cuh"
 #include "lookup.cuh"
 #include "verifier.cuh"
+#include "keygen.cuh"
+
+#include <algorithm>
 
 // ------------------------------------------------------------------------------------------------
 // eval_polynomial / compute_inner_product / kate_division on resident polynomials (polyops.cuh)
@@ -392,4 +396,61 @@ extern "C" int h2_poly_scale_add(uint64_t dst, const void *a, uint64_t src, cons
         LAUNCH(verifier_scale_add_kernel<FqParams>, blocks_for(n, 256), 256, 0, s, d->buf.as<fe>(), sp, host_to_mont<FqParams>(a, repr),
                x ? host_to_mont<FqParams>(b, repr) : fe_zero(), (uint64_t)n);
     return 0;
+}
+
+
+// ------------------------------------------------------------------------------------------------
+// the permutation argument's sigma polynomials (keygen.cuh)
+// ------------------------------------------------------------------------------------------------
+// The mapping goes up in pieces of at most this many (column, row) pairs, so the scratch it needs stays at 32 MB whatever
+// the circuit's size; every piece is ordered on the context's stream behind the kernel that read the previous one.
+#define H2_KEYGEN_CHUNK (1ull << 22)
+template <class P>
+static int permutation_sigma_run(const std::vector<PolyBuf *> &dst, uint32_t k, const uint32_t *mapping, const void *omega, const void *delta, int repr) {
+    Context &X = g_ctx;
+    cudaStream_t s = X.stream;
+    const uint64_t n = 1ull << k, cols = dst.size();
+    const uint64_t tlen = KeygenOps<P>::table_len(k, (uint32_t)cols);
+    const uint64_t piece = n < H2_KEYGEN_CHUNK ? n : H2_KEYGEN_CHUNK;
+    if (scratch_acquire(s)) return 1;
+    if (X.kg_tab.ensure(tlen * sizeof(fe) + 16) || X.kg_map.ensure(piece * sizeof(uint2))) return 1;
+    fe *tab = X.kg_tab.as<fe>();
+    uint32_t *err = reinterpret_cast<uint32_t *>(tab + tlen);
+    uint2 *map = X.kg_map.as<uint2>();
+    CU(cudaMemsetAsync(err, 0, sizeof(uint32_t), s));
+    LAUNCH(keygen_tables_kernel<P>, blocks_for(tlen, 128), 128, 0, s, tab, host_to_mont<P>(omega, repr), host_to_mont<P>(delta, repr), k, (uint32_t)cols);
+    for (uint64_t i = 0; i < cols; i++)
+        for (uint64_t j0 = 0; j0 < n; j0 += piece) {
+            const uint64_t len = n - j0 < piece ? n - j0 : piece;
+            if (upload_async(map, mapping + 2 * (i * n + j0), len * sizeof(uint2), s)) return 1;
+            LAUNCH(keygen_sigma_kernel<P>, blocks_for(len, 256), 256, 0, s, dst[i]->buf.as<fe>() + j0, (const uint2 *)map, (const fe *)tab, k,
+                   (uint32_t)cols, len, err);
+        }
+    uint32_t h_err = 0;
+    CU(cudaMemcpyAsync(&h_err, err, sizeof h_err, cudaMemcpyDeviceToHost, s));
+    if (scratch_release(s)) return 1;
+    CU(cudaStreamSynchronize(s));
+    if (h_err) return fail("h2_poly_permutation_sigma: a mapping entry is outside the permutation's columns or the domain's rows");
+    return 0;
+}
+extern "C" int h2_poly_permutation_sigma(const uint64_t *dst, size_t cols, uint32_t k, const uint32_t *mapping, const void *omega, const void *delta,
+                                         int repr) {
+    CtxLock lk;
+    if (require_ready()) return 1;
+    if (k > 30) return fail("h2_poly_permutation_sigma: k > 30");
+    if (cols == 0) return 0;
+    if (cols >= (1ull << 32)) return fail("h2_poly_permutation_sigma: cols >= 2^32");
+    if (!dst || !mapping || !omega || !delta) return fail("h2_poly_permutation_sigma: null argument");
+    std::vector<PolyBuf *> d(cols);
+    for (size_t i = 0; i < cols; i++) {
+        d[i] = find_poly(dst[i]);
+        if (!d[i]) return fail("h2_poly_permutation_sigma: unknown polynomial handle");
+        if (d[i]->field != d[0]->field) return fail("h2_poly_permutation_sigma: the polynomials live in different fields");
+        if (d[i]->len < ((size_t)1 << k)) return fail("h2_poly_permutation_sigma: a polynomial holds fewer than 2^k elements");
+    }
+    std::vector<PolyBuf *> sorted(d);
+    std::sort(sorted.begin(), sorted.end());
+    if (std::adjacent_find(sorted.begin(), sorted.end()) != sorted.end()) return fail("h2_poly_permutation_sigma: a dst handle appears twice");
+    if (d[0]->field == H2_FIELD_FP) return permutation_sigma_run<FpParams>(d, k, mapping, omega, delta, repr);
+    return permutation_sigma_run<FqParams>(d, k, mapping, omega, delta, repr);
 }

@@ -221,6 +221,16 @@ int h2_poly_compute_s(uint64_t dst, const void *u, uint32_t k, const void *init,
  * `acc.scale(random); acc.add_msm(&msm)` (plonk/verifier/batch.rs:83-93) in one pass.  Asynchronous. */
 int h2_poly_scale_add(uint64_t dst, const void *a, uint64_t src, const void *b, size_t n, int repr);
 
+/* ---- key generation ------------------------------------------------------------------------------------------------ */
+/* The permutation argument's sigma polynomials (plonk/permutation/keygen.rs:102-211) on resident polynomials:
+ * dst[i][j] = delta^c * omega^r for (c, r) = mapping[2 (i n + j)], mapping[2 (i n + j) + 1], i < cols, j < n = 2^k.
+ * mapping: cols * n pairs of uint32 (column, row) in host memory (pageable or pinned) -- the reference's
+ * Assembly::mapping.  omega = domain.get_omega(), delta = F::DELTA, both in `repr`.  Fails when an entry is out of
+ * range (the outputs are then unspecified), a handle is unknown / of another field / shorter than n, two dst handles are
+ * equal, or k > 30; cols == 0 does nothing.  Synchronous. */
+int h2_poly_permutation_sigma(const uint64_t *dst, size_t cols, uint32_t k, const uint32_t *mapping,
+                              const void *omega, const void *delta, int repr);
+
 /* Reference sort of the MSM: by default every (point, window) reference is binned in ONE pass into fixed-capacity
  * per-bucket bins, with an automatic fallback to the exact histogram / scan / scatter sort when a bin overflows
  * (heavily repeated scalars).  exact_only != 0 forces the exact sort.  Same result; for A/B runs and tests. */
