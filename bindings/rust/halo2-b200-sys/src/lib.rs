@@ -70,6 +70,9 @@ extern "C" {
     // keygen: the permutation polynomials from the copy-constraint mapping (plonk/permutation/keygen.rs:102-211)
     pub fn h2_poly_permutation_sigma(dst: *const u64, cols: usize, k: u32, mapping: *const u32, omega: *const c_void, delta: *const c_void,
                                      repr: c_int) -> c_int;
+    // the same polynomials from the copy constraints: Assembly::copy's cycles computed on the device (plonk/permutation/keygen.rs:45-100)
+    pub fn h2_poly_permutation_sigma_copies(dst: *const u64, cols: usize, k: u32, copies: *const u32, m: usize, omega: *const c_void,
+                                            delta: *const c_void, repr: c_int) -> c_int;
     pub fn h2_poly_divide_by_vanishing(poly: u64, ext_k: u32, t_evals: *const c_void, t_len: u32, repr: c_int) -> c_int;
     pub fn h2_poly_eval(polys: *const u64, batch: usize, n: usize, points: *const c_void, repr: c_int, out: *mut c_void) -> c_int;
     pub fn h2_poly_inner_product(a: *const u64, b: *const u64, batch: usize, n: usize, repr: c_int, out: *mut c_void) -> c_int;
@@ -502,6 +505,35 @@ pub fn permutation_polys<F: PrimeField>(field_id: c_int, k: u32, mapping: &[Vec<
     let rc = unsafe {
         h2_poly_permutation_sigma(handles.as_ptr(), handles.len(), k, flat.as_ptr(), w.as_ref().as_ptr() as *const c_void,
                                   d.as_ref().as_ptr() as *const c_void, REPR_CANONICAL)
+    };
+    if rc != 0 {
+        for &h in &handles { unsafe { h2_poly_free(h) }; }
+        check(rc);
+    }
+    handles
+}
+
+/// `permutation_polys` from the copy constraints themselves: `copies` holds one `[left column, left row, right column,
+/// right row]` per `Assembly::copy` call, in synthesis order, columns as indices into the permutation's column list (what
+/// `Assembly::copy` records after its own checks).  The cycles of `Assembly::mapping` are computed on the device, so no
+/// mapping is built on the host.  Returns one polynomial handle per column, owned by the caller's lane.  Panics on a copy
+/// out of range; the message names the first bad copy.
+pub fn permutation_polys_from_copies<F: PrimeField>(field_id: c_int, k: u32, cols: usize, copies: &[[u32; 4]], omega: F, delta: F) -> Vec<u64> {
+    let n = 1usize << k;
+    let mut handles = Vec::with_capacity(cols);
+    for _ in 0..cols {
+        let mut h = 0u64;
+        let rc = unsafe { h2_poly_alloc(field_id, n, &mut h) };
+        if rc != 0 {
+            for h in handles { unsafe { h2_poly_free(h) }; }
+            check(rc);
+        }
+        handles.push(h);
+    }
+    let (w, d) = (omega.to_repr(), delta.to_repr());
+    let rc = unsafe {
+        h2_poly_permutation_sigma_copies(handles.as_ptr(), handles.len(), k, copies.as_ptr() as *const u32, copies.len(),
+                                         w.as_ref().as_ptr() as *const c_void, d.as_ref().as_ptr() as *const c_void, REPR_CANONICAL)
     };
     if rc != 0 {
         for &h in &handles { unsafe { h2_poly_free(h) }; }

@@ -14,11 +14,11 @@ from .poly import (Params, EvaluationDomain, Blind, ResidentPoly, lagrange_gener
 
 from .evaluator import Ast, AstLeaf, Evaluator  # noqa: F401
 from .verifier import MSM, Guard, VerifyError, verify_proof, compute_b  # noqa: F401
-from .keygen import (Assembly, ProvingKey, build_permutation_polys, keygen_vk, keygen_pk,  # noqa: F401
+from .keygen import (Assembly, CopyConstraints, ProvingKey, build_permutation_polys, keygen_vk, keygen_pk,  # noqa: F401
                      batch_invert_assigned_resident)
 from . import multiopen, opening  # noqa: F401
 
-__all__ = ["Ast", "AstLeaf", "Evaluator", "Assembly", "ProvingKey", "build_permutation_polys", "keygen_vk", "keygen_pk",
+__all__ = ["Ast", "AstLeaf", "Evaluator", "Assembly", "CopyConstraints", "ProvingKey", "build_permutation_polys", "keygen_vk", "keygen_pk",
            "batch_invert_assigned_resident", "MSM", "Guard", "VerifyError", "verify_proof", "compute_b", "multiopen", "opening", "H2Error", "Lane", "lib_path", "load", "init", "launch_count", "best_multiexp", "small_multiexp", "best_fft",
            "best_fft_curve", "batch_normalize", "multiexp_window_bits", "Params", "EvaluationDomain", "Blind", "ResidentPoly",
            "lagrange_generators", "compress_points", "decompress_points", "hash_to_curve",

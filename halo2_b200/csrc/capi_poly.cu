@@ -1,11 +1,13 @@
 // C ABI of the engine, part 5 of 5: reductions and elementwise programs on resident polynomials (polyops.cuh, asteval.cuh),
-// the lookup permutation (lookup.cuh), the verifier's MSM scalars (verifier.cuh) and the permutation polynomials (keygen.cuh).
+// the lookup permutation (lookup.cuh), the verifier's MSM scalars (verifier.cuh), the permutation polynomials (keygen.cuh)
+// and their copy cycles (assembly.cuh).
 #include "util_kernels.cuh"
 #include "polyops.cuh"
 #include "asteval.cuh"
 #include "lookup.cuh"
 #include "verifier.cuh"
 #include "keygen.cuh"
+#include "assembly.cuh"
 
 #include <algorithm>
 
@@ -405,32 +407,66 @@ extern "C" int h2_poly_scale_add(uint64_t dst, const void *a, uint64_t src, cons
 // The mapping goes up in pieces of at most this many (column, row) pairs, so the scratch it needs stays at 32 MB whatever
 // the circuit's size; every piece is ordered on the context's stream behind the kernel that read the previous one.
 #define H2_KEYGEN_CHUNK (1ull << 22)
+// The launches both entry points share: the power tables, then one sigma launch per (column, piece) of the mapping, then
+// the error word back.  sigma_tables is called after scratch_acquire; sigma_finish releases the scratch and synchronises.
+template <class P>
+static int sigma_tables(uint32_t k, uint64_t cols, const void *omega, const void *delta, int repr, fe **tab, uint32_t **err) {
+    Context &X = g_ctx;
+    cudaStream_t s = X.stream;
+    const uint64_t tlen = KeygenOps<P>::table_len(k, (uint32_t)cols);
+    if (X.kg_tab.ensure(tlen * sizeof(fe) + 16)) return 1;
+    *tab = X.kg_tab.as<fe>();
+    *err = reinterpret_cast<uint32_t *>(*tab + tlen);
+    CU(cudaMemsetAsync(*err, 0, sizeof(uint32_t), s));
+    LAUNCH(keygen_tables_kernel<P>, blocks_for(tlen, 128), 128, 0, s, *tab, host_to_mont<P>(omega, repr), host_to_mont<P>(delta, repr), k, (uint32_t)cols);
+    return 0;
+}
+template <class P>
+static int sigma_launch(PolyBuf *d, uint64_t j0, const uint2 *map, uint64_t len, uint32_t k, uint64_t cols, const fe *tab, uint32_t *err) {
+    LAUNCH(keygen_sigma_kernel<P>, blocks_for(len, 256), 256, 0, g_ctx.stream, d->buf.as<fe>() + j0, map, tab, k, (uint32_t)cols, len, err);
+    return 0;
+}
+static int sigma_finish(uint32_t *err, const char *who) {
+    cudaStream_t s = g_ctx.stream;
+    uint32_t h_err = 0;
+    CU(cudaMemcpyAsync(&h_err, err, sizeof h_err, cudaMemcpyDeviceToHost, s));
+    if (scratch_release(s)) return 1;
+    CU(cudaStreamSynchronize(s));
+    if (h_err) return fail(std::string(who) + ": a mapping entry is outside the permutation's columns or the domain's rows");
+    return 0;
+}
 template <class P>
 static int permutation_sigma_run(const std::vector<PolyBuf *> &dst, uint32_t k, const uint32_t *mapping, const void *omega, const void *delta, int repr) {
     Context &X = g_ctx;
     cudaStream_t s = X.stream;
     const uint64_t n = 1ull << k, cols = dst.size();
-    const uint64_t tlen = KeygenOps<P>::table_len(k, (uint32_t)cols);
     const uint64_t piece = n < H2_KEYGEN_CHUNK ? n : H2_KEYGEN_CHUNK;
+    fe *tab;
+    uint32_t *err;
     if (scratch_acquire(s)) return 1;
-    if (X.kg_tab.ensure(tlen * sizeof(fe) + 16) || X.kg_map.ensure(piece * sizeof(uint2))) return 1;
-    fe *tab = X.kg_tab.as<fe>();
-    uint32_t *err = reinterpret_cast<uint32_t *>(tab + tlen);
+    if (X.kg_map.ensure(piece * sizeof(uint2)) || sigma_tables<P>(k, cols, omega, delta, repr, &tab, &err)) return 1;
     uint2 *map = X.kg_map.as<uint2>();
-    CU(cudaMemsetAsync(err, 0, sizeof(uint32_t), s));
-    LAUNCH(keygen_tables_kernel<P>, blocks_for(tlen, 128), 128, 0, s, tab, host_to_mont<P>(omega, repr), host_to_mont<P>(delta, repr), k, (uint32_t)cols);
     for (uint64_t i = 0; i < cols; i++)
         for (uint64_t j0 = 0; j0 < n; j0 += piece) {
             const uint64_t len = n - j0 < piece ? n - j0 : piece;
             if (upload_async(map, mapping + 2 * (i * n + j0), len * sizeof(uint2), s)) return 1;
-            LAUNCH(keygen_sigma_kernel<P>, blocks_for(len, 256), 256, 0, s, dst[i]->buf.as<fe>() + j0, (const uint2 *)map, (const fe *)tab, k,
-                   (uint32_t)cols, len, err);
+            if (sigma_launch<P>(dst[i], j0, map, len, k, cols, tab, err)) return 1;
         }
-    uint32_t h_err = 0;
-    CU(cudaMemcpyAsync(&h_err, err, sizeof h_err, cudaMemcpyDeviceToHost, s));
-    if (scratch_release(s)) return 1;
-    CU(cudaStreamSynchronize(s));
-    if (h_err) return fail("h2_poly_permutation_sigma: a mapping entry is outside the permutation's columns or the domain's rows");
+    return sigma_finish(err, "h2_poly_permutation_sigma");
+}
+// the dst checks of both entry points: known handles of one field, at least 2^k elements each, no handle twice
+static int sigma_dst(const char *who, const uint64_t *dst, size_t cols, uint32_t k, std::vector<PolyBuf *> &d) {
+    const std::string w(who);
+    d.resize(cols);
+    for (size_t i = 0; i < cols; i++) {
+        d[i] = find_poly(dst[i]);
+        if (!d[i]) return fail(w + ": unknown polynomial handle");
+        if (d[i]->field != d[0]->field) return fail(w + ": the polynomials live in different fields");
+        if (d[i]->len < ((size_t)1 << k)) return fail(w + ": a polynomial holds fewer than 2^k elements");
+    }
+    std::vector<PolyBuf *> sorted(d);
+    std::sort(sorted.begin(), sorted.end());
+    if (std::adjacent_find(sorted.begin(), sorted.end()) != sorted.end()) return fail(w + ": a dst handle appears twice");
     return 0;
 }
 extern "C" int h2_poly_permutation_sigma(const uint64_t *dst, size_t cols, uint32_t k, const uint32_t *mapping, const void *omega, const void *delta,
@@ -441,16 +477,133 @@ extern "C" int h2_poly_permutation_sigma(const uint64_t *dst, size_t cols, uint3
     if (cols == 0) return 0;
     if (cols >= (1ull << 32)) return fail("h2_poly_permutation_sigma: cols >= 2^32");
     if (!dst || !mapping || !omega || !delta) return fail("h2_poly_permutation_sigma: null argument");
-    std::vector<PolyBuf *> d(cols);
-    for (size_t i = 0; i < cols; i++) {
-        d[i] = find_poly(dst[i]);
-        if (!d[i]) return fail("h2_poly_permutation_sigma: unknown polynomial handle");
-        if (d[i]->field != d[0]->field) return fail("h2_poly_permutation_sigma: the polynomials live in different fields");
-        if (d[i]->len < ((size_t)1 << k)) return fail("h2_poly_permutation_sigma: a polynomial holds fewer than 2^k elements");
-    }
-    std::vector<PolyBuf *> sorted(d);
-    std::sort(sorted.begin(), sorted.end());
-    if (std::adjacent_find(sorted.begin(), sorted.end()) != sorted.end()) return fail("h2_poly_permutation_sigma: a dst handle appears twice");
+    std::vector<PolyBuf *> d;
+    if (sigma_dst("h2_poly_permutation_sigma", dst, cols, k, d)) return 1;
     if (d[0]->field == H2_FIELD_FP) return permutation_sigma_run<FpParams>(d, k, mapping, omega, delta, repr);
     return permutation_sigma_run<FqParams>(d, k, mapping, omega, delta, repr);
+}
+
+
+// ------------------------------------------------------------------------------------------------
+// the permutation argument's copy cycles from the copy constraints (assembly.cuh), then sigma (keygen.cuh)
+// ------------------------------------------------------------------------------------------------
+static int as_read_u32(uint32_t *h, const uint32_t *d, cudaStream_t s) {     // one device word back, synchronously
+    CU(cudaMemcpyAsync(h, d, sizeof(uint32_t), cudaMemcpyDeviceToHost, s));
+    CU(cudaStreamSynchronize(s));
+    return 0;
+}
+// The copy-cycle mapping of m copies (4 uint32 each, synthesis order) over cols * 2^k cells into X.kg_map as (column,
+// row) pairs; *bad = 2 i (column) / 2 i + 1 (row) of the first bad copy i, or ~0.  Scratch in the lane's pools:
+//   as_edge  u32: copies 4m | ea m | eb m | flag m + 1 | live 2 x m | ra m | rb m | keep m + 1 | F m | changed, error word
+//   as_cell  u32: comp N | best N          as_slot  u32: scell S | order 2 x S | nxt 2 x S | digit counts 256 ntiles + 1
+static int assembly_run(uint32_t cols, uint32_t k, const uint32_t *copies, uint64_t m, unsigned long long *bad) {
+    Context &X = g_ctx;
+    cudaStream_t s = X.stream;
+    const uint64_t N = (uint64_t)cols << k;
+    if (X.kg_map.ensure(N * sizeof(uint2)) || X.as_edge.ensure((14 * m + 8) * sizeof(uint32_t))) return 1;
+    uint2 *map = X.kg_map.as<uint2>();
+    unsigned long long *err = X.as_edge.as<unsigned long long>();
+    uint32_t *changed = X.as_edge.as<uint32_t>() + 2;
+    uint32_t *cp = changed + 2, *ea = cp + 4 * m, *eb = ea + m, *flag = eb + m, *live[2] = {flag + m + 1, flag + 2 * m + 1};
+    uint32_t *ra = live[1] + m, *rb = ra + m, *keep = rb + m, *fl = keep + m + 1;
+    CU(cudaMemsetAsync(err, 0xFF, sizeof *err, s));
+    if (m) {
+        if (upload_async(cp, copies, m * 4 * sizeof(uint32_t), s)) return 1;
+        LAUNCH(as_encode_kernel, blocks_for(m + 1, 256), 256, 0, s, (const uint32_t *)cp, (uint32_t)m, cols, k, ea, eb, flag, err);
+    }
+    CU(cudaMemcpyAsync(bad, err, sizeof *bad, cudaMemcpyDeviceToHost, s));
+    CU(cudaStreamSynchronize(s));
+    if (*bad != ~0ull) return 0;
+    LAUNCH(as_identity_kernel, blocks_for(N, 256), 256, 0, s, map, N, k);
+    if (m == 0) return 0;
+    // 2. the spanning forest, Borůvka rounds over the live copies
+    uint32_t L = 0, q = 0;
+    if (lk_scan(flag, m + 1, s) || as_read_u32(&L, flag + m, s)) return 1;
+    LAUNCH(as_compact_kernel, blocks_for(m, 256), 256, 0, s, (const uint32_t *)flag, (uint32_t)m, (const uint32_t *)nullptr, live[0]);
+    CU(cudaMemsetAsync(keep, 0, (m + 1) * sizeof(uint32_t), s));
+    if (L) {
+        if (X.as_cell.ensure(2 * N * sizeof(uint32_t))) return 1;
+        uint32_t *comp = X.as_cell.as<uint32_t>(), *best = comp + N;
+        LAUNCH(as_iota_kernel, blocks_for(N, 256), 256, 0, s, comp, N);
+        uint32_t limit = 0;                                     // after r rounds a component with a live copy has >= 2^r cells
+        while ((2ull << limit) <= N) limit++;
+        for (uint32_t round = 0, cur = 0; L; round++, cur ^= 1) {
+            if (round == limit) return fail("h2_poly_permutation_sigma_copies: internal error: the spanning forest needs more than log2(cells) rounds");
+            const uint32_t *lv = live[cur];
+            LAUNCH(as_roots_kernel, blocks_for(L, 256), 256, 0, s, lv, L, (const uint32_t *)ea, (const uint32_t *)eb, (const uint32_t *)comp, ra, rb, best);
+            LAUNCH(as_best_kernel, blocks_for(L, 256), 256, 0, s, lv, L, (const uint32_t *)ra, (const uint32_t *)rb, best);
+            LAUNCH(as_hook_kernel, blocks_for(L, 256), 256, 0, s, lv, L, (const uint32_t *)ra, (const uint32_t *)rb, (const uint32_t *)best, comp, keep);
+            for (uint32_t h_changed = 1; h_changed;) {
+                CU(cudaMemsetAsync(changed, 0, sizeof(uint32_t), s));
+                LAUNCH(as_jump_kernel, blocks_for(N, 256), 256, 0, s, comp, N, changed);
+                if (as_read_u32(&h_changed, changed, s)) return 1;
+            }
+            LAUNCH(as_split_kernel, blocks_for(L + 1, 256), 256, 0, s, lv, L, (const uint32_t *)ea, (const uint32_t *)eb, (const uint32_t *)comp, flag);
+            if (lk_scan(flag, L + 1, s)) return 1;
+            LAUNCH(as_compact_kernel, blocks_for(L, 256), 256, 0, s, (const uint32_t *)flag, L, lv, live[cur ^ 1]);
+            if (as_read_u32(&L, flag + L, s)) return 1;
+        }
+    }
+    if (lk_scan(keep, m + 1, s) || as_read_u32(&q, keep + m, s)) return 1;
+    if (q == 0) return 0;
+    LAUNCH(as_compact_kernel, blocks_for(m, 256), 256, 0, s, (const uint32_t *)keep, (uint32_t)m, (const uint32_t *)nullptr, fl);
+    // 3. slots, stably sorted by cell
+    const uint64_t S = 2ull * q;
+    if (S >= (1ull << 32)) return fail("h2_poly_permutation_sigma_copies: the spanning forest has 2^31 copies or more");
+    const uint64_t ntiles = (S + H2_AS_TILE - 1) / H2_AS_TILE;
+    if (X.as_slot.ensure((5 * S + H2_AS_TILE * ntiles + 1) * sizeof(uint32_t))) return 1;
+    uint32_t *scell = X.as_slot.as<uint32_t>(), *order[2] = {scell + S, scell + 2 * S}, *nxt[2] = {scell + 3 * S, scell + 4 * S};
+    uint32_t *counts = scell + 5 * S;
+    LAUNCH(as_slots_kernel, blocks_for(S, 256), 256, 0, s, (const uint32_t *)fl, S, (const uint32_t *)ea, (const uint32_t *)eb, scell, order[0]);
+    uint32_t o = 0;
+    for (uint32_t shift = 0; shift == 0 || ((N - 1) >> shift); shift += H2_AS_DIGIT_BITS, o ^= 1) {
+        LAUNCH(as_radix_hist_kernel, (uint32_t)ntiles, H2_AS_TILE, 0, s, (const uint32_t *)order[o], S, (const uint32_t *)scell, shift, ntiles, counts);
+        if (lk_scan(counts, H2_AS_TILE * ntiles + 1, s)) return 1;
+        LAUNCH(as_radix_scatter_kernel, (uint32_t)ntiles, H2_AS_TILE, 0, s, (const uint32_t *)order[o], S, (const uint32_t *)scell, shift,
+               (const uint32_t *)counts, ntiles, order[o ^ 1]);
+    }
+    // 4. successor and pointer jumping: a walk has at most |F| steps < 2^rounds
+    LAUNCH(as_succ_kernel, blocks_for(S, 256), 256, 0, s, (const uint32_t *)order[o], S, (const uint32_t *)scell, nxt[0]);
+    uint32_t t = 0;
+    for (uint64_t len = 1; len <= S; len <<= 1, t ^= 1)
+        LAUNCH(as_jump_slots_kernel, blocks_for(S, 256), 256, 0, s, (const uint32_t *)nxt[t], nxt[t ^ 1], S);
+    LAUNCH(as_final_kernel, blocks_for(S, 256), 256, 0, s, (const uint32_t *)order[o], S, (const uint32_t *)scell, (const uint32_t *)nxt[t], k, map);
+    return 0;
+}
+template <class P>
+static int permutation_sigma_copies_run(const std::vector<PolyBuf *> &dst, uint32_t k, const uint32_t *copies, uint64_t m, const void *omega,
+                                        const void *delta, int repr) {
+    Context &X = g_ctx;
+    cudaStream_t s = X.stream;
+    const uint64_t n = 1ull << k, cols = dst.size();
+    unsigned long long bad = ~0ull;
+    if (scratch_acquire(s)) return 1;
+    if (assembly_run((uint32_t)cols, k, copies, m, &bad)) return 1;
+    if (bad != ~0ull) {
+        if (scratch_release(s)) return 1;
+        return fail("h2_poly_permutation_sigma_copies: copy " + std::to_string(bad >> 1) +
+                    ((bad & 1) ? ": a row is outside the domain (Error::BoundsFailure)" : ": a column is outside the permutation (Error::ColumnNotInPermutation)"));
+    }
+    fe *tab;
+    uint32_t *err;
+    if (sigma_tables<P>(k, cols, omega, delta, repr, &tab, &err)) return 1;
+    const uint2 *map = X.kg_map.as<uint2>();
+    for (uint64_t i = 0; i < cols; i++)
+        if (sigma_launch<P>(dst[i], 0, map + i * n, n, k, cols, tab, err)) return 1;
+    return sigma_finish(err, "h2_poly_permutation_sigma_copies");
+}
+extern "C" int h2_poly_permutation_sigma_copies(const uint64_t *dst, size_t cols, uint32_t k, const uint32_t *copies, size_t m, const void *omega,
+                                                const void *delta, int repr) {
+    CtxLock lk;
+    if (require_ready()) return 1;
+    if (k > 30) return fail("h2_poly_permutation_sigma_copies: k > 30");
+    if (cols == 0) return 0;
+    if (cols >= (1ull << 32)) return fail("h2_poly_permutation_sigma_copies: cols >= 2^32");
+    if (!dst || (m && !copies) || !omega || !delta) return fail("h2_poly_permutation_sigma_copies: null argument");
+    if (((uint64_t)cols << k) >= (1ull << 32)) return fail("h2_poly_permutation_sigma_copies: cols * 2^k >= 2^32 cells");
+    if ((uint64_t)m >= (1ull << 32)) return fail("h2_poly_permutation_sigma_copies: m >= 2^32 copies");
+    std::vector<PolyBuf *> d;
+    if (sigma_dst("h2_poly_permutation_sigma_copies", dst, cols, k, d)) return 1;
+    if (d[0]->field == H2_FIELD_FP) return permutation_sigma_copies_run<FpParams>(d, k, copies, m, omega, delta, repr);
+    return permutation_sigma_copies_run<FqParams>(d, k, copies, m, omega, delta, repr);
 }

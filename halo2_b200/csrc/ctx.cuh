@@ -166,7 +166,8 @@ struct Context {
     DevBuf ast_code, ast_consts;             // asteval.cuh: the postfix program and its constants
     DevBuf po_lvl, po_q, po_pts, po_ptrs;    // polyops.cuh: level arrays, kate carries, per-level points, pointer arrays
     DevBuf lk_keys, lk_left, lk_u32;         // lookup.cuh: sorted canonical keys (input | table), leftover table values, flag / scan arrays
-    DevBuf kg_tab, kg_map;                   // keygen.cuh: power tables + error word, one piece of the copy-constraint mapping
+    DevBuf kg_tab, kg_map;                   // keygen.cuh: power tables + error word, one piece of the copy-constraint mapping (all of it for assembly.cuh)
+    DevBuf as_edge, as_cell, as_slot;        // assembly.cuh: per-copy, per-cell and per-slot u32 arrays
     std::vector<TwiddleEntry *> twiddles;
     uint64_t tw_stamp = 0;
     std::map<uint64_t, BaseSet *> shards;    // this device's shards of multi-GPU base sets (h2_multi_bases_register)

@@ -2,15 +2,17 @@
 (/root/reference/halo2_proofs/src/plonk/keygen.rs:188-336), the permutation argument's Assembly and build_vk / build_pk
 (plonk/permutation/keygen.rs:16-211) and batch_invert_assigned (poly.rs:135-180).
 
-The copy-constraint bookkeeping (`Assembly.copy`) is the reference's sequential algorithm on the host; everything of size
-n per column runs on the device and stays there: the sigma polynomials come from one h2_poly_permutation_sigma call
-(csrc/keygen.cuh), the transforms and commitments are the engine's resident ones.  Circuit synthesis and selector
+The copy-constraint bookkeeping is either the reference's sequential algorithm on the host (`Assembly.copy`, whose mapping
+h2_poly_permutation_sigma turns into sigma) or, with `CopyConstraints`, the list of copies itself, which
+h2_poly_permutation_sigma_copies turns into the same sigma on the device (csrc/assembly.cuh, then csrc/keygen.cuh).
+Everything of size n per column runs on the device and stays there: the transforms and commitments are the engine's
+resident ones.  Circuit synthesis and selector
 compression are the caller's: keygen_vk / keygen_pk take the final fixed columns.
 """
 from __future__ import annotations
 
 import ctypes
-from typing import List, Sequence
+from typing import List, Sequence, Union
 
 import numpy as np
 
@@ -67,20 +69,84 @@ class Assembly:
         return out
 
 
-def build_permutation_polys(domain: EvaluationDomain, assembly: Assembly, delta: int) -> List[ResidentPoly]:
+class CopyConstraints:
+    """The permutation argument's copy constraints as a list, in the order synthesis makes them: what `Assembly` consumes,
+    without replaying its cycle bookkeeping on the host.  build_permutation_polys / keygen_vk / keygen_pk take it in place
+    of an Assembly and get the same key: the cycles are computed on the device from the list (csrc/assembly.cuh).
+    `copies` gives the list as an (m, 4) uint32 array of (left column, left row, right column, right row)."""
+
+    def __init__(self, n: int, num_columns: int):
+        self.n, self.num_columns = int(n), int(num_columns)
+        assert self.n > 0 and self.n & (self.n - 1) == 0, "n = params.n is a power of two"
+        self._arrays: List[np.ndarray] = []
+        self._pending: List[tuple] = []
+
+    def copy(self, left_column: int, left_row: int, right_column: int, right_row: int) -> None:
+        """Assembly.copy's checks, then the copy is recorded: a column outside the permutation raises ValueError
+        (Error::ColumnNotInPermutation), a row outside [0, n) IndexError (Error::BoundsFailure)."""
+        for c in (left_column, right_column):
+            if not 0 <= c < self.num_columns:
+                raise ValueError(f"column {c} is not in the permutation ({self.num_columns} columns)")
+        if not (0 <= left_row < self.n and 0 <= right_row < self.n):
+            raise IndexError(f"row out of bounds: {left_row}, {right_row} (n = {self.n})")
+        self._pending.append((int(left_column), int(left_row), int(right_column), int(right_row)))
+
+    def extend(self, copies) -> None:
+        """Records an (m, 4) integer array of copies, checked as a whole: when a row of it fails copy()'s checks, the first
+        such row raises copy()'s exception (naming its index) and nothing of the array is recorded."""
+        a = np.asarray(copies)
+        if a.size == 0:
+            return
+        if a.ndim != 2 or a.shape[1] != 4 or a.dtype.kind not in "iu":
+            raise TypeError("copies must be an (m, 4) integer array of (left column, left row, right column, right row)")
+        bad_col = ((a[:, [0, 2]] < 0) | (a[:, [0, 2]] >= self.num_columns)).any(axis=1)
+        bad_row = ((a[:, [1, 3]] < 0) | (a[:, [1, 3]] >= self.n)).any(axis=1)
+        bad = np.flatnonzero(bad_col | bad_row)
+        if bad.size:
+            i = int(bad[0])
+            if bad_col[i]:
+                raise ValueError(f"copy {i}: a column of {a[i].tolist()} is not in the permutation ({self.num_columns} columns)")
+            raise IndexError(f"copy {i}: a row of {a[i].tolist()} is out of bounds (n = {self.n})")
+        self._flush()
+        self._arrays.append(a.astype(np.uint32))
+
+    def _flush(self) -> None:
+        if self._pending:
+            self._arrays.append(np.array(self._pending, dtype=np.uint32).reshape(-1, 4))
+            self._pending = []
+
+    def __len__(self) -> int:
+        return sum(a.shape[0] for a in self._arrays) + len(self._pending)
+
+    @property
+    def copies(self) -> np.ndarray:
+        self._flush()
+        if len(self._arrays) != 1:
+            self._arrays = [np.concatenate(self._arrays) if self._arrays else np.zeros((0, 4), dtype=np.uint32)]
+        return self._arrays[0]
+
+
+def build_permutation_polys(domain: EvaluationDomain, assembly: Union[Assembly, CopyConstraints], delta: int) -> List[ResidentPoly]:
     """The permutation polynomials of build_vk / build_pk (permutation/keygen.rs:108-143, :161-198) in the Lagrange basis,
-    resident: sigma_i[j] = delta^c * omega^r for (c, r) = mapping[i][j].  `delta` is F::DELTA."""
+    resident: sigma_i[j] = delta^c * omega^r for (c, r) = mapping[i][j].  `delta` is F::DELTA.  From an Assembly the
+    mapping goes up; from CopyConstraints the copy list goes up and the mapping is computed on the device."""
     if assembly.n != domain.n:
         raise _l.H2Error(f"the assembly has {assembly.n} rows, the domain {domain.n}")
     cols = assembly.num_columns
     polys = [ResidentPoly(domain.field, domain.n) for _ in range(cols)]
     if not cols:
         return polys
-    mapping = np.ascontiguousarray(assembly.mapping)
+    omega, dl = _l.ptr(_l.fe_bytes(domain.omega)), _l.ptr(_l.fe_bytes(int(delta) % domain.m))
     try:
-        _l.check(_l.init().h2_poly_permutation_sigma(_handles(polys), ctypes.c_size_t(cols), ctypes.c_uint32(domain.k),
-                                                     mapping.ctypes.data_as(ctypes.c_void_p), _l.ptr(_l.fe_bytes(domain.omega)),
-                                                     _l.ptr(_l.fe_bytes(int(delta) % domain.m)), _l.REPR_CANONICAL))
+        if isinstance(assembly, CopyConstraints):
+            copies = np.ascontiguousarray(assembly.copies, dtype=np.uint32)
+            _l.check(_l.init().h2_poly_permutation_sigma_copies(_handles(polys), ctypes.c_size_t(cols), ctypes.c_uint32(domain.k),
+                                                                copies.ctypes.data_as(ctypes.c_void_p), ctypes.c_size_t(copies.shape[0]),
+                                                                omega, dl, _l.REPR_CANONICAL))
+        else:
+            mapping = np.ascontiguousarray(assembly.mapping)
+            _l.check(_l.init().h2_poly_permutation_sigma(_handles(polys), ctypes.c_size_t(cols), ctypes.c_uint32(domain.k),
+                                                         mapping.ctypes.data_as(ctypes.c_void_p), omega, dl, _l.REPR_CANONICAL))
     except BaseException:
         for p in polys:
             p.close()
@@ -149,7 +215,7 @@ def _fixed_values(domain: EvaluationDomain, fixed) -> List[ResidentPoly]:
     return out
 
 
-def keygen_vk(params: Params, domain: EvaluationDomain, fixed, assembly: Assembly, delta: int):
+def keygen_vk(params: Params, domain: EvaluationDomain, fixed, assembly: Union[Assembly, CopyConstraints], delta: int):
     """keygen_vk's commitments (keygen.rs:188-236, permutation/keygen.rs:102-153): commit_lagrange of every fixed column and
     every permutation polynomial with Blind::default(), in one pass over the resident generators.  Returns
     (fixed_commitments, permutation_commitments) as affine (m, 64) uint8 arrays in the reference's order."""
@@ -194,7 +260,8 @@ class ProvingKey:
             p.close()
 
 
-def keygen_pk(params: Params, domain: EvaluationDomain, fixed, assembly: Assembly, delta: int, blinding_factors: int) -> ProvingKey:
+def keygen_pk(params: Params, domain: EvaluationDomain, fixed, assembly: Union[Assembly, CopyConstraints], delta: int,
+              blinding_factors: int) -> ProvingKey:
     """keygen_pk (keygen.rs:240-336, permutation/keygen.rs:155-211) on the device: the fixed and permutation columns in all
     three forms, and l_0 / l_blind / l_last (1 on row 0 / on the last `blinding_factors` rows / on row n - blinding_factors - 1,
     :306-325) as extended cosets.  The indicator columns start from a zero allocation and get their ones by add_at."""

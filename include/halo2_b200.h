@@ -230,6 +230,15 @@ int h2_poly_scale_add(uint64_t dst, const void *a, uint64_t src, const void *b, 
  * equal, or k > 30; cols == 0 does nothing.  Synchronous. */
 int h2_poly_permutation_sigma(const uint64_t *dst, size_t cols, uint32_t k, const uint32_t *mapping,
                               const void *omega, const void *delta, int repr);
+/* The same sigma polynomials from the copy constraints themselves: the reference's Assembly (keygen.rs:24-100) runs on
+ * the device (spanning forest of the copies, then the cycles by pointer jumping), with no mapping built or uploaded.
+ * copies: m * 4 uint32 (left column, left row, right column, right row) in host memory, in synthesis order, columns as
+ * indices into the permutation's column list.  Fails, with the index of the first bad copy and whether its column
+ * (Error::ColumnNotInPermutation) or its row (Error::BoundsFailure) is out of range, and then writes nothing to dst.
+ * Also fails on the checks of h2_poly_permutation_sigma, on cols * 2^k >= 2^32 and on m >= 2^32.  m == 0 gives the
+ * identity sigma delta^c omega^r; cols == 0 does nothing.  Synchronous. */
+int h2_poly_permutation_sigma_copies(const uint64_t *dst, size_t cols, uint32_t k, const uint32_t *copies, size_t m,
+                                     const void *omega, const void *delta, int repr);
 
 /* Reference sort of the MSM: by default every (point, window) reference is binned in ONE pass into fixed-capacity
  * per-bucket bins, with an automatic fallback to the exact histogram / scan / scatter sort when a bin overflows

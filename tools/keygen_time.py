@@ -1,7 +1,7 @@
 """Key generation time for the reference's benchmark circuit (benches/plonk.rs, rebuilt in tests/bench_circuit.py: 4 fixed
 columns, 3 permutation columns) on the GPU, the engine's keygen against the path the tests and bench.py take today.
 
-  python tools/keygen_time.py [--ks 14,16,18,20] [--reps 3] [--out keygen_time.json]
+  python tools/keygen_time.py [--ks 14,16,18,20] [--reps 3] [--cycle-k 20] [--out keygen_time.json]
 
 engine   host Assembly (halo2_b200.Assembly, the reference's copy bookkeeping) | sigma (build_permutation_polys: the mapping
          array, its upload and the kernel, one synchronous call) | the rest of keygen_vk + keygen_pk (fixed-column uploads, one
@@ -9,9 +9,15 @@ engine   host Assembly (halo2_b200.Assembly, the reference's copy bookkeeping) |
 current  sigma in Python from the same mapping (the serial omega-power loop and the gather of permutation/keygen.rs:108-143, as
          tests/bench_circuit.py does it) | an upload and a commit_lagrange + batch_normalize per column (bench.py's keygen) | an
          upload and the two transforms per column, and the three indicator columns from host arrays (tests/plonk_prover.py)
-A separate torch.profiler pass per k gives the device time of the sigma kernels and of the mapping's host-to-device copies.
-Medians of `reps` runs after one warm-up; both paths' commitments are compared.  The GPU's name and power limit are read in
-the same run."""
+copies   the copy list instead of the Assembly (halo2_b200.CopyConstraints, h2_poly_permutation_sigma_copies): the whole
+         sigma call (copy-list upload, the assembly kernels of csrc/assembly.cuh, sigma), keygen_vk + keygen_pk from it, and
+         the host baselines on the same (m, 4) copy array: the Python Assembly and the C oracle's sequential loop
+         (orc_assembly of oracle/assembly_oracle.c, compiled -O3).  The copy arrays are generated vectorised; the baselines replay them row by row.
+A separate torch.profiler pass per k gives the device time of the sigma kernels and of the mapping's host-to-device copies,
+and for the copies path that of the copy-list upload, the assembly kernels and sigma.  --cycle-k adds a synthetic list:
+one cycle through every cell of 3 columns, copies in random order, the longest pointer-jumping chains there are.
+Medians of `reps` runs after one warm-up (the host baselines of the synthetic list run once); both paths' commitments and
+sigma columns are compared.  The GPU's name and power limit are read in the same run."""
 import argparse
 import ctypes
 import json
@@ -97,6 +103,82 @@ def sigma_profile(D, asm):
     return out
 
 
+def copies_profile(D, cc):
+    """Device time (ms) inside one build_permutation_polys from CopyConstraints: the copy-list upload, the assembly kernels
+    (as_*), the sigma and table kernels."""
+    from torch.profiler import ProfilerActivity, profile
+    with profile(activities=[ProfilerActivity.CPU, ProfilerActivity.CUDA]) as prof:
+        for p in h2.build_permutation_polys(D, cc, DELTA):
+            p.close()
+        torch.cuda.synchronize()
+    out = {"copies_upload_ms": 0.0, "copies_assembly_kernels_ms": 0.0, "copies_sigma_kernels_ms": 0.0}
+    for ev in prof.key_averages():
+        t = getattr(ev, "device_time_total", None)
+        t = (ev.cuda_time_total if t is None else t) / 1e3
+        if "keygen_sigma_kernel" in ev.key or "keygen_tables_kernel" in ev.key:
+            out["copies_sigma_kernels_ms"] += t
+        elif "HtoD" in ev.key:
+            out["copies_upload_ms"] += t
+        elif "as_" in ev.key or "scan_" in ev.key:
+            out["copies_assembly_kernels_ms"] += t
+    return out
+
+
+def copies_path(D, copies: np.ndarray, cols: int, reps: int, host_reps: int) -> dict:
+    """The sigma call from the copy list, its profile, and the host baselines on the same array; checks the sigma columns
+    against those from the Assembly's mapping."""
+    from oracle import assembly as orc
+    k, n = D.k, D.n
+    res = {"copies": int(copies.shape[0])}
+    cc = h2.CopyConstraints(n, cols)
+    cc.extend(copies)
+
+    def sigma():
+        for p in h2.build_permutation_polys(D, cc, DELTA):
+            p.close()
+    res["copies_sigma_call_s"] = median_of(sigma, reps)
+    res.update(copies_profile(D, cc))
+    rows = copies.tolist()
+
+    def py_assembly():
+        a = h2.Assembly(n, cols)
+        for c in rows:
+            a.copy(*c)
+        return a
+    timed = (lambda fn: median_of(fn, reps)) if host_reps > 1 else once
+    res["python_assembly_s"] = timed(py_assembly)
+    res["orc_assembly_s"] = timed(lambda: orc.assembly(copies, cols, k))
+    mapping, err = orc.assembly(copies, cols, k)
+    assert err is None
+    a = [p for p in h2.build_permutation_polys(D, cc, DELTA)]
+    asm = h2.Assembly(n, cols)
+    asm._mapping = (mapping[..., 0].astype(np.int64) * n + mapping[..., 1]).reshape(-1)   # the oracle's mapping, no second replay
+    b = h2.build_permutation_polys(D, asm, DELTA)
+    res["copies_sigma_identical"] = all((x.download() == y.download()).all() for x, y in zip(a, b))
+    for p in a + b:
+        p.close()
+    return res
+
+
+def once(fn):
+    t0 = time.perf_counter()
+    fn()
+    return time.perf_counter() - t0
+
+
+def run_cycle(k: int, reps: int) -> dict:
+    """The synthetic list: one cycle through all 3 * 2^k cells, copies in random order."""
+    n = 1 << k
+    D = h2.EvaluationDomain("fp", BC.DEGREE, k, ZETA)
+    rng = np.random.default_rng(20)
+    perm = rng.permutation(3 * n).astype(np.int64)
+    nxt = np.roll(perm, -1)
+    cp = np.stack([perm >> k, perm & (n - 1), nxt >> k, nxt & (n - 1)], axis=1)[rng.permutation(3 * n)].astype(np.uint32)
+    res = {"k": k, "list": "one cycle through every cell, random copy order"}
+    res.update(copies_path(D, np.ascontiguousarray(cp), 3, reps, 1))
+    return res
+
+
 def run_k(k: int, reps: int) -> dict:
     n = 1 << k
     D = h2.EvaluationDomain("fp", BC.DEGREE, k, ZETA)
@@ -173,6 +255,20 @@ def run_k(k: int, reps: int) -> dict:
         pk = h2.keygen_pk(prm, D, fixed_b, asm, DELTA, BC.BLINDING_FACTORS)
         res["sigma_identical"] = all((p.download() == s).all() for p, s in zip(pk.permutation.permutations, sig_b))
         pk.close()
+
+        # the copy-list path
+        arr = np.empty((2 * len(copies), 4), dtype=np.uint32)
+        it = np.arange(len(copies), dtype=np.uint32)
+        arr[0::2] = np.stack([0 * it, 2 * it, 0 * it, 2 * it + 1], axis=1)          # copy(a0, a1) ...
+        arr[1::2] = np.stack([0 * it + 1, 2 * it + 1, 0 * it + 2, 2 * it], axis=1)  # ... copy(b1, c0), as assembly() replays them
+        res.update(copies_path(D, arr, 3, reps, reps))
+        cc = h2.CopyConstraints(n, 3)
+        cc.extend(arr)
+        res["copies_keygen_vk_s"] = median_of(lambda: h2.keygen_vk(prm, D, fixed_b, cc, DELTA), reps)
+        res["copies_keygen_pk_s"] = median_of(lambda: h2.keygen_pk(prm, D, fixed_b, cc, DELTA, BC.BLINDING_FACTORS).close(), reps)
+        res["copies_engine_total_s"] = res["copies_keygen_vk_s"] + res["copies_keygen_pk_s"]
+        fcc, pcc = h2.keygen_vk(prm, D, fixed_b, cc, DELTA)
+        res["copies_commitments_identical"] = bool((fcc == fc).all() and (pcc == pc).all())
     finally:
         prm.close()
     return res
@@ -182,12 +278,17 @@ def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--ks", default="14,16,18,20")
     ap.add_argument("--reps", type=int, default=3)
+    ap.add_argument("--cycle-k", type=int, default=20, help="k of the synthetic one-cycle list (0: none)")
     ap.add_argument("--out", default=None)
     a = ap.parse_args()
     L.init()
     out = {"gpu": gpu_info(), "results": []}
     for k in (int(x) for x in a.ks.split(",")):
         r = run_k(k, a.reps)
+        out["results"].append(r)
+        print(json.dumps(r), flush=True)
+    if a.cycle_k:
+        r = run_cycle(a.cycle_k, a.reps)
         out["results"].append(r)
         print(json.dumps(r), flush=True)
     out["gpu_after"] = gpu_info()
