@@ -106,6 +106,8 @@ extern "C" {
     pub fn h2_lane_create(lane: *mut u64) -> c_int;
     pub fn h2_lane_bind(lane: u64) -> c_int;
     pub fn h2_lane_destroy(lane: u64) -> c_int;
+    // shared polynomials: one read-only proving key for every lane
+    pub fn h2_poly_share(polys: *const u64, n: usize) -> c_int;
 }
 
 fn check(rc: c_int) {
@@ -428,7 +430,8 @@ pub fn init(device: i32) {
 /// A prover lane bound to the current thread: every engine call this thread makes while the guard lives runs on a context
 /// of its own (streams, scratch, caches, settings, resident polynomials and IPA sessions), concurrently with threads on other
 /// lanes.  `ResidentBases` are shared by all lanes; resident polynomials (`h2_poly_*`) and IPA sessions belong to the lane
-/// they were created on and are freed with it.  Dropping the guard destroys the lane and puts the thread back on the primary context.
+/// they were created on and are freed with it, except polynomials passed to `share_polys`.  Dropping the guard destroys the
+/// lane and puts the thread back on the primary context.
 /// Binding is per thread, so the guard is `!Send`.
 pub struct Lane {
     handle: u64,
@@ -450,6 +453,16 @@ impl Drop for Lane {
     fn drop(&mut self) {
         unsafe { h2_lane_destroy(self.handle) };
     }
+}
+
+/// Shares resident polynomials of the calling thread's lane (or of the primary context) read-only with every lane and the
+/// primary context (`h2_poly_share`): a proving key built once, on one lane, and read by the provers on all of them.  All or
+/// nothing: every handle must be the caller's or already shared, else the call panics and nothing is shared.  Handles do not
+/// change.  A shared handle may be used from any thread -- wherever a polynomial is only read, and by `h2_poly_free`, which
+/// waits for the reads in progress on every lane -- so a key of shared handles can be `Send + Sync`.  An entry point that
+/// would write a shared polynomial fails with a message saying it is shared; the lane that shared it may be dropped first.
+pub fn share_polys(handles: &[u64]) {
+    check(unsafe { h2_poly_share(handles.as_ptr(), handles.len()) });
 }
 
 /// One process, several GPUs: after `init(primary)`, bind `ngpu` devices; `best_multiexp_multi_gpu` then shards every call

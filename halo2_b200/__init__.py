@@ -10,7 +10,7 @@ from .arithmetic import (best_multiexp, small_multiexp, best_fft, best_fft_curve
                          eval_polynomial, compute_inner_product, kate_division)
 from .poly import (Params, EvaluationDomain, Blind, ResidentPoly, lagrange_generators, compress_points, decompress_points, hash_to_curve,  # noqa: F401
                    eval_polynomial_resident, inner_product_resident, kate_division_resident, batch_invert_resident,
-                   running_product_resident, permute_expression_pair_resident)
+                   running_product_resident, permute_expression_pair_resident, share_resident)
 
 from .evaluator import Ast, AstLeaf, Evaluator  # noqa: F401
 from .verifier import MSM, Guard, VerifyError, verify_proof, compute_b  # noqa: F401
@@ -23,4 +23,5 @@ __all__ = ["Ast", "AstLeaf", "Evaluator", "Assembly", "CopyConstraints", "Provin
            "best_fft_curve", "batch_normalize", "multiexp_window_bits", "Params", "EvaluationDomain", "Blind", "ResidentPoly",
            "lagrange_generators", "compress_points", "decompress_points", "hash_to_curve",
            "eval_polynomial", "compute_inner_product", "kate_division", "eval_polynomial_resident", "inner_product_resident",
-           "kate_division_resident", "batch_invert_resident", "running_product_resident", "permute_expression_pair_resident"]
+           "kate_division_resident", "batch_invert_resident", "running_product_resident", "permute_expression_pair_resident",
+           "share_resident"]

@@ -39,8 +39,23 @@ struct LaneBinding {
 static thread_local LaneBinding g_binding;
 bool on_lane() { return g_binding.slot >= 0; }
 
+// Objects every lane reads -- base sets and shared polynomials -- count the calls in flight that hold them (users, under
+// g_reg_mu).  Their release takes them out of the registry first, so no new call finds them, then waits here.
+static std::condition_variable g_users_cv;   // a shared object's users dropped to 0
+static void user_drop(uint32_t &users) {     // under g_reg_mu
+    if (--users == 0) g_users_cv.notify_all();
+}
+// The object is out of its registry: wait for the calls that hold it, then for the device, which covers the asynchronous
+// reads those calls queued on any lane's stream.  Returns with g_reg_mu released; the caller frees the object.
+static void wait_unused(std::unique_lock<std::mutex> &lk, const uint32_t &users) {
+    g_users_cv.wait(lk, [&users] { return users == 0; });
+    const int dev = g_primary->device;
+    lk.unlock();
+    cudaSetDevice(dev);
+    cudaDeviceSynchronize();
+}
+
 std::map<uint64_t, BaseSet *> g_bases;
-static std::condition_variable g_bases_cv;   // a set's users dropped to 0
 BasesRef::BasesRef(uint64_t handle, bool open_session) {
     std::lock_guard<std::mutex> lk(g_reg_mu);
     auto it = g_bases.find(handle);
@@ -52,7 +67,7 @@ BasesRef::BasesRef(uint64_t handle, bool open_session) {
 BasesRef::~BasesRef() {
     if (!b) return;
     std::lock_guard<std::mutex> lk(g_reg_mu);
-    if (--b->users == 0) g_bases_cv.notify_all();
+    user_drop(b->users);
 }
 void bases_session_end(uint64_t handle) {
     std::lock_guard<std::mutex> lk(g_reg_mu);
@@ -68,12 +83,48 @@ extern "C" int h2_bases_release(uint64_t handle) {
     BaseSet *b = it->second;
     if (b->sessions) return fail("h2_bases_release: an open IPA session uses the base set (h2_ipa_finish it first)");
     g_bases.erase(it);                   // no new user finds it
-    g_bases_cv.wait(lk, [b] { return b->users == 0; });
-    const int dev = g_primary->device;
-    lk.unlock();
-    cudaSetDevice(dev);
-    cudaDeviceSynchronize();
+    wait_unused(lk, b->users);
     bases_free(b);
+    return 0;
+}
+
+std::map<uint64_t, PolyBuf *> g_shared_polys;
+PolyBuf *poly_for_write(uint64_t h, const char *who, const char *unknown) {
+    auto it = g_ctx.polys.find(h);
+    if (it != g_ctx.polys.end()) return it->second;
+    bool shared;
+    {
+        std::lock_guard<std::mutex> lk(g_reg_mu);
+        shared = g_shared_polys.count(h) != 0;
+    }
+    fail(shared ? std::string(who) + ": the polynomial is shared (read-only)" : std::string(unknown));
+    return nullptr;
+}
+PolyBuf *PolyReads::get(uint64_t h) {
+    auto it = g_ctx.polys.find(h);
+    if (it != g_ctx.polys.end()) return it->second;
+    std::lock_guard<std::mutex> lk(g_reg_mu);
+    auto s = g_shared_polys.find(h);
+    if (s == g_shared_polys.end()) return nullptr;
+    s->second->users++;
+    held.push_back(s->second);
+    return s->second;
+}
+PolyReads::~PolyReads() {
+    if (held.empty()) return;
+    std::lock_guard<std::mutex> lk(g_reg_mu);
+    for (PolyBuf *p : held) user_drop(p->users);
+}
+// From any thread and any context: the caller holds no Context mutex.
+int shared_poly_free(uint64_t h) {
+    std::unique_lock<std::mutex> lk(g_reg_mu);
+    auto it = g_shared_polys.find(h);
+    if (it == g_shared_polys.end()) return fail("h2_poly_free: unknown handle");
+    PolyBuf *p = it->second;
+    g_shared_polys.erase(it);            // no new user finds it
+    wait_unused(lk, p->users);
+    p->buf.release();
+    delete p;
     return 0;
 }
 
@@ -430,6 +481,8 @@ extern "C" int h2_shutdown(void) {
     std::lock_guard<std::mutex> reg(g_reg_mu);
     for (auto &kv : g_bases) bases_free(kv.second);
     g_bases.clear();
+    for (auto &kv : g_shared_polys) { kv.second->buf.release(); delete kv.second; }   // every context is idle and synchronised
+    g_shared_polys.clear();
     multi_bases_clear();
     g_multi.clear();
     g_primary = &g_ctxs[0];

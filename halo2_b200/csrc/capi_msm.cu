@@ -82,7 +82,10 @@ static int msm_issue_or_replay(const std::function<int()> &issue, bool graphable
         if (graph) cudaGraphDestroy(graph);
         cudaGetLastError();
         ge->seen = 0;
-        return rc ? rc : issue();            // capture refused: run eagerly
+        // Nothing captured has run, so run eagerly.  The failure need not be this call's: a device-wide synchronisation on
+        // another thread (another lane's cudaFree, cudaDeviceSynchronize, ...) invalidates a capture in progress, and then
+        // every later call of the capture fails.  An error of the pass itself comes back from the eager run.
+        return issue();
     }
     ge->launches = g_launches.load() - l0;
     ce = cudaGraphInstantiate(&ge->exec, graph, 0);
@@ -849,8 +852,9 @@ static int ipa_begin_common(uint64_t bases_handle, uint32_t k, const void *p_pri
     CtxLock lk;
     if (require_ready()) return 1;
     PolyBuf *p_poly = nullptr;
+    PolyReads rd;
     if (p_poly_handle) {   // looked up and used under the one lock
-        p_poly = find_poly(*p_poly_handle);
+        p_poly = rd.get(*p_poly_handle);
         if (!p_poly) return fail("h2_ipa_begin_poly: unknown polynomial handle");
         if (k > 28 || p_poly->len < ((size_t)1 << k)) return fail("h2_ipa_begin_poly: the polynomial holds fewer than 2^k coefficients");
     }
@@ -1023,8 +1027,9 @@ static int msm_registered_polys_impl(uint64_t bases_handle, const uint64_t *poly
         CU(cudaMemcpyAsync(X.misc.p, extra_scalars, batch * sizeof(fe), cudaMemcpyHostToDevice, s));
         if (repr == H2_REPR_CANONICAL && convert_field(scalar_field, X.misc.as<fe>(), batch, 1, s)) return 1;
     }
+    PolyReads rd;
     for (size_t j = 0; j < batch; j++) {
-        PolyBuf *q = find_poly(polys[j]);
+        PolyBuf *q = rd.get(polys[j]);
         if (!q) return fail("h2_msm_registered_polys: unknown polynomial handle");
         if (q->field != scalar_field) return fail("h2_msm_registered_polys: the polynomial is not over the curve's scalar field");
         if (q->len < n) return fail("h2_msm_registered_polys: the polynomial holds fewer than n elements");

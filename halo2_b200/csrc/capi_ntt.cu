@@ -221,13 +221,28 @@ extern "C" int h2_poly_alloc(int field, size_t len, uint64_t *poly) {
     *poly = h;
     return 0;
 }
-extern "C" int h2_poly_free(uint64_t poly) {
+// Moves polynomials of the calling context into the shared registry, all or none (ctx.cuh: g_shared_polys).
+extern "C" int h2_poly_share(const uint64_t *polys, size_t n) {
     CtxLock lk;
+    if (require_ready()) return 1;
+    if (n == 0) return 0;
+    if (!polys) return fail("h2_poly_share: null handle array");
     Context &X = g_ctx;
-    auto it = X.polys.find(poly);
-    if (it == X.polys.end()) return fail("h2_poly_free: unknown handle");
-    PolyBuf *b = it->second;
-    X.polys.erase(it);
+    CU(cudaStreamSynchronize(X.stream));      // every write to them has landed before another context can read them
+    std::lock_guard<std::mutex> reg(g_reg_mu);  // checked and moved under one lock: a shared handle cannot be freed in between
+    for (size_t i = 0; i < n; i++)
+        if (!X.polys.count(polys[i]) && !g_shared_polys.count(polys[i]))
+            return fail("h2_poly_share: unknown polynomial handle (neither the calling context's nor shared)");
+    for (size_t i = 0; i < n; i++) {
+        auto it = X.polys.find(polys[i]);
+        if (it == X.polys.end()) continue;    // already shared, or listed twice
+        g_shared_polys[it->first] = it->second;
+        X.polys.erase(it);
+    }
+    return 0;
+}
+// h2_poly_free of a polynomial the context X owned, taken out of X.polys (X's mutex held)
+static int own_poly_free(Context &X, PolyBuf *b) {
     // every use of a resident polynomial is ordered on the context's stream, and so is its next owner's first write.
     // The pool is first-in first-out: when it is full the OLDEST buffers go (sizes an earlier workload left behind must not
     // pin the pool and push every later free onto the cudaFree + device-sync path, which would make a
@@ -252,6 +267,19 @@ extern "C" int h2_poly_free(uint64_t poly) {
     X.poly_pool_bytes += b->buf.cap;
     return 0;
 }
+extern "C" int h2_poly_free(uint64_t poly) {
+    {
+        CtxLock lk;
+        Context &X = g_ctx;
+        auto it = X.polys.find(poly);
+        if (it != X.polys.end()) {
+            PolyBuf *b = it->second;
+            X.polys.erase(it);
+            return own_poly_free(X, b);
+        }
+    }
+    return shared_poly_free(poly);             // without this context's mutex: it may wait for calls on other lanes
+}
 int convert_field(int field, fe *d, size_t n, int to_mont, cudaStream_t s) {
     if (n == 0) return 0;
     if (field == H2_FIELD_FP) LAUNCH(convert_kernel<FpParams>, blocks_for(n, 256), 256, 0, s, d, (uint64_t)n, to_mont);
@@ -261,8 +289,8 @@ int convert_field(int field, fe *d, size_t n, int to_mont, cudaStream_t s) {
 extern "C" int h2_poly_upload(uint64_t poly, const void *src, size_t len, int repr) {
     CtxLock lk;
     if (require_ready()) return 1;
-    PolyBuf *b = find_poly(poly);
-    if (!b) return fail("h2_poly_upload: unknown handle");
+    PolyBuf *b = poly_for_write(poly, "h2_poly_upload", "h2_poly_upload: unknown handle");
+    if (!b) return 1;
     if (len > b->len) return fail("h2_poly_upload: more elements than the polynomial holds");
     cudaStream_t s = g_ctx.stream;
     if (upload_async(b->buf.p, src, len * sizeof(fe), s)) return 1;
@@ -276,8 +304,8 @@ template <class P> __global__ void poly_add_at_kernel(fe *a, fe delta_mont) { fe
 extern "C" int h2_poly_add_at(uint64_t poly, size_t index, const void *delta, int repr) {
     CtxLock lk;
     if (require_ready()) return 1;
-    PolyBuf *b = find_poly(poly);
-    if (!b) return fail("h2_poly_add_at: unknown handle");
+    PolyBuf *b = poly_for_write(poly, "h2_poly_add_at", "h2_poly_add_at: unknown handle");
+    if (!b) return 1;
     if (index >= b->len) return fail("h2_poly_add_at: index out of range");
     cudaStream_t s = g_ctx.stream;
     if (b->field == H2_FIELD_FP) LAUNCH(poly_add_at_kernel<FpParams>, 1, 1, 0, s, b->buf.as<fe>() + index, host_to_mont<FpParams>(delta, repr));
@@ -289,8 +317,11 @@ extern "C" int h2_poly_add_at(uint64_t poly, size_t index, const void *delta, in
 extern "C" int h2_poly_copy(uint64_t dst, size_t dst_off, uint64_t src, size_t src_off, size_t len) {
     CtxLock lk;
     if (require_ready()) return 1;
-    PolyBuf *d = find_poly(dst), *a = find_poly(src);
-    if (!d || !a) return fail("h2_poly_copy: unknown handle");
+    PolyBuf *d = poly_for_write(dst, "h2_poly_copy", "h2_poly_copy: unknown handle");
+    if (!d) return 1;
+    PolyReads rd;
+    PolyBuf *a = rd.get(src);
+    if (!a) return fail("h2_poly_copy: unknown handle");
     if (d->field != a->field) return fail("h2_poly_copy: the polynomials live in different fields");
     if (dst_off + len > d->len || src_off + len > a->len) return fail("h2_poly_copy: range out of bounds");
     if (d == a && !(dst_off + len <= src_off || src_off + len <= dst_off)) return fail("h2_poly_copy: overlapping ranges");
@@ -300,7 +331,8 @@ extern "C" int h2_poly_copy(uint64_t dst, size_t dst_off, uint64_t src, size_t s
 extern "C" int h2_poly_download(uint64_t poly, void *dst, size_t len, int repr) {
     CtxLock lk;
     if (require_ready()) return 1;
-    PolyBuf *b = find_poly(poly);
+    PolyReads rd;
+    PolyBuf *b = rd.get(poly);
     if (!b) return fail("h2_poly_download: unknown handle");
     if (len > b->len) return fail("h2_poly_download: more elements than the polynomial holds");
     Context &X = g_ctx;
@@ -331,11 +363,14 @@ static int poly_transform(PolyBuf *dst, PolyBuf *src, int mode, uint32_t in_log_
     return scratch_release(s);       // asynchronous: later calls are ordered behind it on the stream
 }
 static int poly_transform_dispatch(uint64_t dst, uint64_t src, int mode, uint32_t in_log_n, uint32_t log_n, const void *omega, const void *zeta,
-                                   const void *divisor, size_t out_len, int repr) {
+                                   const void *divisor, size_t out_len, int repr, const char *who) {
     CtxLock lk;
     if (require_ready()) return 1;
-    PolyBuf *d = find_poly(dst), *a = find_poly(src);
-    if (!d || !a) return fail("resident transform: unknown polynomial handle");
+    PolyBuf *d = poly_for_write(dst, who, "resident transform: unknown polynomial handle");
+    if (!d) return 1;
+    PolyReads rd;
+    PolyBuf *a = rd.get(src);
+    if (!a) return fail("resident transform: unknown polynomial handle");
     if (d->field != a->field) return fail("resident transform: the polynomials live in different fields");
     if (log_n > 30 || in_log_n > log_n) return fail("ntt: bad sizes");
     if (a->len < ((size_t)1 << in_log_n)) return fail("resident transform: the source holds fewer than 2^k elements");
@@ -347,12 +382,12 @@ static int poly_transform_dispatch(uint64_t dst, uint64_t src, int mode, uint32_
     return poly_transform<FqParams>(d, a, mode, in_log_n, log_n, omega, zeta, divisor, out_len, repr);
 }
 extern "C" int h2_poly_lagrange_to_coeff(uint64_t dst, uint64_t src, uint32_t k, const void *omega_inv, const void *divisor, int repr) {
-    return poly_transform_dispatch(dst, src, 1, k, k, omega_inv, nullptr, divisor, (size_t)1 << k, repr);
+    return poly_transform_dispatch(dst, src, 1, k, k, omega_inv, nullptr, divisor, (size_t)1 << k, repr, "h2_poly_lagrange_to_coeff");
 }
 extern "C" int h2_poly_coeff_to_extended(uint64_t dst, uint64_t src, uint32_t k, uint32_t ext_k, const void *zeta, const void *ext_omega, int repr) {
-    return poly_transform_dispatch(dst, src, 2, k, ext_k, ext_omega, zeta, nullptr, (size_t)1 << ext_k, repr);
+    return poly_transform_dispatch(dst, src, 2, k, ext_k, ext_omega, zeta, nullptr, (size_t)1 << ext_k, repr, "h2_poly_coeff_to_extended");
 }
 extern "C" int h2_poly_extended_to_coeff(uint64_t dst, uint64_t src, uint32_t ext_k, const void *ext_omega_inv, const void *ext_divisor,
                                          const void *zeta, size_t out_len, int repr) {
-    return poly_transform_dispatch(dst, src, 3, ext_k, ext_k, ext_omega_inv, zeta, ext_divisor, out_len, repr);
+    return poly_transform_dispatch(dst, src, 3, ext_k, ext_k, ext_omega_inv, zeta, ext_divisor, out_len, repr, "h2_poly_extended_to_coeff");
 }

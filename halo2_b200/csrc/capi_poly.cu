@@ -106,14 +106,16 @@ static int polyops_dispatch(int mode, const uint64_t *ah, const uint64_t *ch, si
     if (n >= (1ull << 32)) return fail(std::string(who) + ": n >= 2^32");
     std::vector<PolyBuf *> a(batch), c;
     if (ch) c.resize(batch);
+    const std::string unknown = std::string(who) + ": unknown polynomial handle";
+    PolyReads rd;
     for (size_t b = 0; b < batch; b++) {
-        a[b] = find_poly(ah[b]);
-        if (!a[b]) return fail(std::string(who) + ": unknown polynomial handle");
+        a[b] = rd.get(ah[b]);
+        if (!a[b]) return fail(unknown);
         if (a[b]->field != a[0]->field) return fail(std::string(who) + ": the polynomials live in different fields");
         if (a[b]->len < n) return fail(std::string(who) + ": a polynomial holds fewer than n coefficients");
-        if (ch) {
-            c[b] = find_poly(ch[b]);
-            if (!c[b]) return fail(std::string(who) + ": unknown polynomial handle");
+        if (ch) {   // kate division writes its quotients; the inner product reads both operands
+            c[b] = mode == 2 ? poly_for_write(ch[b], who, unknown.c_str()) : rd.get(ch[b]);
+            if (!c[b]) return mode == 2 ? 1 : fail(unknown);
             if (c[b]->field != a[0]->field) return fail(std::string(who) + ": the polynomials live in different fields");
             if (c[b]->len + (mode == 2 ? 1 : 0) < n) return fail(std::string(who) + ": the second polynomial is too short");
         }
@@ -160,13 +162,14 @@ extern "C" int h2_poly_eval_ast(uint64_t out, const uint64_t *polys, size_t n_po
                                 const void *consts, size_t n_consts, const void *omega, const void *lin_base, int repr) {
     CtxLock lk;
     if (require_ready()) return 1;
-    PolyBuf *o = find_poly(out);
-    if (!o) return fail("h2_poly_eval_ast: unknown output handle");
+    PolyBuf *o = poly_for_write(out, "h2_poly_eval_ast", "h2_poly_eval_ast: unknown output handle");
+    if (!o) return 1;
     if (log_n > 30 || o->len < ((size_t)1 << log_n)) return fail("h2_poly_eval_ast: the output holds fewer than 2^log_n elements");
     if (n_code == 0 || n_code > (1u << 20)) return fail("h2_poly_eval_ast: empty or oversized program");
     std::vector<PolyBuf *> ps(n_polys);
+    PolyReads rd;
     for (size_t i = 0; i < n_polys; i++) {
-        ps[i] = find_poly(polys[i]);
+        ps[i] = rd.get(polys[i]);
         if (!ps[i]) return fail("h2_poly_eval_ast: unknown polynomial handle");
         if (ps[i]->field != o->field) return fail("h2_poly_eval_ast: the polynomials live in different fields");
         if (ps[i]->len < ((size_t)1 << log_n)) return fail("h2_poly_eval_ast: a polynomial holds fewer than 2^log_n elements");
@@ -197,8 +200,8 @@ extern "C" int h2_poly_eval_ast(uint64_t out, const uint64_t *polys, size_t n_po
 extern "C" int h2_poly_batch_invert(uint64_t poly, size_t n) {
     CtxLock lk;
     if (require_ready()) return 1;
-    PolyBuf *a = find_poly(poly);
-    if (!a) return fail("h2_poly_batch_invert: unknown polynomial handle");
+    PolyBuf *a = poly_for_write(poly, "h2_poly_batch_invert", "h2_poly_batch_invert: unknown polynomial handle");
+    if (!a) return 1;
     if (a->len < n) return fail("h2_poly_batch_invert: the polynomial holds fewer than n elements");
     if (n == 0) return 0;
     cudaStream_t s = g_ctx.stream;
@@ -234,8 +237,11 @@ template <class P> static int grand_product_run(PolyBuf *d, PolyBuf *a, size_t n
 extern "C" int h2_poly_running_product(uint64_t dst, uint64_t src, size_t n, const void *init, int repr) {
     CtxLock lk;
     if (require_ready()) return 1;
-    PolyBuf *d = find_poly(dst), *a = find_poly(src);
-    if (!d || !a) return fail("h2_poly_running_product: unknown polynomial handle");
+    PolyBuf *d = poly_for_write(dst, "h2_poly_running_product", "h2_poly_running_product: unknown polynomial handle");
+    if (!d) return 1;
+    PolyReads rd;
+    PolyBuf *a = rd.get(src);
+    if (!a) return fail("h2_poly_running_product: unknown polynomial handle");
     if (d == a) return fail("h2_poly_running_product: the product cannot overwrite its factors");
     if (d->field != a->field) return fail("h2_poly_running_product: the polynomials live in different fields");
     if (a->len < n || d->len < n) return fail("h2_poly_running_product: a polynomial holds fewer than n elements");
@@ -247,8 +253,8 @@ extern "C" int h2_poly_running_product(uint64_t dst, uint64_t src, size_t n, con
 extern "C" int h2_poly_divide_by_vanishing(uint64_t poly, uint32_t ext_k, const void *t_evals, uint32_t t_len, int repr) {
     CtxLock lk;
     if (require_ready()) return 1;
-    PolyBuf *a = find_poly(poly);
-    if (!a) return fail("h2_poly_divide_by_vanishing: unknown polynomial handle");
+    PolyBuf *a = poly_for_write(poly, "h2_poly_divide_by_vanishing", "h2_poly_divide_by_vanishing: unknown polynomial handle");
+    if (!a) return 1;
     if (ext_k > 30 || a->len < ((size_t)1 << ext_k)) return fail("h2_poly_divide_by_vanishing: the polynomial holds fewer than 2^ext_k elements");
     if (t_len == 0 || (t_len & (t_len - 1)) || t_len > (1u << ext_k)) return fail("h2_poly_divide_by_vanishing: t_len must be a power of two <= 2^ext_k");
     Context &X = g_ctx;
@@ -336,8 +342,13 @@ template <class P> static int lookup_permute_run(PolyBuf *in, PolyBuf *tab, size
 extern "C" int h2_poly_lookup_permute(uint64_t input, uint64_t table, size_t usable_rows, uint64_t out_input, uint64_t out_table) {
     CtxLock lk;
     if (require_ready()) return 1;
-    PolyBuf *a = find_poly(input), *t = find_poly(table), *oa = find_poly(out_input), *ot = find_poly(out_table);
-    if (!a || !t || !oa || !ot) return fail("h2_poly_lookup_permute: unknown polynomial handle");
+    const char *unknown = "h2_poly_lookup_permute: unknown polynomial handle";
+    PolyBuf *oa = poly_for_write(out_input, "h2_poly_lookup_permute", unknown);
+    PolyBuf *ot = oa ? poly_for_write(out_table, "h2_poly_lookup_permute", unknown) : nullptr;
+    if (!oa || !ot) return 1;
+    PolyReads rd;
+    PolyBuf *a = rd.get(input), *t = rd.get(table);
+    if (!a || !t) return fail(unknown);
     if (oa == ot || oa == a || oa == t || ot == a || ot == t) return fail("h2_poly_lookup_permute: the outputs must be two polynomials other than the inputs");
     if (a->field != t->field || a->field != oa->field || a->field != ot->field) return fail("h2_poly_lookup_permute: the polynomials live in different fields");
     if (a->len < usable_rows || t->len < usable_rows || oa->len < usable_rows || ot->len < usable_rows)
@@ -369,8 +380,8 @@ template <class P> static int compute_s_run(PolyBuf *d, const void *u, uint32_t 
 extern "C" int h2_poly_compute_s(uint64_t dst, const void *u, uint32_t k, const void *init, int accumulate, int repr) {
     CtxLock lk;
     if (require_ready()) return 1;
-    PolyBuf *d = find_poly(dst);
-    if (!d) return fail("h2_poly_compute_s: unknown polynomial handle");
+    PolyBuf *d = poly_for_write(dst, "h2_poly_compute_s", "h2_poly_compute_s: unknown polynomial handle");
+    if (!d) return 1;
     if (!u || !init) return fail("h2_poly_compute_s: null challenge vector or init");
     if (k == 0) return fail("h2_poly_compute_s: no challenges (assert!(!u.is_empty()), poly/commitment/verifier.rs:157)");
     if (k > 30 || d->len < ((size_t)1 << k)) return fail("h2_poly_compute_s: the polynomial holds fewer than 2^k elements");
@@ -382,8 +393,11 @@ extern "C" int h2_poly_compute_s(uint64_t dst, const void *u, uint32_t k, const 
 extern "C" int h2_poly_scale_add(uint64_t dst, const void *a, uint64_t src, const void *b, size_t n, int repr) {
     CtxLock lk;
     if (require_ready()) return 1;
-    PolyBuf *d = find_poly(dst), *x = src ? find_poly(src) : nullptr;
-    if (!d || (src && !x)) return fail("h2_poly_scale_add: unknown polynomial handle");
+    PolyBuf *d = poly_for_write(dst, "h2_poly_scale_add", "h2_poly_scale_add: unknown polynomial handle");
+    if (!d) return 1;
+    PolyReads rd;
+    PolyBuf *x = src ? rd.get(src) : nullptr;
+    if (src && !x) return fail("h2_poly_scale_add: unknown polynomial handle");
     if (x == d) return fail("h2_poly_scale_add: src must be another polynomial than dst");
     if (x && x->field != d->field) return fail("h2_poly_scale_add: the polynomials live in different fields");
     if (d->len < n || (x && x->len < n)) return fail("h2_poly_scale_add: a polynomial holds fewer than n elements");
@@ -459,8 +473,8 @@ static int sigma_dst(const char *who, const uint64_t *dst, size_t cols, uint32_t
     const std::string w(who);
     d.resize(cols);
     for (size_t i = 0; i < cols; i++) {
-        d[i] = find_poly(dst[i]);
-        if (!d[i]) return fail(w + ": unknown polynomial handle");
+        d[i] = poly_for_write(dst[i], who, (w + ": unknown polynomial handle").c_str());
+        if (!d[i]) return 1;
         if (d[i]->field != d[0]->field) return fail(w + ": the polynomials live in different fields");
         if (d[i]->len < ((size_t)1 << k)) return fail(w + ": a polynomial holds fewer than 2^k elements");
     }

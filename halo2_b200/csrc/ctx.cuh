@@ -68,7 +68,11 @@ struct BaseSet {
     uint32_t sessions = 0;                 // ... and open IPA sessions on any lane that refer to it; both under g_reg_mu
 };
 
-struct PolyBuf { int field; size_t len; DevBuf buf; PolyBuf() { buf.tracked = false; } };   // device-resident polynomial, Montgomery form, len + 1 slots
+struct PolyBuf {                           // device-resident polynomial, Montgomery form, len + 1 slots
+    int field; size_t len; DevBuf buf;
+    uint32_t users = 0;                    // shared polynomials (g_shared_polys): calls in flight on any context that read it (PolyReads); under g_reg_mu
+    PolyBuf() { buf.tracked = false; }
+};
 struct IpaSession {
     uint64_t bases; uint32_t k, round; int folded; DevBuf p, b, s, scal, out;
     IpaSession() { p.tracked = b.tracked = s.tracked = scal.tracked = out.tracked = false; }
@@ -193,11 +197,14 @@ struct Context {
 //   2. Context::mu    a call on that context, for the whole call.  A thread holds one at a time, except h2_shutdown, which
 //                     takes the primary's and then every live lane's in slot order (every other holder finishes its call
 //                     without waiting for a second context)
-//   3. g_reg_mu       the lane table and bindings, the shared base sets (g_bases) and their counts, g_multi, g_multi_bases;
-//                     held for map lookups only.  h2_bases_release waits on g_bases_cv under it for the set's users
+//   3. g_reg_mu       the lane table and bindings, the shared base sets (g_bases), the shared polynomials (g_shared_polys) and
+//                     their user counts, g_multi, g_multi_bases; held for map lookups only, never while taking a Context
+//                     mutex.  h2_bases_release and h2_poly_free of a shared polynomial hold no Context mutex: they wait on
+//                     g_users_cv under it for the object's users, which drop them without taking a second context
 // Handles of base sets, polynomials, IPA sessions, multi-GPU base sets and lanes come from one process-wide counter
 // (new_handle) that h2_shutdown does not reset: a handle names one object of one kind on one lane, and any other use of it
-// -- a foreign lane, a stale handle from before a shutdown -- finds nothing and is reported as unknown.
+// -- a foreign lane, a stale handle from before a shutdown -- finds nothing and is reported as unknown.  A shared
+// polynomial (h2_poly_share) keeps its handle and is then known, for reading only, on every lane.
 #define H2_MAX_LANES 16
 extern Context g_ctxs[H2_MAX_DEVICES];
 extern Context g_lanes[H2_MAX_LANES];
@@ -265,10 +272,24 @@ template <class P> static fe host_to_mont(const void *bytes, int repr) {
     memcpy(x.v, bytes, 32);
     return repr == H2_REPR_MONTGOMERY ? x : fe_to_mont<P>(x);
 }
-static inline PolyBuf *find_poly(uint64_t h) {
-    auto it = g_ctx.polys.find(h);
-    return it == g_ctx.polys.end() ? nullptr : it->second;
-}
+// Shared polynomials (h2_poly_share): read-only from then on, and readable from every context.  Sharing moves them out of
+// their owner's `polys` into this registry with unchanged handles; they never go into a poly_pool.
+extern std::map<uint64_t, PolyBuf *> g_shared_polys;
+// The write lookup: a polynomial of the calling context.  Any other handle fails -- a shared one with "<who>: the polynomial
+// is shared (read-only)", anything else with `unknown` -- and gives nullptr.
+PolyBuf *poly_for_write(uint64_t h, const char *who, const char *unknown);
+// The read lookup for one call: the calling context's polynomials first, then the shared ones.  A shared polynomial it finds
+// counts the call as a user until the PolyReads is dropped, so h2_poly_free cannot free it meanwhile.  Declared after the
+// call's CtxLock, so it is dropped before the context's mutex.
+struct PolyReads {
+    std::vector<PolyBuf *> held;             // the shared polynomials this call holds
+    PolyBuf *get(uint64_t h);                // nullptr: unknown handle
+    PolyReads() {}
+    ~PolyReads();
+    PolyReads(const PolyReads &) = delete;
+    PolyReads &operator=(const PolyReads &) = delete;
+};
+int shared_poly_free(uint64_t h);            // h2_poly_free of a handle that is not the calling context's
 // what a fixed-base MSM over `b` runs on: the digit-multiples table (mode 2) when there is one, else the window table (mode 1)
 #define H2_FB_BITS_CTX 8u
 static inline const affine *fixed_table(const BaseSet *b, uint32_t *c, uint32_t *mode) {

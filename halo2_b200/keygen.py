@@ -18,7 +18,7 @@ import numpy as np
 
 from . import lib as _l
 from .evaluator import AstLeaf, compile_ast
-from .poly import FIELDS, Blind, EvaluationDomain, Params, ResidentPoly, _handles, batch_invert_resident
+from .poly import FIELDS, Blind, EvaluationDomain, Params, ResidentPoly, _handles, batch_invert_resident, share_resident
 
 
 class Assembly:
@@ -243,7 +243,8 @@ class PermutationProvingKey:
 class ProvingKey:
     """plonk::ProvingKey (plonk.rs) without the verifying key: every polynomial resident.  `fixed_values` / `fixed_polys` /
     `fixed_cosets`, `permutation.{permutations, polys, cosets}`, and the extended cosets `l0`, `l_blind`, `l_last`.  The key
-    belongs to the lane (or the primary context) that built it; close() frees it."""
+    belongs to the lane (or the primary context) that built it until share() makes it readable from every lane; close()
+    frees it."""
 
     def __init__(self, fixed_values, fixed_polys, fixed_cosets, permutation: PermutationProvingKey, l0, l_blind, l_last):
         self.fixed_values, self.fixed_polys, self.fixed_cosets = fixed_values, fixed_polys, fixed_cosets
@@ -254,6 +255,12 @@ class ProvingKey:
         P = self.permutation
         return (list(self.fixed_values) + list(self.fixed_polys) + list(self.fixed_cosets) + list(P.permutations) + list(P.polys)
                 + list(P.cosets) + [p for p in (self.l0, self.l_blind, self.l_last) if p is not None])
+
+    def share(self) -> "ProvingKey":
+        """Shares every polynomial of the key in one h2_poly_share call: one resident copy that provers on every lane read.
+        Call it on the lane that built the key; the key is read-only afterwards.  Returns the key."""
+        share_resident(self._all())
+        return self
 
     def close(self) -> None:
         for p in self._all():

@@ -327,7 +327,12 @@ class Params:
 class ResidentPoly:
     """A polynomial kept in HBM (Montgomery form) between transforms and commits -- SURVEY.md section 8(f) row 3.
     The reference keeps every Polynomial<F, B> in host memory (poly.rs:56-71); this is the handle a patched prover
-    would hold instead while a column travels lagrange -> coeff -> extended."""
+    would hold instead while a column travels lagrange -> coeff -> extended.
+
+    It belongs to the lane (or the primary context) that allocated it until share() makes it read-only and readable from
+    every lane."""
+
+    _shared = False
 
     def __init__(self, field: str, length: int, values=None):
         self.field, self.len = field, int(length)
@@ -356,7 +361,17 @@ class ResidentPoly:
         """a[index] += delta in place (poly/commitment/prover.rs:51, :78: `poly[0] -= value`)."""
         _l.check(_l.init().h2_poly_add_at(self._h, ctypes.c_size_t(int(index)), _l.ptr(_l.fe_bytes(int(delta) % FIELDS[self.field])), _l.REPR_CANONICAL))
 
+    def share(self) -> "ResidentPoly":
+        """h2_poly_share: from now on every lane and the primary context can read the polynomial, and none can write it."""
+        share_resident([self])
+        return self
+
+    @property
+    def shared(self) -> bool:
+        return self._shared
+
     def close(self) -> None:
+        """Frees the polynomial.  A shared one may be closed from any thread: the call waits for reads in progress on every lane."""
         if self._h.value:
             _l.load().h2_poly_free(self._h)
             self._h.value = 0
@@ -370,6 +385,13 @@ class ResidentPoly:
 
 def _handles(polys: Sequence["ResidentPoly"]):
     return (ctypes.c_uint64 * len(polys))(*[p._h.value for p in polys])
+
+
+def share_resident(polys: Sequence["ResidentPoly"]) -> None:
+    """h2_poly_share of all `polys` in one call, all or none: each must belong to the calling thread's lane (or be shared)."""
+    _l.check(_l.init().h2_poly_share(_handles(polys), ctypes.c_size_t(len(polys))))
+    for p in polys:
+        p._shared = True
 
 
 def eval_polynomial_resident(polys: Sequence["ResidentPoly"], points: Sequence[int], n: Optional[int] = None) -> list:

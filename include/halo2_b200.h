@@ -60,8 +60,9 @@ uint32_t h2_abi_version(void);
  *     staging, copy-thread and chunk-cut ones, and h2_test_last_msm_plan act on the calling thread's lane.
  *   - h2_lane_bind(0) goes back to the primary context.  Binding an unknown lane fails.
  *   - Polynomial and IPA-session handles belong to the lane that created them; from any other lane (the primary
- *     included) they are unknown.  Base sets (h2_bases_register*) are shared by every lane.
- *   - h2_lane_destroy frees the lane's polynomials, IPA sessions and pools; it fails while another thread is bound to
+ *     included) they are unknown, until h2_poly_share makes polynomials read-only and readable from every lane and the
+ *     primary context (one proving key for all lanes).  Base sets (h2_bases_register*) are shared by every lane.
+ *   - h2_lane_destroy frees the lane's polynomials (not those it shared), IPA sessions and pools; it fails while another thread is bound to
  *     the lane.  h2_shutdown destroys every lane; lane handles from before it are unknown afterwards, and a thread that
  *     was bound must bind again.
  *   - The h2_multi_* entry points fail on a thread bound to a lane. */
@@ -150,7 +151,19 @@ int h2_set_window_bits(uint32_t c);
  *   h2_poly_download(e, evals, 4 n, repr);                                    // for the h(X) evaluation on the host
  */
 int h2_poly_alloc(int field, size_t len, uint64_t *poly);
+/* A polynomial of the calling context goes back to its pool.  A shared one (h2_poly_share) may be freed from any thread on
+ * any lane or the primary context: no new call finds it, the calls in progress that read it finish, the device is
+ * synchronised (asynchronous reads queued on any lane's stream) and the buffer is freed. */
 int h2_poly_free(uint64_t poly);
+/* Shares the calling context's polynomials polys[0 .. n) read-only with every lane and the primary context: a proving key
+ * built once and read by every prover lane.  Each handle must be the calling context's or already shared (a no-op); any
+ * other handle fails the call and then nothing is shared.  Synchronises the context's stream once, so every write to them
+ * has landed.  Handles do not change.  A shared handle is accepted wherever a polynomial is only read (downloads, the
+ * sources of copies, transforms, running products, Kate divisions and scale_add, the operands of eval_ast / eval /
+ * inner_product, the inputs of lookup_permute, h2_msm_registered_polys*, h2_ipa_begin_poly); every call that would write
+ * one fails with "<entry point>: the polynomial is shared (read-only)" and changes nothing.  h2_lane_destroy of the lane
+ * that shared it leaves it alive; h2_shutdown frees every shared polynomial.  n == 0 does nothing; fails before h2_init. */
+int h2_poly_share(const uint64_t *polys, size_t n);
 int h2_poly_upload(uint64_t poly, const void *src, size_t len, int repr);
 int h2_poly_download(uint64_t poly, void *dst, size_t len, int repr);
 /* a[index] += delta on a resident polynomial: the one-coefficient corrections of the opening argument

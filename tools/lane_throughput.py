@@ -1,14 +1,21 @@
 """Throughput of independent provers on one GPU, one prover lane each (halo2_b200.Lane; DESIGN.md section 9.1).
 
-  python tools/lane_throughput.py [--ks 14,16] [--lanes 1,2,4,8] [--rounds 3] [--out results/lane_throughput.json]
+  python tools/lane_throughput.py [commit] [replay] [real] [--ks 14,16] [--real-ks 16,18] [--lanes 1,2,4,8] [--rounds 3]
+                                  [--out results/lane_throughput.json]
 
-Two workloads, each from 1, 2, 4 and 8 host threads, every thread bound to a lane of its own:
+Three workloads (commit and replay when none is named), each from 1, 2, 4 and 8 host threads, every thread bound to a lane
+of its own:
   commit  a single commit of a 2^k host column against resident generators (h2_msm_registered_batch_affine, batch 1):
           a plain ctypes loop, so the GIL is released for the whole device call;
-  replay  the proof-shaped k-replay of tests/prover_replay.py (GpuArm), whose host glue holds the GIL between calls.
+  replay  the proof-shaped k-replay of tests/prover_replay.py (GpuArm), whose host glue holds the GIL between calls;
+  real    real proofs of the benchmark circuit through tests/plonk_prover.create_proof_engine, once with a private proving
+          key per lane (each lane runs keygen_pk) and once with one key built on the primary context and shared
+          (ProvingKey.share).  Besides the rate it reports the key's bytes, computed from its shapes, and the device's free
+          memory (cudaMemGetInfo) before the keys exist and while they all do; other tenants of the GPU can move the latter.
 Every result is checked: each commit against the same commit run serially on the primary context, each proof byte for byte
-against a serial replay with the same seed.  Runs are alternated -- 1 lane, then N lanes, for every N, `rounds` times -- and the
-medians are reported, with the GPU's name and power limit read in the same run."""
+against a serial run with the same seed (for real: with a private key).  commit and replay alternate their runs -- 1 lane,
+then N lanes, for every N, `rounds` times -- and report the medians; real runs every lane count once per key mode.  The
+GPU's name and power limit are read in the same run."""
 import argparse
 import ctypes
 import json
@@ -35,10 +42,11 @@ def gpu_info():
     return {"name": f[0], "power_limit": f[1], "sm_max_clock": f[2]} if len(f) == 3 else {"raw": q.stdout.strip()}
 
 
-def timed(nlanes, make, reps):
-    """Runs make(i) -> step on nlanes threads, each on its own lane; every thread warms up with 2 steps, then all run `reps`
-    steps at once.  Returns steps per second over the wall time of the timed window."""
-    start, done = threading.Barrier(nlanes + 1), threading.Barrier(nlanes + 1)
+def timed(nlanes, make, reps, warm=2, probe=None):
+    """Runs make(i) -> step on nlanes threads, each on its own lane; every thread warms up with `warm` steps, then all run
+    `reps` steps at once.  Returns steps per second over the wall time of the timed window.  probe(), when given, runs on
+    the calling thread after the window, while every lane still holds what make() built."""
+    start, done, held = threading.Barrier(nlanes + 1), threading.Barrier(nlanes + 1), threading.Barrier(nlanes + 1)
     t_end, errs = [0.0] * nlanes, []
 
     def run(i):
@@ -46,19 +54,21 @@ def timed(nlanes, make, reps):
             with h2.Lane():
                 step, close = make(i)
                 try:
-                    step()
-                    step()
+                    for _ in range(warm):
+                        step()
                     start.wait()
                     for _ in range(reps):
                         step()
                     t_end[i] = time.perf_counter()
                     done.wait()
+                    held.wait()
                 finally:
                     close()
         except BaseException as e:  # noqa: BLE001
             errs.append(e)
             start.abort()
             done.abort()
+            held.abort()
     th = [threading.Thread(target=run, args=(i,)) for i in range(nlanes)]
     for t in th:
         t.start()
@@ -69,6 +79,12 @@ def timed(nlanes, make, reps):
     t0 = time.perf_counter()
     try:
         done.wait()
+        if probe:
+            try:
+                probe()
+            except BaseException as e:  # noqa: BLE001
+                errs.append(e)          # raised below, once the lanes have closed and joined
+        held.wait()
     except threading.BrokenBarrierError:
         pass
     for t in th:
@@ -131,6 +147,70 @@ def replay_bench(k, lanes, rounds, reps):
     return sweep(lanes, rounds, lambda nl: timed(nl, make, reps))
 
 
+def real_bench(k, lanes, reps):
+    """Real proofs on N lanes, with a private key per lane and with one shared key.  Each lane proves with a seed of its
+    own; every proof must equal the serial proof with that seed under a private key on the primary context."""
+    import torch
+    from tests import bench_circuit as BC
+    from tests import multiopen_cases as MC
+    from tests import plonk_api_circuit as circ
+    from tests import plonk_prover as PP
+    from tests import plonk_verifier as PV
+    from tests.test_keygen_oracle import ZETA, bench_copies, delta_of, prover_pk_dict
+    n, m = 1 << k, pasta.P_MOD
+    delta = delta_of(m)
+    dev = L._inited_device or 0
+    free = lambda: int(torch.cuda.mem_get_info(dev)[0])
+    pts = cref.gen_points("vesta", 99, n + 2)
+    prm = h2.Params("vesta", k, pts[:n], h2.lagrange_generators("vesta", k, pts[:n]), pts[n:n + 1], u=pts[n + 1:])
+    D = h2.EvaluationDomain("fp", BC.DEGREE, k, ZETA)
+    fixed, _, adv = BC.columns(k, m, D.omega, delta, circ.A_SMALL * ZETA % m)
+    ab = [cref.ints_to_bytes(c) for c in adv]
+    cc = h2.CopyConstraints(n, 3)
+    cc.extend(np.array(list(bench_copies(k)), dtype=np.uint32))
+    fc, pc = h2.keygen_vk(prm, D, fixed, cc, delta)
+    A = cref.bytes_to_affine
+    vk = PV.PinnedKey(BC.pinned_key_text(k, D.extended_k, pasta.Q_MOD, m, D.omega, [A(x) for x in fc], [A(x) for x in pc]))
+    keygen = lambda: h2.keygen_pk(prm, D, fixed, cc, delta, BC.BLINDING_FACTORS)
+
+    def prove(pk, seed):
+        T = R.Blake2bTranscript(m)
+        PP.create_proof_engine(h2, prm, vk, None, None, [ab], [[]], MC.SeededRng("fp", seed, True), T, ZETA, delta, pk=prover_pk_dict(pk))
+        return bytes(T.proof)
+    seeds = [3000 * k + i for i in range(max(lanes))]
+    pk = keygen()
+    want = [prove(pk, s) for s in seeds]                         # serially, private key, primary context
+    key_bytes = 32 * sum(p.len + 1 for p in pk._all())           # len + 1 slots per resident polynomial
+    arm = PV.EngineArm(h2, "vesta", k, params=prm)
+    if not all(PV.verify_proof(arm, vk, p, [[]], delta) for p in want[:2]):
+        raise AssertionError("the serial proofs do not verify")
+    arm.close()
+    pk.close()
+    free()                                                        # torch's own context exists before the first reading
+    res = {"key_bytes": key_bytes, "key_field_elements_per_n": round(key_bytes / 32 / n, 3)}
+    for mode in ("private", "shared"):
+        res[mode] = {}
+        for nl in lanes:
+            mem = {"free_before_keys": free()}
+            shared = keygen().share() if mode == "shared" else None
+
+            def make(i):
+                key = shared or keygen()
+
+                def step():
+                    if prove(key, seeds[i]) != want[i]:
+                        raise AssertionError(f"real k={k} {mode} lane {i}: proof differs from the serial proof")
+                return step, (lambda: None) if shared else key.close
+            rate = timed(nl, make, reps, warm=1, probe=lambda: mem.update(free_with_keys=free()))
+            if shared:
+                shared.close()
+            mem["keys_and_lanes_bytes"] = mem["free_before_keys"] - mem["free_with_keys"]
+            res[mode][str(nl)] = {"per_s": round(rate, 3), **mem}
+            print(f"real k={k} {mode} {nl} lanes: " + json.dumps(res[mode][str(nl)]), flush=True)
+    prm.close()
+    return res
+
+
 def sweep(lanes, rounds, run):
     """1 lane and N lanes alternated, `rounds` times; medians of the rates."""
     rates = {nl: [] for nl in lanes}
@@ -149,23 +229,36 @@ def sweep(lanes, rounds, run):
 
 def main():
     ap = argparse.ArgumentParser()
+    ap.add_argument("workloads", nargs="*", help="commit, replay and / or real (default: commit replay)")
     ap.add_argument("--ks", default="14,16")
+    ap.add_argument("--real-ks", default="16,18")
     ap.add_argument("--lanes", default="1,2,4,8")
     ap.add_argument("--rounds", type=int, default=3)
     ap.add_argument("--commit-reps", type=int, default=200)
     ap.add_argument("--replay-reps", type=int, default=6)
+    ap.add_argument("--real-reps", type=int, default=2)
     ap.add_argument("--out", default=None)
     a = ap.parse_args()
+    a.workloads = a.workloads or ["commit", "replay"]
+    if set(a.workloads) - {"commit", "replay", "real"}:
+        ap.error("workloads are commit, replay and real")
     L.init()
     ks = [int(x) for x in a.ks.split(",")]
     lanes = sorted({1} | {int(x) for x in a.lanes.split(",")})
-    res = {"gpu": gpu_info(), "lanes": lanes, "rounds": a.rounds, "commit": {}, "replay": {}}
-    for k in ks:
-        res["commit"][str(k)] = commit_bench(k, lanes, a.rounds, a.commit_reps)
-        print(f"commit k={k}: " + json.dumps(res["commit"][str(k)]), flush=True)
-    for k in ks:
-        res["replay"][str(k)] = replay_bench(k, lanes, a.rounds, a.replay_reps)
-        print(f"replay k={k}: " + json.dumps(res["replay"][str(k)]), flush=True)
+    res = {"gpu": gpu_info(), "lanes": lanes, "rounds": a.rounds}
+    for w in a.workloads:
+        res[w] = {}
+    if "commit" in a.workloads:
+        for k in ks:
+            res["commit"][str(k)] = commit_bench(k, lanes, a.rounds, a.commit_reps)
+            print(f"commit k={k}: " + json.dumps(res["commit"][str(k)]), flush=True)
+    if "replay" in a.workloads:
+        for k in ks:
+            res["replay"][str(k)] = replay_bench(k, lanes, a.rounds, a.replay_reps)
+            print(f"replay k={k}: " + json.dumps(res["replay"][str(k)]), flush=True)
+    if "real" in a.workloads:
+        for k in (int(x) for x in a.real_ks.split(",")):
+            res["real"][str(k)] = real_bench(k, lanes, a.real_reps)
     res["gpu_after"] = gpu_info()
     print(json.dumps(res))
     if a.out:
