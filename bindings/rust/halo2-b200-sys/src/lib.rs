@@ -108,6 +108,12 @@ extern "C" {
     pub fn h2_lane_destroy(lane: u64) -> c_int;
     // shared polynomials: one read-only proving key for every lane
     pub fn h2_poly_share(polys: *const u64, n: usize) -> c_int;
+    pub fn h2_poly_permutation_product(z_out: *const u64, proofs: usize, columns: *const u64, sigmas: *const u64, cols: usize, chunk_len: u32,
+                                       k: u32, beta: *const c_void, gamma: *const c_void, omega: *const c_void, delta: *const c_void,
+                                       blinding: *const c_void, blinding_factors: u32, repr: c_int) -> c_int;
+    pub fn h2_poly_lookup_product(z_out: *const u64, count: usize, inputs: *const u64, tables: *const u64, permuted_inputs: *const u64,
+                                  permuted_tables: *const u64, k: u32, beta: *const c_void, gamma: *const c_void, blinding: *const c_void,
+                                  blinding_factors: u32, repr: c_int) -> c_int;
 }
 
 fn check(rc: c_int) {
@@ -547,6 +553,69 @@ pub fn permutation_polys_from_copies<F: PrimeField>(field_id: c_int, k: u32, col
     let rc = unsafe {
         h2_poly_permutation_sigma_copies(handles.as_ptr(), handles.len(), k, copies.as_ptr() as *const u32, copies.len(),
                                          w.as_ref().as_ptr() as *const c_void, d.as_ref().as_ptr() as *const c_void, REPR_CANONICAL)
+    };
+    if rc != 0 {
+        for &h in &handles { unsafe { h2_poly_free(h) }; }
+        check(rc);
+    }
+    handles
+}
+
+/// `count` zero-filled polynomials of n elements on the caller's lane; on a failure the ones already made are freed.
+fn alloc_polys(field_id: c_int, n: usize, count: usize) -> Vec<u64> {
+    let mut handles = Vec::with_capacity(count);
+    for _ in 0..count {
+        let mut h = 0u64;
+        let rc = unsafe { h2_poly_alloc(field_id, n, &mut h) };
+        if rc != 0 {
+            for h in handles { unsafe { h2_poly_free(h) }; }
+            check(rc);
+        }
+        handles.push(h);
+    }
+    handles
+}
+
+/// The permutation argument's product columns, `permutation::Argument::commit` (plonk/permutation/prover.rs:98-168) for every
+/// proof at once: `columns` holds proof p's Lagrange columns at `[p * cols, (p + 1) * cols)` (advice, fixed or instance handles,
+/// in the argument's column order), `sigmas` the key's `cols` permutation polynomials (a shared key works on every lane).
+/// `blinding` holds `blinding_factors` values per (proof, set), in the rng's order.  Returns the z handles (Lagrange basis), set
+/// after set and proof after proof, owned by the caller's lane; the call is asynchronous.  Commit them, then transform them.
+pub fn permutation_products<F: PrimeField>(field_id: c_int, k: u32, columns: &[u64], sigmas: &[u64], chunk_len: u32, beta: F, gamma: F,
+                                           omega: F, delta: F, blinding: &[F], blinding_factors: u32) -> Vec<u64> {
+    assert!(!sigmas.is_empty() && chunk_len > 0 && columns.len() % sigmas.len() == 0, "one column per permutation polynomial and proof");
+    let proofs = columns.len() / sigmas.len();
+    let sets = (sigmas.len() + chunk_len as usize - 1) / chunk_len as usize;
+    assert_eq!(blinding.len(), proofs * sets * blinding_factors as usize, "blinding_factors values per (proof, set)");
+    let handles = alloc_polys(field_id, 1usize << k, proofs * sets);
+    let (b, g, w, d, bl) = (beta.to_repr(), gamma.to_repr(), omega.to_repr(), delta.to_repr(), scalars_to_bytes(blinding));
+    let rc = unsafe {
+        h2_poly_permutation_product(handles.as_ptr(), proofs, columns.as_ptr(), sigmas.as_ptr(), sigmas.len(), chunk_len, k,
+                                    b.as_ref().as_ptr() as *const c_void, g.as_ref().as_ptr() as *const c_void, w.as_ref().as_ptr() as *const c_void,
+                                    d.as_ref().as_ptr() as *const c_void, bl.as_ptr() as *const c_void, blinding_factors, REPR_CANONICAL)
+    };
+    if rc != 0 {
+        for &h in &handles { unsafe { h2_poly_free(h) }; }
+        check(rc);
+    }
+    handles
+}
+
+/// The lookup argument's product columns, `lookup::Permuted::commit_product` (plonk/lookup/prover.rs:279-337), for every lookup
+/// of every proof at once: entry b of the four slices is lookup b's compressed input, compressed table, permuted input and
+/// permuted table (Lagrange handles).  `blinding` holds `blinding_factors` values per lookup.  Returns the z handles
+/// (Lagrange basis), owned by the caller's lane; the call is asynchronous.
+pub fn lookup_products<F: PrimeField>(field_id: c_int, k: u32, inputs: &[u64], tables: &[u64], permuted_inputs: &[u64], permuted_tables: &[u64],
+                                      beta: F, gamma: F, blinding: &[F], blinding_factors: u32) -> Vec<u64> {
+    let count = inputs.len();
+    assert!(tables.len() == count && permuted_inputs.len() == count && permuted_tables.len() == count, "four columns per lookup");
+    assert_eq!(blinding.len(), count * blinding_factors as usize, "blinding_factors values per lookup");
+    let handles = alloc_polys(field_id, 1usize << k, count);
+    let (b, g, bl) = (beta.to_repr(), gamma.to_repr(), scalars_to_bytes(blinding));
+    let rc = unsafe {
+        h2_poly_lookup_product(handles.as_ptr(), count, inputs.as_ptr(), tables.as_ptr(), permuted_inputs.as_ptr(), permuted_tables.as_ptr(), k,
+                               b.as_ref().as_ptr() as *const c_void, g.as_ref().as_ptr() as *const c_void, bl.as_ptr() as *const c_void,
+                               blinding_factors, REPR_CANONICAL)
     };
     if rc != 0 {
         for &h in &handles { unsafe { h2_poly_free(h) }; }

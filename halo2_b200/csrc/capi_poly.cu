@@ -1,6 +1,6 @@
 // C ABI of the engine, part 5 of 5: reductions and elementwise programs on resident polynomials (polyops.cuh, asteval.cuh),
-// the lookup permutation (lookup.cuh), the verifier's MSM scalars (verifier.cuh), the permutation polynomials (keygen.cuh)
-// and their copy cycles (assembly.cuh).
+// the lookup permutation (lookup.cuh), the verifier's MSM scalars (verifier.cuh), the permutation polynomials (keygen.cuh),
+// their copy cycles (assembly.cuh) and the permutation / lookup product columns (grandproduct.cuh).
 #include "util_kernels.cuh"
 #include "polyops.cuh"
 #include "asteval.cuh"
@@ -8,6 +8,7 @@
 #include "verifier.cuh"
 #include "keygen.cuh"
 #include "assembly.cuh"
+#include "grandproduct.cuh"
 
 #include <algorithm>
 
@@ -620,4 +621,134 @@ extern "C" int h2_poly_permutation_sigma_copies(const uint64_t *dst, size_t cols
     if (sigma_dst("h2_poly_permutation_sigma_copies", dst, cols, k, d)) return 1;
     if (d[0]->field == H2_FIELD_FP) return permutation_sigma_copies_run<FpParams>(d, k, copies, m, omega, delta, repr);
     return permutation_sigma_copies_run<FqParams>(d, k, copies, m, omega, delta, repr);
+}
+
+
+// ------------------------------------------------------------------------------------------------
+// the permutation and lookup arguments' product columns, every column of every proof in one call (grandproduct.cuh)
+// ------------------------------------------------------------------------------------------------
+// `ins`: the permutation's proofs x cols column pointers then its cols sigma pointers, or 4 pointers per lookup column.
+// Scratch: gp_val [count][n] (den, den^-1, mv), po_lvl / po_q the tree's levels and exclusive products, gp_aux one upload of
+// the pointer arrays and the blinding values, then the power tables and the carries.
+template <class P>
+static int product_run(bool perm, const std::vector<PolyBuf *> &z, const std::vector<PolyBuf *> &ins, uint32_t ncols, uint32_t chunk_len,
+                       uint32_t sets, uint32_t k, const void *beta, const void *gamma, const void *omega, const void *delta, const void *blinding,
+                       uint32_t bf, int repr) {
+    Context &X = g_ctx;
+    cudaStream_t s = X.stream;
+    const uint64_t n = 1ull << k, count = z.size();
+    GpLevels G{};
+    G.m[0] = n; G.m[1] = (n + H2_POLY_CHUNK - 1) / H2_POLY_CHUNK; G.L = 1;
+    while (G.m[G.L] > H2_POLY_CHUNK) { G.off[G.L + 1] = G.off[G.L] + G.m[G.L] * count; G.m[G.L + 1] = (G.m[G.L] + H2_POLY_CHUNK - 1) / H2_POLY_CHUNK; G.L++; }
+    const uint64_t total = G.off[G.L] + G.m[G.L] * count;
+    const uint64_t nptr = count + ins.size(), ptr_fe = (nptr * sizeof(void *) + sizeof(fe) - 1) / sizeof(fe);
+    const uint64_t tlen = perm ? KeygenOps<P>::table_len(k, ncols) : 0, nblind = count * bf;
+    std::vector<uint8_t> up((ptr_fe + nblind) * sizeof(fe));
+    const fe **hp = reinterpret_cast<const fe **>(up.data());
+    for (uint64_t b = 0; b < count; b++) hp[b] = z[b]->buf.as<fe>();
+    for (size_t i = 0; i < ins.size(); i++) hp[count + i] = ins[i]->buf.as<fe>();
+    if (nblind) memcpy(up.data() + ptr_fe * sizeof(fe), blinding, nblind * sizeof(fe));
+    if (scratch_acquire(s)) return 1;
+    if (X.gp_val.ensure(count * n * sizeof(fe)) || X.po_lvl.ensure(total * sizeof(fe)) || X.po_q.ensure(total * sizeof(fe)) ||
+        X.gp_aux.ensure((ptr_fe + nblind + tlen + count) * sizeof(fe)))
+        return 1;
+    fe *val = X.gp_val.as<fe>(), *lvl = X.po_lvl.as<fe>(), *ex = X.po_q.as<fe>();
+    fe *aux = X.gp_aux.as<fe>(), *blind = aux + ptr_fe, *tab = blind + nblind, *init = tab + tlen;
+    fe *const *zp = reinterpret_cast<fe *const *>(aux);
+    const fe *const *ip = reinterpret_cast<const fe *const *>(aux) + count;
+    CU(cudaMemcpyAsync(aux, up.data(), up.size(), cudaMemcpyHostToDevice, s));
+    if (nblind && repr == H2_REPR_CANONICAL) LAUNCH(convert_kernel<P>, blocks_for(nblind, 64), 64, 0, s, blind, nblind, 1);
+    const fe b_m = host_to_mont<P>(beta, repr), g_m = host_to_mont<P>(gamma, repr);
+    if (perm) {
+        LAUNCH(keygen_tables_kernel<P>, blocks_for(tlen, 128), 128, 0, s, tab, host_to_mont<P>(omega, repr), host_to_mont<P>(delta, repr), k, ncols);
+        LAUNCH(gp_perm_factors_kernel<P>, dim3(blocks_for(n, 128), (uint32_t)count), 128, 0, s, ip, ip + (count / sets) * ncols, ncols, chunk_len, sets,
+               (const fe *)tab, k, b_m, g_m, val, zp);
+    } else {
+        LAUNCH(gp_lookup_factors_kernel<P>, dim3(blocks_for(n, 256), (uint32_t)count), 256, 0, s, ip, n, b_m, g_m, val, zp);
+    }
+    LAUNCH(poly_batch_invert_kernel<P>, blocks_for((count * n + 15) / 16, 64), 64, 0, s, val, count * n);
+    LAUNCH(gp_mv_up_kernel<P>, dim3(blocks_for(G.m[1], 128), (uint32_t)count), 128, 0, s, (const fe *const *)zp, val, n, lvl, G.m[1]);
+    for (uint32_t l = 1; l < G.L; l++)
+        LAUNCH(gp_up_kernel<P>, dim3(blocks_for(G.m[l + 1], 128), (uint32_t)count), 128, 0, s, (const fe *)(lvl + G.off[l]), G.m[l], lvl + G.off[l + 1], G.m[l + 1]);
+    LAUNCH(gp_carry_kernel<P>, blocks_for(count / sets, 64), 64, 0, s, (const fe *)val, (const fe *)lvl, G, n - bf - 1, sets, init, (uint32_t)(count / sets));
+    for (uint32_t l = G.L + 1; l-- > 0;) {
+        const uint64_t chunks = (G.m[l] + H2_POLY_CHUNK - 1) / H2_POLY_CHUNK;
+        LAUNCH(gp_down_kernel<P>, dim3(blocks_for(chunks, 128), (uint32_t)count), 128, 0, s, l == 0 ? (const fe *)val : (const fe *)(lvl + G.off[l]), G.m[l],
+               l == G.L ? (const fe *)nullptr : (const fe *)(ex + G.off[l + 1]), (const fe *)init, l == 0 ? (fe *)nullptr : ex + G.off[l],
+               l == 0 ? zp : (fe *const *)nullptr, chunks);
+    }
+    if (bf) LAUNCH(gp_blind_kernel<P>, blocks_for(nblind, 256), 256, 0, s, zp, n, bf, (const fe *)blind, count);
+    return scratch_release(s);
+}
+// The checks both entry points share, all before any launch: the z_out handles are the calling context's, writable, of one
+// field, hold n elements and are pairwise distinct and none of the inputs; the inputs are readable, of that field, hold n.
+static int product_handles(const char *who, const uint64_t *zh, size_t count, const std::vector<uint64_t> &ih, uint64_t n, PolyReads &rd,
+                           std::vector<PolyBuf *> &z, std::vector<PolyBuf *> &ins) {
+    const std::string w(who), unknown = w + ": unknown polynomial handle";
+    z.resize(count);
+    ins.resize(ih.size());
+    for (size_t b = 0; b < count; b++) {
+        z[b] = poly_for_write(zh[b], who, unknown.c_str());
+        if (!z[b]) return 1;
+        if (z[b]->field != z[0]->field) return fail(w + ": the polynomials live in different fields");
+        if (z[b]->len < n) return fail(w + ": a polynomial holds fewer than 2^k elements");
+    }
+    for (size_t i = 0; i < ih.size(); i++) {
+        ins[i] = rd.get(ih[i]);
+        if (!ins[i]) return fail(unknown);
+        if (ins[i]->field != z[0]->field) return fail(w + ": the polynomials live in different fields");
+        if (ins[i]->len < n) return fail(w + ": a polynomial holds fewer than 2^k elements");
+    }
+    std::vector<PolyBuf *> sz(z), si(ins);
+    std::sort(sz.begin(), sz.end());
+    std::sort(si.begin(), si.end());
+    if (std::adjacent_find(sz.begin(), sz.end()) != sz.end()) return fail(w + ": a z_out handle appears twice");
+    for (PolyBuf *p : sz)
+        if (std::binary_search(si.begin(), si.end(), p)) return fail(w + ": a z_out handle is also an input");
+    return 0;
+}
+static int product_scalars(const char *who, uint32_t k, uint32_t bf) {
+    if (k > 30) return fail(std::string(who) + ": k > 30");
+    if ((uint64_t)bf + 1 >= (1ull << k)) return fail(std::string(who) + ": blinding_factors + 1 >= n");
+    return 0;
+}
+extern "C" int h2_poly_permutation_product(const uint64_t *z_out, size_t proofs, const uint64_t *columns, const uint64_t *sigmas, size_t cols,
+                                           uint32_t chunk_len, uint32_t k, const void *beta, const void *gamma, const void *omega, const void *delta,
+                                           const void *blinding, uint32_t blinding_factors, int repr) {
+    static const char *who = "h2_poly_permutation_product";
+    CtxLock lk;
+    if (require_ready()) return 1;
+    if (product_scalars(who, k, blinding_factors)) return 1;
+    if (chunk_len == 0) return fail(std::string(who) + ": chunk_len == 0");
+    if (proofs == 0 || cols == 0) return 0;
+    if (!z_out || !columns || !sigmas || !beta || !gamma || !omega || !delta || (blinding_factors && !blinding)) return fail(std::string(who) + ": null argument");
+    const uint64_t sets = (cols + chunk_len - 1) / chunk_len;
+    if (cols >= (1ull << 20) || proofs >= (1ull << 16) || proofs * sets > 65535) return fail(std::string(who) + ": more than 65535 product columns");
+    std::vector<uint64_t> ih(columns, columns + proofs * cols);
+    ih.insert(ih.end(), sigmas, sigmas + cols);
+    PolyReads rd;
+    std::vector<PolyBuf *> z, ins;
+    if (product_handles(who, z_out, proofs * sets, ih, 1ull << k, rd, z, ins)) return 1;
+    if (z[0]->field == H2_FIELD_FP)
+        return product_run<FpParams>(true, z, ins, (uint32_t)cols, chunk_len, (uint32_t)sets, k, beta, gamma, omega, delta, blinding, blinding_factors, repr);
+    return product_run<FqParams>(true, z, ins, (uint32_t)cols, chunk_len, (uint32_t)sets, k, beta, gamma, omega, delta, blinding, blinding_factors, repr);
+}
+extern "C" int h2_poly_lookup_product(const uint64_t *z_out, size_t count, const uint64_t *inputs, const uint64_t *tables, const uint64_t *permuted_inputs,
+                                      const uint64_t *permuted_tables, uint32_t k, const void *beta, const void *gamma, const void *blinding,
+                                      uint32_t blinding_factors, int repr) {
+    static const char *who = "h2_poly_lookup_product";
+    CtxLock lk;
+    if (require_ready()) return 1;
+    if (product_scalars(who, k, blinding_factors)) return 1;
+    if (count == 0) return 0;
+    if (!z_out || !inputs || !tables || !permuted_inputs || !permuted_tables || !beta || !gamma || (blinding_factors && !blinding))
+        return fail(std::string(who) + ": null argument");
+    if (count > 65535) return fail(std::string(who) + ": more than 65535 product columns");
+    std::vector<uint64_t> ih;
+    for (size_t b = 0; b < count; b++) ih.insert(ih.end(), {inputs[b], tables[b], permuted_inputs[b], permuted_tables[b]});
+    PolyReads rd;
+    std::vector<PolyBuf *> z, ins;
+    if (product_handles(who, z_out, count, ih, 1ull << k, rd, z, ins)) return 1;
+    if (z[0]->field == H2_FIELD_FP) return product_run<FpParams>(false, z, ins, 0, 1, 1, k, beta, gamma, nullptr, nullptr, blinding, blinding_factors, repr);
+    return product_run<FqParams>(false, z, ins, 0, 1, 1, k, beta, gamma, nullptr, nullptr, blinding, blinding_factors, repr);
 }

@@ -172,6 +172,7 @@ struct Context {
     DevBuf lk_keys, lk_left, lk_u32;         // lookup.cuh: sorted canonical keys (input | table), leftover table values, flag / scan arrays
     DevBuf kg_tab, kg_map;                   // keygen.cuh: power tables + error word, one piece of the copy-constraint mapping (all of it for assembly.cuh)
     DevBuf as_edge, as_cell, as_slot;        // assembly.cuh: per-copy, per-cell and per-slot u32 arrays
+    DevBuf gp_val, gp_aux;                   // grandproduct.cuh: denominators / mv of every column, pointers + tables + carries + blinding values
     std::vector<TwiddleEntry *> twiddles;
     uint64_t tw_stamp = 0;
     std::map<uint64_t, BaseSet *> shards;    // this device's shards of multi-GPU base sets (h2_multi_bases_register)

@@ -1,0 +1,145 @@
+"""The prover's product columns over the C ABI: permutation::Argument::commit
+(/root/reference/halo2_proofs/src/plonk/permutation/prover.rs:47-195) and lookup::Permuted::commit_product
+(plonk/lookup/prover.rs:253-390), every column of every proof in one device call (csrc/grandproduct.cuh).
+
+The library has no transcript: the commit functions return the commitments in the order the reference writes them, and the
+caller writes them to its own transcript.
+"""
+from __future__ import annotations
+
+import ctypes
+from typing import List, Sequence, Tuple
+
+import numpy as np
+
+from . import lib as _l
+from .poly import Blind, EvaluationDomain, Params, ResidentPoly, _handles
+
+_MAX_COMMIT_BATCH = 64   # h2_msm_registered_polys_affine takes at most this many polynomials per pass
+
+
+def _scalars(values, m: int) -> np.ndarray:
+    if not values:
+        return None
+    return np.frombuffer(b"".join((int(v) % m).to_bytes(32, "little") for v in values), dtype=np.uint8).reshape(-1, 32)
+
+
+def _alloc(field: str, n: int, count: int) -> List[ResidentPoly]:
+    return [ResidentPoly(field, n) for _ in range(count)]
+
+
+def _close(polys) -> None:
+    for p in polys:
+        p.close()
+
+
+def permutation_product_resident(domain: EvaluationDomain, columns: Sequence[Sequence[ResidentPoly]], sigmas: Sequence[ResidentPoly], beta: int,
+                                 gamma: int, delta: int, chunk_len: int, blinding_factors: int, blinding: Sequence[int]) -> List[List[ResidentPoly]]:
+    """The permutation argument's product columns z (Lagrange basis, resident) of every proof: `columns[p]` are proof p's
+    resident Lagrange columns in the argument's column order, `sigmas` the key's permutation polynomials, `delta` = F::DELTA.
+    `blinding` holds the blinding rows, proofs x sets x blinding_factors values in the rng's order.  Returns, per proof, its
+    sets' z columns (h2_poly_permutation_product)."""
+    m, n, proofs, cols = domain.m, domain.n, len(columns), len(sigmas)
+    if any(len(c) != cols for c in columns):
+        raise _l.H2Error("every proof needs one column per permutation polynomial")
+    if chunk_len < 1:
+        raise _l.H2Error("chunk_len must be at least 1")
+    sets = -(-cols // chunk_len)
+    if len(blinding) != proofs * sets * blinding_factors:
+        raise _l.H2Error(f"expected {proofs * sets * blinding_factors} blinding values, got {len(blinding)}")
+    z = _alloc(domain.field, n, proofs * sets)
+    try:
+        _l.check(_l.init().h2_poly_permutation_product(
+            _handles(z), ctypes.c_size_t(proofs), _handles([c for per in columns for c in per]), _handles(sigmas), ctypes.c_size_t(cols),
+            ctypes.c_uint32(chunk_len), ctypes.c_uint32(domain.k), _l.ptr(_l.fe_bytes(beta % m)), _l.ptr(_l.fe_bytes(gamma % m)),
+            _l.ptr(_l.fe_bytes(domain.omega)), _l.ptr(_l.fe_bytes(delta % m)), _l.ptr(_scalars(blinding, m)), ctypes.c_uint32(blinding_factors),
+            _l.REPR_CANONICAL))
+    except BaseException:
+        _close(z)
+        raise
+    return [z[p * sets:(p + 1) * sets] for p in range(proofs)]
+
+
+def lookup_product_resident(domain: EvaluationDomain, lookups: Sequence[Sequence[Tuple[ResidentPoly, ResidentPoly, ResidentPoly, ResidentPoly]]],
+                            beta: int, gamma: int, blinding_factors: int, blinding: Sequence[int]) -> List[List[ResidentPoly]]:
+    """The lookup argument's product columns z (Lagrange basis, resident): `lookups[p]` is proof p's list of (compressed input,
+    compressed table, permuted input, permuted table) columns; `blinding` holds blinding_factors values per lookup, in order.
+    Returns, per proof, its lookups' z columns (h2_poly_lookup_product)."""
+    m, n = domain.m, domain.n
+    flat = [lk for per in lookups for lk in per]
+    if len(blinding) != len(flat) * blinding_factors:
+        raise _l.H2Error(f"expected {len(flat) * blinding_factors} blinding values, got {len(blinding)}")
+    z = _alloc(domain.field, n, len(flat))
+    try:
+        parts = [_handles([lk[j] for lk in flat]) for j in range(4)]
+        _l.check(_l.init().h2_poly_lookup_product(_handles(z), ctypes.c_size_t(len(flat)), *parts, ctypes.c_uint32(domain.k),
+                                                   _l.ptr(_l.fe_bytes(beta % m)), _l.ptr(_l.fe_bytes(gamma % m)), _l.ptr(_scalars(blinding, m)),
+                                                   ctypes.c_uint32(blinding_factors), _l.REPR_CANONICAL))
+    except BaseException:
+        _close(z)
+        raise
+    out, at = [], 0
+    for per in lookups:
+        out.append(z[at:at + len(per)])
+        at += len(per)
+    return out
+
+
+def _commit(params: Params, polys: List[ResidentPoly], blinds: List[int]) -> np.ndarray:
+    if not polys:
+        return np.zeros((0, 64), dtype=np.uint8)
+    return np.concatenate([params.commit_resident_affine(polys[i:i + _MAX_COMMIT_BATCH], [Blind(b) for b in blinds[i:i + _MAX_COMMIT_BATCH]],
+                                                         lagrange=True) for i in range(0, len(polys), _MAX_COMMIT_BATCH)])
+
+
+def permutation_commit(params: Params, domain: EvaluationDomain, pk, columns: Sequence[Sequence[ResidentPoly]], beta: int, gamma: int, delta: int,
+                       chunk_len: int, blinding_factors: int, rng):
+    """permutation::Argument::commit (permutation/prover.rs:47-195) for every proof at once.  `pk` is a ProvingKey (its
+    permutation.permutations are the sigma columns), `columns[p]` proof p's columns in the argument's column order, `rng`
+    an object with scalar() -> int, drawn in the reference's order: per proof, per set, blinding_factors values, then the
+    set's blind (:155-171).  One product call, one commitment pass (commit_lagrange), then lagrange_to_coeff and
+    coeff_to_extended per set.  Returns (sets, commitments): sets[p] = [(poly, coset, blind) per set], and the (proofs x sets,
+    64) affine commitments in the order the reference writes them to the transcript."""
+    sigmas = pk.permutation.permutations
+    proofs, sets = len(columns), -(-len(sigmas) // max(int(chunk_len), 1))
+    blinding, blinds = [], []
+    for _ in range(proofs * sets):
+        blinding += [rng.scalar() for _ in range(blinding_factors)]
+        blinds.append(rng.scalar())
+    z = [p for per in permutation_product_resident(domain, columns, sigmas, beta, gamma, delta, chunk_len, blinding_factors, blinding) for p in per]
+    cosets: List[ResidentPoly] = []
+    try:
+        cm = _commit(params, z, blinds)
+        for p in z:
+            domain.lagrange_to_coeff_resident(p)                                  # in place: z becomes permutation_product_poly
+            cosets.append(domain.coeff_to_extended_resident(p))
+    except BaseException:
+        _close(z + cosets)
+        raise
+    return [list(zip(z, cosets, blinds))[p * sets:(p + 1) * sets] for p in range(proofs)], cm
+
+
+def lookup_commit_product(params: Params, domain: EvaluationDomain, lookups, beta: int, gamma: int, blinding_factors: int, rng):
+    """lookup::Permuted::commit_product (lookup/prover.rs:253-390) for every lookup of every proof at once.  `lookups[p]` is
+    proof p's list of (compressed input, compressed table, permuted input, permuted table) Lagrange columns; `rng` is drawn
+    per lookup: blinding_factors values, then product_blind (:317-321, :334).  Returns (products, commitments):
+    products[p] = [(z poly in coefficient form, blind) per lookup], and the affine commitments in write order."""
+    count = sum(len(per) for per in lookups)
+    blinding, blinds = [], []
+    for _ in range(count):
+        blinding += [rng.scalar() for _ in range(blinding_factors)]
+        blinds.append(rng.scalar())
+    z = lookup_product_resident(domain, lookups, beta, gamma, blinding_factors, blinding)
+    flat = [p for per in z for p in per]
+    try:
+        cm = _commit(params, flat, blinds)
+        for p in flat:
+            domain.lagrange_to_coeff_resident(p)
+    except BaseException:
+        _close(flat)
+        raise
+    out, at = [], 0
+    for per in z:
+        out.append(list(zip(per, blinds[at:at + len(per)])))
+        at += len(per)
+    return out, cm

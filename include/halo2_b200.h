@@ -160,7 +160,7 @@ int h2_poly_free(uint64_t poly);
  * other handle fails the call and then nothing is shared.  Synchronises the context's stream once, so every write to them
  * has landed.  Handles do not change.  A shared handle is accepted wherever a polynomial is only read (downloads, the
  * sources of copies, transforms, running products, Kate divisions and scale_add, the operands of eval_ast / eval /
- * inner_product, the inputs of lookup_permute, h2_msm_registered_polys*, h2_ipa_begin_poly); every call that would write
+ * inner_product, the inputs of lookup_permute and of the product columns, h2_msm_registered_polys*, h2_ipa_begin_poly); every call that would write
  * one fails with "<entry point>: the polynomial is shared (read-only)" and changes nothing.  h2_lane_destroy of the lane
  * that shared it leaves it alive; h2_shutdown frees every shared polynomial.  n == 0 does nothing; fails before h2_init. */
 int h2_poly_share(const uint64_t *polys, size_t n);
@@ -252,6 +252,33 @@ int h2_poly_permutation_sigma(const uint64_t *dst, size_t cols, uint32_t k, cons
  * identity sigma delta^c omega^r; cols == 0 does nothing.  Synchronous. */
 int h2_poly_permutation_sigma_copies(const uint64_t *dst, size_t cols, uint32_t k, const uint32_t *copies, size_t m,
                                      const void *omega, const void *delta, int repr);
+
+/* ---- the prover's product columns ------------------------------------------------------------------------------------ */
+/* The permutation argument's product columns, permutation::Argument::commit (plonk/permutation/prover.rs:98-168), for
+ * every set of every proof in one call.  The argument's `cols` columns are split into sets = ceil(cols / chunk_len) sets of
+ * chunk_len (the last may be shorter); columns[p cols + c] is column c of proof p (any resident Lagrange column: advice,
+ * fixed or instance, in the argument's column order), sigmas[c] its permutation polynomial.  z_out[p sets + a] receives
+ * set a of proof p: the running product of
+ *   prod_j (v_j[i] + beta delta^(c0 + j) omega^i + gamma) / (v_j[i] + beta sigma_j[i] + gamma)   (c0 = a chunk_len)
+ * (a zero denominator counts as zero, ff::BatchInvert) starting at ONE for set 0 and at the previous set's row n - bf - 1
+ * after it (last_z), with rows [n - bf, n) = blinding[(p sets + a) bf .. + bf) (the rng's order: per proof, per set).
+ * omega = domain.get_omega(), delta = F::DELTA; scalars and blinding values in `repr`.
+ * The inputs are only read, so shared polynomials (a shared proving key's sigma) work on every lane; z_out must be the
+ * calling context's own, pairwise distinct and none of the inputs.  Every check runs before anything is launched, and a
+ * failed check writes nothing: unknown handle, other field, fewer than n = 2^k elements, shared z_out, aliasing,
+ * chunk_len == 0, blinding_factors + 1 >= n, k > 30, more than 65535 product columns.  proofs == 0 or cols == 0 does
+ * nothing.  Asynchronous. */
+int h2_poly_permutation_product(const uint64_t *z_out, size_t proofs, const uint64_t *columns, const uint64_t *sigmas, size_t cols,
+                                uint32_t chunk_len, uint32_t k, const void *beta, const void *gamma, const void *omega, const void *delta,
+                                const void *blinding, uint32_t blinding_factors, int repr);
+/* The lookup argument's product columns, lookup::Permuted::commit_product (plonk/lookup/prover.rs:279-337), for `count`
+ * lookups (of any number of proofs) in one call: z_out[b][0] = 1, z_out[b][i] = prod_(j < i) (a[j] + beta) (s[j] + gamma) /
+ * ((beta + a'[j]) (gamma + s'[j])) for i < n - bf, rows [n - bf, n) = blinding[b bf .. + bf), where a = inputs[b],
+ * s = tables[b] are the compressed columns and a' = permuted_inputs[b], s' = permuted_tables[b] the permuted ones (blinding
+ * rows included).  Inputs, checks and asynchrony as h2_poly_permutation_product; count == 0 does nothing. */
+int h2_poly_lookup_product(const uint64_t *z_out, size_t count, const uint64_t *inputs, const uint64_t *tables,
+                           const uint64_t *permuted_inputs, const uint64_t *permuted_tables, uint32_t k, const void *beta,
+                           const void *gamma, const void *blinding, uint32_t blinding_factors, int repr);
 
 /* Reference sort of the MSM: by default every (point, window) reference is binned in ONE pass into fixed-capacity
  * per-bucket bins, with an automatic fallback to the exact histogram / scan / scatter sort when a bin overflows
