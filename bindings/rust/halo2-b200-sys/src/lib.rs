@@ -114,6 +114,8 @@ extern "C" {
     pub fn h2_poly_lookup_product(z_out: *const u64, count: usize, inputs: *const u64, tables: *const u64, permuted_inputs: *const u64,
                                   permuted_tables: *const u64, k: u32, beta: *const c_void, gamma: *const c_void, blinding: *const c_void,
                                   blinding_factors: u32, repr: c_int) -> c_int;
+    pub fn h2_poly_lookup_permuted(out_inputs: *const u64, out_tables: *const u64, count: usize, inputs: *const u64, tables: *const u64, k: u32,
+                                   blinding: *const c_void, blinding_factors: u32, repr: c_int) -> c_int;
 }
 
 fn check(rc: c_int) {
@@ -622,6 +624,29 @@ pub fn lookup_products<F: PrimeField>(field_id: c_int, k: u32, inputs: &[u64], t
         check(rc);
     }
     handles
+}
+
+/// The permuted columns of `commit_permuted` (plonk/lookup/prover.rs:76-243) for every lookup of every proof in one call:
+/// `inputs[b]` / `tables[b]` are lookup b's compressed Lagrange columns (handles, 2^k elements; shared ones work on every
+/// lane), `blinding` holds per lookup blinding_factors + 1 input rows then as many table rows, in the rng's order
+/// (:622-624).  Returns (permuted input, permuted table) handles per lookup, blinding rows included.  Panics, naming the lowest
+/// lookup, where the reference returns Error::ConstraintSystemFailure (an input value missing from its table).
+pub fn lookup_permuted<F: PrimeField>(field_id: c_int, k: u32, inputs: &[u64], tables: &[u64], blinding: &[F], blinding_factors: u32) -> Vec<(u64, u64)> {
+    let count = inputs.len();
+    assert_eq!(tables.len(), count, "one table per input");
+    assert_eq!(blinding.len(), count * 2 * (blinding_factors as usize + 1), "2 (blinding_factors + 1) values per lookup");
+    let outs = alloc_polys(field_id, 1usize << k, 2 * count);
+    let (oi, ot): (Vec<u64>, Vec<u64>) = (outs[..count].to_vec(), outs[count..].to_vec());
+    let bl = scalars_to_bytes(blinding);
+    let rc = unsafe {
+        h2_poly_lookup_permuted(oi.as_ptr(), ot.as_ptr(), count, inputs.as_ptr(), tables.as_ptr(), k, bl.as_ptr() as *const c_void, blinding_factors,
+                                REPR_CANONICAL)
+    };
+    if rc != 0 {
+        for &h in &outs { unsafe { h2_poly_free(h) }; }
+        check(rc);
+    }
+    oi.into_iter().zip(ot).collect()
 }
 
 /// The verifier's `g_scalars` (poly/commitment/msm.rs:12) kept in HBM: what `MSM<C>` holds under the `b200` feature instead of

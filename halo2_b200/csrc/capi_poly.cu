@@ -298,66 +298,142 @@ static int lk_scan(uint32_t *d, uint64_t n, cudaStream_t s) {     // exclusive s
     LAUNCH(scan_apply_kernel, nb, H2_SCAN_BLOCK, 0, s, d, n, bs, (const uint32_t *)nullptr);
     return 0;
 }
-template <class P> static int lk_sort(fe *keys, uint64_t N, cudaStream_t s) {    // ascending bitonic sort of N = 2^m canonical keys
+// ascending bitonic sort of `count` arrays of N = 2^m canonical keys each, one per grid.y
+static int lk_sort(fe *keys, uint64_t N, uint32_t count, cudaStream_t s, int field) {
     const uint64_t BL = N < (1ull << H2_LK_BLOCK_LOG) ? N : (1ull << H2_LK_BLOCK_LOG);
     const uint32_t smem = (uint32_t)(BL * sizeof(fe)), thr = (uint32_t)(BL / 2 < 512 ? (BL / 2 ? BL / 2 : 1) : 512);
-    LAUNCH(lk_bitonic_block_kernel, (uint32_t)(N / BL), thr, smem, s, keys, N, (uint64_t)2, 1u);
+    const dim3 blocks((uint32_t)(N / BL), count), stage(blocks_for(N / 2, 256), count);
+    LAUNCH(lk_bitonic_block_kernel, blocks, thr, smem, s, keys, N, (uint64_t)2, 1u);
     for (uint64_t size = 2 * BL; size <= N; size <<= 1) {
-        for (uint64_t stride = size / 2; stride >= BL; stride >>= 1)
-            LAUNCH(lk_bitonic_global_kernel<P>, blocks_for(N / 2, 256), 256, 0, s, keys, N, size, stride);
-        LAUNCH(lk_bitonic_block_kernel, (uint32_t)(N / BL), thr, smem, s, keys, N, size, 0u);
+        for (uint64_t stride = size / 2; stride >= BL; stride >>= 1) {
+            if (field == H2_FIELD_FP) LAUNCH(lk_bitonic_global_kernel<FpParams>, stage, 256, 0, s, keys, N, size, stride);
+            else LAUNCH(lk_bitonic_global_kernel<FqParams>, stage, 256, 0, s, keys, N, size, stride);
+        }
+        LAUNCH(lk_bitonic_block_kernel, blocks, thr, smem, s, keys, N, size, 0u);
     }
     return 0;
 }
-template <class P> static int lookup_permute_run(PolyBuf *in, PolyBuf *tab, size_t u, PolyBuf *out_in, PolyBuf *out_tab) {
+// The permuted columns of `count` lookups of u usable rows (lookup.cuh), and with `blinding` (count x 2 rows values) the
+// blinding rows [u, u + rows) of every output.  Scratch from the lane's pools, per lookup (N = the power of two >= u, >= 2):
+//   lk_keys  32 N bytes (the sorted table)          lk_u32  4 (3 u + 2) bytes (cnt | unconsumed, scanned in one pass; leftovers)
+//   lk_aux   32 bytes of pointers + 64 rows bytes of blinding values;  plus 4 bytes per 8192 scanned words and the error word.
+// One synchronisation; *bad = the lowest lookup with an input value its table lacks, H2_LK_NONE when none -- and then
+// every output is as it was (the one writing kernel runs after the miss is known and checks for it first).
+template <class P>
+static int lookup_permuted_run(const std::vector<PolyBuf *> &outs, const std::vector<PolyBuf *> &ins, uint64_t u, uint64_t rows, const void *blinding,
+                               int repr, uint32_t *bad) {
     Context &X = g_ctx;
     cudaStream_t s = X.stream;
-    if (scratch_acquire(s)) return 1;
+    const uint32_t count = (uint32_t)(ins.size() / 2);
     uint64_t N = 2;
     while (N < u) N <<= 1;
-    // u32 scratch: first flags | their scan (u + 1) | unconsumed flags | their scan (u + 1) | error word
-    const size_t w = u + 1;
-    if (X.lk_keys.ensure(2 * N * sizeof(fe)) || X.lk_left.ensure((u + 1) * sizeof(fe)) || X.lk_u32.ensure((4 * w + 4) * sizeof(uint32_t))) return 1;
-    fe *ka = X.lk_keys.as<fe>(), *kt = ka + N, *left = X.lk_left.as<fe>();
-    uint32_t *first = X.lk_u32.as<uint32_t>(), *first_scan = first + w, *unc = first_scan + w, *unc_scan = unc + w, *err = unc_scan + w;
-    LAUNCH(lk_load_kernel<P>, blocks_for(N, 256), 256, 0, s, (const fe *)in->buf.as<fe>(), (uint64_t)u, ka, N);
-    LAUNCH(lk_load_kernel<P>, blocks_for(N, 256), 256, 0, s, (const fe *)tab->buf.as<fe>(), (uint64_t)u, kt, N);
-    if (lk_sort<P>(ka, N, s) || lk_sort<P>(kt, N, s)) return 1;
-    CU(cudaMemsetAsync(first, 0, (4 * w + 4) * sizeof(uint32_t), s));
-    LAUNCH(lk_fill_u32_kernel, blocks_for(u, 256), 256, 0, s, unc, (uint64_t)u, 1u);
-    LAUNCH(lk_first_kernel<P>, blocks_for(u, 128), 128, 0, s, (const fe *)ka, (const fe *)kt, (uint64_t)u, first, unc, err, out_in->buf.as<fe>(),
-           out_tab->buf.as<fe>());
-    CU(cudaMemcpyAsync(first_scan, first, w * sizeof(uint32_t), cudaMemcpyDeviceToDevice, s));
-    CU(cudaMemcpyAsync(unc_scan, unc, w * sizeof(uint32_t), cudaMemcpyDeviceToDevice, s));
-    if (lk_scan(first_scan, w, s) || lk_scan(unc_scan, w, s)) return 1;
-    LAUNCH(lk_leftover_kernel<P>, blocks_for(u, 256), 256, 0, s, (const fe *)kt, (uint64_t)u, (const uint32_t *)unc, (const uint32_t *)unc_scan, left);
-    LAUNCH(lk_fill_kernel<P>, blocks_for(u, 256), 256, 0, s, (uint64_t)u, (const uint32_t *)first, (const uint32_t *)first_scan, (const fe *)left,
-           out_tab->buf.as<fe>());
-    uint32_t h_err = 0;
-    CU(cudaMemcpyAsync(&h_err, err, sizeof h_err, cudaMemcpyDeviceToHost, s));
+    const uint64_t w = u + 1, nblind = blinding ? (uint64_t)count * 2 * rows : 0, ptr_fe = ((uint64_t)count * 4 * sizeof(void *) + sizeof(fe) - 1) / sizeof(fe);
+    std::vector<uint8_t> up((ptr_fe + nblind) * sizeof(fe));
+    const fe **hp = reinterpret_cast<const fe **>(up.data());
+    for (uint32_t b = 0; b < count; b++) {
+        hp[b] = ins[2 * b]->buf.as<fe>();
+        hp[count + b] = ins[2 * b + 1]->buf.as<fe>();
+        hp[2 * count + b] = outs[2 * b]->buf.as<fe>();
+        hp[3 * count + b] = outs[2 * b + 1]->buf.as<fe>();
+    }
+    if (nblind) memcpy(up.data() + ptr_fe * sizeof(fe), blinding, nblind * sizeof(fe));
+    if (scratch_acquire(s)) return 1;
+    if (X.lk_keys.ensure(count * N * sizeof(fe)) || X.lk_aux.ensure(up.size()) || X.lk_u32.ensure(((2 * w + u) * count + 4) * sizeof(uint32_t))) return 1;
+    fe *keys = X.lk_keys.as<fe>(), *aux = X.lk_aux.as<fe>();
+    uint32_t *sc = X.lk_u32.as<uint32_t>(), *left = sc + 2 * w * count, *err = left + u * count;
+    CU(cudaMemcpyAsync(aux, up.data(), up.size(), cudaMemcpyHostToDevice, s));
+    LkCols c;
+    c.in = reinterpret_cast<const fe *const *>(aux);
+    c.tab = c.in + count;
+    c.out_in = reinterpret_cast<fe *const *>(aux) + 2 * count;
+    c.out_tab = c.out_in + count;
+    c.blind = nblind ? aux + ptr_fe : nullptr;
+    if (nblind && repr == H2_REPR_CANONICAL) LAUNCH(convert_kernel<P>, blocks_for(nblind, 64), 64, 0, s, aux + ptr_fe, nblind, 1);
+    CU(cudaMemsetAsync(sc, 0, w * count * sizeof(uint32_t), s));
+    CU(cudaMemsetAsync(err, 0xFF, sizeof(uint32_t), s));
+    LAUNCH(lk_load_kernel<P>, dim3(blocks_for(N, 256), count), 256, 0, s, c, u, keys, N);
+    if (lk_sort(keys, N, count, s, outs[0]->field)) return 1;
+    LAUNCH(lk_rank_kernel<P>, dim3(blocks_for(u, 128), count), 128, 0, s, c, (const fe *)keys, N, u, sc, err);
+    LAUNCH(lk_unconsumed_kernel, dim3(blocks_for(w, 256), count), 256, 0, s, sc, u, count);
+    if (lk_scan(sc, 2 * w * count, s)) return 1;
+    LAUNCH(lk_leftover_kernel, dim3(blocks_for(u, 256), count), 256, 0, s, (const uint32_t *)sc, u, count, left);
+    LAUNCH(lk_fill_kernel<P>, dim3(blocks_for(u + (nblind ? rows : 0), 256), count), 256, 0, s, c, (const fe *)keys, N, u, rows, (const uint32_t *)sc, count,
+           (const uint32_t *)left, (const uint32_t *)err);
+    CU(cudaMemcpyAsync(bad, err, sizeof *bad, cudaMemcpyDeviceToHost, s));
     if (scratch_release(s)) return 1;
     CU(cudaStreamSynchronize(s));
-    if (h_err) return fail("h2_poly_lookup_permute: an input value does not occur in the table (Error::ConstraintSystemFailure, plonk/lookup/prover.rs:605-608)");
+    return 0;
+}
+static const char *lk_miss = "an input value does not occur in the table (Error::ConstraintSystemFailure, plonk/lookup/prover.rs:605-608)";
+// The checks of both entry points, all before any launch: the outputs are the calling context's, writable, pairwise distinct
+// and none of the inputs; inputs may repeat and may be shared; every polynomial is of one field and holds `len` elements.
+static int lookup_permuted_handles(const char *who, const uint64_t *oh, const uint64_t *ih, size_t nh, uint64_t len, const char *len_name, PolyReads &rd,
+                                   std::vector<PolyBuf *> &outs, std::vector<PolyBuf *> &ins) {
+    const std::string w(who), unknown = w + ": unknown polynomial handle";
+    outs.resize(nh);
+    ins.resize(nh);
+    for (size_t i = 0; i < nh; i++) {
+        outs[i] = poly_for_write(oh[i], who, unknown.c_str());
+        if (!outs[i]) return 1;
+    }
+    for (size_t i = 0; i < nh; i++) {
+        ins[i] = rd.get(ih[i]);
+        if (!ins[i]) return fail(unknown);
+    }
+    for (size_t i = 0; i < nh; i++) {
+        if (outs[i]->field != outs[0]->field || ins[i]->field != outs[0]->field) return fail(w + ": the polynomials live in different fields");
+        if (outs[i]->len < len || ins[i]->len < len) return fail(w + ": a polynomial holds fewer than " + len_name + " elements");
+    }
+    std::vector<PolyBuf *> so(outs), si(ins);
+    std::sort(so.begin(), so.end());
+    std::sort(si.begin(), si.end());
+    if (std::adjacent_find(so.begin(), so.end()) != so.end()) return fail(w + ": an output handle appears twice");
+    for (PolyBuf *p : so)
+        if (std::binary_search(si.begin(), si.end(), p)) return fail(w + ": an output handle is also an input");
     return 0;
 }
 extern "C" int h2_poly_lookup_permute(uint64_t input, uint64_t table, size_t usable_rows, uint64_t out_input, uint64_t out_table) {
+    static const char *who = "h2_poly_lookup_permute";
     CtxLock lk;
     if (require_ready()) return 1;
-    const char *unknown = "h2_poly_lookup_permute: unknown polynomial handle";
-    PolyBuf *oa = poly_for_write(out_input, "h2_poly_lookup_permute", unknown);
-    PolyBuf *ot = oa ? poly_for_write(out_table, "h2_poly_lookup_permute", unknown) : nullptr;
-    if (!oa || !ot) return 1;
+    const uint64_t oh[2] = {out_input, out_table}, ih[2] = {input, table};
     PolyReads rd;
-    PolyBuf *a = rd.get(input), *t = rd.get(table);
-    if (!a || !t) return fail(unknown);
-    if (oa == ot || oa == a || oa == t || ot == a || ot == t) return fail("h2_poly_lookup_permute: the outputs must be two polynomials other than the inputs");
-    if (a->field != t->field || a->field != oa->field || a->field != ot->field) return fail("h2_poly_lookup_permute: the polynomials live in different fields");
-    if (a->len < usable_rows || t->len < usable_rows || oa->len < usable_rows || ot->len < usable_rows)
-        return fail("h2_poly_lookup_permute: a polynomial holds fewer than usable_rows elements");
+    std::vector<PolyBuf *> outs, ins;
+    if (lookup_permuted_handles(who, oh, ih, 2, usable_rows, "usable_rows", rd, outs, ins)) return 1;
     if (usable_rows >= (1ull << 31)) return fail("h2_poly_lookup_permute: usable_rows >= 2^31");
     if (usable_rows == 0) return 0;
-    if (a->field == H2_FIELD_FP) return lookup_permute_run<FpParams>(a, t, usable_rows, oa, ot);
-    return lookup_permute_run<FqParams>(a, t, usable_rows, oa, ot);
+    uint32_t bad = H2_LK_NONE;
+    if (outs[0]->field == H2_FIELD_FP ? lookup_permuted_run<FpParams>(outs, ins, usable_rows, 0, nullptr, H2_REPR_MONTGOMERY, &bad)
+                                      : lookup_permuted_run<FqParams>(outs, ins, usable_rows, 0, nullptr, H2_REPR_MONTGOMERY, &bad))
+        return 1;
+    if (bad != H2_LK_NONE) return fail(std::string(who) + ": " + lk_miss);
+    return 0;
+}
+extern "C" int h2_poly_lookup_permuted(const uint64_t *out_inputs, const uint64_t *out_tables, size_t count, const uint64_t *inputs, const uint64_t *tables,
+                                       uint32_t k, const void *blinding, uint32_t blinding_factors, int repr) {
+    static const char *who = "h2_poly_lookup_permuted";
+    CtxLock lk;
+    if (require_ready()) return 1;
+    if (k > 30) return fail(std::string(who) + ": k > 30");
+    if ((uint64_t)blinding_factors + 1 >= (1ull << k)) return fail(std::string(who) + ": blinding_factors + 1 >= n");
+    if (count == 0) return 0;
+    if (!out_inputs || !out_tables || !inputs || !tables || !blinding) return fail(std::string(who) + ": null argument");
+    if (count > 65535) return fail(std::string(who) + ": more than 65535 lookups");
+    std::vector<uint64_t> oh, ih;
+    for (size_t b = 0; b < count; b++) {
+        oh.insert(oh.end(), {out_inputs[b], out_tables[b]});
+        ih.insert(ih.end(), {inputs[b], tables[b]});
+    }
+    const uint64_t n = 1ull << k, rows = (uint64_t)blinding_factors + 1;
+    PolyReads rd;
+    std::vector<PolyBuf *> outs, ins;
+    if (lookup_permuted_handles(who, oh.data(), ih.data(), 2 * count, n, "2^k", rd, outs, ins)) return 1;
+    uint32_t bad = H2_LK_NONE;
+    if (outs[0]->field == H2_FIELD_FP ? lookup_permuted_run<FpParams>(outs, ins, n - rows, rows, blinding, repr, &bad)
+                                      : lookup_permuted_run<FqParams>(outs, ins, n - rows, rows, blinding, repr, &bad))
+        return 1;
+    if (bad != H2_LK_NONE) return fail(std::string(who) + ": lookup " + std::to_string(bad) + ": " + lk_miss);
+    return 0;
 }
 
 

@@ -169,7 +169,7 @@ struct Context {
     StageRing stage;
     DevBuf ast_code, ast_consts;             // asteval.cuh: the postfix program and its constants
     DevBuf po_lvl, po_q, po_pts, po_ptrs;    // polyops.cuh: level arrays, kate carries, per-level points, pointer arrays
-    DevBuf lk_keys, lk_left, lk_u32;         // lookup.cuh: sorted canonical keys (input | table), leftover table values, flag / scan arrays
+    DevBuf lk_keys, lk_aux, lk_u32;          // lookup.cuh: sorted tables, column pointers + blinding values, histogram / scan / leftover arrays
     DevBuf kg_tab, kg_map;                   // keygen.cuh: power tables + error word, one piece of the copy-constraint mapping (all of it for assembly.cuh)
     DevBuf as_edge, as_cell, as_slot;        // assembly.cuh: per-copy, per-cell and per-slot u32 arrays
     DevBuf gp_val, gp_aux;                   // grandproduct.cuh: denominators / mv of every column, pointers + tables + carries + blinding values

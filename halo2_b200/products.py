@@ -1,6 +1,7 @@
 """The prover's product columns over the C ABI: permutation::Argument::commit
 (/root/reference/halo2_proofs/src/plonk/permutation/prover.rs:47-195) and lookup::Permuted::commit_product
-(plonk/lookup/prover.rs:253-390), every column of every proof in one device call (csrc/grandproduct.cuh).
+(plonk/lookup/prover.rs:253-390), every column of every proof in one device call (csrc/grandproduct.cuh), and the lookup
+argument's permuted columns before them, lookup::Argument::commit_permuted (:76-243), likewise in one call (csrc/lookup.cuh).
 
 The library has no transcript: the commit functions return the commitments in the order the reference writes them, and the
 caller writes them to its own transcript.
@@ -8,11 +9,12 @@ caller writes them to its own transcript.
 from __future__ import annotations
 
 import ctypes
-from typing import List, Sequence, Tuple
+from typing import List, NamedTuple, Sequence, Tuple
 
 import numpy as np
 
 from . import lib as _l
+from .evaluator import Ast
 from .poly import Blind, EvaluationDomain, Params, ResidentPoly, _handles
 
 _MAX_COMMIT_BATCH = 64   # h2_msm_registered_polys_affine takes at most this many polynomials per pass
@@ -142,4 +144,87 @@ def lookup_commit_product(params: Params, domain: EvaluationDomain, lookups, bet
     for per in z:
         out.append(list(zip(per, blinds[at:at + len(per)])))
         at += len(per)
+    return out, cm
+
+
+def lookup_permute_resident(domain: EvaluationDomain, pairs: Sequence[Tuple[ResidentPoly, ResidentPoly]], blinding_factors: int,
+                            blinding: Sequence[int]) -> List[Tuple[ResidentPoly, ResidentPoly]]:
+    """The lookup argument's permuted columns (Lagrange basis, resident) of every (compressed input, compressed table) pair:
+    permute_expression_pair (lookup/prover.rs:563-647) over the usable rows, then the blinding rows (:622-627).  `blinding`
+    holds, per pair, blinding_factors + 1 input rows then as many table rows.  Returns one (permuted input, permuted table)
+    per pair (h2_poly_lookup_permuted); fails, naming the lowest pair, when an input value is missing from its table."""
+    m, n, rows = domain.m, domain.n, blinding_factors + 1
+    if len(blinding) != len(pairs) * 2 * rows:
+        raise _l.H2Error(f"expected {len(pairs) * 2 * rows} blinding values, got {len(blinding)}")
+    out = _alloc(domain.field, n, 2 * len(pairs))
+    try:
+        _l.check(_l.init().h2_poly_lookup_permuted(_handles(out[0::2]), _handles(out[1::2]), ctypes.c_size_t(len(pairs)),
+                                                    _handles([p[0] for p in pairs]), _handles([p[1] for p in pairs]), ctypes.c_uint32(domain.k),
+                                                    _l.ptr(_scalars(blinding, m)), ctypes.c_uint32(blinding_factors), _l.REPR_CANONICAL))
+    except BaseException:
+        _close(out)
+        raise
+    return list(zip(out[0::2], out[1::2]))
+
+
+class Permuted(NamedTuple):
+    """lookup::Permuted (lookup/prover.rs:51-62) on the device.  Its first four items are what lookup_commit_product takes."""
+    compressed_input: ResidentPoly         # Lagrange basis
+    compressed_table: ResidentPoly
+    permuted_input: ResidentPoly           # Lagrange basis, blinding rows included
+    permuted_table: ResidentPoly
+    permuted_input_poly: ResidentPoly      # coefficient form
+    permuted_table_poly: ResidentPoly
+    permuted_input_coset: ResidentPoly     # extended domain
+    permuted_table_coset: ResidentPoly
+    permuted_input_blind: int
+    permuted_table_blind: int
+
+
+def lookup_commit_permuted(params: Params, domain: EvaluationDomain, evaluator, lookups, theta: int, blinding_factors: int, rng):
+    """lookup::Argument::commit_permuted (lookup/prover.rs:76-243) for every lookup of every proof at once.  `evaluator` is a
+    Lagrange-basis Evaluator and `lookups[p]` proof p's list of (input expressions, table expressions), each a list of Ast over
+    it.  Each list is compressed by the fold acc * theta + e from ConstantTerm(0) (:167-176), one Ast program per column; then
+    one permute call, one commitment pass of all columns, and lagrange_to_coeff / coeff_to_extended per column.  `rng` is drawn
+    per proof, per lookup: blinding_factors + 1 input rows, as many table rows, the input blind, the table blind (:622-624,
+    :203-216).  Returns (permuted, commitments): permuted[p] = [Permuted per lookup], which lookup_commit_product takes as it
+    is, and the affine commitments in the order the reference writes them (per proof, per lookup, input then table)."""
+    rows = blinding_factors + 1
+    blinding, blinds = [], []
+    for per in lookups:
+        for _ in per:
+            blinding += [rng.scalar() for _ in range(2 * rows)]
+            blinds += [rng.scalar(), rng.scalar()]
+
+    def compress(exprs):
+        acc = Ast.constant_term(0)
+        for e in exprs:
+            acc = acc * theta + e
+        return evaluator.evaluate(acc)
+
+    compressed: List[ResidentPoly] = []
+    permuted: List[ResidentPoly] = []
+    extra: List[ResidentPoly] = []
+    try:
+        for per in lookups:
+            for inp, tab in per:
+                compressed += [compress(inp), compress(tab)]
+        permuted = [q for pair in lookup_permute_resident(domain, list(zip(compressed[0::2], compressed[1::2])), blinding_factors, blinding)
+                    for q in pair]
+        cm = _commit(params, permuted, blinds)
+        for q in permuted:
+            co = domain.lagrange_to_coeff_resident(q, out=ResidentPoly(domain.field, domain.n))
+            extra.append(co)
+            extra.append(domain.coeff_to_extended_resident(co))
+    except BaseException:
+        _close(compressed + permuted + extra)
+        raise
+    out, at = [], 0
+    for per in lookups:
+        mine = []
+        for _ in per:
+            c, q, e, b = compressed[at:at + 2], permuted[at:at + 2], extra[2 * at:2 * at + 4], blinds[at:at + 2]
+            mine.append(Permuted(c[0], c[1], q[0], q[1], e[0], e[2], e[1], e[3], b[0], b[1]))
+            at += 2
+        out.append(mine)
     return out, cm

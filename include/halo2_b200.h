@@ -206,9 +206,22 @@ int h2_poly_running_product(uint64_t dst, uint64_t src, size_t n, const void *in
  * polynomials: out_input[0, usable_rows) = the input values sorted (ff's Ord = the canonical integers, :577-581);
  * out_table[r] = out_input[r] on the first row of every run of equal values (:595-603), the remaining rows take the table
  * values that are left over, ascending, from the last such row down (:617-622).  Rows from usable_rows on -- the blinding rows,
- * :625-627 -- are not touched: the caller writes its random values there.  Fails (non-zero, nothing useful in the outputs) when
+ * :625-627 -- are not touched: the caller writes its random values there.  Fails (non-zero, the outputs unchanged) when
  * an input value does not occur in the table, the reference's Error::ConstraintSystemFailure (:605-608).  Synchronous. */
 int h2_poly_lookup_permute(uint64_t input, uint64_t table, size_t usable_rows, uint64_t out_input, uint64_t out_table);
+/* The same permuted columns for `count` lookups (of any number of proofs) in one call, blinding rows included:
+ * lookup::Argument::commit_permuted (plonk/lookup/prover.rs:76-243) between compressing the expressions and committing.
+ * Every lookup has n = 2^k rows and u = n - blinding_factors - 1 usable ones: out_inputs[b] / out_tables[b] rows [0, u) =
+ * permute_expression_pair of inputs[b] / tables[b] as h2_poly_lookup_permute gives them, rows [u, n) = the caller's random
+ * values.  blinding: count x 2 (blinding_factors + 1) elements in `repr`, per lookup the input's rows then the table's, the
+ * reference's rng order (:622-624).  The inputs are only read and may repeat, so shared polynomials work on every lane; the
+ * outputs must be the calling context's own, pairwise distinct and none of the inputs.  Every check runs before anything is
+ * launched, and a failed check writes nothing: unknown handle, other field, fewer than n elements, shared output, aliasing,
+ * blinding_factors + 1 >= n, k > 30, count > 65535.  When an input value does not occur in its table
+ * (Error::ConstraintSystemFailure, :605-608) the call fails naming the lowest such lookup b, and no output has changed.
+ * count == 0 does nothing.  Synchronous: one synchronisation whatever count is. */
+int h2_poly_lookup_permuted(const uint64_t *out_inputs, const uint64_t *out_tables, size_t count, const uint64_t *inputs,
+                            const uint64_t *tables, uint32_t k, const void *blinding, uint32_t blinding_factors, int repr);
 /* EvaluationDomain::divide_by_vanishing_poly (poly/domain.rs:329-348) in place on a resident extended-domain polynomial:
  * h[i] *= t_evals[i mod t_len]; t_evals = the domain's t_evaluations (domain.rs:86-128), t_len = 2^(ext_k - k).  Asynchronous. */
 int h2_poly_divide_by_vanishing(uint64_t poly, uint32_t ext_k, const void *t_evals, uint32_t t_len, int repr);
