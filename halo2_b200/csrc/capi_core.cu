@@ -1,6 +1,8 @@
 // C ABI of the engine (include/halo2_b200.h), part 1 of 5: context, device binding, settings, test hooks, utilities.
 #include "util_kernels.cuh"
 
+#include <algorithm>
+
 static thread_local std::string g_err;
 int fail(const std::string &m) { g_err = m; return 1; }
 const std::string &last_error_string() { return g_err; }
@@ -89,28 +91,68 @@ extern "C" int h2_bases_release(uint64_t handle) {
 }
 
 std::map<uint64_t, PolyBuf *> g_shared_polys;
-PolyBuf *poly_for_write(uint64_t h, const char *who, const char *unknown) {
-    auto it = g_ctx.polys.find(h);
-    if (it != g_ctx.polys.end()) return it->second;
-    bool shared;
-    {
-        std::lock_guard<std::mutex> lk(g_reg_mu);
-        shared = g_shared_polys.count(h) != 0;
+PolyBuf *PolyArgs::fits(PolyBuf *p, uint64_t len, const char *len_name) {
+    if (!field_given && field < 0) field = p->field;
+    if (p->field != field) {
+        fail(who + (field_given ? ": the polynomial is not over the curve's scalar field" : ": the polynomials live in different fields"));
+        return nullptr;
     }
-    fail(shared ? std::string(who) + ": the polynomial is shared (read-only)" : std::string(unknown));
-    return nullptr;
+    if (p->len < len) { fail(who + ": a polynomial holds fewer than " + len_name + " elements"); return nullptr; }
+    return p;
 }
-PolyBuf *PolyReads::get(uint64_t h) {
+PolyBuf *PolyArgs::out(uint64_t h, uint64_t len, const char *len_name) {
     auto it = g_ctx.polys.find(h);
-    if (it != g_ctx.polys.end()) return it->second;
-    std::lock_guard<std::mutex> lk(g_reg_mu);
-    auto s = g_shared_polys.find(h);
-    if (s == g_shared_polys.end()) return nullptr;
-    s->second->users++;
-    held.push_back(s->second);
-    return s->second;
+    if (it == g_ctx.polys.end()) {
+        bool shared;
+        {
+            std::lock_guard<std::mutex> lk(g_reg_mu);
+            shared = g_shared_polys.count(h) != 0;
+        }
+        fail(who + (shared ? ": the polynomial is shared (read-only)" : ": unknown polynomial handle"));
+        return nullptr;
+    }
+    outs.push_back(it->second);
+    return fits(it->second, len, len_name);
 }
-PolyReads::~PolyReads() {
+PolyBuf *PolyArgs::in(uint64_t h, uint64_t len, const char *len_name) {
+    auto it = g_ctx.polys.find(h);
+    PolyBuf *p = it != g_ctx.polys.end() ? it->second : nullptr;
+    if (!p) {
+        std::lock_guard<std::mutex> lk(g_reg_mu);
+        auto s = g_shared_polys.find(h);
+        if (s != g_shared_polys.end()) {
+            p = s->second;
+            p->users++;
+            held.push_back(p);
+        }
+    }
+    if (!p) { fail(who + ": unknown polynomial handle"); return nullptr; }
+    ins.push_back(p);
+    return fits(p, len, len_name);
+}
+int PolyArgs::out(const uint64_t *h, size_t n, uint64_t len, const char *len_name, std::vector<PolyBuf *> &v) {
+    v.resize(n);
+    for (size_t i = 0; i < n; i++)
+        if (!(v[i] = out(h[i], len, len_name))) return 1;
+    return 0;
+}
+int PolyArgs::in(const uint64_t *h, size_t n, uint64_t len, const char *len_name, std::vector<PolyBuf *> &v) {
+    v.resize(n);
+    for (size_t i = 0; i < n; i++)
+        if (!(v[i] = in(h[i], len, len_name))) return 1;
+    return 0;
+}
+// Batch slices and product columns run concurrently: an output written twice, or read as another one's input, would race.
+int PolyArgs::distinct(const char *role) {
+    std::vector<PolyBuf *> so(outs), si(ins);
+    std::sort(so.begin(), so.end());
+    std::sort(si.begin(), si.end());
+    if (std::adjacent_find(so.begin(), so.end()) != so.end()) return fail(who + ": " + role + " handle appears twice");
+    for (PolyBuf *p : so)
+        if (std::binary_search(si.begin(), si.end(), p)) return fail(who + ": " + role + " handle is also an input");
+    return 0;
+}
+PolyArgs::~PolyArgs() {
     if (held.empty()) return;
     std::lock_guard<std::mutex> lk(g_reg_mu);
     for (PolyBuf *p : held) user_drop(p->users);
@@ -670,10 +712,10 @@ extern "C" int h2_dev_convert(int field, void *d_a, size_t n, int to_montgomery,
     if (require_ready()) return 1;
     cudaStream_t s = (cudaStream_t)stream;
     if (n == 0) return 0;
-    if (field == H2_FIELD_FP) LAUNCH(convert_kernel<FpParams>, blocks_for(n, 256), 256, 0, s, (fe *)d_a, (uint64_t)n, to_montgomery);
-    else if (field == H2_FIELD_FQ) LAUNCH(convert_kernel<FqParams>, blocks_for(n, 256), 256, 0, s, (fe *)d_a, (uint64_t)n, to_montgomery);
-    else return fail("unknown field id");
-    return 0;
+    return by_field(field, [&](auto p) {
+        LAUNCH(convert_kernel<decltype(p)>, blocks_for(n, 256), 256, 0, s, (fe *)d_a, (uint64_t)n, to_montgomery);
+        return 0;
+    });
 }
 extern "C" int h2_test_field_op(int field, int op, const void *a, const void *b, size_t n, void *out) {
     CtxLock lk;

@@ -851,13 +851,6 @@ static int ipa_begin_common(uint64_t bases_handle, uint32_t k, const void *p_pri
                             uint64_t *session) {
     CtxLock lk;
     if (require_ready()) return 1;
-    PolyBuf *p_poly = nullptr;
-    PolyReads rd;
-    if (p_poly_handle) {   // looked up and used under the one lock
-        p_poly = rd.get(*p_poly_handle);
-        if (!p_poly) return fail("h2_ipa_begin_poly: unknown polynomial handle");
-        if (k > 28 || p_poly->len < ((size_t)1 << k)) return fail("h2_ipa_begin_poly: the polynomial holds fewer than 2^k coefficients");
-    }
     BasesRef ref(bases_handle, true);
     if (!ref.b) return fail("h2_ipa_begin: unknown bases handle");
     BaseSet *b = ref.b;
@@ -869,13 +862,15 @@ static int ipa_begin_common(uint64_t bases_handle, uint32_t k, const void *p_pri
     if (k == 0 || k > 28) return fail("h2_ipa_begin: k out of range");
     if (b->n != (1ull << k) + 2) return fail("h2_ipa_begin: the base set must hold g[0..2^k) || w || u");
     if (!b->table.p) return fail("h2_ipa_begin: the base set has no window table (register with H2_BASES_PRECOMPUTE)");
+    PolyArgs g("h2_ipa_begin_poly", b->curve == H2_CURVE_PALLAS ? H2_FIELD_FQ : H2_FIELD_FP);
+    PolyBuf *p_poly = nullptr;
+    if (p_poly_handle && !(p_poly = g.in(*p_poly_handle, 1ull << k, "2^k"))) return 1;   // looked up and used under the one lock
     IpaSession *q;
     if (!g_ctx.ipa_pool.empty()) { q = g_ctx.ipa_pool.back(); g_ctx.ipa_pool.pop_back(); }
     else q = new IpaSession();
     q->bases = bases_handle; q->k = k; q->round = 0; q->folded = 1;
     cudaStream_t s = g_ctx.stream;
     if (scratch_acquire(s)) { ipa_free(q); return 1; }   // pow2 is shared scratch
-    if (p_poly && p_poly->field != (b->curve == H2_CURVE_PALLAS ? H2_FIELD_FQ : H2_FIELD_FP)) { ipa_free(q); return fail("h2_ipa_begin_poly: the polynomial is not over the curve's scalar field"); }
     int rc = b->curve == H2_CURVE_PALLAS ? ipa_begin_impl<FqParams>(q, p_prime, p_poly, x3, repr, s) : ipa_begin_impl<FpParams>(q, p_prime, p_poly, x3, repr, s);
     if (rc) { ipa_free(q); return 1; }
     if (scratch_release(s)) { ipa_free(q); return 1; }
@@ -1018,6 +1013,9 @@ static int msm_registered_polys_impl(uint64_t bases_handle, const uint64_t *poly
     const size_t total = n + (extra_scalars ? 1 : 0);
     if (total > b->n) return fail("h2_msm_registered_polys: more scalars than registered bases");
     const int scalar_field = b->curve == H2_CURVE_PALLAS ? H2_FIELD_FQ : H2_FIELD_FP;
+    PolyArgs g("h2_msm_registered_polys", scalar_field);
+    std::vector<PolyBuf *> q;
+    if (g.in(polys, batch, n, "n", q)) return 1;
     Context &X = g_ctx;
     cudaStream_t s = X.stream;
     if (scratch_acquire(s)) return 1;
@@ -1027,13 +1025,8 @@ static int msm_registered_polys_impl(uint64_t bases_handle, const uint64_t *poly
         CU(cudaMemcpyAsync(X.misc.p, extra_scalars, batch * sizeof(fe), cudaMemcpyHostToDevice, s));
         if (repr == H2_REPR_CANONICAL && convert_field(scalar_field, X.misc.as<fe>(), batch, 1, s)) return 1;
     }
-    PolyReads rd;
     for (size_t j = 0; j < batch; j++) {
-        PolyBuf *q = rd.get(polys[j]);
-        if (!q) return fail("h2_msm_registered_polys: unknown polynomial handle");
-        if (q->field != scalar_field) return fail("h2_msm_registered_polys: the polynomial is not over the curve's scalar field");
-        if (q->len < n) return fail("h2_msm_registered_polys: the polynomial holds fewer than n elements");
-        CU(cudaMemcpyAsync(d + j * total, q->buf.p, n * sizeof(fe), cudaMemcpyDeviceToDevice, s));
+        CU(cudaMemcpyAsync(d + j * total, q[j]->buf.p, n * sizeof(fe), cudaMemcpyDeviceToDevice, s));
         if (extra_scalars) CU(cudaMemcpyAsync(d + j * total + n, X.misc.as<fe>() + j, sizeof(fe), cudaMemcpyDeviceToDevice, s));
     }
     uint32_t tc = 0, tmode = 0;

@@ -137,9 +137,7 @@ static int ntt_host_dispatch(int field, int mode, const void *a_in, uint32_t in_
     CtxLock lk;
     if (require_ready()) return 1;
     if (log_n > 30 || in_log_n > log_n) return fail("ntt: bad sizes");
-    if (field == H2_FIELD_FP) return ntt_host<FpParams>(field, mode, a_in, in_log_n, log_n, omega, zeta, divisor, out_len, out, repr);
-    if (field == H2_FIELD_FQ) return ntt_host<FqParams>(field, mode, a_in, in_log_n, log_n, omega, zeta, divisor, out_len, out, repr);
-    return fail("unknown field id");
+    return by_field(field, [&](auto p) { return ntt_host<decltype(p)>(field, mode, a_in, in_log_n, log_n, omega, zeta, divisor, out_len, out, repr); });
 }
 extern "C" int h2_ntt(int field, void *a, const void *omega, uint32_t log_n, int repr) {
     return ntt_host_dispatch(field, 0, a, log_n, log_n, omega, nullptr, nullptr, (size_t)1 << log_n, a, repr);
@@ -161,11 +159,11 @@ extern "C" int h2_ntt_dev(int field, const void *d_in, void *d_out, const void *
     cudaStream_t s = (cudaStream_t)stream;
     if (scratch_acquire(s)) return 1;
     NttScales sc;   // Montgomery in, Montgomery out, no scaling
-    int rc;
-    if (field == H2_FIELD_FP) rc = ntt_run<FpParams>(field, (const fe *)d_in, log_n, (fe *)d_out, log_n, host_to_mont<FpParams>(omega, omega_repr), sc, 1ull << log_n, s);
-    else if (field == H2_FIELD_FQ) rc = ntt_run<FqParams>(field, (const fe *)d_in, log_n, (fe *)d_out, log_n, host_to_mont<FqParams>(omega, omega_repr), sc, 1ull << log_n, s);
-    else return fail("unknown field id");
-    if (rc) return rc;
+    if (by_field(field, [&](auto p) {
+            using P = decltype(p);
+            return ntt_run<P>(field, (const fe *)d_in, log_n, (fe *)d_out, log_n, host_to_mont<P>(omega, omega_repr), sc, 1ull << log_n, s);
+        }))
+        return 1;
     return scratch_release(s);
 }
 // test / bench hook: 1 = the bulk-copy (TMA) persistent pass kernel where it applies, 0 = the classic kernel (default; ctx.cuh)
@@ -184,9 +182,7 @@ extern "C" int h2_ntt_clear_cache(void) {
 }
 
 int get_twiddles_any(int field, const fe &omega_mont, uint32_t log_n, cudaStream_t s, const fe **out) {
-    if (field == H2_FIELD_FP) return get_twiddles<FpParams>(field, omega_mont, log_n, s, out);
-    if (field == H2_FIELD_FQ) return get_twiddles<FqParams>(field, omega_mont, log_n, s, out);
-    return fail("unknown field id");
+    return by_field(field, [&](auto p) { return get_twiddles<decltype(p)>(field, omega_mont, log_n, s, out); });
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -282,16 +278,17 @@ extern "C" int h2_poly_free(uint64_t poly) {
 }
 int convert_field(int field, fe *d, size_t n, int to_mont, cudaStream_t s) {
     if (n == 0) return 0;
-    if (field == H2_FIELD_FP) LAUNCH(convert_kernel<FpParams>, blocks_for(n, 256), 256, 0, s, d, (uint64_t)n, to_mont);
-    else LAUNCH(convert_kernel<FqParams>, blocks_for(n, 256), 256, 0, s, d, (uint64_t)n, to_mont);
-    return 0;
+    return by_field(field, [&](auto p) {
+        LAUNCH(convert_kernel<decltype(p)>, blocks_for(n, 256), 256, 0, s, d, (uint64_t)n, to_mont);
+        return 0;
+    });
 }
 extern "C" int h2_poly_upload(uint64_t poly, const void *src, size_t len, int repr) {
     CtxLock lk;
     if (require_ready()) return 1;
-    PolyBuf *b = poly_for_write(poly, "h2_poly_upload", "h2_poly_upload: unknown handle");
+    PolyArgs g("h2_poly_upload");
+    PolyBuf *b = g.out(poly, len, "len");
     if (!b) return 1;
-    if (len > b->len) return fail("h2_poly_upload: more elements than the polynomial holds");
     cudaStream_t s = g_ctx.stream;
     if (upload_async(b->buf.p, src, len * sizeof(fe), s)) return 1;
     if (repr == H2_REPR_CANONICAL && convert_field(b->field, b->buf.as<fe>(), len, 1, s)) return 1;
@@ -304,26 +301,27 @@ template <class P> __global__ void poly_add_at_kernel(fe *a, fe delta_mont) { fe
 extern "C" int h2_poly_add_at(uint64_t poly, size_t index, const void *delta, int repr) {
     CtxLock lk;
     if (require_ready()) return 1;
-    PolyBuf *b = poly_for_write(poly, "h2_poly_add_at", "h2_poly_add_at: unknown handle");
+    PolyArgs g("h2_poly_add_at");
+    PolyBuf *b = g.out(poly, 0, "0");
     if (!b) return 1;
     if (index >= b->len) return fail("h2_poly_add_at: index out of range");
     cudaStream_t s = g_ctx.stream;
-    if (b->field == H2_FIELD_FP) LAUNCH(poly_add_at_kernel<FpParams>, 1, 1, 0, s, b->buf.as<fe>() + index, host_to_mont<FpParams>(delta, repr));
-    else LAUNCH(poly_add_at_kernel<FqParams>, 1, 1, 0, s, b->buf.as<fe>() + index, host_to_mont<FqParams>(delta, repr));
-    return 0;
+    return by_field(b->field, [&](auto p) {
+        using P = decltype(p);
+        LAUNCH(poly_add_at_kernel<P>, 1, 1, 0, s, b->buf.as<fe>() + index, host_to_mont<P>(delta, repr));
+        return 0;
+    });
 }
 // dst[dst_off .. dst_off + len) = src[src_off .. src_off + len) on the device: the h(X) pieces (plonk/vanishing/prover.rs:95-100
 // `h_poly.chunks_exact(n)`), or a copy of a column that an in-place step is about to overwrite
 extern "C" int h2_poly_copy(uint64_t dst, size_t dst_off, uint64_t src, size_t src_off, size_t len) {
     CtxLock lk;
     if (require_ready()) return 1;
-    PolyBuf *d = poly_for_write(dst, "h2_poly_copy", "h2_poly_copy: unknown handle");
+    PolyArgs g("h2_poly_copy");
+    PolyBuf *d = g.out(dst, dst_off + len, "dst_off + len");
     if (!d) return 1;
-    PolyReads rd;
-    PolyBuf *a = rd.get(src);
-    if (!a) return fail("h2_poly_copy: unknown handle");
-    if (d->field != a->field) return fail("h2_poly_copy: the polynomials live in different fields");
-    if (dst_off + len > d->len || src_off + len > a->len) return fail("h2_poly_copy: range out of bounds");
+    PolyBuf *a = g.in(src, src_off + len, "src_off + len");
+    if (!a) return 1;
     if (d == a && !(dst_off + len <= src_off || src_off + len <= dst_off)) return fail("h2_poly_copy: overlapping ranges");
     if (len) CU(cudaMemcpyAsync(d->buf.as<fe>() + dst_off, a->buf.as<fe>() + src_off, len * sizeof(fe), cudaMemcpyDeviceToDevice, g_ctx.stream));
     return 0;
@@ -331,10 +329,9 @@ extern "C" int h2_poly_copy(uint64_t dst, size_t dst_off, uint64_t src, size_t s
 extern "C" int h2_poly_download(uint64_t poly, void *dst, size_t len, int repr) {
     CtxLock lk;
     if (require_ready()) return 1;
-    PolyReads rd;
-    PolyBuf *b = rd.get(poly);
-    if (!b) return fail("h2_poly_download: unknown handle");
-    if (len > b->len) return fail("h2_poly_download: more elements than the polynomial holds");
+    PolyArgs g("h2_poly_download");
+    PolyBuf *b = g.in(poly, len, "len");
+    if (!b) return 1;
     Context &X = g_ctx;
     cudaStream_t s = X.stream;
     const fe *from = b->buf.as<fe>();
@@ -363,31 +360,28 @@ static int poly_transform(PolyBuf *dst, PolyBuf *src, int mode, uint32_t in_log_
     return scratch_release(s);       // asynchronous: later calls are ordered behind it on the stream
 }
 static int poly_transform_dispatch(uint64_t dst, uint64_t src, int mode, uint32_t in_log_n, uint32_t log_n, const void *omega, const void *zeta,
-                                   const void *divisor, size_t out_len, int repr, const char *who) {
+                                   const void *divisor, size_t out_len, int repr, const char *who, const char *in_name, const char *out_name) {
     CtxLock lk;
     if (require_ready()) return 1;
-    PolyBuf *d = poly_for_write(dst, who, "resident transform: unknown polynomial handle");
-    if (!d) return 1;
-    PolyReads rd;
-    PolyBuf *a = rd.get(src);
-    if (!a) return fail("resident transform: unknown polynomial handle");
-    if (d->field != a->field) return fail("resident transform: the polynomials live in different fields");
     if (log_n > 30 || in_log_n > log_n) return fail("ntt: bad sizes");
-    if (a->len < ((size_t)1 << in_log_n)) return fail("resident transform: the source holds fewer than 2^k elements");
     if (out_len > ((size_t)1 << log_n)) out_len = (size_t)1 << log_n;
-    if (d->len < out_len) return fail("resident transform: the destination is too short");
-    if (d == a && out_len != ((size_t)1 << log_n)) return fail("resident transform: in place needs out_len == 2^log_n");
-    if (d == a && in_log_n != log_n) return fail("resident transform: in place needs equal input and output sizes");
-    if (a->field == H2_FIELD_FP) return poly_transform<FpParams>(d, a, mode, in_log_n, log_n, omega, zeta, divisor, out_len, repr);
-    return poly_transform<FqParams>(d, a, mode, in_log_n, log_n, omega, zeta, divisor, out_len, repr);
+    PolyArgs g(who);
+    PolyBuf *d = g.out(dst, out_len, out_name);
+    if (!d) return 1;
+    PolyBuf *a = g.in(src, (size_t)1 << in_log_n, in_name);
+    if (!a) return 1;
+    if (d == a && out_len != ((size_t)1 << log_n)) return fail(std::string(who) + ": in place needs out_len == 2^log_n");
+    if (d == a && in_log_n != log_n) return fail(std::string(who) + ": in place needs equal input and output sizes");
+    return by_field(a->field, [&](auto p) { return poly_transform<decltype(p)>(d, a, mode, in_log_n, log_n, omega, zeta, divisor, out_len, repr); });
 }
 extern "C" int h2_poly_lagrange_to_coeff(uint64_t dst, uint64_t src, uint32_t k, const void *omega_inv, const void *divisor, int repr) {
-    return poly_transform_dispatch(dst, src, 1, k, k, omega_inv, nullptr, divisor, (size_t)1 << k, repr, "h2_poly_lagrange_to_coeff");
+    return poly_transform_dispatch(dst, src, 1, k, k, omega_inv, nullptr, divisor, (size_t)1 << k, repr, "h2_poly_lagrange_to_coeff", "2^k", "2^k");
 }
 extern "C" int h2_poly_coeff_to_extended(uint64_t dst, uint64_t src, uint32_t k, uint32_t ext_k, const void *zeta, const void *ext_omega, int repr) {
-    return poly_transform_dispatch(dst, src, 2, k, ext_k, ext_omega, zeta, nullptr, (size_t)1 << ext_k, repr, "h2_poly_coeff_to_extended");
+    return poly_transform_dispatch(dst, src, 2, k, ext_k, ext_omega, zeta, nullptr, (size_t)1 << ext_k, repr, "h2_poly_coeff_to_extended", "2^k", "2^ext_k");
 }
 extern "C" int h2_poly_extended_to_coeff(uint64_t dst, uint64_t src, uint32_t ext_k, const void *ext_omega_inv, const void *ext_divisor,
                                          const void *zeta, size_t out_len, int repr) {
-    return poly_transform_dispatch(dst, src, 3, ext_k, ext_k, ext_omega_inv, zeta, ext_divisor, out_len, repr, "h2_poly_extended_to_coeff");
+    return poly_transform_dispatch(dst, src, 3, ext_k, ext_k, ext_omega_inv, zeta, ext_divisor, out_len, repr, "h2_poly_extended_to_coeff", "2^ext_k",
+                                   "out_len");
 }

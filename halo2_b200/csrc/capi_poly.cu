@@ -10,8 +10,6 @@
 #include "assembly.cuh"
 #include "grandproduct.cuh"
 
-#include <algorithm>
-
 // ------------------------------------------------------------------------------------------------
 // eval_polynomial / compute_inner_product / kate_division on resident polynomials (polyops.cuh)
 // ------------------------------------------------------------------------------------------------
@@ -105,30 +103,14 @@ static int polyops_dispatch(int mode, const uint64_t *ah, const uint64_t *ch, si
     if (batch == 0) return 0;
     if (batch > 256) return fail(std::string(who) + ": batch > 256");
     if (n >= (1ull << 32)) return fail(std::string(who) + ": n >= 2^32");
-    std::vector<PolyBuf *> a(batch), c;
-    if (ch) c.resize(batch);
-    const std::string unknown = std::string(who) + ": unknown polynomial handle";
-    PolyReads rd;
-    for (size_t b = 0; b < batch; b++) {
-        a[b] = rd.get(ah[b]);
-        if (!a[b]) return fail(unknown);
-        if (a[b]->field != a[0]->field) return fail(std::string(who) + ": the polynomials live in different fields");
-        if (a[b]->len < n) return fail(std::string(who) + ": a polynomial holds fewer than n coefficients");
-        if (ch) {   // kate division writes its quotients; the inner product reads both operands
-            c[b] = mode == 2 ? poly_for_write(ch[b], who, unknown.c_str()) : rd.get(ch[b]);
-            if (!c[b]) return mode == 2 ? 1 : fail(unknown);
-            if (c[b]->field != a[0]->field) return fail(std::string(who) + ": the polynomials live in different fields");
-            if (c[b]->len + (mode == 2 ? 1 : 0) < n) return fail(std::string(who) + ": the second polynomial is too short");
-        }
+    PolyArgs g(who);
+    std::vector<PolyBuf *> a, c;
+    if (mode == 2) {   // kate division writes quotients of n - 1 coefficients; the inner product reads both operands
+        if (g.out(ch, batch, n - 1, "n - 1", c) || g.in(ah, batch, n, "n", a) || g.distinct("a quotient")) return 1;
+    } else if (g.in(ah, batch, n, "n", a) || (ch && g.in(ch, batch, n, "n", c))) {
+        return 1;
     }
-    if (mode == 2)   // batch slices run concurrently: no quotient may be another slice's dividend, or be written twice
-        for (size_t b = 0; b < batch; b++)
-            for (size_t b2 = 0; b2 < batch; b2++) {
-                if (c[b] == a[b2]) return fail(std::string(who) + ": the quotient cannot overwrite a dividend");
-                if (b2 < b && c[b] == c[b2]) return fail(std::string(who) + ": a quotient handle appears twice");
-            }
-    if (a[0]->field == H2_FIELD_FP) return polyops_run<FpParams>(mode, a, c, n, points, repr, out);
-    return polyops_run<FqParams>(mode, a, c, n, points, repr, out);
+    return by_field(a[0]->field, [&](auto p) { return polyops_run<decltype(p)>(mode, a, c, n, points, repr, out); });
 }
 // Evaluator::evaluate (poly/evaluator.rs:129-228) on resident polynomials: `code` is the postfix form of the Ast (asteval.cuh),
 // validated here so that the kernel's operand stack can neither overflow nor underflow.
@@ -163,19 +145,12 @@ extern "C" int h2_poly_eval_ast(uint64_t out, const uint64_t *polys, size_t n_po
                                 const void *consts, size_t n_consts, const void *omega, const void *lin_base, int repr) {
     CtxLock lk;
     if (require_ready()) return 1;
-    PolyBuf *o = poly_for_write(out, "h2_poly_eval_ast", "h2_poly_eval_ast: unknown output handle");
-    if (!o) return 1;
-    if (log_n > 30 || o->len < ((size_t)1 << log_n)) return fail("h2_poly_eval_ast: the output holds fewer than 2^log_n elements");
+    if (log_n > 30) return fail("h2_poly_eval_ast: log_n > 30");
     if (n_code == 0 || n_code > (1u << 20)) return fail("h2_poly_eval_ast: empty or oversized program");
-    std::vector<PolyBuf *> ps(n_polys);
-    PolyReads rd;
-    for (size_t i = 0; i < n_polys; i++) {
-        ps[i] = rd.get(polys[i]);
-        if (!ps[i]) return fail("h2_poly_eval_ast: unknown polynomial handle");
-        if (ps[i]->field != o->field) return fail("h2_poly_eval_ast: the polynomials live in different fields");
-        if (ps[i]->len < ((size_t)1 << log_n)) return fail("h2_poly_eval_ast: a polynomial holds fewer than 2^log_n elements");
-        if (ps[i] == o) return fail("h2_poly_eval_ast: the output cannot be one of the operands (rotated reads)");
-    }
+    PolyArgs g("h2_poly_eval_ast");
+    std::vector<PolyBuf *> ps;
+    PolyBuf *o = g.out(out, (size_t)1 << log_n, "2^log_n");
+    if (!o || g.in(polys, n_polys, (size_t)1 << log_n, "2^log_n", ps) || g.distinct("an output")) return 1;   // operands are read at other rows
     const AstInstr *prog = reinterpret_cast<const AstInstr *>(code);
     int depth = 0;
     bool has_linear = false;
@@ -194,22 +169,24 @@ extern "C" int h2_poly_eval_ast(uint64_t out, const uint64_t *polys, size_t n_po
     }
     if (depth != 1) return fail("h2_poly_eval_ast: the program must leave exactly one value");
     if (has_linear && (!omega || !lin_base)) return fail("h2_poly_eval_ast: a LinearTerm needs omega and the coset generator");
-    if (o->field == H2_FIELD_FP) return ast_run<FpParams>(o, ps, log_n, prog, n_code, consts, n_consts, omega, lin_base, repr, has_linear);
-    return ast_run<FqParams>(o, ps, log_n, prog, n_code, consts, n_consts, omega, lin_base, repr, has_linear);
+    return by_field(o->field, [&](auto p) { return ast_run<decltype(p)>(o, ps, log_n, prog, n_code, consts, n_consts, omega, lin_base, repr, has_linear); });
 }
 // ff::BatchInvert on the first n elements of a resident polynomial, in place (zeros stay zero)
 extern "C" int h2_poly_batch_invert(uint64_t poly, size_t n) {
     CtxLock lk;
     if (require_ready()) return 1;
-    PolyBuf *a = poly_for_write(poly, "h2_poly_batch_invert", "h2_poly_batch_invert: unknown polynomial handle");
+    PolyArgs g("h2_poly_batch_invert");
+    PolyBuf *a = g.out(poly, n, "n");
     if (!a) return 1;
-    if (a->len < n) return fail("h2_poly_batch_invert: the polynomial holds fewer than n elements");
     if (n == 0) return 0;
     cudaStream_t s = g_ctx.stream;
     if (scratch_acquire(s)) return 1;
     const uint32_t nb = blocks_for((n + 15) / 16, 64);
-    if (a->field == H2_FIELD_FP) LAUNCH(poly_batch_invert_kernel<FpParams>, nb, 64, 0, s, a->buf.as<fe>(), (uint64_t)n);
-    else LAUNCH(poly_batch_invert_kernel<FqParams>, nb, 64, 0, s, a->buf.as<fe>(), (uint64_t)n);
+    if (by_field(a->field, [&](auto p) {
+            LAUNCH(poly_batch_invert_kernel<decltype(p)>, nb, 64, 0, s, a->buf.as<fe>(), (uint64_t)n);
+            return 0;
+        }))
+        return 1;
     return scratch_release(s);
 }
 // dst[0] = init, dst[i] = dst[i - 1] * src[i - 1] for i < n: the running product of plonk/permutation/prover.rs:150-156
@@ -238,25 +215,20 @@ template <class P> static int grand_product_run(PolyBuf *d, PolyBuf *a, size_t n
 extern "C" int h2_poly_running_product(uint64_t dst, uint64_t src, size_t n, const void *init, int repr) {
     CtxLock lk;
     if (require_ready()) return 1;
-    PolyBuf *d = poly_for_write(dst, "h2_poly_running_product", "h2_poly_running_product: unknown polynomial handle");
-    if (!d) return 1;
-    PolyReads rd;
-    PolyBuf *a = rd.get(src);
-    if (!a) return fail("h2_poly_running_product: unknown polynomial handle");
-    if (d == a) return fail("h2_poly_running_product: the product cannot overwrite its factors");
-    if (d->field != a->field) return fail("h2_poly_running_product: the polynomials live in different fields");
-    if (a->len < n || d->len < n) return fail("h2_poly_running_product: a polynomial holds fewer than n elements");
+    PolyArgs g("h2_poly_running_product");
+    PolyBuf *d, *a;
+    if (!(d = g.out(dst, n, "n")) || !(a = g.in(src, n, "n")) || g.distinct("a dst")) return 1;
     if (n == 0) return 0;
-    if (a->field == H2_FIELD_FP) return grand_product_run<FpParams>(d, a, n, init, repr);
-    return grand_product_run<FqParams>(d, a, n, init, repr);
+    return by_field(a->field, [&](auto p) { return grand_product_run<decltype(p)>(d, a, n, init, repr); });
 }
 // divide_by_vanishing_poly on a resident extended-domain polynomial; t_evals: t_len = 2^(ext_k - k) host elements
 extern "C" int h2_poly_divide_by_vanishing(uint64_t poly, uint32_t ext_k, const void *t_evals, uint32_t t_len, int repr) {
     CtxLock lk;
     if (require_ready()) return 1;
-    PolyBuf *a = poly_for_write(poly, "h2_poly_divide_by_vanishing", "h2_poly_divide_by_vanishing: unknown polynomial handle");
+    if (ext_k > 30) return fail("h2_poly_divide_by_vanishing: ext_k > 30");
+    PolyArgs g("h2_poly_divide_by_vanishing");
+    PolyBuf *a = g.out(poly, (size_t)1 << ext_k, "2^ext_k");
     if (!a) return 1;
-    if (ext_k > 30 || a->len < ((size_t)1 << ext_k)) return fail("h2_poly_divide_by_vanishing: the polynomial holds fewer than 2^ext_k elements");
     if (t_len == 0 || (t_len & (t_len - 1)) || t_len > (1u << ext_k)) return fail("h2_poly_divide_by_vanishing: t_len must be a power of two <= 2^ext_k");
     Context &X = g_ctx;
     cudaStream_t s = X.stream;
@@ -265,8 +237,11 @@ extern "C" int h2_poly_divide_by_vanishing(uint64_t poly, uint32_t ext_k, const 
     CU(cudaMemcpyAsync(X.po_pts.p, t_evals, (size_t)t_len * sizeof(fe), cudaMemcpyHostToDevice, s));
     if (repr == H2_REPR_CANONICAL && convert_field(a->field, X.po_pts.as<fe>(), t_len, 1, s)) return 1;
     const uint64_t n = 1ull << ext_k;
-    if (a->field == H2_FIELD_FP) LAUNCH(poly_vanish_div_kernel<FpParams>, blocks_for(n, 256), 256, 0, s, a->buf.as<fe>(), n, (const fe *)X.po_pts.as<fe>(), t_len - 1);
-    else LAUNCH(poly_vanish_div_kernel<FqParams>, blocks_for(n, 256), 256, 0, s, a->buf.as<fe>(), n, (const fe *)X.po_pts.as<fe>(), t_len - 1);
+    if (by_field(a->field, [&](auto p) {
+            LAUNCH(poly_vanish_div_kernel<decltype(p)>, blocks_for(n, 256), 256, 0, s, a->buf.as<fe>(), n, (const fe *)X.po_pts.as<fe>(), t_len - 1);
+            return 0;
+        }))
+        return 1;
     return scratch_release(s);
 }
 extern "C" int h2_poly_eval(const uint64_t *polys, size_t batch, size_t n, const void *points, int repr, void *out) {
@@ -299,15 +274,14 @@ static int lk_scan(uint32_t *d, uint64_t n, cudaStream_t s) {     // exclusive s
     return 0;
 }
 // ascending bitonic sort of `count` arrays of N = 2^m canonical keys each, one per grid.y
-static int lk_sort(fe *keys, uint64_t N, uint32_t count, cudaStream_t s, int field) {
+template <class P> static int lk_sort(fe *keys, uint64_t N, uint32_t count, cudaStream_t s) {
     const uint64_t BL = N < (1ull << H2_LK_BLOCK_LOG) ? N : (1ull << H2_LK_BLOCK_LOG);
     const uint32_t smem = (uint32_t)(BL * sizeof(fe)), thr = (uint32_t)(BL / 2 < 512 ? (BL / 2 ? BL / 2 : 1) : 512);
     const dim3 blocks((uint32_t)(N / BL), count), stage(blocks_for(N / 2, 256), count);
     LAUNCH(lk_bitonic_block_kernel, blocks, thr, smem, s, keys, N, (uint64_t)2, 1u);
     for (uint64_t size = 2 * BL; size <= N; size <<= 1) {
         for (uint64_t stride = size / 2; stride >= BL; stride >>= 1) {
-            if (field == H2_FIELD_FP) LAUNCH(lk_bitonic_global_kernel<FpParams>, stage, 256, 0, s, keys, N, size, stride);
-            else LAUNCH(lk_bitonic_global_kernel<FqParams>, stage, 256, 0, s, keys, N, size, stride);
+            LAUNCH(lk_bitonic_global_kernel<P>, stage, 256, 0, s, keys, N, size, stride);
         }
         LAUNCH(lk_bitonic_block_kernel, blocks, thr, smem, s, keys, N, size, 0u);
     }
@@ -352,7 +326,7 @@ static int lookup_permuted_run(const std::vector<PolyBuf *> &outs, const std::ve
     CU(cudaMemsetAsync(sc, 0, w * count * sizeof(uint32_t), s));
     CU(cudaMemsetAsync(err, 0xFF, sizeof(uint32_t), s));
     LAUNCH(lk_load_kernel<P>, dim3(blocks_for(N, 256), count), 256, 0, s, c, u, keys, N);
-    if (lk_sort(keys, N, count, s, outs[0]->field)) return 1;
+    if (lk_sort<P>(keys, N, count, s)) return 1;
     LAUNCH(lk_rank_kernel<P>, dim3(blocks_for(u, 128), count), 128, 0, s, c, (const fe *)keys, N, u, sc, err);
     LAUNCH(lk_unconsumed_kernel, dim3(blocks_for(w, 256), count), 256, 0, s, sc, u, count);
     if (lk_scan(sc, 2 * w * count, s)) return 1;
@@ -365,46 +339,18 @@ static int lookup_permuted_run(const std::vector<PolyBuf *> &outs, const std::ve
     return 0;
 }
 static const char *lk_miss = "an input value does not occur in the table (Error::ConstraintSystemFailure, plonk/lookup/prover.rs:605-608)";
-// The checks of both entry points, all before any launch: the outputs are the calling context's, writable, pairwise distinct
-// and none of the inputs; inputs may repeat and may be shared; every polynomial is of one field and holds `len` elements.
-static int lookup_permuted_handles(const char *who, const uint64_t *oh, const uint64_t *ih, size_t nh, uint64_t len, const char *len_name, PolyReads &rd,
-                                   std::vector<PolyBuf *> &outs, std::vector<PolyBuf *> &ins) {
-    const std::string w(who), unknown = w + ": unknown polynomial handle";
-    outs.resize(nh);
-    ins.resize(nh);
-    for (size_t i = 0; i < nh; i++) {
-        outs[i] = poly_for_write(oh[i], who, unknown.c_str());
-        if (!outs[i]) return 1;
-    }
-    for (size_t i = 0; i < nh; i++) {
-        ins[i] = rd.get(ih[i]);
-        if (!ins[i]) return fail(unknown);
-    }
-    for (size_t i = 0; i < nh; i++) {
-        if (outs[i]->field != outs[0]->field || ins[i]->field != outs[0]->field) return fail(w + ": the polynomials live in different fields");
-        if (outs[i]->len < len || ins[i]->len < len) return fail(w + ": a polynomial holds fewer than " + len_name + " elements");
-    }
-    std::vector<PolyBuf *> so(outs), si(ins);
-    std::sort(so.begin(), so.end());
-    std::sort(si.begin(), si.end());
-    if (std::adjacent_find(so.begin(), so.end()) != so.end()) return fail(w + ": an output handle appears twice");
-    for (PolyBuf *p : so)
-        if (std::binary_search(si.begin(), si.end(), p)) return fail(w + ": an output handle is also an input");
-    return 0;
-}
 extern "C" int h2_poly_lookup_permute(uint64_t input, uint64_t table, size_t usable_rows, uint64_t out_input, uint64_t out_table) {
     static const char *who = "h2_poly_lookup_permute";
     CtxLock lk;
     if (require_ready()) return 1;
     const uint64_t oh[2] = {out_input, out_table}, ih[2] = {input, table};
-    PolyReads rd;
+    PolyArgs g(who);
     std::vector<PolyBuf *> outs, ins;
-    if (lookup_permuted_handles(who, oh, ih, 2, usable_rows, "usable_rows", rd, outs, ins)) return 1;
+    if (g.out(oh, 2, usable_rows, "usable_rows", outs) || g.in(ih, 2, usable_rows, "usable_rows", ins) || g.distinct("an output")) return 1;
     if (usable_rows >= (1ull << 31)) return fail("h2_poly_lookup_permute: usable_rows >= 2^31");
     if (usable_rows == 0) return 0;
     uint32_t bad = H2_LK_NONE;
-    if (outs[0]->field == H2_FIELD_FP ? lookup_permuted_run<FpParams>(outs, ins, usable_rows, 0, nullptr, H2_REPR_MONTGOMERY, &bad)
-                                      : lookup_permuted_run<FqParams>(outs, ins, usable_rows, 0, nullptr, H2_REPR_MONTGOMERY, &bad))
+    if (by_field(outs[0]->field, [&](auto p) { return lookup_permuted_run<decltype(p)>(outs, ins, usable_rows, 0, nullptr, H2_REPR_MONTGOMERY, &bad); }))
         return 1;
     if (bad != H2_LK_NONE) return fail(std::string(who) + ": " + lk_miss);
     return 0;
@@ -425,13 +371,11 @@ extern "C" int h2_poly_lookup_permuted(const uint64_t *out_inputs, const uint64_
         ih.insert(ih.end(), {inputs[b], tables[b]});
     }
     const uint64_t n = 1ull << k, rows = (uint64_t)blinding_factors + 1;
-    PolyReads rd;
+    PolyArgs g(who);
     std::vector<PolyBuf *> outs, ins;
-    if (lookup_permuted_handles(who, oh.data(), ih.data(), 2 * count, n, "2^k", rd, outs, ins)) return 1;
+    if (g.out(oh.data(), 2 * count, n, "2^k", outs) || g.in(ih.data(), 2 * count, n, "2^k", ins) || g.distinct("an output")) return 1;
     uint32_t bad = H2_LK_NONE;
-    if (outs[0]->field == H2_FIELD_FP ? lookup_permuted_run<FpParams>(outs, ins, n - rows, rows, blinding, repr, &bad)
-                                      : lookup_permuted_run<FqParams>(outs, ins, n - rows, rows, blinding, repr, &bad))
-        return 1;
+    if (by_field(outs[0]->field, [&](auto p) { return lookup_permuted_run<decltype(p)>(outs, ins, n - rows, rows, blinding, repr, &bad); })) return 1;
     if (bad != H2_LK_NONE) return fail(std::string(who) + ": lookup " + std::to_string(bad) + ": " + lk_miss);
     return 0;
 }
@@ -457,38 +401,32 @@ template <class P> static int compute_s_run(PolyBuf *d, const void *u, uint32_t 
 extern "C" int h2_poly_compute_s(uint64_t dst, const void *u, uint32_t k, const void *init, int accumulate, int repr) {
     CtxLock lk;
     if (require_ready()) return 1;
-    PolyBuf *d = poly_for_write(dst, "h2_poly_compute_s", "h2_poly_compute_s: unknown polynomial handle");
-    if (!d) return 1;
     if (!u || !init) return fail("h2_poly_compute_s: null challenge vector or init");
     if (k == 0) return fail("h2_poly_compute_s: no challenges (assert!(!u.is_empty()), poly/commitment/verifier.rs:157)");
-    if (k > 30 || d->len < ((size_t)1 << k)) return fail("h2_poly_compute_s: the polynomial holds fewer than 2^k elements");
-    if (d->field == H2_FIELD_FP) return compute_s_run<FpParams>(d, u, k, init, accumulate, repr);
-    return compute_s_run<FqParams>(d, u, k, init, accumulate, repr);
+    if (k > 30) return fail("h2_poly_compute_s: k > 30");
+    PolyArgs g("h2_poly_compute_s");
+    PolyBuf *d = g.out(dst, (size_t)1 << k, "2^k");
+    if (!d) return 1;
+    return by_field(d->field, [&](auto p) { return compute_s_run<decltype(p)>(d, u, k, init, accumulate, repr); });
 }
 // dst[i] = a * dst[i] + b * src[i], i < n (src == 0: dst[i] *= a): MSM::scale and the g_scalars part of MSM::add_msm
 // (poly/commitment/msm.rs:126-139, :37-62); BatchVerifier's accumulate_msm (plonk/verifier/batch.rs:83-93) is one call
 extern "C" int h2_poly_scale_add(uint64_t dst, const void *a, uint64_t src, const void *b, size_t n, int repr) {
     CtxLock lk;
     if (require_ready()) return 1;
-    PolyBuf *d = poly_for_write(dst, "h2_poly_scale_add", "h2_poly_scale_add: unknown polynomial handle");
-    if (!d) return 1;
-    PolyReads rd;
-    PolyBuf *x = src ? rd.get(src) : nullptr;
-    if (src && !x) return fail("h2_poly_scale_add: unknown polynomial handle");
-    if (x == d) return fail("h2_poly_scale_add: src must be another polynomial than dst");
-    if (x && x->field != d->field) return fail("h2_poly_scale_add: the polynomials live in different fields");
-    if (d->len < n || (x && x->len < n)) return fail("h2_poly_scale_add: a polynomial holds fewer than n elements");
+    PolyArgs g("h2_poly_scale_add");
+    PolyBuf *d = g.out(dst, n, "n"), *x = nullptr;
+    if (!d || (src && !(x = g.in(src, n, "n"))) || g.distinct("a dst")) return 1;
     if (!a || (x && !b)) return fail("h2_poly_scale_add: null factor");
     if (n == 0) return 0;
     cudaStream_t s = g_ctx.stream;
     const fe *sp = x ? x->buf.as<fe>() : nullptr;
-    if (d->field == H2_FIELD_FP)
-        LAUNCH(verifier_scale_add_kernel<FpParams>, blocks_for(n, 256), 256, 0, s, d->buf.as<fe>(), sp, host_to_mont<FpParams>(a, repr),
-               x ? host_to_mont<FpParams>(b, repr) : fe_zero(), (uint64_t)n);
-    else
-        LAUNCH(verifier_scale_add_kernel<FqParams>, blocks_for(n, 256), 256, 0, s, d->buf.as<fe>(), sp, host_to_mont<FqParams>(a, repr),
-               x ? host_to_mont<FqParams>(b, repr) : fe_zero(), (uint64_t)n);
-    return 0;
+    return by_field(d->field, [&](auto p) {
+        using P = decltype(p);
+        LAUNCH(verifier_scale_add_kernel<P>, blocks_for(n, 256), 256, 0, s, d->buf.as<fe>(), sp, host_to_mont<P>(a, repr), x ? host_to_mont<P>(b, repr) : fe_zero(),
+               (uint64_t)n);
+        return 0;
+    });
 }
 
 
@@ -545,21 +483,6 @@ static int permutation_sigma_run(const std::vector<PolyBuf *> &dst, uint32_t k, 
         }
     return sigma_finish(err, "h2_poly_permutation_sigma");
 }
-// the dst checks of both entry points: known handles of one field, at least 2^k elements each, no handle twice
-static int sigma_dst(const char *who, const uint64_t *dst, size_t cols, uint32_t k, std::vector<PolyBuf *> &d) {
-    const std::string w(who);
-    d.resize(cols);
-    for (size_t i = 0; i < cols; i++) {
-        d[i] = poly_for_write(dst[i], who, (w + ": unknown polynomial handle").c_str());
-        if (!d[i]) return 1;
-        if (d[i]->field != d[0]->field) return fail(w + ": the polynomials live in different fields");
-        if (d[i]->len < ((size_t)1 << k)) return fail(w + ": a polynomial holds fewer than 2^k elements");
-    }
-    std::vector<PolyBuf *> sorted(d);
-    std::sort(sorted.begin(), sorted.end());
-    if (std::adjacent_find(sorted.begin(), sorted.end()) != sorted.end()) return fail(w + ": a dst handle appears twice");
-    return 0;
-}
 extern "C" int h2_poly_permutation_sigma(const uint64_t *dst, size_t cols, uint32_t k, const uint32_t *mapping, const void *omega, const void *delta,
                                          int repr) {
     CtxLock lk;
@@ -568,10 +491,10 @@ extern "C" int h2_poly_permutation_sigma(const uint64_t *dst, size_t cols, uint3
     if (cols == 0) return 0;
     if (cols >= (1ull << 32)) return fail("h2_poly_permutation_sigma: cols >= 2^32");
     if (!dst || !mapping || !omega || !delta) return fail("h2_poly_permutation_sigma: null argument");
+    PolyArgs g("h2_poly_permutation_sigma");
     std::vector<PolyBuf *> d;
-    if (sigma_dst("h2_poly_permutation_sigma", dst, cols, k, d)) return 1;
-    if (d[0]->field == H2_FIELD_FP) return permutation_sigma_run<FpParams>(d, k, mapping, omega, delta, repr);
-    return permutation_sigma_run<FqParams>(d, k, mapping, omega, delta, repr);
+    if (g.out(dst, cols, (size_t)1 << k, "2^k", d) || g.distinct("a dst")) return 1;
+    return by_field(d[0]->field, [&](auto p) { return permutation_sigma_run<decltype(p)>(d, k, mapping, omega, delta, repr); });
 }
 
 
@@ -693,10 +616,10 @@ extern "C" int h2_poly_permutation_sigma_copies(const uint64_t *dst, size_t cols
     if (!dst || (m && !copies) || !omega || !delta) return fail("h2_poly_permutation_sigma_copies: null argument");
     if (((uint64_t)cols << k) >= (1ull << 32)) return fail("h2_poly_permutation_sigma_copies: cols * 2^k >= 2^32 cells");
     if ((uint64_t)m >= (1ull << 32)) return fail("h2_poly_permutation_sigma_copies: m >= 2^32 copies");
+    PolyArgs g("h2_poly_permutation_sigma_copies");
     std::vector<PolyBuf *> d;
-    if (sigma_dst("h2_poly_permutation_sigma_copies", dst, cols, k, d)) return 1;
-    if (d[0]->field == H2_FIELD_FP) return permutation_sigma_copies_run<FpParams>(d, k, copies, m, omega, delta, repr);
-    return permutation_sigma_copies_run<FqParams>(d, k, copies, m, omega, delta, repr);
+    if (g.out(dst, cols, (size_t)1 << k, "2^k", d) || g.distinct("a dst")) return 1;
+    return by_field(d[0]->field, [&](auto p) { return permutation_sigma_copies_run<decltype(p)>(d, k, copies, m, omega, delta, repr); });
 }
 
 
@@ -756,33 +679,6 @@ static int product_run(bool perm, const std::vector<PolyBuf *> &z, const std::ve
     if (bf) LAUNCH(gp_blind_kernel<P>, blocks_for(nblind, 256), 256, 0, s, zp, n, bf, (const fe *)blind, count);
     return scratch_release(s);
 }
-// The checks both entry points share, all before any launch: the z_out handles are the calling context's, writable, of one
-// field, hold n elements and are pairwise distinct and none of the inputs; the inputs are readable, of that field, hold n.
-static int product_handles(const char *who, const uint64_t *zh, size_t count, const std::vector<uint64_t> &ih, uint64_t n, PolyReads &rd,
-                           std::vector<PolyBuf *> &z, std::vector<PolyBuf *> &ins) {
-    const std::string w(who), unknown = w + ": unknown polynomial handle";
-    z.resize(count);
-    ins.resize(ih.size());
-    for (size_t b = 0; b < count; b++) {
-        z[b] = poly_for_write(zh[b], who, unknown.c_str());
-        if (!z[b]) return 1;
-        if (z[b]->field != z[0]->field) return fail(w + ": the polynomials live in different fields");
-        if (z[b]->len < n) return fail(w + ": a polynomial holds fewer than 2^k elements");
-    }
-    for (size_t i = 0; i < ih.size(); i++) {
-        ins[i] = rd.get(ih[i]);
-        if (!ins[i]) return fail(unknown);
-        if (ins[i]->field != z[0]->field) return fail(w + ": the polynomials live in different fields");
-        if (ins[i]->len < n) return fail(w + ": a polynomial holds fewer than 2^k elements");
-    }
-    std::vector<PolyBuf *> sz(z), si(ins);
-    std::sort(sz.begin(), sz.end());
-    std::sort(si.begin(), si.end());
-    if (std::adjacent_find(sz.begin(), sz.end()) != sz.end()) return fail(w + ": a z_out handle appears twice");
-    for (PolyBuf *p : sz)
-        if (std::binary_search(si.begin(), si.end(), p)) return fail(w + ": a z_out handle is also an input");
-    return 0;
-}
 static int product_scalars(const char *who, uint32_t k, uint32_t bf) {
     if (k > 30) return fail(std::string(who) + ": k > 30");
     if ((uint64_t)bf + 1 >= (1ull << k)) return fail(std::string(who) + ": blinding_factors + 1 >= n");
@@ -802,12 +698,12 @@ extern "C" int h2_poly_permutation_product(const uint64_t *z_out, size_t proofs,
     if (cols >= (1ull << 20) || proofs >= (1ull << 16) || proofs * sets > 65535) return fail(std::string(who) + ": more than 65535 product columns");
     std::vector<uint64_t> ih(columns, columns + proofs * cols);
     ih.insert(ih.end(), sigmas, sigmas + cols);
-    PolyReads rd;
+    PolyArgs g(who);
     std::vector<PolyBuf *> z, ins;
-    if (product_handles(who, z_out, proofs * sets, ih, 1ull << k, rd, z, ins)) return 1;
-    if (z[0]->field == H2_FIELD_FP)
-        return product_run<FpParams>(true, z, ins, (uint32_t)cols, chunk_len, (uint32_t)sets, k, beta, gamma, omega, delta, blinding, blinding_factors, repr);
-    return product_run<FqParams>(true, z, ins, (uint32_t)cols, chunk_len, (uint32_t)sets, k, beta, gamma, omega, delta, blinding, blinding_factors, repr);
+    if (g.out(z_out, proofs * sets, 1ull << k, "2^k", z) || g.in(ih.data(), ih.size(), 1ull << k, "2^k", ins) || g.distinct("a z_out")) return 1;
+    return by_field(z[0]->field, [&](auto p) {
+        return product_run<decltype(p)>(true, z, ins, (uint32_t)cols, chunk_len, (uint32_t)sets, k, beta, gamma, omega, delta, blinding, blinding_factors, repr);
+    });
 }
 extern "C" int h2_poly_lookup_product(const uint64_t *z_out, size_t count, const uint64_t *inputs, const uint64_t *tables, const uint64_t *permuted_inputs,
                                       const uint64_t *permuted_tables, uint32_t k, const void *beta, const void *gamma, const void *blinding,
@@ -822,9 +718,8 @@ extern "C" int h2_poly_lookup_product(const uint64_t *z_out, size_t count, const
     if (count > 65535) return fail(std::string(who) + ": more than 65535 product columns");
     std::vector<uint64_t> ih;
     for (size_t b = 0; b < count; b++) ih.insert(ih.end(), {inputs[b], tables[b], permuted_inputs[b], permuted_tables[b]});
-    PolyReads rd;
+    PolyArgs g(who);
     std::vector<PolyBuf *> z, ins;
-    if (product_handles(who, z_out, count, ih, 1ull << k, rd, z, ins)) return 1;
-    if (z[0]->field == H2_FIELD_FP) return product_run<FpParams>(false, z, ins, 0, 1, 1, k, beta, gamma, nullptr, nullptr, blinding, blinding_factors, repr);
-    return product_run<FqParams>(false, z, ins, 0, 1, 1, k, beta, gamma, nullptr, nullptr, blinding, blinding_factors, repr);
+    if (g.out(z_out, count, 1ull << k, "2^k", z) || g.in(ih.data(), ih.size(), 1ull << k, "2^k", ins) || g.distinct("a z_out")) return 1;
+    return by_field(z[0]->field, [&](auto p) { return product_run<decltype(p)>(false, z, ins, 0, 1, 1, k, beta, gamma, nullptr, nullptr, blinding, blinding_factors, repr); });
 }

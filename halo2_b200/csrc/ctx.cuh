@@ -70,7 +70,7 @@ struct BaseSet {
 
 struct PolyBuf {                           // device-resident polynomial, Montgomery form, len + 1 slots
     int field; size_t len; DevBuf buf;
-    uint32_t users = 0;                    // shared polynomials (g_shared_polys): calls in flight on any context that read it (PolyReads); under g_reg_mu
+    uint32_t users = 0;                    // shared polynomials (g_shared_polys): calls in flight on any context that read it (PolyArgs); under g_reg_mu
     PolyBuf() { buf.tracked = false; }
 };
 struct IpaSession {
@@ -276,21 +276,40 @@ template <class P> static fe host_to_mont(const void *bytes, int repr) {
 // Shared polynomials (h2_poly_share): read-only from then on, and readable from every context.  Sharing moves them out of
 // their owner's `polys` into this registry with unchanged handles; they never go into a poly_pool.
 extern std::map<uint64_t, PolyBuf *> g_shared_polys;
-// The write lookup: a polynomial of the calling context.  Any other handle fails -- a shared one with "<who>: the polynomial
-// is shared (read-only)", anything else with `unknown` -- and gives nullptr.
-PolyBuf *poly_for_write(uint64_t h, const char *who, const char *unknown);
-// The read lookup for one call: the calling context's polynomials first, then the shared ones.  A shared polynomial it finds
-// counts the call as a user until the PolyReads is dropped, so h2_poly_free cannot free it meanwhile.  Declared after the
-// call's CtxLock, so it is dropped before the context's mutex.
-struct PolyReads {
-    std::vector<PolyBuf *> held;             // the shared polynomials this call holds
-    PolyBuf *get(uint64_t h);                // nullptr: unknown handle
-    PolyReads() {}
-    ~PolyReads();
-    PolyReads(const PolyReads &) = delete;
-    PolyReads &operator=(const PolyReads &) = delete;
+// The resident-polynomial arguments of one entry point `who`, all checked before it launches anything:
+//   - an output is a polynomial of the calling context; a shared one fails with "<who>: the polynomial is shared (read-only)";
+//   - an input is the calling context's or a shared one, and a shared input counts the call as a user until the PolyArgs is
+//     dropped, so h2_poly_free cannot free it meanwhile.  Declared after the call's CtxLock, so it is dropped before the
+//     context's mutex;
+//   - every polynomial is over one field (`field`, the curve's scalar field for the MSM-side calls, or else the first
+//     polynomial's) and holds at least the `len` elements its lookup asks for, named `len_name` in the message;
+//   - with distinct(), no output is listed twice or is also an input; calls that work in place do not ask for it.
+// Every failure sets "<who>: <reason>"; a lookup then gives nullptr, the other members 1.
+struct PolyArgs {
+    explicit PolyArgs(const char *who, int field = -1) : who(who), field(field), field_given(field >= 0) {}
+    ~PolyArgs();
+    PolyBuf *out(uint64_t h, uint64_t len, const char *len_name);
+    PolyBuf *in(uint64_t h, uint64_t len, const char *len_name);
+    int out(const uint64_t *h, size_t n, uint64_t len, const char *len_name, std::vector<PolyBuf *> &v);
+    int in(const uint64_t *h, size_t n, uint64_t len, const char *len_name, std::vector<PolyBuf *> &v);
+    int distinct(const char *role);          // role with its article: "<who>: a dst handle appears twice"
+    PolyArgs(const PolyArgs &) = delete;
+    PolyArgs &operator=(const PolyArgs &) = delete;
+
+  private:
+    std::string who;
+    int field;
+    bool field_given;
+    std::vector<PolyBuf *> outs, ins, held;  // held: the shared polynomials this call is a user of
+    PolyBuf *fits(PolyBuf *p, uint64_t len, const char *len_name);
 };
 int shared_poly_free(uint64_t h);            // h2_poly_free of a handle that is not the calling context's
+// f(FpParams{}) or f(FqParams{}) for a field id; any other id fails
+template <class F> static int by_field(int field, F &&f) {
+    if (field == H2_FIELD_FP) return f(FpParams{});
+    if (field == H2_FIELD_FQ) return f(FqParams{});
+    return fail("unknown field id");
+}
 // what a fixed-base MSM over `b` runs on: the digit-multiples table (mode 2) when there is one, else the window table (mode 1)
 #define H2_FB_BITS_CTX 8u
 static inline const affine *fixed_table(const BaseSet *b, uint32_t *c, uint32_t *mode) {

@@ -127,7 +127,7 @@ class FakeLib:
         self._log("h2_poly_scale_add")
         n = _v(n)
         if _v(src) and _v(src) == _v(dst):
-            return self._fail("h2_poly_scale_add: src must be another polynomial than dst")
+            return self._fail("h2_poly_scale_add: a dst handle is also an input")
         f, d = self.polys[_v(dst)]
         buf = np.ascontiguousarray(d[:n])
         sb = np.ascontiguousarray(self.polys[_v(src)][1][:n]) if _v(src) else None
@@ -213,7 +213,7 @@ class FakeLib:
         pts = _rd(points, 32 * batch).reshape(-1, 32)
         for i in range(batch):
             if int(dst[i]) == int(src[i]):
-                return self._fail("h2_poly_kate_division: dst aliases src")
+                return self._fail("h2_poly_kate_division: a quotient handle is also an input")
             f, a = self.polys[int(src[i])]
             q = cref.kate_division(f, a[:n], int.from_bytes(pts[i].tobytes(), "little"))
             d = self.polys[int(dst[i])][1]
@@ -272,7 +272,7 @@ class FakeLib:
         if depth != 1:
             return self._fail("h2_poly_eval_ast: the program leaves more than one value")
         if _v(out) in [int(polys[i]) for i in range(n_polys)]:
-            return self._fail("h2_poly_eval_ast: the output cannot be one of the operands")
+            return self._fail("h2_poly_eval_ast: an output handle is also an input")
         f = self.polys[_v(out)][0]
         if self.polys[_v(out)][1].shape[0] < n or any(self.polys[int(polys[i])][1].shape[0] < n for i in range(n_polys)):
             return self._fail("h2_poly_eval_ast: a polynomial holds fewer than 2^log_n elements")
@@ -296,7 +296,7 @@ class FakeLib:
     def h2_poly_running_product(self, dst, src, n, init, repr_):
         self._log("h2_poly_running_product")
         if _v(dst) == _v(src):
-            return self._fail("h2_poly_running_product: the product cannot overwrite its factors")
+            return self._fail("h2_poly_running_product: a dst handle is also an input")
         f, a = self.polys[_v(src)]
         n = _v(n)
         res = np.zeros((n, 32), dtype=np.uint8)
