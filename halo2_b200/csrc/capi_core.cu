@@ -701,11 +701,10 @@ extern "C" int h2_dev_gen_points(int curve, uint64_t seed, uint64_t first, size_
     CtxLock lk;
     if (require_ready()) return 1;
     cudaStream_t s = (cudaStream_t)stream;
-    if (n == 0) return 0;
-    if (curve == H2_CURVE_PALLAS) LAUNCH(gen_points_kernel<FpParams>, blocks_for(n, 128), 128, 0, s, (affine *)d_out, seed, first, (uint64_t)n);
-    else if (curve == H2_CURVE_VESTA) LAUNCH(gen_points_kernel<FqParams>, blocks_for(n, 128), 128, 0, s, (affine *)d_out, seed, first, (uint64_t)n);
-    else return fail("unknown curve id");
-    return 0;
+    return by_curve(curve, [&](auto p, auto) {
+        if (n) LAUNCH(gen_points_kernel<decltype(p)>, blocks_for(n, 128), 128, 0, s, (affine *)d_out, seed, first, (uint64_t)n);
+        return 0;
+    });
 }
 extern "C" int h2_dev_convert(int field, void *d_a, size_t n, int to_montgomery, void *stream) {
     CtxLock lk;
@@ -727,8 +726,11 @@ extern "C" int h2_test_field_op(int field, int op, const void *a, const void *b,
     fe *da = X.misc.as<fe>(), *db = da + n, *dout = db + n;
     CU(cudaMemcpyAsync(da, a, n * sizeof(fe), cudaMemcpyHostToDevice, s));
     CU(cudaMemcpyAsync(db, b, n * sizeof(fe), cudaMemcpyHostToDevice, s));
-    if (field == H2_FIELD_FP) LAUNCH(test_field_kernel<FpParams>, blocks_for(n, 128), 128, 0, s, da, db, dout, (uint64_t)n, op);
-    else LAUNCH(test_field_kernel<FqParams>, blocks_for(n, 128), 128, 0, s, da, db, dout, (uint64_t)n, op);
+    if (by_field(field, [&](auto p) {
+            LAUNCH(test_field_kernel<decltype(p)>, blocks_for(n, 128), 128, 0, s, da, db, dout, (uint64_t)n, op);
+            return 0;
+        }))
+        return 1;
     CU(cudaMemcpyAsync(out, dout, n * sizeof(fe), cudaMemcpyDeviceToHost, s));
     if (scratch_release(s)) return 1;
     CU(cudaStreamSynchronize(s));
@@ -744,8 +746,11 @@ extern "C" int h2_test_curve_op(int curve, int op, const void *a_xy, const void 
     affine *da = X.misc.as<affine>(), *db = da + n, *dout = db + n;
     CU(cudaMemcpyAsync(da, a_xy, n * sizeof(affine), cudaMemcpyHostToDevice, s));
     CU(cudaMemcpyAsync(db, b_xy, n * sizeof(affine), cudaMemcpyHostToDevice, s));
-    if (curve == H2_CURVE_PALLAS) LAUNCH(test_curve_kernel<FpParams>, blocks_for(n, 64), 64, 0, s, da, db, dout, (uint64_t)n, op);
-    else LAUNCH(test_curve_kernel<FqParams>, blocks_for(n, 64), 64, 0, s, da, db, dout, (uint64_t)n, op);
+    if (by_curve(curve, [&](auto p, auto) {
+            LAUNCH(test_curve_kernel<decltype(p)>, blocks_for(n, 64), 64, 0, s, da, db, dout, (uint64_t)n, op);
+            return 0;
+        }))
+        return 1;
     CU(cudaMemcpyAsync(out_xy, dout, n * sizeof(affine), cudaMemcpyDeviceToHost, s));
     if (scratch_release(s)) return 1;
     CU(cudaStreamSynchronize(s));

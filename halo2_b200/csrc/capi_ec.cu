@@ -11,9 +11,9 @@
 // ------------------------------------------------------------------------------------------------
 // the log n butterfly stages (+ the optional `*g *= scale` pass) on an XYZZ work array already in network order
 template <class P, class PS>
-static int ecfft_stages(int scalar_field, xyzz *work, uint32_t log_n, const fe &omega_mont, const fe *scale_canon, cudaStream_t s) {
+static int ecfft_stages(xyzz *work, uint32_t log_n, const fe &omega_mont, const fe *scale_canon, cudaStream_t s) {
     const fe *tw = nullptr;
-    if (get_twiddles_any(scalar_field, omega_mont, log_n, s, &tw)) return 1;
+    if (get_twiddles_any(PS::ID, omega_mont, log_n, s, &tw)) return 1;
     const uint64_t n = 1ull << log_n;
     // one QUAD of lanes per butterfly (ecfft.cuh) unless the test hook asks for the one-thread form
     // A quad level costs ~3 multiply latencies (selects, call, 32 shuffles, limb carries), so the quad form only
@@ -32,7 +32,7 @@ static int ecfft_stages(int scalar_field, xyzz *work, uint32_t log_n, const fe &
 // mode 0: Jacobian in -> Jacobian out (h2_ec_fft); mode 1: affine in -> scaled, normalised affine out (h2_params_lagrange)
 // `in` == nullptr: the input is already in X.ec_io on the device (h2_params_new), scratch acquired by the caller
 template <class P, class PS>
-static int ecfft_host(int scalar_field, int mode, const void *in, uint32_t log_n, const void *omega, const void *scale, int repr, void *out) {
+static int ecfft_host(int mode, const void *in, uint32_t log_n, const void *omega, const void *scale, int repr, void *out) {
     Context &X = g_ctx;
     cudaStream_t s = X.stream;
     const uint64_t n = 1ull << log_n;
@@ -58,7 +58,7 @@ static int ecfft_host(int scalar_field, int mode, const void *in, uint32_t log_n
         if (!canon) sc = fe_from_mont<PS>(sc);
         scp = &sc;
     }
-    if (ecfft_stages<P, PS>(scalar_field, work, log_n, host_to_mont<PS>(omega, repr), scp, s)) return 1;
+    if (ecfft_stages<P, PS>(work, log_n, host_to_mont<PS>(omega, repr), scp, s)) return 1;
     if (mode == 0) {
         auto k = ecfft_store_jac_kernel<P, PS>;
         LAUNCH(k, blocks_for(n, 128), 128, 0, s, work, X.ec_io.as<jacobian>(), canon, n);
@@ -76,9 +76,7 @@ static int ecfft_host_dispatch(int curve, int mode, const void *in, uint32_t log
     CtxLock lk;
     if (require_ready()) return 1;
     if (log_n > 26) return fail("ec_fft: log_n > 26 not supported");
-    if (curve == H2_CURVE_PALLAS) return ecfft_host<FpParams, FqParams>(H2_FIELD_FQ, mode, in, log_n, omega, scale, repr, out);
-    if (curve == H2_CURVE_VESTA) return ecfft_host<FqParams, FpParams>(H2_FIELD_FP, mode, in, log_n, omega, scale, repr, out);
-    return fail("unknown curve id");
+    return by_curve(curve, [&](auto p, auto ps) { return ecfft_host<decltype(p), decltype(ps)>(mode, in, log_n, omega, scale, repr, out); });
 }
 extern "C" int h2_ec_fft(int curve, void *points_xyz, const void *omega, uint32_t log_n, const void *scale, int repr) {
     return ecfft_host_dispatch(curve, 0, points_xyz, log_n, omega, scale, repr, points_xyz);
@@ -123,19 +121,18 @@ static int hash_to_curve_host(const char *domain_prefix, const void *msgs, size_
 extern "C" int h2_hash_to_curve(int curve, const char *domain_prefix, const void *messages, size_t msg_len, size_t n, int repr, void *out_xy) {
     CtxLock lk;
     if (require_ready()) return 1;
-    if (curve != H2_CURVE_PALLAS && curve != H2_CURVE_VESTA) return fail("unknown curve id");
+    if (check_curve(curve)) return 1;
     if (!domain_prefix) return fail("h2_hash_to_curve: domain_prefix is NULL");
     if (msg_len && !messages && n) return fail("h2_hash_to_curve: messages is NULL");
     if (msg_len >= (1ull << 31) || n >= (1ull << 32)) return fail("h2_hash_to_curve: message or batch too large");
     if (n == 0) return 0;
     static const uint8_t empty = 0;
     const void *m = messages ? messages : &empty;      // msg_len == 0: n hashes of the empty message
-    return curve == H2_CURVE_PALLAS ? hash_to_curve_host<FpParams>(domain_prefix, m, msg_len, n, repr, out_xy)
-                                    : hash_to_curve_host<FqParams>(domain_prefix, m, msg_len, n, repr, out_xy);
+    return by_curve(curve, [&](auto p, auto) { return hash_to_curve_host<decltype(p)>(domain_prefix, m, msg_len, n, repr, out_xy); });
 }
 // Params::new: g[i] = H(0 || i), w = H(1), u = H(2) with H = hash_to_curve("Halo2-Parameters"), then g_lagrange from g
 template <class P, class PS>
-static int params_new_host(int scalar_field, uint32_t k, int repr, void *g_xy, void *gl_xy, void *w_xy, void *u_xy) {
+static int params_new_host(uint32_t k, int repr, void *g_xy, void *gl_xy, void *w_xy, void *u_xy) {
     Context &X = g_ctx;
     cudaStream_t s = X.stream;
     const uint64_t n = 1ull << k;
@@ -158,21 +155,21 @@ static int params_new_host(int scalar_field, uint32_t k, int repr, void *g_xy, v
     CU(cudaMemcpyAsync(g_xy, d_g, n * sizeof(affine), cudaMemcpyDeviceToHost, s));
     CU(cudaMemcpyAsync(w_xy, d_g + n, sizeof(affine), cudaMemcpyDeviceToHost, s));
     CU(cudaMemcpyAsync(u_xy, d_g + n + 1, sizeof(affine), cudaMemcpyDeviceToHost, s));
-    return ecfft_host<P, PS>(scalar_field, 1, nullptr, k, alpha_inv.v, minv.v, repr, gl_xy);   // releases the scratch, synchronises
+    return ecfft_host<P, PS>(1, nullptr, k, alpha_inv.v, minv.v, repr, gl_xy);   // releases the scratch, synchronises
 }
 extern "C" int h2_params_new(int curve, uint32_t k, int repr, void *out_g_xy, void *out_g_lagrange_xy, void *out_w_xy, void *out_u_xy) {
     CtxLock lk;
     if (require_ready()) return 1;
     if (k > 26) return fail("h2_params_new: k > 26 not supported");
     if (!out_g_xy || !out_g_lagrange_xy || !out_w_xy || !out_u_xy) return fail("h2_params_new: NULL output");
-    if (curve == H2_CURVE_PALLAS) return params_new_host<FpParams, FqParams>(H2_FIELD_FQ, k, repr, out_g_xy, out_g_lagrange_xy, out_w_xy, out_u_xy);
-    if (curve == H2_CURVE_VESTA) return params_new_host<FqParams, FpParams>(H2_FIELD_FP, k, repr, out_g_xy, out_g_lagrange_xy, out_w_xy, out_u_xy);
-    return fail("unknown curve id");
+    return by_curve(curve, [&](auto p, auto ps) {
+        return params_new_host<decltype(p), decltype(ps)>(k, repr, out_g_xy, out_g_lagrange_xy, out_w_xy, out_u_xy);
+    });
 }
 extern "C" int h2_batch_normalize(int curve, const void *points_xyz, size_t n, int repr, void *out_xy) {
     CtxLock lk;
     if (require_ready()) return 1;
-    if (curve != H2_CURVE_PALLAS && curve != H2_CURVE_VESTA) return fail("unknown curve id");
+    if (check_curve(curve)) return 1;
     if (n == 0) return 0;
     Context &X = g_ctx;
     cudaStream_t s = X.stream;
@@ -181,10 +178,11 @@ extern "C" int h2_batch_normalize(int curve, const void *points_xyz, size_t n, i
     if (X.ec_io.ensure(n * sizeof(jacobian)) || X.ec_out.ensure(n * sizeof(affine))) return 1;
     CU(cudaMemcpyAsync(X.ec_io.p, points_xyz, n * sizeof(jacobian), cudaMemcpyHostToDevice, s));
     const uint32_t nb = blocks_for((n + H2_NORM_CHUNK - 1) / H2_NORM_CHUNK, 64);
-    if (curve == H2_CURVE_PALLAS)
-        LAUNCH(normalize_kernel<FpParams>, nb, 64, 0, s, (const xyzz *)nullptr, X.ec_io.as<jacobian>(), canon, X.ec_out.as<affine>(), canon, (uint64_t)n);
-    else
-        LAUNCH(normalize_kernel<FqParams>, nb, 64, 0, s, (const xyzz *)nullptr, X.ec_io.as<jacobian>(), canon, X.ec_out.as<affine>(), canon, (uint64_t)n);
+    if (by_curve(curve, [&](auto p, auto) {
+            LAUNCH(normalize_kernel<decltype(p)>, nb, 64, 0, s, (const xyzz *)nullptr, X.ec_io.as<jacobian>(), canon, X.ec_out.as<affine>(), canon, (uint64_t)n);
+            return 0;
+        }))
+        return 1;
     CU(cudaMemcpyAsync(out_xy, X.ec_out.p, n * sizeof(affine), cudaMemcpyDeviceToHost, s));
     if (scratch_release(s)) return 1;
     CU(cudaStreamSynchronize(s));
@@ -222,10 +220,10 @@ template <class P> static int points_codec(int decompress, const void *in, size_
 static int points_codec_dispatch(int curve, int decompress, const void *in, size_t n, int repr, void *out) {
     CtxLock lk;
     if (require_ready()) return 1;
-    if (curve != H2_CURVE_PALLAS && curve != H2_CURVE_VESTA) return fail("unknown curve id");
+    if (check_curve(curve)) return 1;
     if (n >= (1ull << 32)) return fail("points codec: n >= 2^32");
     if (n == 0) return 0;
-    return curve == H2_CURVE_PALLAS ? points_codec<FpParams>(decompress, in, n, repr, out) : points_codec<FqParams>(decompress, in, n, repr, out);
+    return by_curve(curve, [&](auto p, auto) { return points_codec<decltype(p)>(decompress, in, n, repr, out); });
 }
 extern "C" int h2_points_compress(int curve, const void *points_xy, size_t n, int repr, void *out_bytes) {
     return points_codec_dispatch(curve, 0, points_xy, n, repr, out_bytes);

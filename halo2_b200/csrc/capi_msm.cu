@@ -8,7 +8,15 @@
 #include "ntt.cuh"
 #include "ecfft.cuh"
 #include "fixedbase.cuh"
-static_assert(H2_FB_BITS == H2_FB_BITS_CTX, "ctx.cuh: fixed_table");
+
+// What an MSM pass runs on: a registered set's digit-multiples table (mode 2, H2_FB_BITS) or window table (mode 1, window c, `stride`
+// points per window), or plain bases (mode 0, window c; 0: chosen by size)
+struct PassBases { const affine *bases; uint32_t c = 0, mode = 0; uint64_t stride = 0; };
+static PassBases pass_bases(const BaseSet *b) {
+    if (b->dtable.p) return {b->dtable.as<affine>(), H2_FB_BITS, 2, b->n};
+    if (b->table.p) return {b->table.as<affine>(), b->c, 1, b->n};
+    return {b->buf.as<affine>()};
+}
 
 
 // ------------------------------------------------------------------------------------------------
@@ -42,13 +50,13 @@ static inline size_t chunk_first(size_t n, uint32_t k, uint32_t j) {
 // A fixed-base MSM over resident bases is launched with the same parameters call after call: the second call with a given
 // key is captured into a CUDA graph, later ones replay it.
 static int msm_issue_or_replay(const std::function<int()> &issue, bool graphable, const void *d_scalars, const void *d_bases, const void *d_out,
-                               size_t n, uint64_t stride, uint32_t c, uint32_t sets, int scalars_mont, int out_canonical, cudaStream_t s) {
+                               size_t n, uint64_t stride, uint32_t c, uint32_t sets, int scalars_mont, int out_canonical, bool fast, cudaStream_t s) {
     Context &X = g_ctx;
     if (!(graphable && X.graphs_on && !g_prof_on)) return issue();
     MsmGraph *ge = nullptr;
     for (auto &e : X.graphs)
         if (e.scalars == d_scalars && e.bases == d_bases && e.out == d_out && e.n == n && e.stride == stride && e.c == c && e.sets == sets &&
-            e.scalars_mont == scalars_mont && e.out_canonical == out_canonical && e.fast == (X.fast_now ? 1u : 0u)) { ge = &e; break; }
+            e.scalars_mont == scalars_mont && e.out_canonical == out_canonical && e.fast == (fast ? 1u : 0u)) { ge = &e; break; }
     if (ge && ge->gen != g_alloc_gen) {   // some buffer moved since the capture
         if (ge->exec) cudaGraphExecDestroy(ge->exec);
         ge->exec = nullptr; ge->seen = 0; ge->gen = g_alloc_gen;
@@ -62,7 +70,7 @@ static int msm_issue_or_replay(const std::function<int()> &issue, bool graphable
         }
         MsmGraph e;
         e.scalars = d_scalars; e.bases = d_bases; e.out = d_out; e.n = n; e.stride = stride; e.gen = g_alloc_gen; e.c = c; e.sets = sets;
-        e.scalars_mont = scalars_mont; e.out_canonical = out_canonical; e.fast = X.fast_now ? 1u : 0u;
+        e.scalars_mont = scalars_mont; e.out_canonical = out_canonical; e.fast = fast ? 1u : 0u;
         X.graphs.push_back(e);
         ge = &X.graphs.back();
     }
@@ -99,10 +107,15 @@ static int msm_issue_or_replay(const std::function<int()> &issue, bool graphable
 // bc != nullptr: the bases arrive chunk by chunk while this runs.  Each chunk is then sorted and accumulated on its own
 // (own bins, work items and bucket sums) as soon as it has landed, and the bucket reduce adds the per-chunk bucket sums:
 // the upload of all but the first chunk hides behind the accumulation.
+// fast: a pass over a window table with bins and without chunks may run without its fallback kernels (MsmPlan::fast); *ran_fast (if
+// given) tells whether it did, and then its result is valid only if both device flags come back clear (msm_pass).  rerun: the pass
+// re-runs, in full, a fast one whose flags came back set.
 template <class P, class PS>
 static int msm_run(const fe *d_scalars, int scalars_mont, const affine *d_bases, size_t n, uint32_t c, uint32_t fixed, uint64_t stride,
-                   jacobian *d_out, int out_canonical, cudaStream_t s, const BasesChunks *bc = nullptr, uint32_t sets = 1) {
+                   jacobian *d_out, int out_canonical, cudaStream_t s, const BasesChunks *bc, uint32_t sets, bool fast, bool rerun,
+                   bool *ran_fast) {
     Context &X = g_ctx;
+    if (ran_fast) *ran_fast = false;
     if (n == 0) {   // empty sum = identity, one per scalar vector
         jacobian id;
         id.x = fe_zero(); id.y = out_canonical ? fe_zero() : fe_one<P>(); id.z = fe_zero();
@@ -115,8 +128,8 @@ static int msm_run(const fe *d_scalars, int scalars_mont, const affine *d_bases,
     std::function<int()> issue;
     // h2_test_last_msm_plan: mode, c, W, sets, accumulation, natural, fast, re-run of a fast pass -- recorded here on the host,
     // so a pass replayed from a captured graph reports the same
-    auto record = [&X](uint32_t mode, uint32_t c_, uint32_t W, uint32_t sets_, uint32_t accum, uint32_t natural, uint32_t fast) {
-        const uint32_t v[8] = {mode, c_, W, sets_, accum, natural, fast, X.fast_retry ? 1u : 0u};
+    auto record = [&X, rerun](uint32_t mode, uint32_t c_, uint32_t W, uint32_t sets_, uint32_t accum, uint32_t natural, uint32_t fast_) {
+        const uint32_t v[8] = {mode, c_, W, sets_, accum, natural, fast_, rerun ? 1u : 0u};
         memcpy(X.last_plan, v, sizeof v);
         X.have_plan = true;
     };
@@ -145,7 +158,7 @@ static int msm_run(const fe *d_scalars, int scalars_mont, const affine *d_bases,
             }
             return 0;
         };
-        return msm_issue_or_replay(issue, !bc, d_scalars, d_bases, d_out, n, stride, H2_FB_BITS, fp.sets, scalars_mont, out_canonical, s);
+        return msm_issue_or_replay(issue, !bc, d_scalars, d_bases, d_out, n, stride, H2_FB_BITS, fp.sets, scalars_mont, out_canonical, fast, s);
     }
     const uint32_t glv = (!fixed && X.glv_on && n < (1ull << 30)) ? 1u : 0u;
     if (c == 0) c = X.window_override ? X.window_override : msm_default_window(n, glv);
@@ -155,9 +168,8 @@ static int msm_run(const fe *d_scalars, int scalars_mont, const affine *d_bases,
     MsmPlan p;                       // the whole problem: bucket reduce and window combine
     msm_make_plan(p, n, c, 0, 0, fixed, stride, glv, sets, force_cap);
     p.chunks = K;
-    // fast fixed-base pass: no fallback kernels; the caller checks the flags (fixed_pass_ok) and re-runs with fast_now = false
-    p.fast = (fixed == 1 && !bc && X.fast_now && p.cap != 0) ? 1u : 0u;
-    X.last_fast = p.fast != 0;
+    p.fast = (fixed == 1 && !bc && fast && p.cap != 0) ? 1u : 0u;
+    if (ran_fast) *ran_fast = p.fast != 0;
     // ... whose work items are whole buckets: with T >= the bin capacity a bucket can only exceed T by overflowing its bin, so
     // "a bucket was split" (flags[0], ~5 buckets of a k = 14 commit at T = 32) never fails a pass that the sort flag would not
     if (p.fast && p.T < p.cap) { p.T = p.cap; p.acc_chunk[0] = p.T; }
@@ -331,29 +343,59 @@ static int msm_run(const fe *d_scalars, int scalars_mont, const affine *d_bases,
         LAUNCH(k_final, 1, 64, 0, s, p, M, (uint32_t)out_canonical);
         return 0;
     };
-    return msm_issue_or_replay(issue, fixed && !bc, d_scalars, d_bases, d_out, n, stride, c, sets, scalars_mont, out_canonical, s);
+    return msm_issue_or_replay(issue, fixed && !bc, d_scalars, d_bases, d_out, n, stride, c, sets, scalars_mont, out_canonical, fast, s);
 }
 
-int msm_dispatch(int curve, const fe *d_scalars, int scalars_mont, const affine *d_bases, size_t n, uint32_t c,
-                 jacobian *d_out, int out_canonical, cudaStream_t s, uint32_t fixed, uint64_t stride,
-                 const BasesChunks *bc, uint32_t sets) {
-    if (curve == H2_CURVE_PALLAS) return msm_run<FpParams, FqParams>(d_scalars, scalars_mont, d_bases, n, c, fixed, stride, d_out, out_canonical, s, bc, sets);
-    if (curve == H2_CURVE_VESTA) return msm_run<FqParams, FpParams>(d_scalars, scalars_mont, d_bases, n, c, fixed, stride, d_out, out_canonical, s, bc, sets);
-    return fail("unknown curve id");
+static int msm_dispatch(int curve, const fe *d_scalars, int scalars_mont, const PassBases &B, size_t n, jacobian *d_out, int out_canonical,
+                        cudaStream_t s, const BasesChunks *bc, uint32_t sets, bool fast = false, bool rerun = false, bool *ran_fast = nullptr) {
+    return by_curve(curve, [&](auto p, auto ps) {
+        return msm_run<decltype(p), decltype(ps)>(d_scalars, scalars_mont, B.bases, n, B.c, B.mode, B.stride, d_out, out_canonical, s, bc, sets,
+                                                  fast, rerun, ran_fast);
+    });
 }
-// The fast fixed-base pass (MsmPlan::fast): callers queue `fixed_pass_flags` right behind the pass (with the copy of the result),
-// synchronise, and ask `fixed_pass_ok`; false = a bin overflowed or a bucket was split, the result is not valid: issue the pass again
-// with X.fast_now = false.
-int fixed_pass_flags(cudaStream_t s) {
+
+// Where the result of an msm_pass goes: `sets` Jacobian points to host memory, or (affine) as many affine points after
+// batch_normalize on the device, or one Jacobian point to `peer` on device `peer_dev` (a multi-GPU worker's partial sum).
+struct PassOut { void *host; bool affine = false; void *peer = nullptr; int peer_dev = -1; };
+// One MSM pass whose result leaves the device, with the scratch acquired by the caller: issued, normalised (to.affine), copied out,
+// the scratch released and the stream synchronised.  A pass over a window table runs fast first (MsmPlan::fast) unless fast passes
+// are off (h2_test_set_fast_fixed) or its bases arrive in chunks; if either device flag comes back set -- a bin overflowed or a
+// bucket was split -- its result is not valid and the pass runs again, in full.  `issued`, if given, runs after each issue with the
+// issue's return code and returns the code to go on with.
+static int msm_pass(int curve, const fe *d_scalars, int scalars_mont, const PassBases &B, size_t n, uint32_t sets, jacobian *d_result,
+                    int canon, const PassOut &to, const BasesChunks *bc = nullptr, const std::function<int(int)> &issued = nullptr) {
     Context &X = g_ctx;
-    if (!X.last_fast) return 0;
-    if (!X.h_flags) CU(cudaHostAlloc((void **)&X.h_flags, 2 * sizeof(uint32_t), cudaHostAllocDefault));
-    CU(cudaMemcpyAsync(X.h_flags, X.last_flags, 2 * sizeof(uint32_t), cudaMemcpyDeviceToHost, s));
+    cudaStream_t s = X.stream;
+    if (to.affine && X.ec_out.ensure(sets * sizeof(affine))) return 1;
+    for (int attempt = 0; attempt < 2; attempt++) {
+        bool fast = false;
+        int rc = msm_dispatch(curve, d_scalars, scalars_mont, B, n, d_result, to.affine ? 0 : canon, s, bc, sets,
+                              attempt == 0 && B.mode == 1 && X.fast_on && !bc, attempt == 1, &fast);
+        if (issued) rc = issued(rc);
+        if (rc) return rc;
+        if (to.affine) {
+            const uint32_t nb = blocks_for((sets + H2_NORM_CHUNK - 1) / H2_NORM_CHUNK, 64);
+            auto normalize = [&](auto p, auto) {
+                LAUNCH(normalize_kernel<decltype(p)>, nb, 64, 0, s, (const xyzz *)nullptr, d_result, 0, X.ec_out.as<affine>(), canon, (uint64_t)sets);
+                return 0;
+            };
+            if (by_curve(curve, normalize)) return 1;
+            CU(cudaMemcpyAsync(to.host, X.ec_out.p, sets * sizeof(affine), cudaMemcpyDeviceToHost, s));
+        } else if (to.peer) {
+            CU(cudaMemcpyPeerAsync(to.peer, to.peer_dev, d_result, X.device, sets * sizeof(jacobian), s));
+        } else {
+            CU(cudaMemcpyAsync(to.host, d_result, sets * sizeof(jacobian), cudaMemcpyDeviceToHost, s));
+        }
+        if (fast) {
+            if (!X.h_flags) CU(cudaHostAlloc((void **)&X.h_flags, 2 * sizeof(uint32_t), cudaHostAllocDefault));
+            CU(cudaMemcpyAsync(X.h_flags, X.last_flags, 2 * sizeof(uint32_t), cudaMemcpyDeviceToHost, s));
+        }
+        if (scratch_release(s)) return 1;
+        CU(cudaStreamSynchronize(s));
+        if (!fast || (X.h_flags[0] == 0 && X.h_flags[1] == 0)) break;
+        if (scratch_acquire(s)) return 1;
+    }
     return 0;
-}
-bool fixed_pass_ok() {
-    Context &X = g_ctx;
-    return !X.last_fast || (X.h_flags[0] == 0 && X.h_flags[1] == 0);
 }
 // window size for a precomputed table over n bases: few references per bucket (short serial chains)
 // for small n, fewer windows for large n
@@ -377,13 +419,12 @@ static int build_table(BaseSet *b, uint32_t c, cudaStream_t s) {
     uint32_t W = (256 + c - 1) / c;
     if ((uint64_t)W * b->n >= (1ull << 31)) return fail("window table: too many points");
     if (b->table.ensure((size_t)W * b->n * sizeof(affine))) return 1;
-    if (b->curve == H2_CURVE_PALLAS) {
-        auto k = msm_table_kernel<FpParams, FqParams>;
-        LAUNCH(k, blocks_for(b->n, 128), 128, 0, s, b->buf.as<affine>(), b->table.as<affine>(), (uint64_t)b->n, (uint64_t)b->n, c, W);
-    } else {
-        auto k = msm_table_kernel<FqParams, FpParams>;
-        LAUNCH(k, blocks_for(b->n, 128), 128, 0, s, b->buf.as<affine>(), b->table.as<affine>(), (uint64_t)b->n, (uint64_t)b->n, c, W);
-    }
+    if (by_curve(b->curve, [&](auto p, auto ps) {
+            auto k = msm_table_kernel<decltype(p), decltype(ps)>;
+            LAUNCH(k, blocks_for(b->n, 128), 128, 0, s, b->buf.as<affine>(), b->table.as<affine>(), (uint64_t)b->n, (uint64_t)b->n, c, W);
+            return 0;
+        }))
+        return 1;
     b->c = c; b->W = W;
     return 0;
 }
@@ -394,20 +435,17 @@ static int build_direct(BaseSet *b, cudaStream_t s) {
     if (b->c != H2_FB_BITS || b->W != H2_FB_WINDOWS) return fail("H2_BASES_DIRECT: needs the 8-bit window table");
     if (b->dtable.ensure((size_t)H2_FB_WINDOWS * H2_FB_MULTIPLES * b->n * sizeof(affine))) return 1;
     const uint64_t threads = (uint64_t)H2_FB_WINDOWS * b->n;
-    if (b->curve == H2_CURVE_PALLAS) {
-        auto k = fb_table_kernel<FpParams, FqParams>;
+    return by_curve(b->curve, [&](auto p, auto ps) {
+        auto k = fb_table_kernel<decltype(p), decltype(ps)>;
         LAUNCH(k, blocks_for(threads, 128), 128, 0, s, (const affine *)b->table.as<affine>(), b->dtable.as<affine>(), (uint64_t)b->n, (uint64_t)b->n);
-    } else {
-        auto k = fb_table_kernel<FqParams, FpParams>;
-        LAUNCH(k, blocks_for(threads, 128), 128, 0, s, (const affine *)b->table.as<affine>(), b->dtable.as<affine>(), (uint64_t)b->n, (uint64_t)b->n);
-    }
-    return 0;
+        return 0;
+    });
 }
 int convert_points(int curve, affine *d, size_t n, int to_mont, cudaStream_t s) {
-    if (n == 0) return 0;
-    if (curve == H2_CURVE_PALLAS) LAUNCH(convert_points_kernel<FpParams>, blocks_for(n, 256), 256, 0, s, d, (uint64_t)n, to_mont);
-    else LAUNCH(convert_points_kernel<FqParams>, blocks_for(n, 256), 256, 0, s, d, (uint64_t)n, to_mont);
-    return 0;
+    return by_curve(curve, [&](auto p, auto) {
+        if (n) LAUNCH(convert_points_kernel<decltype(p)>, blocks_for(n, 256), 256, 0, s, d, (uint64_t)n, to_mont);
+        return 0;
+    });
 }
 
 extern "C" int h2_msm_dev(int curve, const void *d_scalars, int scalars_repr, const void *d_bases, size_t n, uint32_t window_bits,
@@ -416,18 +454,16 @@ extern "C" int h2_msm_dev(int curve, const void *d_scalars, int scalars_repr, co
     if (require_ready()) return 1;
     cudaStream_t s = (cudaStream_t)stream;
     if (scratch_acquire(s)) return 1;
-    int rc = msm_dispatch(curve, (const fe *)d_scalars, scalars_repr == H2_REPR_MONTGOMERY, (const affine *)d_bases, n, window_bits,
-                          (jacobian *)d_out_xyz, 0, s);
+    int rc = msm_dispatch(curve, (const fe *)d_scalars, scalars_repr == H2_REPR_MONTGOMERY, PassBases{(const affine *)d_bases, window_bits}, n,
+                          (jacobian *)d_out_xyz, 0, s, nullptr, 1);
     if (rc) return rc;
     return scratch_release(s);
 }
 
 // host_bases != nullptr: one-shot MSM -- the bases are uploaded (and converted) on the copy stream AFTER the
-// scalars, overlapping the digit/sort kernels, which only read scalars.
-// d_result_peer != nullptr (multi-GPU worker): the 96-byte result goes to that address on device `peer_dev` instead of the host.
-static int msm_host_common(int curve, const void *scalars, size_t n_scalars, const void *extra_scalar, const affine *d_bases,
-                           size_t n_total, int repr, void *out_xyz, uint32_t c = 0, uint32_t fixed = 0, uint64_t stride = 0,
-                           const void *host_bases = nullptr, void *d_result_peer = nullptr, int peer_dev = -1) {
+// scalars, overlapping the digit/sort kernels, which only read scalars (B.bases is where they go).
+static int msm_host_common(int curve, const void *scalars, size_t n_scalars, const void *extra_scalar, const PassBases &B,
+                           size_t n_total, int repr, const PassOut &to, const void *host_bases = nullptr) {
     Context &X = g_ctx;
     cudaStream_t s = X.stream;
     if (scratch_acquire(s)) return 1;
@@ -448,7 +484,7 @@ static int msm_host_common(int curve, const void *scalars, size_t n_scalars, con
         bc.k = 1;
         if (n_total >= ((size_t)1 << X.chunk_min_log) && n_total >= 16 * H2_MAX_UPLOAD_CHUNKS)
             bc.k = n_total >= ((size_t)8 << X.chunk_min_log) ? H2_MAX_UPLOAD_CHUNKS : n_total >= ((size_t)2 << X.chunk_min_log) ? 3u : 2u;
-        affine *db = const_cast<affine *>(d_bases);
+        affine *db = const_cast<affine *>(B.bases);
         for (uint32_t j = 0; j < bc.k; j++) { bc.ev_scal[j] = X.ev_scal_up[j]; bc.ev[j] = X.ev_bases_up[j]; }
         bc.recorded = &recorded; bc.failed = &up_failed;
         Context *ctx = &X;
@@ -479,35 +515,24 @@ static int msm_host_common(int curve, const void *scalars, size_t n_scalars, con
         if (n_scalars && upload_async(X.scal_in.p, scalars, n_scalars * sizeof(fe), s)) return 1;
         if (extra_scalar) CU(cudaMemcpyAsync(X.scal_in.as<fe>() + n_scalars, extra_scalar, sizeof(fe), cudaMemcpyHostToDevice, s));
     }
-    for (int attempt = 0; attempt < 2; attempt++) {   // fixed-base: the fast pass first, the full one if its flags came back set
-        X.fast_now = attempt == 0 && fixed == 1 && X.fast_on && !bc.k;
-        X.fast_retry = attempt == 1;
-        int rc = msm_dispatch(curve, X.scal_in.as<fe>(), repr == H2_REPR_MONTGOMERY, d_bases, n_total, c, X.result.as<jacobian>(),
-                              repr == H2_REPR_CANONICAL, s, fixed, stride, bc.k ? &bc : nullptr);
-        X.fast_now = X.fast_retry = false;
+    auto joined = [&](int rc) -> int {   // the upload's failure is the one to report
         if (uploader.joinable()) uploader.join();
         if (up_failed.load()) { cudaStreamSynchronize(s); cudaStreamSynchronize(X.copy_stream); return fail(up_err); }
-        if (rc) return rc;
-        if (d_result_peer) CU(cudaMemcpyPeerAsync(d_result_peer, peer_dev, X.result.p, X.device, sizeof(jacobian), s));
-        else CU(cudaMemcpyAsync(out_xyz, X.result.p, sizeof(jacobian), cudaMemcpyDeviceToHost, s));
-        if (fixed_pass_flags(s)) return 1;
-        if (scratch_release(s)) return 1;
-        CU(cudaStreamSynchronize(s));
-        if (fixed_pass_ok()) break;
-        if (scratch_acquire(s)) return 1;
-    }
-    return 0;
+        return rc;
+    };
+    return msm_pass(curve, X.scal_in.as<fe>(), repr == H2_REPR_MONTGOMERY, B, n_total, 1, X.result.as<jacobian>(), repr == H2_REPR_CANONICAL, to,
+                    bc.k ? &bc : nullptr, joined);
 }
 
 extern "C" int h2_msm(int curve, const void *scalars, const void *bases_xy, size_t n, int repr, void *out_xyz) {
     CtxLock lk;
     if (require_ready()) return 1;
-    if (curve != H2_CURVE_PALLAS && curve != H2_CURVE_VESTA) return fail("unknown curve id");
+    if (check_curve(curve)) return 1;
     Context &X = g_ctx;
     cudaStream_t s = X.stream;
     if (scratch_acquire(s)) return 1;
     if (X.bases_in.ensure((n + 1) * sizeof(affine))) return 1;
-    return msm_host_common(curve, scalars, n, nullptr, X.bases_in.as<affine>(), n, repr, out_xyz, 0, 0, 0, bases_xy);
+    return msm_host_common(curve, scalars, n, nullptr, {X.bases_in.as<affine>()}, n, repr, {out_xyz}, bases_xy);
 }
 
 static int bases_register_impl(int curve, const void *bases_xy, size_t n, int repr, uint32_t window_bits, uint32_t flags, uint64_t *handle);
@@ -520,7 +545,7 @@ extern "C" int h2_bases_register_ex(int curve, const void *bases_xy, size_t n, i
 static int bases_register_impl(int curve, const void *bases_xy, size_t n, int repr, uint32_t window_bits, uint32_t flags, uint64_t *handle) {
     CtxLock lk;
     if (require_ready()) return 1;
-    if (curve != H2_CURVE_PALLAS && curve != H2_CURVE_VESTA) return fail("unknown curve id");
+    if (check_curve(curve)) return 1;
     BaseSet *b = new BaseSet();
     b->curve = curve; b->n = n;
     if (b->buf.ensure((n + 1) * sizeof(affine))) { delete b; return 1; }
@@ -548,12 +573,7 @@ extern "C" int h2_msm_registered(uint64_t handle, const void *scalars, size_t n,
     BaseSet *b = ref.b;
     size_t total = n + (extra_scalar ? 1 : 0);
     if (total > b->n) return fail("h2_msm_registered: more scalars than registered bases");
-    if (b->table.p) {   // fixed-base path: digit-multiples table (direct sum) or window table (one shared bucket set)
-        uint32_t c, mode;
-        const affine *t = fixed_table(b, &c, &mode);
-        return msm_host_common(b->curve, scalars, n, extra_scalar, t, total, repr, out_xyz, c, mode, b->n);
-    }
-    return msm_host_common(b->curve, scalars, n, extra_scalar, b->buf.as<affine>(), total, repr, out_xyz);
+    return msm_host_common(b->curve, scalars, n, extra_scalar, pass_bases(b), total, repr, {out_xyz});
 }
 
 // `batch` scalar vectors of n entries (+ one extra scalar each, the blinds) against a registered base set with a
@@ -593,34 +613,8 @@ static int msm_registered_batch_impl(uint64_t handle, const void *scalars, size_
         CU(cudaMemcpy2DAsync(d, total * sizeof(fe), scalars, n * sizeof(fe), n * sizeof(fe), batch, cudaMemcpyHostToDevice, s));
         CU(cudaMemcpy2DAsync(d + n, total * sizeof(fe), extra_scalars, sizeof(fe), sizeof(fe), batch, cudaMemcpyHostToDevice, s));
     }
-    const int canon = repr == H2_REPR_CANONICAL;
-    uint32_t tc, tmode;
-    const affine *tbl = fixed_table(b, &tc, &tmode);
-    if (affine_out && X.ec_out.ensure(batch * sizeof(affine))) return 1;
-    for (int attempt = 0; attempt < 2; attempt++) {   // the fast pass first, the full one if its flags came back set
-        X.fast_now = attempt == 0 && tmode == 1 && X.fast_on;
-        X.fast_retry = attempt == 1;
-        int rc = msm_dispatch(b->curve, d, repr == H2_REPR_MONTGOMERY, tbl, total, tc, X.result.as<jacobian>(),
-                              affine_out ? 0 : canon, s, tmode, b->n, nullptr, (uint32_t)batch);
-        X.fast_now = X.fast_retry = false;
-        if (rc) return rc;
-        if (affine_out) {
-            const uint32_t nb = blocks_for((batch + H2_NORM_CHUNK - 1) / H2_NORM_CHUNK, 64);
-            if (b->curve == H2_CURVE_PALLAS)
-                LAUNCH(normalize_kernel<FpParams>, nb, 64, 0, s, (const xyzz *)nullptr, X.result.as<jacobian>(), 0, X.ec_out.as<affine>(), canon, (uint64_t)batch);
-            else
-                LAUNCH(normalize_kernel<FqParams>, nb, 64, 0, s, (const xyzz *)nullptr, X.result.as<jacobian>(), 0, X.ec_out.as<affine>(), canon, (uint64_t)batch);
-            CU(cudaMemcpyAsync(out_xyz, X.ec_out.p, batch * sizeof(affine), cudaMemcpyDeviceToHost, s));
-        } else {
-            CU(cudaMemcpyAsync(out_xyz, X.result.p, batch * sizeof(jacobian), cudaMemcpyDeviceToHost, s));
-        }
-        if (fixed_pass_flags(s)) return 1;
-        if (scratch_release(s)) return 1;
-        CU(cudaStreamSynchronize(s));
-        if (fixed_pass_ok()) break;
-        if (scratch_acquire(s)) return 1;
-    }
-    return 0;
+    return msm_pass(b->curve, d, repr == H2_REPR_MONTGOMERY, pass_bases(b), total, (uint32_t)batch, X.result.as<jacobian>(),
+                    repr == H2_REPR_CANONICAL, {out_xyz, affine_out != 0});
 }
 
 extern "C" int h2_point_sum(int curve, const void *points_xyz, size_t g, int repr, void *out_xyz) {
@@ -632,9 +626,11 @@ extern "C" int h2_point_sum(int curve, const void *points_xyz, size_t g, int rep
     if (X.misc.ensure((g + 1) * sizeof(jacobian)) || X.result.ensure(sizeof(jacobian))) return 1;
     if (g) CU(cudaMemcpyAsync(X.misc.p, points_xyz, g * sizeof(jacobian), cudaMemcpyHostToDevice, s));
     int canon = repr == H2_REPR_CANONICAL;
-    if (curve == H2_CURVE_PALLAS) LAUNCH(point_sum_kernel<FpParams>, 1, 32, 0, s, X.misc.as<jacobian>(), (uint32_t)g, canon, X.result.as<jacobian>());
-    else if (curve == H2_CURVE_VESTA) LAUNCH(point_sum_kernel<FqParams>, 1, 32, 0, s, X.misc.as<jacobian>(), (uint32_t)g, canon, X.result.as<jacobian>());
-    else return fail("unknown curve id");
+    if (by_curve(curve, [&](auto p, auto) {
+            LAUNCH(point_sum_kernel<decltype(p)>, 1, 32, 0, s, X.misc.as<jacobian>(), (uint32_t)g, canon, X.result.as<jacobian>());
+            return 0;
+        }))
+        return 1;
     CU(cudaMemcpyAsync(out_xyz, X.result.p, sizeof(jacobian), cudaMemcpyDeviceToHost, s));
     if (scratch_release(s)) return 1;
     CU(cudaStreamSynchronize(s));
@@ -647,10 +643,10 @@ extern "C" int h2_point_sum_dev(int curve, const void *d_points_xyz, size_t g, v
     CtxLock lk;
     if (require_ready()) return 1;
     cudaStream_t s = (cudaStream_t)stream;
-    if (curve == H2_CURVE_PALLAS) LAUNCH(point_sum_kernel<FpParams>, 1, 32, 0, s, (const jacobian *)d_points_xyz, (uint32_t)g, 0, (jacobian *)d_out_xyz);
-    else if (curve == H2_CURVE_VESTA) LAUNCH(point_sum_kernel<FqParams>, 1, 32, 0, s, (const jacobian *)d_points_xyz, (uint32_t)g, 0, (jacobian *)d_out_xyz);
-    else return fail("unknown curve id");
-    return 0;
+    return by_curve(curve, [&](auto p, auto) {
+        LAUNCH(point_sum_kernel<decltype(p)>, 1, 32, 0, s, (const jacobian *)d_points_xyz, (uint32_t)g, 0, (jacobian *)d_out_xyz);
+        return 0;
+    });
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -689,8 +685,11 @@ static int multi_finish(int curve, int repr, void *out_xyz) {     // the G-term 
     const size_t G = g_multi.size();
     const int canon = repr == H2_REPR_CANONICAL;
     if (X.result.ensure(sizeof(jacobian))) return 1;
-    if (curve == H2_CURVE_PALLAS) LAUNCH(point_sum_kernel<FpParams>, 1, 32, 0, s, X.multi_parts.as<jacobian>(), (uint32_t)G, canon, X.result.as<jacobian>());
-    else LAUNCH(point_sum_kernel<FqParams>, 1, 32, 0, s, X.multi_parts.as<jacobian>(), (uint32_t)G, canon, X.result.as<jacobian>());
+    if (by_curve(curve, [&](auto p, auto) {
+            LAUNCH(point_sum_kernel<decltype(p)>, 1, 32, 0, s, X.multi_parts.as<jacobian>(), (uint32_t)G, canon, X.result.as<jacobian>());
+            return 0;
+        }))
+        return 1;
     CU(cudaMemcpyAsync(out_xyz, X.result.p, sizeof(jacobian), cudaMemcpyDeviceToHost, s));
     CU(cudaStreamSynchronize(s));
     return 0;
@@ -705,7 +704,7 @@ extern "C" int h2_msm_multi_gpu(int curve, const void *scalars, const void *base
     if (multi_refuse_lane("h2_msm_multi_gpu")) return 1;
     CtxLock lk;
     if (require_ready()) return 1;
-    if (curve != H2_CURVE_PALLAS && curve != H2_CURVE_VESTA) return fail("unknown curve id");
+    if (check_curve(curve)) return 1;
     if (g_multi.empty()) return fail("h2_msm_multi_gpu: call h2_multi_init first");
     const size_t G = g_multi.size();
     Context &P0 = *g_primary;
@@ -718,8 +717,8 @@ extern "C" int h2_msm_multi_gpu(int curve, const void *scalars, const void *base
         shard_range(n, g, G, &lo, &hi);
         if (scratch_acquire(X.stream)) return 1;
         if (X.bases_in.ensure((hi - lo + 1) * sizeof(affine))) return 1;
-        return msm_host_common(curve, (const fe *)scalars + lo, hi - lo, nullptr, X.bases_in.as<affine>(), hi - lo, repr, nullptr, 0, 0, 0,
-                               (const affine *)bases_xy + lo, parts + g, prim);
+        return msm_host_common(curve, (const fe *)scalars + lo, hi - lo, nullptr, {X.bases_in.as<affine>()}, hi - lo, repr,
+                               {nullptr, false, parts + g, prim}, (const affine *)bases_xy + lo);
     });
     if (rc) return rc;
     return multi_finish(curve, repr, out_xyz);
@@ -733,7 +732,7 @@ extern "C" int h2_multi_bases_register(int curve, const void *bases_xy, size_t n
     if (multi_refuse_lane("h2_multi_bases_register")) return 1;
     CtxLock lk;
     if (require_ready()) return 1;
-    if (curve != H2_CURVE_PALLAS && curve != H2_CURVE_VESTA) return fail("unknown curve id");
+    if (check_curve(curve)) return 1;
     if (g_multi.empty()) return fail("h2_multi_bases_register: call h2_multi_init first");
     const size_t G = g_multi.size();
     MultiBases mb;
@@ -804,8 +803,8 @@ extern "C" int h2_msm_multi_registered(uint64_t handle, const void *scalars, siz
         shard_range(n, g, G, &lo, &hi);
         auto ib = X.shards.find(mb.handles[g]);
         if (ib == X.shards.end()) return fail("h2_msm_multi_registered: a shard was released");
-        return msm_host_common(mb.curve, (const fe *)scalars + lo, hi - lo, nullptr, ib->second->buf.as<affine>(), hi - lo, repr, nullptr, 0, 0, 0,
-                               nullptr, parts + g, prim);
+        return msm_host_common(mb.curve, (const fe *)scalars + lo, hi - lo, nullptr, {ib->second->buf.as<affine>()}, hi - lo, repr,
+                               {nullptr, false, parts + g, prim});
     });
     if (rc) return rc;
     return multi_finish(mb.curve, repr, out_xyz);
@@ -862,35 +861,27 @@ static int ipa_begin_common(uint64_t bases_handle, uint32_t k, const void *p_pri
     if (k == 0 || k > 28) return fail("h2_ipa_begin: k out of range");
     if (b->n != (1ull << k) + 2) return fail("h2_ipa_begin: the base set must hold g[0..2^k) || w || u");
     if (!b->table.p) return fail("h2_ipa_begin: the base set has no window table (register with H2_BASES_PRECOMPUTE)");
-    PolyArgs g("h2_ipa_begin_poly", b->curve == H2_CURVE_PALLAS ? H2_FIELD_FQ : H2_FIELD_FP);
-    PolyBuf *p_poly = nullptr;
-    if (p_poly_handle && !(p_poly = g.in(*p_poly_handle, 1ull << k, "2^k"))) return 1;   // looked up and used under the one lock
-    IpaSession *q;
-    if (!g_ctx.ipa_pool.empty()) { q = g_ctx.ipa_pool.back(); g_ctx.ipa_pool.pop_back(); }
-    else q = new IpaSession();
-    q->bases = bases_handle; q->k = k; q->round = 0; q->folded = 1;
-    cudaStream_t s = g_ctx.stream;
-    if (scratch_acquire(s)) { ipa_free(q); return 1; }   // pow2 is shared scratch
-    int rc = b->curve == H2_CURVE_PALLAS ? ipa_begin_impl<FqParams>(q, p_prime, p_poly, x3, repr, s) : ipa_begin_impl<FpParams>(q, p_prime, p_poly, x3, repr, s);
-    if (rc) { ipa_free(q); return 1; }
-    if (scratch_release(s)) { ipa_free(q); return 1; }
-    cudaError_t e = cudaStreamSynchronize(s);   // p_prime may be pageable host memory
-    if (e != cudaSuccess) { ipa_free(q); return fail(std::string("h2_ipa_begin: ") + cudaGetErrorString(e)); }
-    uint64_t h = new_handle();
-    g_ctx.ipa[h] = q;
-    *session = h;
-    opened = true;
-    return 0;
-}
-template <class PS> static int ipa_round_impl(IpaSession *q, BaseSet *b, const void *z, const void *l_rand, const void *r_rand, int repr, int out_canonical, cudaStream_t s) {
-    const uint64_t n = 1ull << q->k;
-    const uint32_t bit = q->k - 1 - q->round;
-    IpaState S = ipa_state(q);
-    LAUNCH(ipa_prep_kernel<PS>, blocks_for(n, 256), 256, 0, s, S, bit);
-    LAUNCH(ipa_inner_kernel<PS>, 1, 512, 0, s, S, bit, host_to_mont<PS>(z, repr), host_to_mont<PS>(l_rand, repr), host_to_mont<PS>(r_rand, repr));
-    uint32_t tc, tmode;
-    const affine *tbl = fixed_table(b, &tc, &tmode);
-    return msm_dispatch(b->curve, S.scal, 1, tbl, n + 2, tc, q->out.as<jacobian>(), out_canonical, s, tmode, b->n, nullptr, 2);
+    return by_curve(b->curve, [&](auto, auto ps) {
+        using PS = decltype(ps);
+        PolyArgs g("h2_ipa_begin_poly", PS::ID);
+        PolyBuf *p_poly = nullptr;
+        if (p_poly_handle && !(p_poly = g.in(*p_poly_handle, 1ull << k, "2^k"))) return 1;   // looked up and used under the one lock
+        IpaSession *q;
+        if (!g_ctx.ipa_pool.empty()) { q = g_ctx.ipa_pool.back(); g_ctx.ipa_pool.pop_back(); }
+        else q = new IpaSession();
+        q->bases = bases_handle; q->k = k; q->round = 0; q->folded = 1;
+        cudaStream_t s = g_ctx.stream;
+        if (scratch_acquire(s)) { ipa_free(q); return 1; }   // pow2 is shared scratch
+        if (ipa_begin_impl<PS>(q, p_prime, p_poly, x3, repr, s)) { ipa_free(q); return 1; }
+        if (scratch_release(s)) { ipa_free(q); return 1; }
+        cudaError_t e = cudaStreamSynchronize(s);   // p_prime may be pageable host memory
+        if (e != cudaSuccess) { ipa_free(q); return fail(std::string("h2_ipa_begin: ") + cudaGetErrorString(e)); }
+        uint64_t h = new_handle();
+        g_ctx.ipa[h] = q;
+        *session = h;
+        opened = true;
+        return 0;
+    });
 }
 static int ipa_round_common(uint64_t session, const void *z, const void *l_rand, const void *r_rand, int repr, void *out, int affine_out);
 extern "C" int h2_ipa_round(uint64_t session, const void *z, const void *l_rand, const void *r_rand, int repr, void *out_lr_xyz) {
@@ -913,29 +904,18 @@ static int ipa_round_common(uint64_t session, const void *z, const void *l_rand,
     BaseSet *b = ref.b;
     cudaStream_t s = g_ctx.stream;
     if (scratch_acquire(s)) return 1;
-    const int oc = affine_out ? 0 : repr == H2_REPR_CANONICAL;
-    if (affine_out && g_ctx.ec_out.ensure(2 * sizeof(affine))) return 1;
-    uint32_t tc0, tmode0;
-    fixed_table(b, &tc0, &tmode0);
-    for (int attempt = 0; attempt < 2; attempt++) {   // the fast pass first, the full one if its flags came back set (the prep / inner kernels are idempotent)
-        g_ctx.fast_now = attempt == 0 && tmode0 == 1 && g_ctx.fast_on;
-        g_ctx.fast_retry = attempt == 1;
-        int rc = b->curve == H2_CURVE_PALLAS ? ipa_round_impl<FqParams>(q, b, z, l_rand, r_rand, repr, oc, s) : ipa_round_impl<FpParams>(q, b, z, l_rand, r_rand, repr, oc, s);
-        g_ctx.fast_now = g_ctx.fast_retry = false;
-        if (rc) return rc;
-        if (affine_out) {
-            const int canon = repr == H2_REPR_CANONICAL;
-            if (b->curve == H2_CURVE_PALLAS) LAUNCH(normalize_kernel<FpParams>, 1, 64, 0, s, (const xyzz *)nullptr, q->out.as<jacobian>(), 0, g_ctx.ec_out.as<affine>(), canon, (uint64_t)2);
-            else LAUNCH(normalize_kernel<FqParams>, 1, 64, 0, s, (const xyzz *)nullptr, q->out.as<jacobian>(), 0, g_ctx.ec_out.as<affine>(), canon, (uint64_t)2);
-            CU(cudaMemcpyAsync(out_lr_xyz, g_ctx.ec_out.p, 2 * sizeof(affine), cudaMemcpyDeviceToHost, s));
-        } else
-            CU(cudaMemcpyAsync(out_lr_xyz, q->out.p, 2 * sizeof(jacobian), cudaMemcpyDeviceToHost, s));
-        if (fixed_pass_flags(s)) return 1;
-        if (scratch_release(s)) return 1;
-        CU(cudaStreamSynchronize(s));
-        if (fixed_pass_ok()) break;
-        if (scratch_acquire(s)) return 1;
-    }
+    const uint64_t n = 1ull << q->k;
+    const IpaState S = ipa_state(q);
+    // S.scal from p, b and s: a re-run of the pass reads them again, as no MSM kernel writes its scalars
+    int rc = by_curve(b->curve, [&](auto, auto ps) {
+        using PS = decltype(ps);
+        const uint32_t bit = q->k - 1 - q->round;
+        LAUNCH(ipa_prep_kernel<PS>, blocks_for(n, 256), 256, 0, s, S, bit);
+        LAUNCH(ipa_inner_kernel<PS>, 1, 512, 0, s, S, bit, host_to_mont<PS>(z, repr), host_to_mont<PS>(l_rand, repr), host_to_mont<PS>(r_rand, repr));
+        return 0;
+    });
+    if (rc || msm_pass(b->curve, S.scal, 1, pass_bases(b), n + 2, 2, q->out.as<jacobian>(), repr == H2_REPR_CANONICAL, {out_lr_xyz, affine_out != 0}))
+        return 1;
     q->folded = 0;
     return 0;
 }
@@ -952,8 +932,12 @@ extern "C" int h2_ipa_fold(uint64_t session, const void *u, const void *u_inv, i
     const uint32_t bit = q->k - 1 - q->round;
     cudaStream_t s = g_ctx.stream;
     IpaState S = ipa_state(q);
-    if (ref.b->curve == H2_CURVE_PALLAS) LAUNCH(ipa_fold_kernel<FqParams>, blocks_for(n, 256), 256, 0, s, S, bit, host_to_mont<FqParams>(u, repr), host_to_mont<FqParams>(u_inv, repr));
-    else LAUNCH(ipa_fold_kernel<FpParams>, blocks_for(n, 256), 256, 0, s, S, bit, host_to_mont<FpParams>(u, repr), host_to_mont<FpParams>(u_inv, repr));
+    if (by_curve(ref.b->curve, [&](auto, auto ps) {
+            using PS = decltype(ps);
+            LAUNCH(ipa_fold_kernel<PS>, blocks_for(n, 256), 256, 0, s, S, bit, host_to_mont<PS>(u, repr), host_to_mont<PS>(u_inv, repr));
+            return 0;
+        }))
+        return 1;
     q->round++; q->folded = 1;   // asynchronous: the next round (or finish) is ordered behind it on the stream
     return 0;
 }
@@ -972,11 +956,12 @@ extern "C" int h2_ipa_finish(uint64_t session, int repr, void *out_c_b) {
         else {
             IpaState S = ipa_state(q);
             fe *out = q->scal.as<fe>();
-            if (ref.b->curve == H2_CURVE_PALLAS) ipa_result_kernel<FqParams><<<1, 32, 0, s>>>(S, repr == H2_REPR_CANONICAL, out);
-            else ipa_result_kernel<FpParams><<<1, 32, 0, s>>>(S, repr == H2_REPR_CANONICAL, out);
-            g_launches.fetch_add(1, std::memory_order_relaxed);
-            cudaError_t e = cudaMemcpyAsync(out_c_b, out, 2 * sizeof(fe), cudaMemcpyDeviceToHost, s);
-            if (e != cudaSuccess) rc = fail(std::string("h2_ipa_finish: ") + cudaGetErrorString(e));
+            rc = by_curve(ref.b->curve, [&](auto, auto ps) {
+                ipa_result_kernel<decltype(ps)><<<1, 32, 0, s>>>(S, repr == H2_REPR_CANONICAL, out);
+                g_launches.fetch_add(1, std::memory_order_relaxed);
+                cudaError_t e = cudaMemcpyAsync(out_c_b, out, 2 * sizeof(fe), cudaMemcpyDeviceToHost, s);
+                return e != cudaSuccess ? fail(std::string("h2_ipa_finish: ") + cudaGetErrorString(e)) : 0;
+            });
         }
     }
     cudaError_t e = cudaStreamSynchronize(s);
@@ -1012,52 +997,25 @@ static int msm_registered_polys_impl(uint64_t bases_handle, const uint64_t *poly
     if (batch > 1 && !b->table.p) return fail("h2_msm_registered_polys: a batch needs a base set with a window table (H2_BASES_PRECOMPUTE)");
     const size_t total = n + (extra_scalars ? 1 : 0);
     if (total > b->n) return fail("h2_msm_registered_polys: more scalars than registered bases");
-    const int scalar_field = b->curve == H2_CURVE_PALLAS ? H2_FIELD_FQ : H2_FIELD_FP;
-    PolyArgs g("h2_msm_registered_polys", scalar_field);
-    std::vector<PolyBuf *> q;
-    if (g.in(polys, batch, n, "n", q)) return 1;
-    Context &X = g_ctx;
-    cudaStream_t s = X.stream;
-    if (scratch_acquire(s)) return 1;
-    if (X.scal_in.ensure(batch * total * sizeof(fe)) || X.result.ensure(batch * sizeof(jacobian)) || X.misc.ensure(batch * sizeof(fe) + 64)) return 1;
-    fe *d = X.scal_in.as<fe>();
-    if (extra_scalars) {   // the blinds: Montgomery form like the resident data
-        CU(cudaMemcpyAsync(X.misc.p, extra_scalars, batch * sizeof(fe), cudaMemcpyHostToDevice, s));
-        if (repr == H2_REPR_CANONICAL && convert_field(scalar_field, X.misc.as<fe>(), batch, 1, s)) return 1;
-    }
-    for (size_t j = 0; j < batch; j++) {
-        CU(cudaMemcpyAsync(d + j * total, q[j]->buf.p, n * sizeof(fe), cudaMemcpyDeviceToDevice, s));
-        if (extra_scalars) CU(cudaMemcpyAsync(d + j * total + n, X.misc.as<fe>() + j, sizeof(fe), cudaMemcpyDeviceToDevice, s));
-    }
-    uint32_t tc = 0, tmode = 0;
-    const affine *tbl = b->table.p ? fixed_table(b, &tc, &tmode) : nullptr;
-    const int canon = repr == H2_REPR_CANONICAL;
-    if (affine_out && X.ec_out.ensure(batch * sizeof(affine))) return 1;
-    for (int attempt = 0; attempt < 2; attempt++) {   // the fast pass first, the full one if its flags came back set
-        int rc;
-        X.fast_now = attempt == 0 && tbl && tmode == 1 && X.fast_on;
-        X.fast_retry = attempt == 1;
-        if (tbl) rc = msm_dispatch(b->curve, d, 1, tbl, total, tc, X.result.as<jacobian>(), affine_out ? 0 : canon, s, tmode, b->n,
-                                   nullptr, (uint32_t)batch);
-        else rc = msm_dispatch(b->curve, d, 1, b->buf.as<affine>(), total, 0, X.result.as<jacobian>(), affine_out ? 0 : canon, s);
-        X.fast_now = X.fast_retry = false;
-        if (rc) return rc;
-        if (affine_out) {
-            const uint32_t nb = blocks_for((batch + H2_NORM_CHUNK - 1) / H2_NORM_CHUNK, 64);
-            if (b->curve == H2_CURVE_PALLAS)
-                LAUNCH(normalize_kernel<FpParams>, nb, 64, 0, s, (const xyzz *)nullptr, X.result.as<jacobian>(), 0, X.ec_out.as<affine>(), canon, (uint64_t)batch);
-            else
-                LAUNCH(normalize_kernel<FqParams>, nb, 64, 0, s, (const xyzz *)nullptr, X.result.as<jacobian>(), 0, X.ec_out.as<affine>(), canon, (uint64_t)batch);
-            CU(cudaMemcpyAsync(out_xyz, X.ec_out.p, batch * sizeof(affine), cudaMemcpyDeviceToHost, s));
-        } else {
-            CU(cudaMemcpyAsync(out_xyz, X.result.p, batch * sizeof(jacobian), cudaMemcpyDeviceToHost, s));
-        }
-        if (fixed_pass_flags(s)) return 1;
-        if (scratch_release(s)) return 1;
-        CU(cudaStreamSynchronize(s));
-        if (fixed_pass_ok()) break;
+    return by_curve(b->curve, [&](auto, auto ps) {
+        PolyArgs g("h2_msm_registered_polys", decltype(ps)::ID);
+        std::vector<PolyBuf *> q;
+        if (g.in(polys, batch, n, "n", q)) return 1;
+        Context &X = g_ctx;
+        cudaStream_t s = X.stream;
         if (scratch_acquire(s)) return 1;
-    }
-    return 0;
+        if (X.scal_in.ensure(batch * total * sizeof(fe)) || X.result.ensure(batch * sizeof(jacobian)) || X.misc.ensure(batch * sizeof(fe) + 64)) return 1;
+        fe *d = X.scal_in.as<fe>();
+        if (extra_scalars) {   // the blinds: Montgomery form like the resident data
+            CU(cudaMemcpyAsync(X.misc.p, extra_scalars, batch * sizeof(fe), cudaMemcpyHostToDevice, s));
+            if (repr == H2_REPR_CANONICAL && convert_field(decltype(ps)::ID, X.misc.as<fe>(), batch, 1, s)) return 1;
+        }
+        for (size_t j = 0; j < batch; j++) {
+            CU(cudaMemcpyAsync(d + j * total, q[j]->buf.p, n * sizeof(fe), cudaMemcpyDeviceToDevice, s));
+            if (extra_scalars) CU(cudaMemcpyAsync(d + j * total + n, X.misc.as<fe>() + j, sizeof(fe), cudaMemcpyDeviceToDevice, s));
+        }
+        return msm_pass(b->curve, d, 1, pass_bases(b), total, (uint32_t)batch, X.result.as<jacobian>(), repr == H2_REPR_CANONICAL,
+                        {out_xyz, affine_out != 0});
+    });
 }
 

@@ -130,9 +130,6 @@ struct Context {
     uint64_t natural_max_buckets = 1ull << 14;   // fast passes with up to this many buckets take them in index order (MsmPlan::natural).  At k = 14
                                              // (one lane pair per bucket) 2^14 buckets are a single commit, 2^15 an IPA round's two sets and 2^16 four
                                              // batched commits: only a pass that is resident at once gains
-    bool fast_now = false;                   // ... the pass being issued is such a fast one
-    bool last_fast = false;                  // ... the most recent pass was
-    bool fast_retry = false;                 // the pass being issued re-runs, in full, a fast pass whose flags came back set
     uint32_t last_plan[8] = {};              // what the most recent MSM pass ran, recorded on the host (h2_test_last_msm_plan)
     bool have_plan = false;
     uint32_t *h_flags = nullptr;             // pinned host copy of the two flags
@@ -310,13 +307,13 @@ template <class F> static int by_field(int field, F &&f) {
     if (field == H2_FIELD_FQ) return f(FqParams{});
     return fail("unknown field id");
 }
-// what a fixed-base MSM over `b` runs on: the digit-multiples table (mode 2) when there is one, else the window table (mode 1)
-#define H2_FB_BITS_CTX 8u
-static inline const affine *fixed_table(const BaseSet *b, uint32_t *c, uint32_t *mode) {
-    if (b->dtable.p) { *c = H2_FB_BITS_CTX; *mode = 2; return b->dtable.as<affine>(); }
-    *c = b->c; *mode = 1;
-    return b->table.as<affine>();
+// f(FpParams{}, FqParams{}) for Pallas, f(FqParams{}, FpParams{}) for Vesta: (base field, scalar field); any other id fails
+template <class F> static int by_curve(int curve, F &&f) {
+    if (curve == H2_CURVE_PALLAS) return f(FpParams{}, FqParams{});
+    if (curve == H2_CURVE_VESTA) return f(FqParams{}, FpParams{});
+    return fail("unknown curve id");
 }
+static inline int check_curve(int curve) { return by_curve(curve, [](auto, auto) { return 0; }); }   // for entry points that check up front
 
 // ---- functions one TU defines and others call -------------------------------------------------------------------
 // Arrival of a one-shot MSM's inputs in k chunks: events on the copy stream -- bases / scalars of chunk j have landed.
@@ -338,9 +335,6 @@ struct BasesChunks {
     }
 };
 // capi_msm.cu
-int msm_dispatch(int curve, const fe *d_scalars, int scalars_mont, const affine *d_bases, size_t n, uint32_t c,
-                 jacobian *d_out, int out_canonical, cudaStream_t s, uint32_t fixed = 0, uint64_t stride = 0,
-                 const BasesChunks *bc = nullptr, uint32_t sets = 1);
 int convert_points(int curve, affine *d, size_t n, int to_mont, cudaStream_t s);
 // capi_ntt.cu
 int get_twiddles_any(int field, const fe &omega_mont, uint32_t log_n, cudaStream_t s, const fe **out);

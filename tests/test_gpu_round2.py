@@ -276,10 +276,29 @@ def test_fast_fixed_base_pass_and_its_fallback(eng):
     """Fixed-base passes run without their fallback kernels first and re-run in full when a device flag comes back set
     (h2_test_set_fast_fixed): ordinary polynomials take the fast pass, constant / 0-1 / all-equal columns overflow the sort bins
     and take the re-run -- same points either way, through every entry point that issues such a pass (single and batched commits,
-    commits of resident polynomials with batch_normalize, the IPA round loop), eager, captured and replayed."""
+    commits of resident polynomials with batch_normalize, the IPA round loop), eager, captured and replayed.  After each pass,
+    h2_test_last_msm_plan reports (fast, re-run): with fast passes on, a pass either ran fast and stood (1, 0) or re-ran in full
+    (0, 1); with them off, every pass runs in full once (0, 0)."""
     import halo2_b200 as h2
     from halo2_b200 import lib as L
     lib = L.init()
+
+    def fast_rerun():
+        out = (ctypes.c_uint32 * 8)()
+        L.check(lib.h2_test_last_msm_plan(out))
+        return out[6], out[7]
+
+    def check_plan(on, want=None):
+        got = fast_rerun()
+        if not on:
+            assert got == (0, 0), got
+        elif want is not None:
+            assert got == want, got
+        else:
+            assert got in ((1, 0), (0, 1)), got
+    # a single commit: the random column stands, the all-ones, 0/1 and all-(r - 1) columns re-run; the all-zero column's scalars
+    # may add no references at all
+    single_want = [(1, 0), None, (0, 1), (0, 1), (0, 1), None]
     curve, c, k = "vesta", pasta.VESTA, 9
     n = 1 << k
     g = cref.gen_points(curve, SEED + 700, n + 2)
@@ -297,16 +316,24 @@ def test_fast_fixed_base_pass_and_its_fallback(eng):
             L.check(lib.h2_test_set_fast_fixed(on))
             params = h2.Params(curve, k, g[:n], g[:n], g[n:n + 1], u=g[n + 1:n + 2])
             for rep in range(3):
-                assert [_affine(curve, params.commit(p, blind)) for p in polys] == wants, (on, rep)
+                for p, want, plan in zip(polys, wants, single_want):
+                    assert _affine(curve, params.commit(p, blind)) == want, (on, rep)
+                    check_plan(on, plan)
             assert [_affine(curve, m) for m in params.commit_many(polys, [blind] * len(polys))] == wants, on
+            check_plan(on, (0, 1))
             res = [h2.ResidentPoly(c.scalar, n, p) for p in polys]
             for rep in range(3):
                 aff = params.commit_resident_affine(res, [blind] * len(res))
                 assert [cref.bytes_to_affine(a) for a in aff] == wants, (on, rep)
+                check_plan(on, (0, 1))
+
+            def challenge(j, a, b):   # right after round j's pass; whether a round of a constant p' re-runs depends on the challenges
+                check_plan(on)
+                return ch[j]
             for name, pp in (("random", polys[0]), ("constant", polys[4])):
                 wl, wr, wc = ipa_want[name]
                 for rep in range(2):
-                    gl_, gr_, gc_ = params.ipa_rounds(pp, 3, 5, lambda j, a, b: ch[j], lr, lr)
+                    gl_, gr_, gc_ = params.ipa_rounds(pp, 3, 5, challenge, lr, lr)
                     assert gc_ == wc, (on, name)
                     for j in range(k):
                         assert (cref.jac_to_affine(curve, gl_[j]) == wl[j]).all() and (cref.jac_to_affine(curve, gr_[j]) == wr[j]).all(), (on, name, j)
