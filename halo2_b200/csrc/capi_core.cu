@@ -738,6 +738,10 @@ extern "C" int h2_test_field_op(int field, int op, const void *a, const void *b,
 }
 extern "C" int h2_test_curve_op(int curve, int op, const void *a_xy, const void *b_xy, size_t n, void *out_xy) {
     CtxLock lk;
+    if (op < 0 || op > 13)
+        return fail("h2_test_curve_op: op must be 0 (mixed and full add), 1 (double), 2 (scalar mul), 3 .. 6 (xyzz_add, xyzz_add_mixed, "
+                    "xyzz_double, xyzz_shift), 7 .. 10 (xyzz_add_quad, xyzz_add_mixed_quad, xyzz_add_mixed_pair, xyzz_shift_quad), "
+                    "11 / 12 (xyzz_addsub_q sum / difference) or 13 (xyzz_double_q)");
     if (require_ready()) return 1;
     Context &X = g_ctx;
     cudaStream_t s = X.stream;
@@ -747,7 +751,8 @@ extern "C" int h2_test_curve_op(int curve, int op, const void *a_xy, const void 
     CU(cudaMemcpyAsync(da, a_xy, n * sizeof(affine), cudaMemcpyHostToDevice, s));
     CU(cudaMemcpyAsync(db, b_xy, n * sizeof(affine), cudaMemcpyHostToDevice, s));
     if (by_curve(curve, [&](auto p, auto) {
-            LAUNCH(test_curve_kernel<decltype(p)>, blocks_for(n, 64), 64, 0, s, da, db, dout, (uint64_t)n, op);
+            if (op <= 6) LAUNCH(test_curve_kernel<decltype(p)>, blocks_for(n, 64), 64, 0, s, da, db, dout, (uint64_t)n, op);
+            else LAUNCH(test_curve_coop_kernel<decltype(p)>, blocks_for(n * (op == 9 ? 2 : 4), 64), 64, 0, s, da, db, dout, (uint64_t)n, op);   // whole warps
             return 0;
         }))
         return 1;

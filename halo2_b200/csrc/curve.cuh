@@ -49,6 +49,35 @@ template <class P> H2_HD xyzz xyzz_from_affine(const affine &p) {
     r.x = p.x; r.y = p.y; r.zz = fe_one<P>(); r.zzz = fe_one<P>();
     return r;
 }
+// The same point in another representation: (l^2 X, l^3 Y, l^2 ZZ, l^3 ZZZ) for l != 0; the identity stays (0, 0, 0, 0).
+// Only the group-law self-tests use it (h2_test_curve_op, tests/kernel_emul), to give every form operands with ZZ != 1.
+template <class P> H2_HD xyzz xyzz_rescale(const xyzz &p, const fe &l) {
+    if (xyzz_is_identity(p)) return xyzz_identity();
+    const fe l2 = fe_sqr<P>(l), l3 = fe_mul<P>(l2, l);
+    xyzz r;
+    r.x = fe_mul<P>(p.x, l2); r.y = fe_mul<P>(p.y, l3); r.zz = fe_mul<P>(p.zz, l2); r.zzz = fe_mul<P>(p.zzz, l3);
+    return r;
+}
+H2_HD uint64_t splitmix64(uint64_t x) {
+    x += 0x9E3779B97F4A7C15ULL;
+    x = (x ^ (x >> 30)) * 0xBF58476D1CE4E5B9ULL;
+    x = (x ^ (x >> 27)) * 0x94D049BB133111EBULL;
+    return x ^ (x >> 31);
+}
+// The rescaling factor of operand `which` of self-test element i: 1 for i % 4 == 0 (the ZZ = 1 case stays covered), otherwise
+// a non-zero field element below 2^254 mixed from (i, which) -- the device kernel and its host emulation draw the same one.
+template <class P> H2_HD fe test_lambda(uint64_t i, uint32_t which) {
+    if (i % 4 == 0) return fe_one<P>();
+    fe l;
+    uint64_t s = splitmix64(i * 2 + which);
+    for (int j = 0; j < 8; j += 2) {
+        s = splitmix64(s);
+        l.v[j] = (uint32_t)s; l.v[j + 1] = (uint32_t)(s >> 32);
+    }
+    l.v[7] &= 0x3fffffffu;
+    if (fe_is_zero(l)) l = fe_one<P>();
+    return l;
+}
 template <class P> H2_HD void xyzz_neg(xyzz &p) { p.y = fe_neg<P>(p.y); }
 template <class P> H2_HD affine affine_neg(const affine &p) {
     affine r; r.x = p.x; r.y = fe_neg<P>(p.y);   // -(0,0) = (0,0): fe_neg(0) = 0

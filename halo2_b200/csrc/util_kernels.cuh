@@ -3,6 +3,7 @@
 #pragma once
 #include "ctx.cuh"
 #include "msm.cuh"   // ld_affine / st_affine, xyzz helpers
+#include "ecfft.cuh" // the EC-FFT's warp-uniform group law (self-test kernel)
 
 // ------------------------------------------------------------------------------------------------
 // small kernels: conversions, generators, self-tests
@@ -21,12 +22,6 @@ template <class P> __global__ void convert_points_kernel(affine *a, uint64_t n, 
     if (to_mont) { p.x = fe_to_mont<P>(p.x); p.y = fe_to_mont<P>(p.y); }
     else { p.x = fe_from_mont<P>(p.x); p.y = fe_from_mont<P>(p.y); }
     st_affine(a + i, p);
-}
-__device__ __forceinline__ uint64_t splitmix64(uint64_t x) {
-    x += 0x9E3779B97F4A7C15ULL;
-    x = (x ^ (x >> 30)) * 0xBF58476D1CE4E5B9ULL;
-    x = (x ^ (x >> 27)) * 0x94D049BB133111EBULL;
-    return x ^ (x >> 31);
 }
 template <class P> __device__ affine xyzz_to_affine_dev(const xyzz &p) {
     affine r;
@@ -64,33 +59,93 @@ template <class P> __global__ void test_field_kernel(const fe *a, const fe *b, f
     }
     fe_store(out + i, fe_from_mont<P>(r));
 }
+// Group-law self-tests (h2_test_curve_op; the ops are listed in include/halo2_b200.h).  Points arrive and leave as canonical
+// affine points.  Ops 3 .. 13 rescale their XYZZ operands by test_lambda, so the formulas see ZZ != 1 (except on every 4th
+// element); the result is compared as an affine point, which does not depend on the representation.
+template <class P> __device__ void mont_point(affine &p) {
+    if (!affine_is_identity(p)) { p.x = fe_to_mont<P>(p.x); p.y = fe_to_mont<P>(p.y); }
+}
+template <class P> __device__ void st_canonical(affine *out, affine o) {
+    o.x = fe_from_mont<P>(o.x); o.y = fe_from_mont<P>(o.y);
+    st_affine(out, o);
+}
+template <class P> __device__ affine poison_point() {   // (1, 0) canonical: not on the curve
+    affine o; o.x = fe_one<P>(); o.y = fe_zero();
+    return o;
+}
 template <class P> __global__ void __launch_bounds__(64) test_curve_kernel(const affine *a, const affine *b, affine *out, uint64_t n, int op) {
     uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
     affine pa = ld_affine(a + i), pb = ld_affine(b + i);
-    if (!affine_is_identity(pa)) { pa.x = fe_to_mont<P>(pa.x); pa.y = fe_to_mont<P>(pa.y); }
+    mont_point<P>(pa);
     xyzz r = xyzz_from_affine<P>(pa);
     if (op == 0) {
-        if (!affine_is_identity(pb)) { pb.x = fe_to_mont<P>(pb.x); pb.y = fe_to_mont<P>(pb.y); }
+        mont_point<P>(pb);
         xyzz t = r;
         xyzz_add_mixed<P>(r, pb);                         // mixed path
         xyzz full = xyzz_from_affine<P>(pb);
         xyzz_add<P>(t, full);                             // full-add path must agree
         affine r1 = xyzz_to_affine_dev<P>(r), r2 = xyzz_to_affine_dev<P>(t);
-        if (!(fe_eq(r1.x, r2.x) && fe_eq(r1.y, r2.y))) { r1.x = fe_one<P>(); r1.y = fe_zero(); }   // poison
-        r1.x = fe_from_mont<P>(r1.x); r1.y = fe_from_mont<P>(r1.y);
-        st_affine(out + i, r1);
+        if (!(fe_eq(r1.x, r2.x) && fe_eq(r1.y, r2.y))) r1 = poison_point<P>();
+        st_canonical<P>(out + i, r1);
         return;
     } else if (op == 1) {
         xyzz_double<P>(r);
-    } else {
+    } else if (op == 2) {
         uint32_t k[8];
         for (int j = 0; j < 8; j++) k[j] = pb.x.v[j];
         r = xyzz_scalar_mul<P>(pa, k);
+    } else {                                              // 3 .. 6: the serial forms on rescaled operands
+        r = xyzz_rescale<P>(r, test_lambda<P>(i, 0));
+        if (op == 6) xyzz_shift<P>(r, pb.x.v[0]);         // k = the low 32 bits of b.x
+        else if (op == 5) xyzz_double<P>(r);
+        else {
+            mont_point<P>(pb);
+            if (op == 4) xyzz_add_mixed<P>(r, pb);
+            else xyzz_add<P>(r, xyzz_rescale<P>(xyzz_from_affine<P>(pb), test_lambda<P>(i, 1)));
+        }
     }
-    affine o = xyzz_to_affine_dev<P>(r);
-    o.x = fe_from_mont<P>(o.x); o.y = fe_from_mont<P>(o.y);
-    st_affine(out + i, o);
+    st_canonical<P>(out + i, xyzz_to_affine_dev<P>(r));
+}
+// Ops 7 .. 13: the lane-cooperative forms, `lanes` consecutive lanes per element (2 for the pair of op 9, 4 otherwise).  The
+// launch is whole warps and nothing returns before the group law: lanes past n hold identity operands and still reach every
+// shuffle, as xyzz_addsub_q / xyzz_double_q require of the full warp.  Every lane of a group computes the result; if any lane's
+// XYZZ words differ from the group's first lane the element gets the poison point -- the forms rely on the lanes staying equal.
+template <class P> __global__ void __launch_bounds__(64) test_curve_coop_kernel(const affine *a, const affine *b, affine *out, uint64_t n, int op) {
+    const uint32_t lanes = op == 9 ? 2u : 4u;
+    const uint64_t i = ((uint64_t)blockIdx.x * blockDim.x + threadIdx.x) / lanes;
+    affine pa, pb;
+    pa.x = pa.y = pb.x = pb.y = fe_zero();
+    if (i < n) { pa = ld_affine(a + i); pb = ld_affine(b + i); }
+    mont_point<P>(pa);
+    const uint32_t k = pb.x.v[0];                         // op 10: the shift count, the low 32 bits of b.x
+    if (op != 10) mont_point<P>(pb);
+    xyzz r = xyzz_rescale<P>(xyzz_from_affine<P>(pa), test_lambda<P>(i, 0));
+    const xyzz q = xyzz_rescale<P>(xyzz_from_affine<P>(pb), test_lambda<P>(i, 1));
+    switch (op) {
+    case 7: xyzz_add_quad<P>(r, q); break;
+    case 8: xyzz_add_mixed_quad<P>(r, pb); break;
+    case 9: xyzz_add_mixed_pair<P>(r, pb); break;
+    case 10: xyzz_shift_quad<P>(r, k); break;
+    case 11: case 12: {
+        xyzz sum, diff;
+        xyzz_addsub_q<P, true>(r, q, sum, diff);
+        r = op == 11 ? sum : diff;
+        break;
+    }
+    default: xyzz_double_q<P>(r); break;
+    }
+    uint32_t differ = 0;
+#pragma unroll
+    for (int j = 0; j < 8; j++) {
+        differ |= r.x.v[j] ^ __shfl_sync(0xffffffffu, r.x.v[j], 0, lanes);
+        differ |= r.y.v[j] ^ __shfl_sync(0xffffffffu, r.y.v[j], 0, lanes);
+        differ |= r.zz.v[j] ^ __shfl_sync(0xffffffffu, r.zz.v[j], 0, lanes);
+        differ |= r.zzz.v[j] ^ __shfl_sync(0xffffffffu, r.zzz.v[j], 0, lanes);
+    }
+    for (uint32_t o = 1; o < lanes; o <<= 1) differ |= __shfl_xor_sync(0xffffffffu, differ, o, lanes);
+    if (i >= n || (threadIdx.x & (lanes - 1))) return;
+    st_canonical<P>(out + i, differ ? poison_point<P>() : xyzz_to_affine_dev<P>(r));
 }
 // throughput microbenchmark: 4 independent dependent-chains per thread
 template <class P, bool SQR> __global__ void bench_mul_kernel(fe *io, uint32_t iters) {

@@ -449,8 +449,19 @@ int h2_test_set_accum_ways(uint32_t ways);
  * host buffers.  op: 0 add, 1 sub, 2 mul, 3 inverse(a) by the Fermat ladder,
  * 4 square(a), 5 inverse(a) by division steps (fe_inv_gcd, what the kernels use). */
 int h2_test_field_op(int field, int op, const void *a, const void *b, size_t n, void *out);
-/* out[i] = affine(a[i] + b[i]) (op 0), affine(2 a[i]) (op 1), affine(k[i] * a[i]) with b = 32-byte
- * scalars padded to 64 B (op 2); canonical affine, host buffers. */
+/* Self-test of the device group law; canonical affine points in and out, identity = (0, 0), host buffers.
+ *   op 0  a[i] + b[i] by the mixed and the full addition (the poison point (1, 0) if they disagree)
+ *   op 1  2 a[i]            op 2  k[i] * a[i], b = 32-byte scalars padded to 64 B
+ * Ops 3 .. 13 run one form each on XYZZ operands rescaled by a per-element factor l (X = l^2 x, Y = l^3 y, ZZ = l^2,
+ * ZZZ = l^3; l = 1 for i % 4 == 0), the two operands of a full addition with independent factors:
+ *   op 3  xyzz_add            a[i] + b[i]     op 4  xyzz_add_mixed   a[i] + b[i] (b affine)
+ *   op 5  xyzz_double         2 a[i]          op 6  xyzz_shift       2^k a[i], k = the low 32 bits of b[i].x
+ * Ops 7 .. 13 are the lane-cooperative forms, 4 lanes per element (op 9: 2); the result is the poison point if the lanes
+ * of an element end with different values:
+ *   op 7  xyzz_add_quad       a[i] + b[i]     op 8  xyzz_add_mixed_quad   a[i] + b[i] (b affine)
+ *   op 9  xyzz_add_mixed_pair a[i] + b[i]     op 10 xyzz_shift_quad       2^k a[i], k as in op 6
+ *   op 11 / 12  xyzz_addsub_q<P, true>   a[i] + b[i] / a[i] - b[i]        op 13 xyzz_double_q   2 a[i]
+ * Any other op fails. */
 int h2_test_curve_op(int curve, int op, const void *a_xy, const void *b_xy, size_t n, void *out_xy);
 /* Times `iters` dependent field multiplications per thread over `threads` threads; returns
  * elapsed milliseconds in *ms (microbenchmark for the roofline discussion in DESIGN.md). */

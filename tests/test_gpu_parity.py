@@ -728,8 +728,9 @@ def test_small_multiexp_and_batch_normalize(eng):
 
 def test_accum_ways(eng):
     """Small MSMs accumulate with 1, 2 or 4 quads of lanes per work item (msm_accum0_multi_kernel) or one pair of lanes
-    (ways = 0, msm_accum0_pair_kernel): same points -- incl. a 0/1/2 column and a constant column, whose buckets are full of
-    repeated points (P + P in the pair / quad formulas)."""
+    (ways = 0, msm_accum0_pair_kernel): same points -- incl. a 0/1/2 column and a constant column, which crowd the references
+    into a few buckets.  The window-table entries of distinct generators are distinct, so those buckets still sum distinct
+    points; the P + P / P + (-P) branches of the pair and quad formulas are run by tests/test_gpu_group_law.py."""
     from halo2_b200 import lib as L
     lib = L.init()
     curve, c, k = "vesta", pasta.VESTA, 10

@@ -45,29 +45,45 @@ def test_emul_field(emu, field):
         assert _fop(emu, field, 7, a) == (pow(a, m - 2, m) if a else 0), hex(a)
 
 
-def _cop(emu, curve, op, a, b):
+def _cop(emu, curve, op, a, b, i=0):
     out = np.zeros(64, dtype=np.uint8)
-    emu.emu_curve_op(cref.CURVE_ID[curve], op, cref._p(np.ascontiguousarray(a)), cref._p(np.ascontiguousarray(b)), cref._p(out))
+    emu.emu_curve_op(cref.CURVE_ID[curve], op, cref._p(np.ascontiguousarray(a)), cref._p(np.ascontiguousarray(b)), ctypes.c_uint64(i),
+                     cref._p(out))
     return cref.bytes_to_affine(out)
 
 
 @pytest.mark.parametrize("curve", ["pallas", "vesta"])
 def test_emul_curve(emu, curve):
+    """The serial XYZZ group law against the oracle: on affine operands (ZZ = 1, ops 0 - 2) and, as h2_test_curve_op's ops 3 - 6
+    run it on the device, on operands rescaled to ZZ != 1 (element index i % 4 != 0; i % 4 == 0 keeps ZZ = 1)."""
     c = pasta.CURVES[curve]
     pts = pasta.gen_points(c, 5, 8)
     g = pasta.generator(c)
+    two = lambda p: pasta.to_affine(c, pasta.jac_double(c, pasta.to_jac(p)))   # noqa: E731
     cases = [(pts[0], pts[1]), (pts[2], pts[2]), (pts[3], (pts[3][0], c.p - pts[3][1])), (None, pts[4]), (pts[5], None),
-             (None, None), (g, g)]
-    for a, b in cases:
+             (None, None), (g, g), (g, (g[0], c.p - g[1])), (pts[6], two(pts[6])), (two(pts[6]), pts[6])]
+    for j, (a, b) in enumerate(cases):
         A, B = cref.affines_to_bytes([a])[0], cref.affines_to_bytes([b])[0]
         want = pasta.to_affine(c, pasta.jac_add(c, pasta.to_jac(a), pasta.to_jac(b)))
+        dbl = pasta.to_affine(c, pasta.jac_double(c, pasta.to_jac(a)))
         assert _cop(emu, curve, 0, A, B) == want
         assert _cop(emu, curve, 1, A, B) == want
-        assert _cop(emu, curve, 2, A, B) == pasta.to_affine(c, pasta.jac_double(c, pasta.to_jac(a)))
+        assert _cop(emu, curve, 2, A, B) == dbl
+        for i in (4 * j, 4 * j + 1, 4 * j + 2, 4 * j + 7):
+            assert _cop(emu, curve, 3, A, B, i) == want, (j, i)
+            assert _cop(emu, curve, 4, A, B, i) == want, (j, i)
+            assert _cop(emu, curve, 5, A, B, i) == dbl, (j, i)
+    for j, k in enumerate(list(range(0, 21)) + [63, 64, 255, 256, 270]):
+        for a in (pts[7], g, None):
+            kb = np.zeros(64, dtype=np.uint8)
+            kb[:4] = np.frombuffer(int(k).to_bytes(4, "little"), dtype=np.uint8)
+            want = pasta.to_affine(c, pasta.scalar_mul(c, pow(2, k, c.r), a))
+            for i in (4 * j, 4 * j + 3):
+                assert _cop(emu, curve, 6, cref.affines_to_bytes([a])[0], kb, i) == want, (k, i)
     for k in pasta.gen_scalars(c.scalar, 3, 3) + [0, 1, c.r - 1]:
         kb = np.zeros(64, dtype=np.uint8)
         kb[:32] = cref._fe(k)
-        assert _cop(emu, curve, 4, cref.affines_to_bytes([pts[7]])[0], kb) == pasta.to_affine(c, pasta.scalar_mul(c, k, pts[7]))
+        assert _cop(emu, curve, 8, cref.affines_to_bytes([pts[7]])[0], kb) == pasta.to_affine(c, pasta.scalar_mul(c, k, pts[7]))
 
 
 def _ntt(emu, f, mode, a, in_log, log_n, omega, zeta=None, div=None, out_len=None, nthr=64):
