@@ -157,6 +157,26 @@ PolyArgs::~PolyArgs() {
     std::lock_guard<std::mutex> lk(g_reg_mu);
     for (PolyBuf *p : held) user_drop(p->users);
 }
+int HostArgs::check(std::initializer_list<Need> needs) const {
+    if (!canon() && !mont()) return fail(std::string(who) + ": unknown repr");
+    for (const Need &n : needs)
+        if (n.required && !n.p) return fail(std::string(who) + ": null " + n.name);
+    return 0;
+}
+int HostArgs::up(int field, fe *d, const void *h, size_t n, cudaStream_t s) const {
+    if (upload_async(d, h, n * sizeof(fe), s)) return 1;
+    return to_mont(field, d, n, s);
+}
+int HostArgs::to_mont(int field, fe *d, size_t n, cudaStream_t s) const { return canon() ? convert_field(field, d, n, 1, s) : 0; }
+int HostArgs::from_mont(int field, fe *d, size_t n, cudaStream_t s) const { return canon() ? convert_field(field, d, n, 0, s) : 0; }
+int HostArgs::down(int field, void *h, const fe *d, size_t n, cudaStream_t s) const {
+    if (mont()) return download_sync(h, d, n * sizeof(fe), s);
+    Context &X = g_ctx;
+    if (scratch_acquire(s) || X.ntt_out.ensure(n * sizeof(fe))) return 1;
+    CU(cudaMemcpyAsync(X.ntt_out.p, d, n * sizeof(fe), cudaMemcpyDeviceToDevice, s));
+    if (from_mont(field, X.ntt_out.as<fe>(), n, s) || download_sync(h, X.ntt_out.p, n * sizeof(fe), s)) return 1;
+    return scratch_release(s);
+}
 // From any thread and any context: the caller holds no Context mutex.
 int shared_poly_free(uint64_t h) {
     std::unique_lock<std::mutex> lk(g_reg_mu);

@@ -32,11 +32,11 @@ static int ecfft_stages(xyzz *work, uint32_t log_n, const fe &omega_mont, const 
 // mode 0: Jacobian in -> Jacobian out (h2_ec_fft); mode 1: affine in -> scaled, normalised affine out (h2_params_lagrange)
 // `in` == nullptr: the input is already in X.ec_io on the device (h2_params_new), scratch acquired by the caller
 template <class P, class PS>
-static int ecfft_host(int mode, const void *in, uint32_t log_n, const void *omega, const void *scale, int repr, void *out) {
+static int ecfft_host(int mode, const void *in, uint32_t log_n, const void *omega, const void *scale, const HostArgs &h, void *out) {
     Context &X = g_ctx;
     cudaStream_t s = X.stream;
     const uint64_t n = 1ull << log_n;
-    const int canon = repr == H2_REPR_CANONICAL;
+    const int canon = h.canon();
     const size_t in_sz = mode == 0 ? sizeof(jacobian) : sizeof(affine);
     if (in) {
         if (scratch_acquire(s)) return 1;
@@ -58,7 +58,7 @@ static int ecfft_host(int mode, const void *in, uint32_t log_n, const void *omeg
         if (!canon) sc = fe_from_mont<PS>(sc);
         scp = &sc;
     }
-    if (ecfft_stages<P, PS>(work, log_n, host_to_mont<PS>(omega, repr), scp, s)) return 1;
+    if (ecfft_stages<P, PS>(work, log_n, h.elem<PS>(omega), scp, s)) return 1;
     if (mode == 0) {
         auto k = ecfft_store_jac_kernel<P, PS>;
         LAUNCH(k, blocks_for(n, 128), 128, 0, s, work, X.ec_io.as<jacobian>(), canon, n);
@@ -72,18 +72,20 @@ static int ecfft_host(int mode, const void *in, uint32_t log_n, const void *omeg
     CU(cudaStreamSynchronize(s));
     return 0;
 }
-static int ecfft_host_dispatch(int curve, int mode, const void *in, uint32_t log_n, const void *omega, const void *scale, int repr, void *out) {
+static int ecfft_host_dispatch(int curve, int mode, const void *in, uint32_t log_n, const void *omega, const void *scale, const HostArgs &h,
+                               std::initializer_list<HostArgs::Need> needs, void *out) {
     CtxLock lk;
-    if (require_ready()) return 1;
+    if (require_ready() || h.check(needs)) return 1;
     if (log_n > 26) return fail("ec_fft: log_n > 26 not supported");
-    return by_curve(curve, [&](auto p, auto ps) { return ecfft_host<decltype(p), decltype(ps)>(mode, in, log_n, omega, scale, repr, out); });
+    return by_curve(curve, [&](auto p, auto ps) { return ecfft_host<decltype(p), decltype(ps)>(mode, in, log_n, omega, scale, h, out); });
 }
 extern "C" int h2_ec_fft(int curve, void *points_xyz, const void *omega, uint32_t log_n, const void *scale, int repr) {
-    return ecfft_host_dispatch(curve, 0, points_xyz, log_n, omega, scale, repr, points_xyz);
+    return ecfft_host_dispatch(curve, 0, points_xyz, log_n, omega, scale, {"h2_ec_fft", repr}, {{points_xyz, "points_xyz"}, {omega, "omega"}}, points_xyz);
 }
+// minv is required here (poly/commitment.rs:83)
 extern "C" int h2_params_lagrange(int curve, const void *g_xy, uint32_t k, const void *omega_inv, const void *minv, int repr, void *out_xy) {
-    if (!minv) return fail("h2_params_lagrange: minv is required (poly/commitment.rs:83)");
-    return ecfft_host_dispatch(curve, 1, g_xy, k, omega_inv, minv, repr, out_xy);
+    return ecfft_host_dispatch(curve, 1, g_xy, k, omega_inv, minv, {"h2_params_lagrange", repr},
+                               {{g_xy, "g_xy"}, {omega_inv, "omega_inv"}, {minv, "minv"}, {out_xy, "out_g_lagrange_xy"}}, out_xy);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -92,7 +94,7 @@ extern "C" int h2_params_lagrange(int curve, const void *g_xy, uint32_t k, const
 // n messages -> n affine points in X.ec_io (device, `repr`); scratch held by the caller.  msgs == nullptr: generator
 // messages 0 || (first + i) as u32 LE
 template <class P>
-static int h2c_issue(const H2cConst &K, const void *msgs, size_t msg_len, uint64_t first, size_t n, int repr, affine *d_out, cudaStream_t s) {
+static int h2c_issue(const H2cConst &K, const void *msgs, size_t msg_len, uint64_t first, size_t n, const HostArgs &h, affine *d_out, cudaStream_t s) {
     Context &X = g_ctx;
     const uint8_t *d_msgs = nullptr;
     if (msgs && n * msg_len) {
@@ -100,19 +102,19 @@ static int h2c_issue(const H2cConst &K, const void *msgs, size_t msg_len, uint64
         CU(cudaMemcpyAsync(X.misc.p, msgs, n * msg_len, cudaMemcpyHostToDevice, s));
         d_msgs = X.misc.as<uint8_t>();
     }
-    LAUNCH(h2c_kernel<P>, blocks_for(n, 64), 64, 0, s, d_msgs, (uint32_t)msg_len, msgs ? 0 : 1, first, K, d_out, repr == H2_REPR_MONTGOMERY ? 1 : 0,
+    LAUNCH(h2c_kernel<P>, blocks_for(n, 64), 64, 0, s, d_msgs, (uint32_t)msg_len, msgs ? 0 : 1, first, K, d_out, h.mont() ? 1 : 0,
            (uint64_t)n);
     return 0;
 }
 template <class P>
-static int hash_to_curve_host(const char *domain_prefix, const void *msgs, size_t msg_len, size_t n, int repr, void *out_xy) {
+static int hash_to_curve_host(const char *domain_prefix, const void *msgs, size_t msg_len, size_t n, const HostArgs &h, void *out_xy) {
     Context &X = g_ctx;
     cudaStream_t s = X.stream;
     const H2cConst K = make_h2c_const<P>(domain_prefix);
     if (!K.ok) return fail("h2_hash_to_curve: domain prefix too long (DST must be < 256 bytes)");
     if (scratch_acquire(s)) return 1;
     if (X.ec_io.ensure(n * sizeof(affine))) return 1;
-    if (h2c_issue<P>(K, msgs, msg_len, 0, n, repr, X.ec_io.as<affine>(), s)) return 1;
+    if (h2c_issue<P>(K, msgs, msg_len, 0, n, h, X.ec_io.as<affine>(), s)) return 1;
     CU(cudaMemcpyAsync(out_xy, X.ec_io.p, n * sizeof(affine), cudaMemcpyDeviceToHost, s));
     if (scratch_release(s)) return 1;
     CU(cudaStreamSynchronize(s));
@@ -120,19 +122,19 @@ static int hash_to_curve_host(const char *domain_prefix, const void *msgs, size_
 }
 extern "C" int h2_hash_to_curve(int curve, const char *domain_prefix, const void *messages, size_t msg_len, size_t n, int repr, void *out_xy) {
     CtxLock lk;
-    if (require_ready()) return 1;
-    if (check_curve(curve)) return 1;
+    const HostArgs h("h2_hash_to_curve", repr);
+    if (require_ready() || check_curve(curve) || h.check({{out_xy, "out_xy", n != 0}})) return 1;
     if (!domain_prefix) return fail("h2_hash_to_curve: domain_prefix is NULL");
     if (msg_len && !messages && n) return fail("h2_hash_to_curve: messages is NULL");
     if (msg_len >= (1ull << 31) || n >= (1ull << 32)) return fail("h2_hash_to_curve: message or batch too large");
     if (n == 0) return 0;
     static const uint8_t empty = 0;
     const void *m = messages ? messages : &empty;      // msg_len == 0: n hashes of the empty message
-    return by_curve(curve, [&](auto p, auto) { return hash_to_curve_host<decltype(p)>(domain_prefix, m, msg_len, n, repr, out_xy); });
+    return by_curve(curve, [&](auto p, auto) { return hash_to_curve_host<decltype(p)>(domain_prefix, m, msg_len, n, h, out_xy); });
 }
 // Params::new: g[i] = H(0 || i), w = H(1), u = H(2) with H = hash_to_curve("Halo2-Parameters"), then g_lagrange from g
 template <class P, class PS>
-static int params_new_host(uint32_t k, int repr, void *g_xy, void *gl_xy, void *w_xy, void *u_xy) {
+static int params_new_host(uint32_t k, const HostArgs &h, void *g_xy, void *gl_xy, void *w_xy, void *u_xy) {
     Context &X = g_ctx;
     cudaStream_t s = X.stream;
     const uint64_t n = 1ull << k;
@@ -145,35 +147,35 @@ static int params_new_host(uint32_t k, int repr, void *g_xy, void *gl_xy, void *
     const fe two_inv = fe_inv<PS>(fe_dbl<PS>(fe_one<PS>()));
     fe minv = fe_one<PS>();
     for (uint32_t i = 0; i < k; i++) minv = fe_mul<PS>(minv, two_inv);
-    if (repr == H2_REPR_CANONICAL) { alpha_inv = fe_from_mont<PS>(alpha_inv); minv = fe_from_mont<PS>(minv); }
+    if (h.canon()) { alpha_inv = fe_from_mont<PS>(alpha_inv); minv = fe_from_mont<PS>(minv); }   // ecfft_host reads them in repr
     if (scratch_acquire(s)) return 1;
     if (X.ec_io.ensure((n + 2) * sizeof(jacobian))) return 1;
     affine *d_g = X.ec_io.as<affine>();
     static const uint8_t wu[2] = {1, 2};
-    if (h2c_issue<P>(K, wu, 1, 0, 2, repr, d_g + n, s)) return 1;       // w, u behind g
-    if (h2c_issue<P>(K, nullptr, 0, 0, n, repr, d_g, s)) return 1;
+    if (h2c_issue<P>(K, wu, 1, 0, 2, h, d_g + n, s)) return 1;       // w, u behind g
+    if (h2c_issue<P>(K, nullptr, 0, 0, n, h, d_g, s)) return 1;
     CU(cudaMemcpyAsync(g_xy, d_g, n * sizeof(affine), cudaMemcpyDeviceToHost, s));
     CU(cudaMemcpyAsync(w_xy, d_g + n, sizeof(affine), cudaMemcpyDeviceToHost, s));
     CU(cudaMemcpyAsync(u_xy, d_g + n + 1, sizeof(affine), cudaMemcpyDeviceToHost, s));
-    return ecfft_host<P, PS>(1, nullptr, k, alpha_inv.v, minv.v, repr, gl_xy);   // releases the scratch, synchronises
+    return ecfft_host<P, PS>(1, nullptr, k, alpha_inv.v, minv.v, h, gl_xy);   // releases the scratch, synchronises
 }
 extern "C" int h2_params_new(int curve, uint32_t k, int repr, void *out_g_xy, void *out_g_lagrange_xy, void *out_w_xy, void *out_u_xy) {
     CtxLock lk;
-    if (require_ready()) return 1;
+    const HostArgs h("h2_params_new", repr);
+    if (require_ready() || h.check({{out_g_xy, "out_g_xy"}, {out_g_lagrange_xy, "out_g_lagrange_xy"}, {out_w_xy, "out_w_xy"}, {out_u_xy, "out_u_xy"}})) return 1;
     if (k > 26) return fail("h2_params_new: k > 26 not supported");
-    if (!out_g_xy || !out_g_lagrange_xy || !out_w_xy || !out_u_xy) return fail("h2_params_new: NULL output");
     return by_curve(curve, [&](auto p, auto ps) {
-        return params_new_host<decltype(p), decltype(ps)>(k, repr, out_g_xy, out_g_lagrange_xy, out_w_xy, out_u_xy);
+        return params_new_host<decltype(p), decltype(ps)>(k, h, out_g_xy, out_g_lagrange_xy, out_w_xy, out_u_xy);
     });
 }
 extern "C" int h2_batch_normalize(int curve, const void *points_xyz, size_t n, int repr, void *out_xy) {
     CtxLock lk;
-    if (require_ready()) return 1;
-    if (check_curve(curve)) return 1;
+    const HostArgs h("h2_batch_normalize", repr);
+    if (require_ready() || check_curve(curve) || h.check({{points_xyz, "points_xyz", n != 0}, {out_xy, "out_xy", n != 0}})) return 1;
     if (n == 0) return 0;
     Context &X = g_ctx;
     cudaStream_t s = X.stream;
-    const int canon = repr == H2_REPR_CANONICAL;
+    const int canon = h.canon();
     if (scratch_acquire(s)) return 1;
     if (X.ec_io.ensure(n * sizeof(jacobian)) || X.ec_out.ensure(n * sizeof(affine))) return 1;
     CU(cudaMemcpyAsync(X.ec_io.p, points_xyz, n * sizeof(jacobian), cudaMemcpyHostToDevice, s));
@@ -193,10 +195,10 @@ extern "C" int h2_batch_normalize(int curve, const void *points_xyz, size_t n, i
 // point (de)compression (codec.cuh): C::to_bytes / C::from_bytes, the encoding of Params::{write, read} and of every
 // point in a proof transcript
 // ------------------------------------------------------------------------------------------------
-template <class P> static int points_codec(int decompress, const void *in, size_t n, int repr, void *out) {
+template <class P> static int points_codec(int decompress, const void *in, size_t n, const HostArgs &h, void *out) {
     Context &X = g_ctx;
     cudaStream_t s = X.stream;
-    const int mont = repr == H2_REPR_MONTGOMERY;
+    const int mont = h.mont();
     if (scratch_acquire(s)) return 1;
     if (X.ec_io.ensure(n * sizeof(affine)) || X.ec_out.ensure(n * sizeof(affine)) || X.misc.ensure(64)) return 1;
     uint32_t bad = 0xffffffffu;
@@ -217,18 +219,19 @@ template <class P> static int points_codec(int decompress, const void *in, size_
     if (bad != 0xffffffffu) return fail("h2_points_decompress: invalid point encoding at index " + std::to_string(bad));
     return 0;
 }
-static int points_codec_dispatch(int curve, int decompress, const void *in, size_t n, int repr, void *out) {
+static int points_codec_dispatch(int curve, int decompress, const void *in, size_t n, const HostArgs &h, std::initializer_list<HostArgs::Need> needs,
+                                 void *out) {
     CtxLock lk;
-    if (require_ready()) return 1;
-    if (check_curve(curve)) return 1;
+    if (require_ready() || check_curve(curve) || h.check(needs)) return 1;
     if (n >= (1ull << 32)) return fail("points codec: n >= 2^32");
     if (n == 0) return 0;
-    return by_curve(curve, [&](auto p, auto) { return points_codec<decltype(p)>(decompress, in, n, repr, out); });
+    return by_curve(curve, [&](auto p, auto) { return points_codec<decltype(p)>(decompress, in, n, h, out); });
 }
 extern "C" int h2_points_compress(int curve, const void *points_xy, size_t n, int repr, void *out_bytes) {
-    return points_codec_dispatch(curve, 0, points_xy, n, repr, out_bytes);
+    return points_codec_dispatch(curve, 0, points_xy, n, {"h2_points_compress", repr}, {{points_xy, "points_xy", n != 0}, {out_bytes, "out_bytes", n != 0}},
+                                 out_bytes);
 }
 extern "C" int h2_points_decompress(int curve, const void *bytes, size_t n, int repr, void *out_xy) {
-    return points_codec_dispatch(curve, 1, bytes, n, repr, out_xy);
+    return points_codec_dispatch(curve, 1, bytes, n, {"h2_points_decompress", repr}, {{bytes, "bytes", n != 0}, {out_xy, "out_xy", n != 0}}, out_xy);
 }
 

@@ -451,10 +451,11 @@ int convert_points(int curve, affine *d, size_t n, int to_mont, cudaStream_t s) 
 extern "C" int h2_msm_dev(int curve, const void *d_scalars, int scalars_repr, const void *d_bases, size_t n, uint32_t window_bits,
                           void *d_out_xyz, void *stream) {
     CtxLock lk;
-    if (require_ready()) return 1;
+    const HostArgs h("h2_msm_dev", scalars_repr);
+    if (require_ready() || h.check()) return 1;
     cudaStream_t s = (cudaStream_t)stream;
     if (scratch_acquire(s)) return 1;
-    int rc = msm_dispatch(curve, (const fe *)d_scalars, scalars_repr == H2_REPR_MONTGOMERY, PassBases{(const affine *)d_bases, window_bits}, n,
+    int rc = msm_dispatch(curve, (const fe *)d_scalars, h.mont(), PassBases{(const affine *)d_bases, window_bits}, n,
                           (jacobian *)d_out_xyz, 0, s, nullptr, 1);
     if (rc) return rc;
     return scratch_release(s);
@@ -463,7 +464,7 @@ extern "C" int h2_msm_dev(int curve, const void *d_scalars, int scalars_repr, co
 // host_bases != nullptr: one-shot MSM -- the bases are uploaded (and converted) on the copy stream AFTER the
 // scalars, overlapping the digit/sort kernels, which only read scalars (B.bases is where they go).
 static int msm_host_common(int curve, const void *scalars, size_t n_scalars, const void *extra_scalar, const PassBases &B,
-                           size_t n_total, int repr, const PassOut &to, const void *host_bases = nullptr) {
+                           size_t n_total, const HostArgs &h, const PassOut &to, const void *host_bases = nullptr) {
     Context &X = g_ctx;
     cudaStream_t s = X.stream;
     if (scratch_acquire(s)) return 1;
@@ -501,7 +502,7 @@ static int msm_host_common(int curve, const void *scalars, size_t n_scalars, con
                     CU(cudaEventRecord(ctx->ev_scal_up[j], cs));
                     recorded.store(2 * j + 1, std::memory_order_release);
                     if (upload_async(db + lo, (const affine *)host_bases + lo, (hi - lo) * sizeof(affine), cs)) return 1;
-                    if (repr == H2_REPR_CANONICAL && convert_points(curve, db + lo, hi - lo, 1, cs)) return 1;
+                    if (h.canon() && convert_points(curve, db + lo, hi - lo, 1, cs)) return 1;
                     CU(cudaEventRecord(ctx->ev_bases_up[j], cs));
                     recorded.store(2 * j + 2, std::memory_order_release);
                 }
@@ -520,60 +521,60 @@ static int msm_host_common(int curve, const void *scalars, size_t n_scalars, con
         if (up_failed.load()) { cudaStreamSynchronize(s); cudaStreamSynchronize(X.copy_stream); return fail(up_err); }
         return rc;
     };
-    return msm_pass(curve, X.scal_in.as<fe>(), repr == H2_REPR_MONTGOMERY, B, n_total, 1, X.result.as<jacobian>(), repr == H2_REPR_CANONICAL, to,
+    return msm_pass(curve, X.scal_in.as<fe>(), h.mont(), B, n_total, 1, X.result.as<jacobian>(), h.canon(), to,
                     bc.k ? &bc : nullptr, joined);
 }
 
 extern "C" int h2_msm(int curve, const void *scalars, const void *bases_xy, size_t n, int repr, void *out_xyz) {
     CtxLock lk;
-    if (require_ready()) return 1;
-    if (check_curve(curve)) return 1;
+    const HostArgs h("h2_msm", repr);
+    if (require_ready() || check_curve(curve) || h.check({{scalars, "scalars", n != 0}, {bases_xy, "bases_xy", n != 0}, {out_xyz, "out_xyz"}})) return 1;
     Context &X = g_ctx;
     cudaStream_t s = X.stream;
     if (scratch_acquire(s)) return 1;
     if (X.bases_in.ensure((n + 1) * sizeof(affine))) return 1;
-    return msm_host_common(curve, scalars, n, nullptr, {X.bases_in.as<affine>()}, n, repr, {out_xyz}, bases_xy);
+    return msm_host_common(curve, scalars, n, nullptr, {X.bases_in.as<affine>()}, n, h, {out_xyz}, bases_xy);
 }
 
-static int bases_register_impl(int curve, const void *bases_xy, size_t n, int repr, uint32_t window_bits, uint32_t flags, uint64_t *handle);
+static int bases_register_impl(int curve, const void *bases_xy, size_t n, const HostArgs &h, uint32_t window_bits, uint32_t flags, uint64_t *handle);
 extern "C" int h2_bases_register(int curve, const void *bases_xy, size_t n, int repr, uint64_t *handle) {
-    return bases_register_impl(curve, bases_xy, n, repr, 0, 0, handle);
+    return bases_register_impl(curve, bases_xy, n, {"h2_bases_register", repr}, 0, 0, handle);
 }
 extern "C" int h2_bases_register_ex(int curve, const void *bases_xy, size_t n, int repr, uint32_t window_bits, uint32_t flags, uint64_t *handle) {
-    return bases_register_impl(curve, bases_xy, n, repr, window_bits, flags, handle);
+    return bases_register_impl(curve, bases_xy, n, {"h2_bases_register_ex", repr}, window_bits, flags, handle);
 }
-static int bases_register_impl(int curve, const void *bases_xy, size_t n, int repr, uint32_t window_bits, uint32_t flags, uint64_t *handle) {
+static int bases_register_impl(int curve, const void *bases_xy, size_t n, const HostArgs &h, uint32_t window_bits, uint32_t flags, uint64_t *handle) {
     CtxLock lk;
-    if (require_ready()) return 1;
-    if (check_curve(curve)) return 1;
+    if (require_ready() || check_curve(curve) || h.check({{bases_xy, "bases_xy", n != 0}})) return 1;
     BaseSet *b = new BaseSet();
     b->curve = curve; b->n = n;
     if (b->buf.ensure((n + 1) * sizeof(affine))) { delete b; return 1; }
     cudaStream_t s = g_ctx.stream;
     auto drop = [&]() { cudaStreamSynchronize(s); b->buf.release(); b->table.release(); b->dtable.release(); delete b; return 1; };
     if (n && upload_async(b->buf.p, bases_xy, n * sizeof(affine), s)) return drop();
-    if (repr == H2_REPR_CANONICAL && convert_points(curve, b->buf.as<affine>(), n, 1, s)) return drop();
+    if (h.canon() && convert_points(curve, b->buf.as<affine>(), n, 1, s)) return drop();
     const bool direct = (flags & H2_BASES_DIRECT) && (flags & H2_BASES_PRECOMPUTE) && n > 0;
     if ((flags & H2_BASES_PRECOMPUTE) && n > 0 && build_table(b, direct ? H2_FB_BITS : window_bits, s)) return drop();
     if (direct && build_direct(b, s)) return drop();
     if (cudaStreamSynchronize(s) != cudaSuccess) { fail("h2_bases_register: device error while building the tables"); return drop(); }
-    const uint64_t h = new_handle();
+    const uint64_t id = new_handle();
     {   // shared by every lane from here on (h2_bases_release: capi_core.cu)
         std::lock_guard<std::mutex> reg(g_reg_mu);
-        g_bases[h] = b;
+        g_bases[id] = b;
     }
-    *handle = h;
+    *handle = id;
     return 0;
 }
 extern "C" int h2_msm_registered(uint64_t handle, const void *scalars, size_t n, const void *extra_scalar, int repr, void *out_xyz) {
     CtxLock lk;
-    if (require_ready()) return 1;
+    const HostArgs h("h2_msm_registered", repr);
+    if (require_ready() || h.check({{scalars, "scalars", n != 0}, {out_xyz, "out_xyz"}})) return 1;
     BasesRef ref(handle);
     if (!ref.b) return fail("h2_msm_registered: unknown handle");
     BaseSet *b = ref.b;
     size_t total = n + (extra_scalar ? 1 : 0);
     if (total > b->n) return fail("h2_msm_registered: more scalars than registered bases");
-    return msm_host_common(b->curve, scalars, n, extra_scalar, pass_bases(b), total, repr, {out_xyz});
+    return msm_host_common(b->curve, scalars, n, extra_scalar, pass_bases(b), total, h, {out_xyz});
 }
 
 // `batch` scalar vectors of n entries (+ one extra scalar each, the blinds) against a registered base set with a
@@ -593,7 +594,8 @@ extern "C" int h2_msm_registered_batch_affine(uint64_t handle, const void *scala
 static int msm_registered_batch_impl(uint64_t handle, const void *scalars, size_t n, const void *extra_scalars, size_t batch, int repr,
                                      void *out_xyz, int affine_out) {
     CtxLock lk;
-    if (require_ready()) return 1;
+    const HostArgs h(affine_out ? "h2_msm_registered_batch_affine" : "h2_msm_registered_batch", repr);
+    if (require_ready() || h.check({{scalars, "scalars", n * batch != 0}, {out_xyz, affine_out ? "out_xy" : "out_xyz", batch != 0}})) return 1;
     BasesRef ref(handle);
     if (!ref.b) return fail("h2_msm_registered_batch: unknown handle");
     BaseSet *b = ref.b;
@@ -613,19 +615,19 @@ static int msm_registered_batch_impl(uint64_t handle, const void *scalars, size_
         CU(cudaMemcpy2DAsync(d, total * sizeof(fe), scalars, n * sizeof(fe), n * sizeof(fe), batch, cudaMemcpyHostToDevice, s));
         CU(cudaMemcpy2DAsync(d + n, total * sizeof(fe), extra_scalars, sizeof(fe), sizeof(fe), batch, cudaMemcpyHostToDevice, s));
     }
-    return msm_pass(b->curve, d, repr == H2_REPR_MONTGOMERY, pass_bases(b), total, (uint32_t)batch, X.result.as<jacobian>(),
-                    repr == H2_REPR_CANONICAL, {out_xyz, affine_out != 0});
+    return msm_pass(b->curve, d, h.mont(), pass_bases(b), total, (uint32_t)batch, X.result.as<jacobian>(), h.canon(), {out_xyz, affine_out != 0});
 }
 
 extern "C" int h2_point_sum(int curve, const void *points_xyz, size_t g, int repr, void *out_xyz) {
     CtxLock lk;
-    if (require_ready()) return 1;
+    const HostArgs h("h2_point_sum", repr);
+    if (require_ready() || h.check({{points_xyz, "points_xyz", g != 0}, {out_xyz, "out_xyz"}})) return 1;
     Context &X = g_ctx;
     cudaStream_t s = X.stream;
     if (scratch_acquire(s)) return 1;
     if (X.misc.ensure((g + 1) * sizeof(jacobian)) || X.result.ensure(sizeof(jacobian))) return 1;
     if (g) CU(cudaMemcpyAsync(X.misc.p, points_xyz, g * sizeof(jacobian), cudaMemcpyHostToDevice, s));
-    int canon = repr == H2_REPR_CANONICAL;
+    const int canon = h.canon();
     if (by_curve(curve, [&](auto p, auto) {
             LAUNCH(point_sum_kernel<decltype(p)>, 1, 32, 0, s, X.misc.as<jacobian>(), (uint32_t)g, canon, X.result.as<jacobian>());
             return 0;
@@ -679,11 +681,11 @@ static int multi_run(const std::function<int(size_t)> &fn) {
     for (size_t g = 0; g < G; g++) if (rcs[g]) return fail("device " + std::to_string(g_multi[g]) + ": " + errs[g]);
     return 0;
 }
-static int multi_finish(int curve, int repr, void *out_xyz) {     // the G-term sum on the primary device
+static int multi_finish(int curve, const HostArgs &h, void *out_xyz) {     // the G-term sum on the primary device
     Context &X = g_ctx;
     cudaStream_t s = X.stream;
     const size_t G = g_multi.size();
-    const int canon = repr == H2_REPR_CANONICAL;
+    const int canon = h.canon();
     if (X.result.ensure(sizeof(jacobian))) return 1;
     if (by_curve(curve, [&](auto p, auto) {
             LAUNCH(point_sum_kernel<decltype(p)>, 1, 32, 0, s, X.multi_parts.as<jacobian>(), (uint32_t)G, canon, X.result.as<jacobian>());
@@ -703,8 +705,8 @@ static int multi_refuse_lane(const char *who) {
 extern "C" int h2_msm_multi_gpu(int curve, const void *scalars, const void *bases_xy, size_t n, int repr, void *out_xyz) {
     if (multi_refuse_lane("h2_msm_multi_gpu")) return 1;
     CtxLock lk;
-    if (require_ready()) return 1;
-    if (check_curve(curve)) return 1;
+    const HostArgs h("h2_msm_multi_gpu", repr);
+    if (require_ready() || check_curve(curve) || h.check({{scalars, "scalars", n != 0}, {bases_xy, "bases_xy", n != 0}, {out_xyz, "out_xyz"}})) return 1;
     if (g_multi.empty()) return fail("h2_msm_multi_gpu: call h2_multi_init first");
     const size_t G = g_multi.size();
     Context &P0 = *g_primary;
@@ -717,11 +719,11 @@ extern "C" int h2_msm_multi_gpu(int curve, const void *scalars, const void *base
         shard_range(n, g, G, &lo, &hi);
         if (scratch_acquire(X.stream)) return 1;
         if (X.bases_in.ensure((hi - lo + 1) * sizeof(affine))) return 1;
-        return msm_host_common(curve, (const fe *)scalars + lo, hi - lo, nullptr, {X.bases_in.as<affine>()}, hi - lo, repr,
+        return msm_host_common(curve, (const fe *)scalars + lo, hi - lo, nullptr, {X.bases_in.as<affine>()}, hi - lo, h,
                                {nullptr, false, parts + g, prim}, (const affine *)bases_xy + lo);
     });
     if (rc) return rc;
-    return multi_finish(curve, repr, out_xyz);
+    return multi_finish(curve, h, out_xyz);
 }
 // resident shards: bases[lo_g, hi_g) live on device g, in that device context's `shards` (handle valid for
 // h2_msm_multi_registered only).  Handles come from new_handle(), so one from before an h2_shutdown is unknown after it.
@@ -731,8 +733,8 @@ void multi_bases_clear() { g_multi_bases.clear(); }   // h2_shutdown (the shards
 extern "C" int h2_multi_bases_register(int curve, const void *bases_xy, size_t n, int repr, uint64_t *handle) {
     if (multi_refuse_lane("h2_multi_bases_register")) return 1;
     CtxLock lk;
-    if (require_ready()) return 1;
-    if (check_curve(curve)) return 1;
+    const HostArgs h("h2_multi_bases_register", repr);
+    if (require_ready() || check_curve(curve) || h.check({{bases_xy, "bases_xy", n != 0}})) return 1;
     if (g_multi.empty()) return fail("h2_multi_bases_register: call h2_multi_init first");
     const size_t G = g_multi.size();
     MultiBases mb;
@@ -746,7 +748,7 @@ extern "C" int h2_multi_bases_register(int curve, const void *bases_xy, size_t n
         if (b->buf.ensure((hi - lo + 1) * sizeof(affine))) { delete b; return 1; }
         cudaStream_t s = X.stream;
         if (upload_async(b->buf.p, (const affine *)bases_xy + lo, (hi - lo) * sizeof(affine), s) ||
-            (repr == H2_REPR_CANONICAL && convert_points(curve, b->buf.as<affine>(), hi - lo, 1, s)) ||
+            (h.canon() && convert_points(curve, b->buf.as<affine>(), hi - lo, 1, s)) ||
             cudaStreamSynchronize(s) != cudaSuccess) {
             cudaStreamSynchronize(s); b->buf.release(); delete b;
             return fail("h2_multi_bases_register: upload failed");
@@ -786,7 +788,8 @@ extern "C" int h2_multi_bases_release(uint64_t handle) {
 extern "C" int h2_msm_multi_registered(uint64_t handle, const void *scalars, size_t n, int repr, void *out_xyz) {
     if (multi_refuse_lane("h2_msm_multi_registered")) return 1;
     CtxLock lk;
-    if (require_ready()) return 1;
+    const HostArgs h("h2_msm_multi_registered", repr);
+    if (require_ready() || h.check({{scalars, "scalars", n != 0}, {out_xyz, "out_xyz"}})) return 1;
     auto it = g_multi_bases.find(handle);
     if (it == g_multi_bases.end()) return fail("h2_msm_multi_registered: unknown handle");
     const MultiBases &mb = it->second;
@@ -803,11 +806,11 @@ extern "C" int h2_msm_multi_registered(uint64_t handle, const void *scalars, siz
         shard_range(n, g, G, &lo, &hi);
         auto ib = X.shards.find(mb.handles[g]);
         if (ib == X.shards.end()) return fail("h2_msm_multi_registered: a shard was released");
-        return msm_host_common(mb.curve, (const fe *)scalars + lo, hi - lo, nullptr, {ib->second->buf.as<affine>()}, hi - lo, repr,
+        return msm_host_common(mb.curve, (const fe *)scalars + lo, hi - lo, nullptr, {ib->second->buf.as<affine>()}, hi - lo, h,
                                {nullptr, false, parts + g, prim});
     });
     if (rc) return rc;
-    return multi_finish(mb.curve, repr, out_xyz);
+    return multi_finish(mb.curve, h, out_xyz);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -820,7 +823,7 @@ static IpaState ipa_state(IpaSession *q) {
     S.p = q->p.as<fe>(); S.b = q->b.as<fe>(); S.s = q->s.as<fe>(); S.scal = q->scal.as<fe>(); S.n = 1ull << q->k;
     return S;
 }
-template <class PS> static int ipa_begin_impl(IpaSession *q, const void *p_prime, PolyBuf *p_poly, const void *x3, int repr, cudaStream_t s) {
+template <class PS> static int ipa_begin_impl(IpaSession *q, const void *p_prime, PolyBuf *p_poly, const void *x3, const HostArgs &h, cudaStream_t s) {
     Context &X = g_ctx;
     const uint64_t n = 1ull << q->k;
     if (q->p.ensure(n * sizeof(fe)) || q->b.ensure(n * sizeof(fe)) || q->s.ensure(n * sizeof(fe)) || q->scal.ensure(2 * (n + 2) * sizeof(fe)) ||
@@ -829,10 +832,9 @@ template <class PS> static int ipa_begin_impl(IpaSession *q, const void *p_prime
     if (p_poly) CU(cudaMemcpyAsync(q->p.p, p_poly->buf.p, n * sizeof(fe), cudaMemcpyDeviceToDevice, s));
     else if (upload_async(q->p.p, p_prime, n * sizeof(fe), s)) return 1;
     IpaState S = ipa_state(q);
-    LAUNCH(ipa_init_kernel<PS>, blocks_for(n, 256), 256, 0, s, S, p_poly ? 1 : repr == H2_REPR_MONTGOMERY);
+    LAUNCH(ipa_init_kernel<PS>, blocks_for(n, 256), 256, 0, s, S, p_poly ? 1 : h.mont());
     // b_t = x3^t (prover.rs:86-93) with the NTT twiddle generator
-    fe x = host_to_mont<PS>(x3, repr);
-    LAUNCH(twiddle_pow2_kernel<PS>, 1, 32, 0, s, X.pow2.as<fe>(), x, q->k + 1);
+    LAUNCH(twiddle_pow2_kernel<PS>, 1, 32, 0, s, X.pow2.as<fe>(), h.elem<PS>(x3), q->k + 1);
     LAUNCH(twiddle_fill_kernel<PS>, blocks_for((n + 31) / 32, 128), 128, 0, s, S.b, X.pow2.as<fe>(), n);
     return 0;
 }
@@ -849,7 +851,8 @@ extern "C" int h2_ipa_begin_poly(uint64_t bases_handle, uint32_t k, uint64_t p_p
 static int ipa_begin_common(uint64_t bases_handle, uint32_t k, const void *p_prime, const uint64_t *p_poly_handle, const void *x3, int repr,
                             uint64_t *session) {
     CtxLock lk;
-    if (require_ready()) return 1;
+    const HostArgs h(p_poly_handle ? "h2_ipa_begin_poly" : "h2_ipa_begin", repr);
+    if (require_ready() || h.check({{p_prime, "p_prime", !p_poly_handle}, {x3, "x3"}})) return 1;
     BasesRef ref(bases_handle, true);
     if (!ref.b) return fail("h2_ipa_begin: unknown bases handle");
     BaseSet *b = ref.b;
@@ -872,13 +875,13 @@ static int ipa_begin_common(uint64_t bases_handle, uint32_t k, const void *p_pri
         q->bases = bases_handle; q->k = k; q->round = 0; q->folded = 1;
         cudaStream_t s = g_ctx.stream;
         if (scratch_acquire(s)) { ipa_free(q); return 1; }   // pow2 is shared scratch
-        if (ipa_begin_impl<PS>(q, p_prime, p_poly, x3, repr, s)) { ipa_free(q); return 1; }
+        if (ipa_begin_impl<PS>(q, p_prime, p_poly, x3, h, s)) { ipa_free(q); return 1; }
         if (scratch_release(s)) { ipa_free(q); return 1; }
         cudaError_t e = cudaStreamSynchronize(s);   // p_prime may be pageable host memory
         if (e != cudaSuccess) { ipa_free(q); return fail(std::string("h2_ipa_begin: ") + cudaGetErrorString(e)); }
-        uint64_t h = new_handle();
-        g_ctx.ipa[h] = q;
-        *session = h;
+        uint64_t id = new_handle();
+        g_ctx.ipa[id] = q;
+        *session = id;
         opened = true;
         return 0;
     });
@@ -893,7 +896,8 @@ extern "C" int h2_ipa_round_affine(uint64_t session, const void *z, const void *
 }
 static int ipa_round_common(uint64_t session, const void *z, const void *l_rand, const void *r_rand, int repr, void *out_lr_xyz, int affine_out) {
     CtxLock lk;
-    if (require_ready()) return 1;
+    const HostArgs h(affine_out ? "h2_ipa_round_affine" : "h2_ipa_round", repr);
+    if (require_ready() || h.check({{z, "z"}, {l_rand, "l_rand"}, {r_rand, "r_rand"}, {out_lr_xyz, affine_out ? "out_lr_xy" : "out_lr_xyz"}})) return 1;
     auto it = g_ctx.ipa.find(session);
     if (it == g_ctx.ipa.end()) return fail("h2_ipa_round: unknown session");
     IpaSession *q = it->second;
@@ -911,17 +915,18 @@ static int ipa_round_common(uint64_t session, const void *z, const void *l_rand,
         using PS = decltype(ps);
         const uint32_t bit = q->k - 1 - q->round;
         LAUNCH(ipa_prep_kernel<PS>, blocks_for(n, 256), 256, 0, s, S, bit);
-        LAUNCH(ipa_inner_kernel<PS>, 1, 512, 0, s, S, bit, host_to_mont<PS>(z, repr), host_to_mont<PS>(l_rand, repr), host_to_mont<PS>(r_rand, repr));
+        LAUNCH(ipa_inner_kernel<PS>, 1, 512, 0, s, S, bit, h.elem<PS>(z), h.elem<PS>(l_rand), h.elem<PS>(r_rand));
         return 0;
     });
-    if (rc || msm_pass(b->curve, S.scal, 1, pass_bases(b), n + 2, 2, q->out.as<jacobian>(), repr == H2_REPR_CANONICAL, {out_lr_xyz, affine_out != 0}))
+    if (rc || msm_pass(b->curve, S.scal, 1, pass_bases(b), n + 2, 2, q->out.as<jacobian>(), h.canon(), {out_lr_xyz, affine_out != 0}))
         return 1;
     q->folded = 0;
     return 0;
 }
 extern "C" int h2_ipa_fold(uint64_t session, const void *u, const void *u_inv, int repr) {
     CtxLock lk;
-    if (require_ready()) return 1;
+    const HostArgs h("h2_ipa_fold", repr);
+    if (require_ready() || h.check({{u, "u"}, {u_inv, "u_inv"}})) return 1;
     auto it = g_ctx.ipa.find(session);
     if (it == g_ctx.ipa.end()) return fail("h2_ipa_fold: unknown session");
     IpaSession *q = it->second;
@@ -934,16 +939,18 @@ extern "C" int h2_ipa_fold(uint64_t session, const void *u, const void *u_inv, i
     IpaState S = ipa_state(q);
     if (by_curve(ref.b->curve, [&](auto, auto ps) {
             using PS = decltype(ps);
-            LAUNCH(ipa_fold_kernel<PS>, blocks_for(n, 256), 256, 0, s, S, bit, host_to_mont<PS>(u, repr), host_to_mont<PS>(u_inv, repr));
+            LAUNCH(ipa_fold_kernel<PS>, blocks_for(n, 256), 256, 0, s, S, bit, h.elem<PS>(u), h.elem<PS>(u_inv));
             return 0;
         }))
         return 1;
     q->round++; q->folded = 1;   // asynchronous: the next round (or finish) is ordered behind it on the stream
     return 0;
 }
+// out_c_b == NULL aborts the session whatever repr is, so that cleanup cannot fail
 extern "C" int h2_ipa_finish(uint64_t session, int repr, void *out_c_b) {
     CtxLock lk;
-    if (require_ready()) return 1;
+    const HostArgs h("h2_ipa_finish", repr);
+    if (require_ready() || (out_c_b && h.check())) return 1;
     auto it = g_ctx.ipa.find(session);
     if (it == g_ctx.ipa.end()) return fail("h2_ipa_finish: unknown session");
     IpaSession *q = it->second;
@@ -957,7 +964,7 @@ extern "C" int h2_ipa_finish(uint64_t session, int repr, void *out_c_b) {
             IpaState S = ipa_state(q);
             fe *out = q->scal.as<fe>();
             rc = by_curve(ref.b->curve, [&](auto, auto ps) {
-                ipa_result_kernel<decltype(ps)><<<1, 32, 0, s>>>(S, repr == H2_REPR_CANONICAL, out);
+                ipa_result_kernel<decltype(ps)><<<1, 32, 0, s>>>(S, h.canon(), out);
                 g_launches.fetch_add(1, std::memory_order_relaxed);
                 cudaError_t e = cudaMemcpyAsync(out_c_b, out, 2 * sizeof(fe), cudaMemcpyDeviceToHost, s);
                 return e != cudaSuccess ? fail(std::string("h2_ipa_finish: ") + cudaGetErrorString(e)) : 0;
@@ -988,7 +995,8 @@ extern "C" int h2_msm_registered_polys_affine(uint64_t bases_handle, const uint6
 static int msm_registered_polys_impl(uint64_t bases_handle, const uint64_t *polys, size_t batch, size_t n, const void *extra_scalars, int repr,
                                      void *out_xyz, int affine_out) {
     CtxLock lk;
-    if (require_ready()) return 1;
+    const HostArgs h(affine_out ? "h2_msm_registered_polys_affine" : "h2_msm_registered_polys", repr);
+    if (require_ready() || h.check({{out_xyz, affine_out ? "out_xy" : "out_xyz", batch != 0}})) return 1;
     BasesRef ref(bases_handle);
     if (!ref.b) return fail("h2_msm_registered_polys: unknown bases handle");
     BaseSet *b = ref.b;
@@ -1006,16 +1014,12 @@ static int msm_registered_polys_impl(uint64_t bases_handle, const uint64_t *poly
         if (scratch_acquire(s)) return 1;
         if (X.scal_in.ensure(batch * total * sizeof(fe)) || X.result.ensure(batch * sizeof(jacobian)) || X.misc.ensure(batch * sizeof(fe) + 64)) return 1;
         fe *d = X.scal_in.as<fe>();
-        if (extra_scalars) {   // the blinds: Montgomery form like the resident data
-            CU(cudaMemcpyAsync(X.misc.p, extra_scalars, batch * sizeof(fe), cudaMemcpyHostToDevice, s));
-            if (repr == H2_REPR_CANONICAL && convert_field(decltype(ps)::ID, X.misc.as<fe>(), batch, 1, s)) return 1;
-        }
+        if (extra_scalars && h.up(decltype(ps)::ID, X.misc.as<fe>(), extra_scalars, batch, s)) return 1;   // the blinds: Montgomery form like the resident data
         for (size_t j = 0; j < batch; j++) {
             CU(cudaMemcpyAsync(d + j * total, q[j]->buf.p, n * sizeof(fe), cudaMemcpyDeviceToDevice, s));
             if (extra_scalars) CU(cudaMemcpyAsync(d + j * total + n, X.misc.as<fe>() + j, sizeof(fe), cudaMemcpyDeviceToDevice, s));
         }
-        return msm_pass(b->curve, d, 1, pass_bases(b), total, (uint32_t)batch, X.result.as<jacobian>(), repr == H2_REPR_CANONICAL,
-                        {out_xyz, affine_out != 0});
+        return msm_pass(b->curve, d, 1, pass_bases(b), total, (uint32_t)batch, X.result.as<jacobian>(), h.canon(), {out_xyz, affine_out != 0});
     });
 }
 

@@ -89,12 +89,12 @@ static int ntt_run(int field, const fe *d_in, uint32_t in_log_n, fe *d_out, uint
     return 0;
 }
 
-// Builds the in/out scale constants.  data_repr is the encoding of the data entering and leaving.
+// Builds the in/out scale constants.  canon: the data enters and leaves in canonical form.
 //   zeta_in  != null : multiply element j by zeta^(j mod 3)            (coeff_to_extended)
 //   divisor  != null : multiply every output by divisor                (ifft)
 //   zeta_out != null : multiply output p by [1, zeta^2, zeta][p mod 3] (extended_to_coeff)
 template <class P>
-static NttScales make_scales(int data_repr, const fe *zeta_in, const fe *divisor, const fe *zeta_out) {
+static NttScales make_scales(bool canon, const fe *zeta_in, const fe *divisor, const fe *zeta_out) {
     NttScales sc;
     fe one = fe_one<P>();
     fe in_c[3] = {one, one, one}, out_c[3] = {one, one, one};
@@ -102,7 +102,7 @@ static NttScales make_scales(int data_repr, const fe *zeta_in, const fe *divisor
     if (zeta_in) { in_c[1] = *zeta_in; in_c[2] = fe_sqr<P>(*zeta_in); in_needed = true; }
     if (divisor) { for (int k = 0; k < 3; k++) out_c[k] = *divisor; out_needed = true; }
     if (zeta_out) { out_c[1] = fe_mul<P>(out_c[1], fe_sqr<P>(*zeta_out)); out_c[2] = fe_mul<P>(out_c[2], *zeta_out); out_needed = true; }
-    if (data_repr == H2_REPR_CANONICAL) {
+    if (canon) {
         // canonical -> Montgomery on the way in:  mont_mul(a, c R^2) = a c R
         for (int k = 0; k < 3; k++) in_c[k] = fe_mul<P>(in_c[k], fe_r2<P>());
         // Montgomery -> canonical on the way out: mont_mul(x R, c) = x c
@@ -114,54 +114,60 @@ static NttScales make_scales(int data_repr, const fe *zeta_in, const fe *divisor
     return sc;
 }
 
+// zeta / divisor: nullptr in the modes that have none (the entry points have checked the others)
+template <class P> static NttScales host_scales(const HostArgs &h, bool canon, int mode, const void *zeta, const void *divisor) {
+    const fe z = zeta ? h.elem<P>(zeta) : fe_zero(), d = divisor ? h.elem<P>(divisor) : fe_zero();
+    return make_scales<P>(canon, mode == 2 ? &z : nullptr, (mode == 1 || mode == 3) ? &d : nullptr, mode == 3 ? &z : nullptr);
+}
 template <class P>
 static int ntt_host(int field, int mode, const void *a_in, uint32_t in_log_n, uint32_t log_n, const void *omega, const void *zeta,
-                    const void *divisor, size_t out_len, void *out, int repr) {
+                    const void *divisor, size_t out_len, void *out, const HostArgs &h) {
     Context &X = g_ctx;
     cudaStream_t s = X.stream;
     if (scratch_acquire(s)) return 1;
     uint64_t n = 1ull << log_n, n_in = 1ull << in_log_n;
     if (out_len > n) out_len = n;
     if (X.ntt_io.ensure(n_in * sizeof(fe)) || X.ntt_out.ensure(n * sizeof(fe))) return 1;
-    fe w = host_to_mont<P>(omega, repr), z, d;
-    if (zeta) z = host_to_mont<P>(zeta, repr);
-    if (divisor) d = host_to_mont<P>(divisor, repr);
-    NttScales sc = make_scales<P>(repr, mode == 2 ? &z : nullptr, (mode == 1 || mode == 3) ? &d : nullptr, mode == 3 ? &z : nullptr);
+    const NttScales sc = host_scales<P>(h, h.canon(), mode, zeta, divisor);
     if (upload_async(X.ntt_io.p, a_in, n_in * sizeof(fe), s)) return 1;
-    if (ntt_run<P>(field, X.ntt_io.as<fe>(), in_log_n, X.ntt_out.as<fe>(), log_n, w, sc, out_len, s)) return 1;
+    if (ntt_run<P>(field, X.ntt_io.as<fe>(), in_log_n, X.ntt_out.as<fe>(), log_n, h.elem<P>(omega), sc, out_len, s)) return 1;
     if (download_sync(out, X.ntt_out.p, out_len * sizeof(fe), s)) return 1;
     return scratch_release(s);
 }
 static int ntt_host_dispatch(int field, int mode, const void *a_in, uint32_t in_log_n, uint32_t log_n, const void *omega, const void *zeta,
-                             const void *divisor, size_t out_len, void *out, int repr) {
+                             const void *divisor, size_t out_len, void *out, const HostArgs &h, std::initializer_list<HostArgs::Need> needs) {
     CtxLock lk;
-    if (require_ready()) return 1;
+    if (require_ready() || h.check(needs)) return 1;
     if (log_n > 30 || in_log_n > log_n) return fail("ntt: bad sizes");
-    return by_field(field, [&](auto p) { return ntt_host<decltype(p)>(field, mode, a_in, in_log_n, log_n, omega, zeta, divisor, out_len, out, repr); });
+    return by_field(field, [&](auto p) { return ntt_host<decltype(p)>(field, mode, a_in, in_log_n, log_n, omega, zeta, divisor, out_len, out, h); });
 }
 extern "C" int h2_ntt(int field, void *a, const void *omega, uint32_t log_n, int repr) {
-    return ntt_host_dispatch(field, 0, a, log_n, log_n, omega, nullptr, nullptr, (size_t)1 << log_n, a, repr);
+    return ntt_host_dispatch(field, 0, a, log_n, log_n, omega, nullptr, nullptr, (size_t)1 << log_n, a, {"h2_ntt", repr}, {{a, "a"}, {omega, "omega"}});
 }
 extern "C" int h2_intt_scaled(int field, void *a, const void *omega_inv, const void *divisor, uint32_t log_n, int repr) {
-    return ntt_host_dispatch(field, 1, a, log_n, log_n, omega_inv, nullptr, divisor, (size_t)1 << log_n, a, repr);
+    return ntt_host_dispatch(field, 1, a, log_n, log_n, omega_inv, nullptr, divisor, (size_t)1 << log_n, a, {"h2_intt_scaled", repr},
+                             {{a, "a"}, {omega_inv, "omega_inv"}, {divisor, "divisor"}});
 }
 extern "C" int h2_coeff_to_extended(int field, const void *a, uint32_t k, uint32_t ext_k, const void *zeta, const void *ext_omega,
                                     void *out, int repr) {
-    return ntt_host_dispatch(field, 2, a, k, ext_k, ext_omega, zeta, nullptr, (size_t)1 << ext_k, out, repr);
+    return ntt_host_dispatch(field, 2, a, k, ext_k, ext_omega, zeta, nullptr, (size_t)1 << ext_k, out, {"h2_coeff_to_extended", repr},
+                             {{a, "a"}, {zeta, "zeta"}, {ext_omega, "ext_omega"}, {out, "out"}});
 }
 extern "C" int h2_extended_to_coeff(int field, const void *a, uint32_t ext_k, const void *ext_omega_inv, const void *ext_divisor,
                                     const void *zeta, size_t out_len, void *out, int repr) {
-    return ntt_host_dispatch(field, 3, a, ext_k, ext_k, ext_omega_inv, zeta, ext_divisor, out_len, out, repr);
+    return ntt_host_dispatch(field, 3, a, ext_k, ext_k, ext_omega_inv, zeta, ext_divisor, out_len, out, {"h2_extended_to_coeff", repr},
+                             {{a, "a"}, {ext_omega_inv, "ext_omega_inv"}, {ext_divisor, "ext_divisor"}, {zeta, "zeta"}, {out, "out", out_len != 0}});
 }
 extern "C" int h2_ntt_dev(int field, const void *d_in, void *d_out, const void *omega, int omega_repr, uint32_t log_n, void *stream) {
     CtxLock lk;
-    if (require_ready()) return 1;
+    const HostArgs h("h2_ntt_dev", omega_repr);
+    if (require_ready() || h.check({{omega, "omega"}})) return 1;
     cudaStream_t s = (cudaStream_t)stream;
     if (scratch_acquire(s)) return 1;
     NttScales sc;   // Montgomery in, Montgomery out, no scaling
     if (by_field(field, [&](auto p) {
             using P = decltype(p);
-            return ntt_run<P>(field, (const fe *)d_in, log_n, (fe *)d_out, log_n, host_to_mont<P>(omega, omega_repr), sc, 1ull << log_n, s);
+            return ntt_run<P>(field, (const fe *)d_in, log_n, (fe *)d_out, log_n, h.elem<P>(omega), sc, 1ull << log_n, s);
         }))
         return 1;
     return scratch_release(s);
@@ -285,13 +291,13 @@ int convert_field(int field, fe *d, size_t n, int to_mont, cudaStream_t s) {
 }
 extern "C" int h2_poly_upload(uint64_t poly, const void *src, size_t len, int repr) {
     CtxLock lk;
-    if (require_ready()) return 1;
+    const HostArgs h("h2_poly_upload", repr);
+    if (require_ready() || h.check({{src, "src", len != 0}})) return 1;
     PolyArgs g("h2_poly_upload");
     PolyBuf *b = g.out(poly, len, "len");
     if (!b) return 1;
     cudaStream_t s = g_ctx.stream;
-    if (upload_async(b->buf.p, src, len * sizeof(fe), s)) return 1;
-    if (repr == H2_REPR_CANONICAL && convert_field(b->field, b->buf.as<fe>(), len, 1, s)) return 1;
+    if (h.up(b->field, b->buf.as<fe>(), src, len, s)) return 1;
     CU(cudaStreamSynchronize(s));      // src may be pageable
     return 0;
 }
@@ -300,7 +306,8 @@ extern "C" int h2_poly_upload(uint64_t poly, const void *src, size_t len, int re
 template <class P> __global__ void poly_add_at_kernel(fe *a, fe delta_mont) { fe_store(a, fe_add<P>(fe_load(a), delta_mont)); }
 extern "C" int h2_poly_add_at(uint64_t poly, size_t index, const void *delta, int repr) {
     CtxLock lk;
-    if (require_ready()) return 1;
+    const HostArgs h("h2_poly_add_at", repr);
+    if (require_ready() || h.check({{delta, "delta"}})) return 1;
     PolyArgs g("h2_poly_add_at");
     PolyBuf *b = g.out(poly, 0, "0");
     if (!b) return 1;
@@ -308,7 +315,7 @@ extern "C" int h2_poly_add_at(uint64_t poly, size_t index, const void *delta, in
     cudaStream_t s = g_ctx.stream;
     return by_field(b->field, [&](auto p) {
         using P = decltype(p);
-        LAUNCH(poly_add_at_kernel<P>, 1, 1, 0, s, b->buf.as<fe>() + index, host_to_mont<P>(delta, repr));
+        LAUNCH(poly_add_at_kernel<P>, 1, 1, 0, s, b->buf.as<fe>() + index, h.elem<P>(delta));
         return 0;
     });
 }
@@ -328,41 +335,29 @@ extern "C" int h2_poly_copy(uint64_t dst, size_t dst_off, uint64_t src, size_t s
 }
 extern "C" int h2_poly_download(uint64_t poly, void *dst, size_t len, int repr) {
     CtxLock lk;
-    if (require_ready()) return 1;
+    const HostArgs h("h2_poly_download", repr);
+    if (require_ready() || h.check({{dst, "dst", len != 0}})) return 1;
     PolyArgs g("h2_poly_download");
     PolyBuf *b = g.in(poly, len, "len");
     if (!b) return 1;
-    Context &X = g_ctx;
-    cudaStream_t s = X.stream;
-    const fe *from = b->buf.as<fe>();
-    if (repr == H2_REPR_CANONICAL) {   // convert a copy: the resident data stays in Montgomery form
-        if (scratch_acquire(s)) return 1;
-        if (X.ntt_out.ensure(len * sizeof(fe))) return 1;
-        CU(cudaMemcpyAsync(X.ntt_out.p, from, len * sizeof(fe), cudaMemcpyDeviceToDevice, s));
-        if (convert_field(b->field, X.ntt_out.as<fe>(), len, 0, s)) return 1;
-        from = X.ntt_out.as<fe>();
-    }
-    if (download_sync(dst, from, len * sizeof(fe), s)) return 1;
-    if (repr == H2_REPR_CANONICAL && scratch_release(s)) return 1;
-    return 0;
+    return h.down(b->field, dst, b->buf.as<fe>(), len, g_ctx.stream);
 }
 // mode as in ntt_host: 1 = inverse transform with divisor, 2 = coeff_to_extended, 3 = extended_to_coeff
 template <class P>
 static int poly_transform(PolyBuf *dst, PolyBuf *src, int mode, uint32_t in_log_n, uint32_t log_n, const void *omega, const void *zeta,
-                          const void *divisor, size_t out_len, int repr) {
+                          const void *divisor, size_t out_len, const HostArgs &h) {
     cudaStream_t s = g_ctx.stream;
     if (scratch_acquire(s)) return 1;
-    fe w = host_to_mont<P>(omega, repr), z, d;
-    if (zeta) z = host_to_mont<P>(zeta, repr);
-    if (divisor) d = host_to_mont<P>(divisor, repr);
-    NttScales sc = make_scales<P>(H2_REPR_MONTGOMERY, mode == 2 ? &z : nullptr, (mode == 1 || mode == 3) ? &d : nullptr, mode == 3 ? &z : nullptr);
-    if (ntt_run<P>(src->field, src->buf.as<fe>(), in_log_n, dst->buf.as<fe>(), log_n, w, sc, out_len, s)) return 1;
+    const NttScales sc = host_scales<P>(h, false, mode, zeta, divisor);   // resident data: Montgomery in and out
+    if (ntt_run<P>(src->field, src->buf.as<fe>(), in_log_n, dst->buf.as<fe>(), log_n, h.elem<P>(omega), sc, out_len, s)) return 1;
     return scratch_release(s);       // asynchronous: later calls are ordered behind it on the stream
 }
 static int poly_transform_dispatch(uint64_t dst, uint64_t src, int mode, uint32_t in_log_n, uint32_t log_n, const void *omega, const void *zeta,
-                                   const void *divisor, size_t out_len, int repr, const char *who, const char *in_name, const char *out_name) {
+                                   const void *divisor, size_t out_len, const HostArgs &h, std::initializer_list<HostArgs::Need> needs,
+                                   const char *in_name, const char *out_name) {
+    const char *who = h.who;
     CtxLock lk;
-    if (require_ready()) return 1;
+    if (require_ready() || h.check(needs)) return 1;
     if (log_n > 30 || in_log_n > log_n) return fail("ntt: bad sizes");
     if (out_len > ((size_t)1 << log_n)) out_len = (size_t)1 << log_n;
     PolyArgs g(who);
@@ -372,16 +367,18 @@ static int poly_transform_dispatch(uint64_t dst, uint64_t src, int mode, uint32_
     if (!a) return 1;
     if (d == a && out_len != ((size_t)1 << log_n)) return fail(std::string(who) + ": in place needs out_len == 2^log_n");
     if (d == a && in_log_n != log_n) return fail(std::string(who) + ": in place needs equal input and output sizes");
-    return by_field(a->field, [&](auto p) { return poly_transform<decltype(p)>(d, a, mode, in_log_n, log_n, omega, zeta, divisor, out_len, repr); });
+    return by_field(a->field, [&](auto p) { return poly_transform<decltype(p)>(d, a, mode, in_log_n, log_n, omega, zeta, divisor, out_len, h); });
 }
 extern "C" int h2_poly_lagrange_to_coeff(uint64_t dst, uint64_t src, uint32_t k, const void *omega_inv, const void *divisor, int repr) {
-    return poly_transform_dispatch(dst, src, 1, k, k, omega_inv, nullptr, divisor, (size_t)1 << k, repr, "h2_poly_lagrange_to_coeff", "2^k", "2^k");
+    return poly_transform_dispatch(dst, src, 1, k, k, omega_inv, nullptr, divisor, (size_t)1 << k, {"h2_poly_lagrange_to_coeff", repr},
+                                   {{omega_inv, "omega_inv"}, {divisor, "divisor"}}, "2^k", "2^k");
 }
 extern "C" int h2_poly_coeff_to_extended(uint64_t dst, uint64_t src, uint32_t k, uint32_t ext_k, const void *zeta, const void *ext_omega, int repr) {
-    return poly_transform_dispatch(dst, src, 2, k, ext_k, ext_omega, zeta, nullptr, (size_t)1 << ext_k, repr, "h2_poly_coeff_to_extended", "2^k", "2^ext_k");
+    return poly_transform_dispatch(dst, src, 2, k, ext_k, ext_omega, zeta, nullptr, (size_t)1 << ext_k, {"h2_poly_coeff_to_extended", repr},
+                                   {{zeta, "zeta"}, {ext_omega, "ext_omega"}}, "2^k", "2^ext_k");
 }
 extern "C" int h2_poly_extended_to_coeff(uint64_t dst, uint64_t src, uint32_t ext_k, const void *ext_omega_inv, const void *ext_divisor,
                                          const void *zeta, size_t out_len, int repr) {
-    return poly_transform_dispatch(dst, src, 3, ext_k, ext_k, ext_omega_inv, zeta, ext_divisor, out_len, repr, "h2_poly_extended_to_coeff", "2^ext_k",
-                                   "out_len");
+    return poly_transform_dispatch(dst, src, 3, ext_k, ext_k, ext_omega_inv, zeta, ext_divisor, out_len, {"h2_poly_extended_to_coeff", repr},
+                                   {{ext_omega_inv, "ext_omega_inv"}, {ext_divisor, "ext_divisor"}, {zeta, "zeta"}}, "2^ext_k", "out_len");
 }

@@ -15,7 +15,8 @@
 // ------------------------------------------------------------------------------------------------
 // mode 0: eval (points: batch x 32 host), 1: inner product of a[i] and c[i], 2: kate division of a[i] by (X - point_i) into c[i]
 template <class P>
-static int polyops_run(int mode, const std::vector<PolyBuf *> &a, const std::vector<PolyBuf *> &c, size_t n, const void *points, int repr, void *out) {
+static int polyops_run(int mode, const std::vector<PolyBuf *> &a, const std::vector<PolyBuf *> &c, size_t n, const void *points, const HostArgs &h,
+                       void *out) {
     Context &X = g_ctx;
     cudaStream_t s = X.stream;
     const uint32_t batch = (uint32_t)a.size();
@@ -40,16 +41,15 @@ static int polyops_run(int mode, const std::vector<PolyBuf *> &a, const std::vec
     // points of level 0 (Montgomery): the caller's, or 1 for the plain sums of the inner product
     if (mode == 1) {
         LAUNCH(fe_fill_kernel<P>, blocks_for(batch, 64), 64, 0, s, pts, batch, fe_one<P>());
-    } else {
-        CU(cudaMemcpyAsync(pts, points, batch * sizeof(fe), cudaMemcpyHostToDevice, s));
-        if (repr == H2_REPR_CANONICAL) LAUNCH(convert_kernel<P>, blocks_for(batch, 64), 64, 0, s, pts, (uint64_t)batch, 1);
+    } else if (h.up(P::ID, pts, points, batch, s)) {
+        return 1;
     }
     if (mode != 1 && n <= (1ull << 16) && n >= 2 && X.poly_cta) {
         // small polynomials: one CTA per polynomial does the whole reduction (polyops.cuh poly_eval_cta_kernel / poly_kate_cta_kernel)
         if (mode == 0) {
             fe *res = X.misc.as<fe>();
             LAUNCH(poly_eval_cta_kernel<P>, batch, H2_POLY_CTA, 0, s, d_a, (uint64_t)n, (const fe *)pts, res);
-            if (repr == H2_REPR_CANONICAL) LAUNCH(convert_kernel<P>, blocks_for(batch, 64), 64, 0, s, res, (uint64_t)batch, 0);
+            if (h.from_mont(P::ID, res, batch, s)) return 1;
             CU(cudaMemcpyAsync(out, res, batch * sizeof(fe), cudaMemcpyDeviceToHost, s));
             if (scratch_release(s)) return 1;
             CU(cudaStreamSynchronize(s));
@@ -76,7 +76,7 @@ static int polyops_run(int mode, const std::vector<PolyBuf *> &a, const std::vec
         } else {
             CU(cudaMemcpyAsync(res, level(L), batch * sizeof(fe), cudaMemcpyDeviceToDevice, s));   // m[L] == 1: [batch][1]
         }
-        if (repr == H2_REPR_CANONICAL) LAUNCH(convert_kernel<P>, blocks_for(batch, 64), 64, 0, s, res, (uint64_t)batch, 0);
+        if (h.from_mont(P::ID, res, batch, s)) return 1;
         CU(cudaMemcpyAsync(out, res, batch * sizeof(fe), cudaMemcpyDeviceToHost, s));
         if (scratch_release(s)) return 1;
         CU(cudaStreamSynchronize(s));
@@ -96,8 +96,9 @@ static int polyops_run(int mode, const std::vector<PolyBuf *> &a, const std::vec
     for (uint32_t b = 0; b < batch; b++) CU(cudaMemsetAsync(c[b]->buf.as<fe>() + (n - 1), 0, sizeof(fe), s));
     return scratch_release(s);
 }
-static int polyops_dispatch(int mode, const uint64_t *ah, const uint64_t *ch, size_t batch, size_t n, const void *points, int repr, void *out,
-                            const char *who) {
+// h: checked by the caller
+static int polyops_dispatch(int mode, const uint64_t *ah, const uint64_t *ch, size_t batch, size_t n, const void *points, const HostArgs &h, void *out) {
+    const char *who = h.who;
     CtxLock lk;
     if (require_ready()) return 1;
     if (batch == 0) return 0;
@@ -110,13 +111,13 @@ static int polyops_dispatch(int mode, const uint64_t *ah, const uint64_t *ch, si
     } else if (g.in(ah, batch, n, "n", a) || (ch && g.in(ch, batch, n, "n", c))) {
         return 1;
     }
-    return by_field(a[0]->field, [&](auto p) { return polyops_run<decltype(p)>(mode, a, c, n, points, repr, out); });
+    return by_field(a[0]->field, [&](auto p) { return polyops_run<decltype(p)>(mode, a, c, n, points, h, out); });
 }
 // Evaluator::evaluate (poly/evaluator.rs:129-228) on resident polynomials: `code` is the postfix form of the Ast (asteval.cuh),
 // validated here so that the kernel's operand stack can neither overflow nor underflow.
 template <class P>
 static int ast_run(PolyBuf *out, const std::vector<PolyBuf *> &polys, uint32_t log_n, const AstInstr *code, size_t n_code, const void *consts,
-                   size_t n_consts, const void *omega, const void *lin_base, int repr, bool has_linear) {
+                   size_t n_consts, const void *omega, const void *lin_base, const HostArgs &h, bool has_linear) {
     Context &X = g_ctx;
     cudaStream_t s = X.stream;
     const uint64_t n = 1ull << log_n;
@@ -127,16 +128,13 @@ static int ast_run(PolyBuf *out, const std::vector<PolyBuf *> &polys, uint32_t l
     for (size_t i = 0; i < polys.size(); i++) hp[i] = polys[i]->buf.as<fe>();
     CU(cudaMemcpyAsync(X.po_ptrs.p, hp.data(), hp.size() * sizeof(void *), cudaMemcpyHostToDevice, s));
     CU(cudaMemcpyAsync(X.ast_code.p, code, n_code * sizeof(AstInstr), cudaMemcpyHostToDevice, s));
-    if (n_consts) {
-        CU(cudaMemcpyAsync(X.ast_consts.p, consts, n_consts * sizeof(fe), cudaMemcpyHostToDevice, s));
-        if (repr == H2_REPR_CANONICAL) LAUNCH(convert_kernel<P>, blocks_for(n_consts, 64), 64, 0, s, X.ast_consts.as<fe>(), (uint64_t)n_consts, 1);
-    }
+    if (h.up(P::ID, X.ast_consts.as<fe>(), consts, n_consts, s)) return 1;
     AstArgs A;
     A.polys = X.po_ptrs.as<const fe *>(); A.code = X.ast_code.as<AstInstr>(); A.n_code = (uint32_t)n_code; A.consts = X.ast_consts.as<fe>();
     A.tw = nullptr; A.lin_base = fe_one<P>(); A.log_n = log_n; A.out = out->buf.as<fe>();
     if (has_linear) {
-        if (get_twiddles_any(out->field, host_to_mont<P>(omega, repr), log_n, s, &A.tw)) return 1;
-        A.lin_base = host_to_mont<P>(lin_base, repr);
+        if (get_twiddles_any(out->field, h.elem<P>(omega), log_n, s, &A.tw)) return 1;
+        A.lin_base = h.elem<P>(lin_base);
     }
     LAUNCH(ast_eval_kernel<P>, blocks_for(n, 128), 128, 0, s, A);
     return scratch_release(s);
@@ -168,8 +166,9 @@ extern "C" int h2_poly_eval_ast(uint64_t out, const uint64_t *polys, size_t n_po
         if (depth > H2_AST_STACK) return fail("h2_poly_eval_ast: expression deeper than the operand stack (24)");
     }
     if (depth != 1) return fail("h2_poly_eval_ast: the program must leave exactly one value");
-    if (has_linear && (!omega || !lin_base)) return fail("h2_poly_eval_ast: a LinearTerm needs omega and the coset generator");
-    return by_field(o->field, [&](auto p) { return ast_run<decltype(p)>(o, ps, log_n, prog, n_code, consts, n_consts, omega, lin_base, repr, has_linear); });
+    const HostArgs h("h2_poly_eval_ast", repr);   // a LinearTerm needs omega and the coset generator
+    if (h.check({{consts, "consts", n_consts != 0}, {omega, "omega", has_linear}, {lin_base, "lin_base", has_linear}})) return 1;
+    return by_field(o->field, [&](auto p) { return ast_run<decltype(p)>(o, ps, log_n, prog, n_code, consts, n_consts, omega, lin_base, h, has_linear); });
 }
 // ff::BatchInvert on the first n elements of a resident polynomial, in place (zeros stay zero)
 extern "C" int h2_poly_batch_invert(uint64_t poly, size_t n) {
@@ -190,7 +189,7 @@ extern "C" int h2_poly_batch_invert(uint64_t poly, size_t n) {
     return scratch_release(s);
 }
 // dst[0] = init, dst[i] = dst[i - 1] * src[i - 1] for i < n: the running product of plonk/permutation/prover.rs:150-156
-template <class P> static int grand_product_run(PolyBuf *d, PolyBuf *a, size_t n, const void *init, int repr) {
+template <class P> static int grand_product_run(PolyBuf *d, PolyBuf *a, size_t n, const void *init, const HostArgs &h) {
     Context &X = g_ctx;
     cudaStream_t s = X.stream;
     std::vector<uint64_t> m{(uint64_t)n}, off{0};
@@ -202,7 +201,7 @@ template <class P> static int grand_product_run(PolyBuf *d, PolyBuf *a, size_t n
     if (X.po_lvl.ensure(total * sizeof(fe)) || X.po_q.ensure(total * sizeof(fe))) return 1;
     fe *lvl = X.po_lvl.as<fe>(), *ex = X.po_q.as<fe>();
     const fe *src = a->buf.as<fe>();
-    const fe in0 = host_to_mont<P>(init, repr);
+    const fe in0 = h.elem<P>(init);
     for (size_t l = 0; l < L; l++)
         LAUNCH(poly_product_up_kernel<P>, blocks_for(m[l + 1], 128), 128, 0, s, l == 0 ? src : (const fe *)(lvl + off[l]), m[l], lvl + off[l + 1], m[l + 1]);
     for (size_t l = L + 1; l-- > 0;) {
@@ -214,17 +213,19 @@ template <class P> static int grand_product_run(PolyBuf *d, PolyBuf *a, size_t n
 }
 extern "C" int h2_poly_running_product(uint64_t dst, uint64_t src, size_t n, const void *init, int repr) {
     CtxLock lk;
-    if (require_ready()) return 1;
+    const HostArgs h("h2_poly_running_product", repr);
+    if (require_ready() || h.check({{init, "init", n != 0}})) return 1;
     PolyArgs g("h2_poly_running_product");
     PolyBuf *d, *a;
     if (!(d = g.out(dst, n, "n")) || !(a = g.in(src, n, "n")) || g.distinct("a dst")) return 1;
     if (n == 0) return 0;
-    return by_field(a->field, [&](auto p) { return grand_product_run<decltype(p)>(d, a, n, init, repr); });
+    return by_field(a->field, [&](auto p) { return grand_product_run<decltype(p)>(d, a, n, init, h); });
 }
 // divide_by_vanishing_poly on a resident extended-domain polynomial; t_evals: t_len = 2^(ext_k - k) host elements
 extern "C" int h2_poly_divide_by_vanishing(uint64_t poly, uint32_t ext_k, const void *t_evals, uint32_t t_len, int repr) {
     CtxLock lk;
-    if (require_ready()) return 1;
+    const HostArgs h("h2_poly_divide_by_vanishing", repr);
+    if (require_ready() || h.check({{t_evals, "t_evals"}})) return 1;
     if (ext_k > 30) return fail("h2_poly_divide_by_vanishing: ext_k > 30");
     PolyArgs g("h2_poly_divide_by_vanishing");
     PolyBuf *a = g.out(poly, (size_t)1 << ext_k, "2^ext_k");
@@ -234,8 +235,7 @@ extern "C" int h2_poly_divide_by_vanishing(uint64_t poly, uint32_t ext_k, const 
     cudaStream_t s = X.stream;
     if (scratch_acquire(s)) return 1;
     if (X.po_pts.ensure((size_t)t_len * sizeof(fe))) return 1;
-    CU(cudaMemcpyAsync(X.po_pts.p, t_evals, (size_t)t_len * sizeof(fe), cudaMemcpyHostToDevice, s));
-    if (repr == H2_REPR_CANONICAL && convert_field(a->field, X.po_pts.as<fe>(), t_len, 1, s)) return 1;
+    if (h.up(a->field, X.po_pts.as<fe>(), t_evals, t_len, s)) return 1;
     const uint64_t n = 1ull << ext_k;
     if (by_field(a->field, [&](auto p) {
             LAUNCH(poly_vanish_div_kernel<decltype(p)>, blocks_for(n, 256), 256, 0, s, a->buf.as<fe>(), n, (const fe *)X.po_pts.as<fe>(), t_len - 1);
@@ -245,17 +245,23 @@ extern "C" int h2_poly_divide_by_vanishing(uint64_t poly, uint32_t ext_k, const 
     return scratch_release(s);
 }
 extern "C" int h2_poly_eval(const uint64_t *polys, size_t batch, size_t n, const void *points, int repr, void *out) {
+    const HostArgs h("h2_poly_eval", repr);
+    if (h.check({{points, "points", batch != 0 && n != 0}, {out, "out", batch != 0}})) return 1;
     if (n == 0) { memset(out, 0, batch * 32); return 0; }            // the empty sum (fold over nothing, arithmetic.rs:300-302)
-    return polyops_dispatch(0, polys, nullptr, batch, n, points, repr, out, "h2_poly_eval");
+    return polyops_dispatch(0, polys, nullptr, batch, n, points, h, out);
 }
 extern "C" int h2_poly_inner_product(const uint64_t *a, const uint64_t *b, size_t batch, size_t n, int repr, void *out) {
+    const HostArgs h("h2_poly_inner_product", repr);
+    if (h.check({{out, "out", batch != 0}})) return 1;
     if (n == 0) { memset(out, 0, batch * 32); return 0; }
-    return polyops_dispatch(1, a, b, batch, n, nullptr, repr, out, "h2_poly_inner_product");
+    return polyops_dispatch(1, a, b, batch, n, nullptr, h, out);
 }
 extern "C" int h2_poly_kate_division(const uint64_t *dst, const uint64_t *src, size_t batch, size_t n, const void *points, int repr) {
+    const HostArgs h("h2_poly_kate_division", repr);
+    if (h.check({{points, "points", batch != 0 && n > 1}})) return 1;
     if (n == 0) return fail("h2_poly_kate_division: empty polynomial (the reference underflows a.len() - 1, arithmetic.rs:329)");
     if (n == 1) return 0;                                             // quotient of a constant: no coefficients
-    return polyops_dispatch(2, src, dst, batch, n, points, repr, nullptr, "h2_poly_kate_division");
+    return polyops_dispatch(2, src, dst, batch, n, points, h, nullptr);
 }
 
 
@@ -291,11 +297,12 @@ template <class P> static int lk_sort(fe *keys, uint64_t N, uint32_t count, cuda
 // blinding rows [u, u + rows) of every output.  Scratch from the lane's pools, per lookup (N = the power of two >= u, >= 2):
 //   lk_keys  32 N bytes (the sorted table)          lk_u32  4 (3 u + 2) bytes (cnt | unconsumed, scanned in one pass; leftovers)
 //   lk_aux   32 bytes of pointers + 64 rows bytes of blinding values;  plus 4 bytes per 8192 scanned words and the error word.
-// One synchronisation; *bad = the lowest lookup with an input value its table lacks, H2_LK_NONE when none -- and then
-// every output is as it was (the one writing kernel runs after the miss is known and checks for it first).
+// `h`: the encoding of the blinding values (nullptr without them).  One synchronisation; *bad = the lowest lookup with an input value
+// its table lacks, H2_LK_NONE when none -- and then every output is as it was (the one writing kernel runs after the miss is known and
+// checks for it first).
 template <class P>
 static int lookup_permuted_run(const std::vector<PolyBuf *> &outs, const std::vector<PolyBuf *> &ins, uint64_t u, uint64_t rows, const void *blinding,
-                               int repr, uint32_t *bad) {
+                               const HostArgs *h, uint32_t *bad) {
     Context &X = g_ctx;
     cudaStream_t s = X.stream;
     const uint32_t count = (uint32_t)(ins.size() / 2);
@@ -322,7 +329,7 @@ static int lookup_permuted_run(const std::vector<PolyBuf *> &outs, const std::ve
     c.out_in = reinterpret_cast<fe *const *>(aux) + 2 * count;
     c.out_tab = c.out_in + count;
     c.blind = nblind ? aux + ptr_fe : nullptr;
-    if (nblind && repr == H2_REPR_CANONICAL) LAUNCH(convert_kernel<P>, blocks_for(nblind, 64), 64, 0, s, aux + ptr_fe, nblind, 1);
+    if (nblind && h->to_mont(P::ID, aux + ptr_fe, nblind, s)) return 1;
     CU(cudaMemsetAsync(sc, 0, w * count * sizeof(uint32_t), s));
     CU(cudaMemsetAsync(err, 0xFF, sizeof(uint32_t), s));
     LAUNCH(lk_load_kernel<P>, dim3(blocks_for(N, 256), count), 256, 0, s, c, u, keys, N);
@@ -350,7 +357,7 @@ extern "C" int h2_poly_lookup_permute(uint64_t input, uint64_t table, size_t usa
     if (usable_rows >= (1ull << 31)) return fail("h2_poly_lookup_permute: usable_rows >= 2^31");
     if (usable_rows == 0) return 0;
     uint32_t bad = H2_LK_NONE;
-    if (by_field(outs[0]->field, [&](auto p) { return lookup_permuted_run<decltype(p)>(outs, ins, usable_rows, 0, nullptr, H2_REPR_MONTGOMERY, &bad); }))
+    if (by_field(outs[0]->field, [&](auto p) { return lookup_permuted_run<decltype(p)>(outs, ins, usable_rows, 0, nullptr, nullptr, &bad); }))
         return 1;
     if (bad != H2_LK_NONE) return fail(std::string(who) + ": " + lk_miss);
     return 0;
@@ -359,11 +366,12 @@ extern "C" int h2_poly_lookup_permuted(const uint64_t *out_inputs, const uint64_
                                        uint32_t k, const void *blinding, uint32_t blinding_factors, int repr) {
     static const char *who = "h2_poly_lookup_permuted";
     CtxLock lk;
-    if (require_ready()) return 1;
+    const HostArgs h(who, repr);
+    if (require_ready() || h.check({{blinding, "blinding", count != 0}})) return 1;
     if (k > 30) return fail(std::string(who) + ": k > 30");
     if ((uint64_t)blinding_factors + 1 >= (1ull << k)) return fail(std::string(who) + ": blinding_factors + 1 >= n");
     if (count == 0) return 0;
-    if (!out_inputs || !out_tables || !inputs || !tables || !blinding) return fail(std::string(who) + ": null argument");
+    if (!out_inputs || !out_tables || !inputs || !tables) return fail(std::string(who) + ": null argument");
     if (count > 65535) return fail(std::string(who) + ": more than 65535 lookups");
     std::vector<uint64_t> oh, ih;
     for (size_t b = 0; b < count; b++) {
@@ -375,7 +383,7 @@ extern "C" int h2_poly_lookup_permuted(const uint64_t *out_inputs, const uint64_
     std::vector<PolyBuf *> outs, ins;
     if (g.out(oh.data(), 2 * count, n, "2^k", outs) || g.in(ih.data(), 2 * count, n, "2^k", ins) || g.distinct("an output")) return 1;
     uint32_t bad = H2_LK_NONE;
-    if (by_field(outs[0]->field, [&](auto p) { return lookup_permuted_run<decltype(p)>(outs, ins, n - rows, rows, blinding, repr, &bad); })) return 1;
+    if (by_field(outs[0]->field, [&](auto p) { return lookup_permuted_run<decltype(p)>(outs, ins, n - rows, rows, blinding, &h, &bad); })) return 1;
     if (bad != H2_LK_NONE) return fail(std::string(who) + ": lookup " + std::to_string(bad) + ": " + lk_miss);
     return 0;
 }
@@ -386,45 +394,43 @@ extern "C" int h2_poly_lookup_permuted(const uint64_t *out_inputs, const uint64_
 // ------------------------------------------------------------------------------------------------
 // dst[i] (+)= init * prod_{j : bit j of i} u[k - 1 - j], i < 2^k: compute_s (poly/commitment/verifier.rs:156-171); with
 // `accumulate` the add_to_g_scalars of Guard::use_challenges (:36-41, msm.rs:104-113) in the same pass
-template <class P> static int compute_s_run(PolyBuf *d, const void *u, uint32_t k, const void *init, int accumulate, int repr) {
+template <class P> static int compute_s_run(PolyBuf *d, const void *u, uint32_t k, const void *init, int accumulate, const HostArgs &h) {
     Context &X = g_ctx;
     cudaStream_t s = X.stream;
     if (scratch_acquire(s)) return 1;
     if (X.po_pts.ensure((size_t)k * sizeof(fe))) return 1;
     fe *du = X.po_pts.as<fe>();
-    CU(cudaMemcpyAsync(du, u, (size_t)k * sizeof(fe), cudaMemcpyHostToDevice, s));
-    if (repr == H2_REPR_CANONICAL) LAUNCH(convert_kernel<P>, blocks_for(k, 64), 64, 0, s, du, (uint64_t)k, 1);
+    if (h.up(P::ID, du, u, k, s)) return 1;
     const uint64_t groups = 1ull << (k - (k < 2 ? k : 2));
-    LAUNCH(verifier_compute_s_kernel<P>, blocks_for(groups, 128), 128, 0, s, d->buf.as<fe>(), (const fe *)du, k, host_to_mont<P>(init, repr), accumulate);
+    LAUNCH(verifier_compute_s_kernel<P>, blocks_for(groups, 128), 128, 0, s, d->buf.as<fe>(), (const fe *)du, k, h.elem<P>(init), accumulate);
     return scratch_release(s);
 }
 extern "C" int h2_poly_compute_s(uint64_t dst, const void *u, uint32_t k, const void *init, int accumulate, int repr) {
     CtxLock lk;
-    if (require_ready()) return 1;
-    if (!u || !init) return fail("h2_poly_compute_s: null challenge vector or init");
+    const HostArgs h("h2_poly_compute_s", repr);
+    if (require_ready() || h.check({{u, "u"}, {init, "init"}})) return 1;
     if (k == 0) return fail("h2_poly_compute_s: no challenges (assert!(!u.is_empty()), poly/commitment/verifier.rs:157)");
     if (k > 30) return fail("h2_poly_compute_s: k > 30");
     PolyArgs g("h2_poly_compute_s");
     PolyBuf *d = g.out(dst, (size_t)1 << k, "2^k");
     if (!d) return 1;
-    return by_field(d->field, [&](auto p) { return compute_s_run<decltype(p)>(d, u, k, init, accumulate, repr); });
+    return by_field(d->field, [&](auto p) { return compute_s_run<decltype(p)>(d, u, k, init, accumulate, h); });
 }
 // dst[i] = a * dst[i] + b * src[i], i < n (src == 0: dst[i] *= a): MSM::scale and the g_scalars part of MSM::add_msm
 // (poly/commitment/msm.rs:126-139, :37-62); BatchVerifier's accumulate_msm (plonk/verifier/batch.rs:83-93) is one call
 extern "C" int h2_poly_scale_add(uint64_t dst, const void *a, uint64_t src, const void *b, size_t n, int repr) {
     CtxLock lk;
-    if (require_ready()) return 1;
+    const HostArgs h("h2_poly_scale_add", repr);
+    if (require_ready() || h.check({{a, "a"}, {b, "b", src != 0}})) return 1;
     PolyArgs g("h2_poly_scale_add");
     PolyBuf *d = g.out(dst, n, "n"), *x = nullptr;
     if (!d || (src && !(x = g.in(src, n, "n"))) || g.distinct("a dst")) return 1;
-    if (!a || (x && !b)) return fail("h2_poly_scale_add: null factor");
     if (n == 0) return 0;
     cudaStream_t s = g_ctx.stream;
     const fe *sp = x ? x->buf.as<fe>() : nullptr;
     return by_field(d->field, [&](auto p) {
         using P = decltype(p);
-        LAUNCH(verifier_scale_add_kernel<P>, blocks_for(n, 256), 256, 0, s, d->buf.as<fe>(), sp, host_to_mont<P>(a, repr), x ? host_to_mont<P>(b, repr) : fe_zero(),
-               (uint64_t)n);
+        LAUNCH(verifier_scale_add_kernel<P>, blocks_for(n, 256), 256, 0, s, d->buf.as<fe>(), sp, h.elem<P>(a), x ? h.elem<P>(b) : fe_zero(), (uint64_t)n);
         return 0;
     });
 }
@@ -439,7 +445,7 @@ extern "C" int h2_poly_scale_add(uint64_t dst, const void *a, uint64_t src, cons
 // The launches both entry points share: the power tables, then one sigma launch per (column, piece) of the mapping, then
 // the error word back.  sigma_tables is called after scratch_acquire; sigma_finish releases the scratch and synchronises.
 template <class P>
-static int sigma_tables(uint32_t k, uint64_t cols, const void *omega, const void *delta, int repr, fe **tab, uint32_t **err) {
+static int sigma_tables(uint32_t k, uint64_t cols, const void *omega, const void *delta, const HostArgs &h, fe **tab, uint32_t **err) {
     Context &X = g_ctx;
     cudaStream_t s = X.stream;
     const uint64_t tlen = KeygenOps<P>::table_len(k, (uint32_t)cols);
@@ -447,7 +453,7 @@ static int sigma_tables(uint32_t k, uint64_t cols, const void *omega, const void
     *tab = X.kg_tab.as<fe>();
     *err = reinterpret_cast<uint32_t *>(*tab + tlen);
     CU(cudaMemsetAsync(*err, 0, sizeof(uint32_t), s));
-    LAUNCH(keygen_tables_kernel<P>, blocks_for(tlen, 128), 128, 0, s, *tab, host_to_mont<P>(omega, repr), host_to_mont<P>(delta, repr), k, (uint32_t)cols);
+    LAUNCH(keygen_tables_kernel<P>, blocks_for(tlen, 128), 128, 0, s, *tab, h.elem<P>(omega), h.elem<P>(delta), k, (uint32_t)cols);
     return 0;
 }
 template <class P>
@@ -465,7 +471,8 @@ static int sigma_finish(uint32_t *err, const char *who) {
     return 0;
 }
 template <class P>
-static int permutation_sigma_run(const std::vector<PolyBuf *> &dst, uint32_t k, const uint32_t *mapping, const void *omega, const void *delta, int repr) {
+static int permutation_sigma_run(const std::vector<PolyBuf *> &dst, uint32_t k, const uint32_t *mapping, const void *omega, const void *delta,
+                                 const HostArgs &h) {
     Context &X = g_ctx;
     cudaStream_t s = X.stream;
     const uint64_t n = 1ull << k, cols = dst.size();
@@ -473,7 +480,7 @@ static int permutation_sigma_run(const std::vector<PolyBuf *> &dst, uint32_t k, 
     fe *tab;
     uint32_t *err;
     if (scratch_acquire(s)) return 1;
-    if (X.kg_map.ensure(piece * sizeof(uint2)) || sigma_tables<P>(k, cols, omega, delta, repr, &tab, &err)) return 1;
+    if (X.kg_map.ensure(piece * sizeof(uint2)) || sigma_tables<P>(k, cols, omega, delta, h, &tab, &err)) return 1;
     uint2 *map = X.kg_map.as<uint2>();
     for (uint64_t i = 0; i < cols; i++)
         for (uint64_t j0 = 0; j0 < n; j0 += piece) {
@@ -486,15 +493,16 @@ static int permutation_sigma_run(const std::vector<PolyBuf *> &dst, uint32_t k, 
 extern "C" int h2_poly_permutation_sigma(const uint64_t *dst, size_t cols, uint32_t k, const uint32_t *mapping, const void *omega, const void *delta,
                                          int repr) {
     CtxLock lk;
-    if (require_ready()) return 1;
+    const HostArgs h("h2_poly_permutation_sigma", repr);
+    if (require_ready() || h.check({{omega, "omega", cols != 0}, {delta, "delta", cols != 0}})) return 1;
     if (k > 30) return fail("h2_poly_permutation_sigma: k > 30");
     if (cols == 0) return 0;
     if (cols >= (1ull << 32)) return fail("h2_poly_permutation_sigma: cols >= 2^32");
-    if (!dst || !mapping || !omega || !delta) return fail("h2_poly_permutation_sigma: null argument");
+    if (!dst || !mapping) return fail("h2_poly_permutation_sigma: null argument");
     PolyArgs g("h2_poly_permutation_sigma");
     std::vector<PolyBuf *> d;
     if (g.out(dst, cols, (size_t)1 << k, "2^k", d) || g.distinct("a dst")) return 1;
-    return by_field(d[0]->field, [&](auto p) { return permutation_sigma_run<decltype(p)>(d, k, mapping, omega, delta, repr); });
+    return by_field(d[0]->field, [&](auto p) { return permutation_sigma_run<decltype(p)>(d, k, mapping, omega, delta, h); });
 }
 
 
@@ -586,7 +594,7 @@ static int assembly_run(uint32_t cols, uint32_t k, const uint32_t *copies, uint6
 }
 template <class P>
 static int permutation_sigma_copies_run(const std::vector<PolyBuf *> &dst, uint32_t k, const uint32_t *copies, uint64_t m, const void *omega,
-                                        const void *delta, int repr) {
+                                        const void *delta, const HostArgs &h) {
     Context &X = g_ctx;
     cudaStream_t s = X.stream;
     const uint64_t n = 1ull << k, cols = dst.size();
@@ -600,7 +608,7 @@ static int permutation_sigma_copies_run(const std::vector<PolyBuf *> &dst, uint3
     }
     fe *tab;
     uint32_t *err;
-    if (sigma_tables<P>(k, cols, omega, delta, repr, &tab, &err)) return 1;
+    if (sigma_tables<P>(k, cols, omega, delta, h, &tab, &err)) return 1;
     const uint2 *map = X.kg_map.as<uint2>();
     for (uint64_t i = 0; i < cols; i++)
         if (sigma_launch<P>(dst[i], 0, map + i * n, n, k, cols, tab, err)) return 1;
@@ -609,17 +617,18 @@ static int permutation_sigma_copies_run(const std::vector<PolyBuf *> &dst, uint3
 extern "C" int h2_poly_permutation_sigma_copies(const uint64_t *dst, size_t cols, uint32_t k, const uint32_t *copies, size_t m, const void *omega,
                                                 const void *delta, int repr) {
     CtxLock lk;
-    if (require_ready()) return 1;
+    const HostArgs h("h2_poly_permutation_sigma_copies", repr);
+    if (require_ready() || h.check({{omega, "omega", cols != 0}, {delta, "delta", cols != 0}})) return 1;
     if (k > 30) return fail("h2_poly_permutation_sigma_copies: k > 30");
     if (cols == 0) return 0;
     if (cols >= (1ull << 32)) return fail("h2_poly_permutation_sigma_copies: cols >= 2^32");
-    if (!dst || (m && !copies) || !omega || !delta) return fail("h2_poly_permutation_sigma_copies: null argument");
+    if (!dst || (m && !copies)) return fail("h2_poly_permutation_sigma_copies: null argument");
     if (((uint64_t)cols << k) >= (1ull << 32)) return fail("h2_poly_permutation_sigma_copies: cols * 2^k >= 2^32 cells");
     if ((uint64_t)m >= (1ull << 32)) return fail("h2_poly_permutation_sigma_copies: m >= 2^32 copies");
     PolyArgs g("h2_poly_permutation_sigma_copies");
     std::vector<PolyBuf *> d;
     if (g.out(dst, cols, (size_t)1 << k, "2^k", d) || g.distinct("a dst")) return 1;
-    return by_field(d[0]->field, [&](auto p) { return permutation_sigma_copies_run<decltype(p)>(d, k, copies, m, omega, delta, repr); });
+    return by_field(d[0]->field, [&](auto p) { return permutation_sigma_copies_run<decltype(p)>(d, k, copies, m, omega, delta, h); });
 }
 
 
@@ -632,7 +641,7 @@ extern "C" int h2_poly_permutation_sigma_copies(const uint64_t *dst, size_t cols
 template <class P>
 static int product_run(bool perm, const std::vector<PolyBuf *> &z, const std::vector<PolyBuf *> &ins, uint32_t ncols, uint32_t chunk_len,
                        uint32_t sets, uint32_t k, const void *beta, const void *gamma, const void *omega, const void *delta, const void *blinding,
-                       uint32_t bf, int repr) {
+                       uint32_t bf, const HostArgs &h) {
     Context &X = g_ctx;
     cudaStream_t s = X.stream;
     const uint64_t n = 1ull << k, count = z.size();
@@ -656,10 +665,10 @@ static int product_run(bool perm, const std::vector<PolyBuf *> &z, const std::ve
     fe *const *zp = reinterpret_cast<fe *const *>(aux);
     const fe *const *ip = reinterpret_cast<const fe *const *>(aux) + count;
     CU(cudaMemcpyAsync(aux, up.data(), up.size(), cudaMemcpyHostToDevice, s));
-    if (nblind && repr == H2_REPR_CANONICAL) LAUNCH(convert_kernel<P>, blocks_for(nblind, 64), 64, 0, s, blind, nblind, 1);
-    const fe b_m = host_to_mont<P>(beta, repr), g_m = host_to_mont<P>(gamma, repr);
+    if (h.to_mont(P::ID, blind, nblind, s)) return 1;
+    const fe b_m = h.elem<P>(beta), g_m = h.elem<P>(gamma);
     if (perm) {
-        LAUNCH(keygen_tables_kernel<P>, blocks_for(tlen, 128), 128, 0, s, tab, host_to_mont<P>(omega, repr), host_to_mont<P>(delta, repr), k, ncols);
+        LAUNCH(keygen_tables_kernel<P>, blocks_for(tlen, 128), 128, 0, s, tab, h.elem<P>(omega), h.elem<P>(delta), k, ncols);
         LAUNCH(gp_perm_factors_kernel<P>, dim3(blocks_for(n, 128), (uint32_t)count), 128, 0, s, ip, ip + (count / sets) * ncols, ncols, chunk_len, sets,
                (const fe *)tab, k, b_m, g_m, val, zp);
     } else {
@@ -689,11 +698,15 @@ extern "C" int h2_poly_permutation_product(const uint64_t *z_out, size_t proofs,
                                            const void *blinding, uint32_t blinding_factors, int repr) {
     static const char *who = "h2_poly_permutation_product";
     CtxLock lk;
-    if (require_ready()) return 1;
+    const HostArgs h(who, repr);
+    const bool work = proofs != 0 && cols != 0;
+    if (require_ready() || h.check({{beta, "beta", work}, {gamma, "gamma", work}, {omega, "omega", work}, {delta, "delta", work},
+                                    {blinding, "blinding", work && blinding_factors != 0}}))
+        return 1;
     if (product_scalars(who, k, blinding_factors)) return 1;
     if (chunk_len == 0) return fail(std::string(who) + ": chunk_len == 0");
     if (proofs == 0 || cols == 0) return 0;
-    if (!z_out || !columns || !sigmas || !beta || !gamma || !omega || !delta || (blinding_factors && !blinding)) return fail(std::string(who) + ": null argument");
+    if (!z_out || !columns || !sigmas) return fail(std::string(who) + ": null argument");
     const uint64_t sets = (cols + chunk_len - 1) / chunk_len;
     if (cols >= (1ull << 20) || proofs >= (1ull << 16) || proofs * sets > 65535) return fail(std::string(who) + ": more than 65535 product columns");
     std::vector<uint64_t> ih(columns, columns + proofs * cols);
@@ -702,7 +715,7 @@ extern "C" int h2_poly_permutation_product(const uint64_t *z_out, size_t proofs,
     std::vector<PolyBuf *> z, ins;
     if (g.out(z_out, proofs * sets, 1ull << k, "2^k", z) || g.in(ih.data(), ih.size(), 1ull << k, "2^k", ins) || g.distinct("a z_out")) return 1;
     return by_field(z[0]->field, [&](auto p) {
-        return product_run<decltype(p)>(true, z, ins, (uint32_t)cols, chunk_len, (uint32_t)sets, k, beta, gamma, omega, delta, blinding, blinding_factors, repr);
+        return product_run<decltype(p)>(true, z, ins, (uint32_t)cols, chunk_len, (uint32_t)sets, k, beta, gamma, omega, delta, blinding, blinding_factors, h);
     });
 }
 extern "C" int h2_poly_lookup_product(const uint64_t *z_out, size_t count, const uint64_t *inputs, const uint64_t *tables, const uint64_t *permuted_inputs,
@@ -710,16 +723,17 @@ extern "C" int h2_poly_lookup_product(const uint64_t *z_out, size_t count, const
                                       uint32_t blinding_factors, int repr) {
     static const char *who = "h2_poly_lookup_product";
     CtxLock lk;
-    if (require_ready()) return 1;
+    const HostArgs h(who, repr);
+    const bool work = count != 0;
+    if (require_ready() || h.check({{beta, "beta", work}, {gamma, "gamma", work}, {blinding, "blinding", work && blinding_factors != 0}})) return 1;
     if (product_scalars(who, k, blinding_factors)) return 1;
     if (count == 0) return 0;
-    if (!z_out || !inputs || !tables || !permuted_inputs || !permuted_tables || !beta || !gamma || (blinding_factors && !blinding))
-        return fail(std::string(who) + ": null argument");
+    if (!z_out || !inputs || !tables || !permuted_inputs || !permuted_tables) return fail(std::string(who) + ": null argument");
     if (count > 65535) return fail(std::string(who) + ": more than 65535 product columns");
     std::vector<uint64_t> ih;
     for (size_t b = 0; b < count; b++) ih.insert(ih.end(), {inputs[b], tables[b], permuted_inputs[b], permuted_tables[b]});
     PolyArgs g(who);
     std::vector<PolyBuf *> z, ins;
     if (g.out(z_out, count, 1ull << k, "2^k", z) || g.in(ih.data(), ih.size(), 1ull << k, "2^k", ins) || g.distinct("a z_out")) return 1;
-    return by_field(z[0]->field, [&](auto p) { return product_run<decltype(p)>(false, z, ins, 0, 1, 1, k, beta, gamma, nullptr, nullptr, blinding, blinding_factors, repr); });
+    return by_field(z[0]->field, [&](auto p) { return product_run<decltype(p)>(false, z, ins, 0, 1, 1, k, beta, gamma, nullptr, nullptr, blinding, blinding_factors, h); });
 }

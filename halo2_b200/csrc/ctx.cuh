@@ -265,11 +265,32 @@ int scratch_acquire(cudaStream_t s);     // make `s` wait for whatever last used
 int scratch_release(cudaStream_t s);
 static inline uint32_t blocks_for(uint64_t n, uint32_t bs) { return (uint32_t)((n + bs - 1) / bs); }
 
-template <class P> static fe host_to_mont(const void *bytes, int repr) {
-    fe x;
-    memcpy(x.v, bytes, 32);
-    return repr == H2_REPR_MONTGOMERY ? x : fe_to_mont<P>(x);
-}
+// The host-side field elements and points of one entry point `who`, in the encoding `repr` (include/halo2_b200.h).
+// check() runs before the call acquires scratch, copies or launches anything:
+//   - repr is H2_REPR_CANONICAL or H2_REPR_MONTGOMERY, else "<who>: unknown repr";
+//   - every required host pointer is set, else "<who>: null <name>" (name as in the header); a Need whose `required` is
+//     false (an optional pointer, or an array of no elements) is not checked.
+// Then a single element is read into Montgomery form (elem), an array goes to the device and into Montgomery form (up, or
+// to_mont after a copy of the caller's own), and device elements come back in repr (down from resident data, which stays
+// in Montgomery form; from_mont on scratch).  canon() / mont() are for kernels that take the encoding as a flag.
+struct HostArgs {
+    struct Need { const void *p; const char *name; bool required = true; };
+    HostArgs(const char *who, int repr) : who(who), repr(repr) {}
+    int check(std::initializer_list<Need> needs = {}) const;
+    bool canon() const { return repr == H2_REPR_CANONICAL; }
+    bool mont() const { return repr == H2_REPR_MONTGOMERY; }
+    template <class P> fe elem(const void *bytes) const {
+        fe x;
+        memcpy(x.v, bytes, 32);
+        return mont() ? x : fe_to_mont<P>(x);
+    }
+    int up(int field, fe *d, const void *h, size_t n, cudaStream_t s) const;   // upload_async, then to_mont
+    int to_mont(int field, fe *d, size_t n, cudaStream_t s) const;             // device elements in repr -> Montgomery, in place
+    int from_mont(int field, fe *d, size_t n, cudaStream_t s) const;           // Montgomery -> repr, in place (scratch only)
+    int down(int field, void *h, const fe *d, size_t n, cudaStream_t s) const; // to the host in repr; canonical converts a scratch copy
+    const char *who;
+    int repr;
+};
 // Shared polynomials (h2_poly_share): read-only from then on, and readable from every context.  Sharing moves them out of
 // their owner's `polys` into this registry with unchanged handles; they never go into a poly_pool.
 extern std::map<uint64_t, PolyBuf *> g_shared_polys;

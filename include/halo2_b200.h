@@ -13,6 +13,12 @@
  *   - Field element = 32 bytes = 4 x u64 little-endian limbs.  `repr` selects the encoding:
  *       H2_REPR_CANONICAL   the integer itself (ff::PrimeField::to_repr, arithmetic.rs:77)
  *       H2_REPR_MONTGOMERY  x * 2^256 mod m (pasta_curves' in-memory form: zero-copy path)
+ *     for every host element and point a call takes or returns (coordinate by coordinate).  Before it copies or
+ *     launches anything, a call fails with "<entry point>: unknown repr" for any other value, and with
+ *     "<entry point>: null <parameter>" when a host element or element array it reads or writes is NULL.  An array of
+ *     no elements may be NULL, and so may an element the call does not touch: every element of a call with nothing
+ *     to do (count, cols or proofs == 0), the init of a running product of n == 0, the points of an evaluation of
+ *     n == 0 or of a Kate division of n <= 1; so may the optional pointers documented below.  repr is checked even then.
  *   - Affine point = x || y (64 bytes); the identity is 64 zero bytes
  *     (book/src/background/curves.md:226-230).  Results are Jacobian x || y || z (96 bytes,
  *     the layout of pasta's Ep/Eq); identity has z = 0.  Only the group element is defined
