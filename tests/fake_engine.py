@@ -260,6 +260,8 @@ class FakeLib:
         self._log("h2_poly_eval_ast")
         n_polys, log_n, n_code, n_consts = _v(n_polys), _v(log_n), _v(n_code), _v(n_consts)
         n = 1 << log_n
+        if n_code == 0 or n_code > 1 << 20:
+            return self._fail("h2_poly_eval_ast: empty or oversized program")
         prog = np.frombuffer(ctypes.string_at(_v(code), 16 * n_code), dtype=np.uint32).reshape(-1, 4).copy()
         depth = 0                                                 # the library's own validation (capi_poly.cu): operand stack of 24
         for op, arg, _, _ in prog:

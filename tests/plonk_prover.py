@@ -297,6 +297,82 @@ def _to_ast(eng, e, fixed_l, advice_l, instance_l):
     raise ValueError(name)
 
 
+# The Ast programs create_proof_engine evaluates, built from leaves alone so that a test can run exactly the prover's programs
+# over columns of its own.  Column arguments are lists of leaves; a permutation or lookup argument's leaves come in its order.
+def lookup_compression(eng, exprs, theta: int, fixed, advice, instance):
+    """compress_expressions of lookup/prover.rs commit_permuted: a lookup's input or table expressions compressed by powers of theta (Lagrange basis)."""
+    acc = eng.Ast.constant_term(0)
+    for e in exprs:
+        acc = acc * theta + _to_ast(eng, e, fixed, advice, instance)
+    return acc
+
+
+def permutation_denominator(eng, cols, sigmas, beta: int, gamma: int):
+    """permutation/prover.rs commit, before batch_invert: prod_j (beta * sigma_j + gamma + column_j) over one chunk of columns (Lagrange basis)."""
+    den = None
+    for col, sl in zip(cols, sigmas):
+        term = sl * beta + eng.Ast.constant_term(gamma) + col
+        den = term if den is None else den * term
+    return den
+
+
+def permutation_numerator(eng, inv_den, cols, first: int, beta: int, gamma: int, delta: int, m: int):
+    """permutation/prover.rs commit, after batch_invert: 1 / den * prod_j (beta * delta^(first + j) * omega^row + gamma + column_j); `first` is the
+    chunk's first global column index (Lagrange basis)."""
+    num = inv_den
+    for j, col in enumerate(cols):
+        num = num * (eng.Ast.linear_term(pow(delta, first + j, m) * beta % m) + eng.Ast.constant_term(gamma) + col)
+    return num
+
+
+def lookup_product_denominator(eng, permuted_input, permuted_table, beta: int, gamma: int):
+    """lookup/prover.rs commit_product, before batch_invert: (A' + beta) (S' + gamma) (Lagrange basis)."""
+    return (permuted_input + eng.Ast.constant_term(beta)) * (permuted_table + eng.Ast.constant_term(gamma))
+
+
+def lookup_product_numerator(eng, inv_den, input_, table, beta: int, gamma: int):
+    """lookup/prover.rs commit_product, after batch_invert: 1 / den * (A + beta) (S + gamma), A and S the compressed columns (Lagrange basis)."""
+    return inv_den * (input_ + eng.Ast.constant_term(beta)) * (table + eng.Ast.constant_term(gamma))
+
+
+def vanishing_expressions(eng, vk: PV.PinnedKey, beta: int, gamma: int, delta: int, fixed, sigmas, lagrange, advice, instance, perm_z, lookups):
+    """The h(X) constraints of one proof over the extended coset, in the reference's order (prover.rs:460-564): the gates, the
+    permutation argument's (permutation/prover.rs construct), then each lookup's (lookup/prover.rs construct).  `lagrange`: the
+    (l_0, l_blind, l_last) leaves; `perm_z`: one leaf per permutation set; `lookups`: (Z, A', S', A, S) leaves per lookup."""
+    Ast = eng.Ast
+    m = vk.scalar_modulus
+    chunk_len = vk.degree() - 2
+    last_rot = -(vk.blinding_factors() + 1)
+    L0, LB, LL = lagrange
+    one = Ast.constant_term(1)
+    active = one - (LL + LB)
+    exprs = [_to_ast(eng, gate, fixed, advice, instance) for gate in vk.gates]
+    if perm_z:
+        exprs.append((one - perm_z[0]) * L0)
+        exprs.append((perm_z[-1] * perm_z[-1] - perm_z[-1]) * LL)
+        for a in range(1, len(perm_z)):
+            exprs.append((perm_z[a] - perm_z[a - 1].with_rotation(last_rot)) * L0)
+        colc = lambda col: {"Advice": advice, "Fixed": fixed, "Instance": instance}[col[0]][col[1]]
+        for a in range(len(perm_z)):
+            cols = vk.permutation_columns[a * chunk_len:(a + 1) * chunk_len]
+            left = perm_z[a].with_rotation(1)
+            for col, sc in zip(cols, sigmas[a * chunk_len:(a + 1) * chunk_len]):
+                left = left * (colc(col) + sc * beta + Ast.constant_term(gamma))
+            right = perm_z[a]
+            for j, col in enumerate(cols):
+                right = right * (colc(col) + Ast.linear_term(beta * pow(delta, a * chunk_len + j, m) % m) + Ast.constant_term(gamma))
+            exprs.append((left - right) * active)
+    for Z_, A_, S_, CI_, CT_ in lookups:
+        exprs.append((one - Z_) * L0)
+        exprs.append((Z_ * Z_ - Z_) * LL)
+        left = Z_.with_rotation(1) * (A_ + Ast.constant_term(beta)) * (S_ + Ast.constant_term(gamma))
+        right = Z_ * (CI_ + Ast.constant_term(beta)) * (CT_ + Ast.constant_term(gamma))
+        exprs.append((left - right) * active)
+        exprs.append((A_ - S_) * L0)
+        exprs.append((A_ - S_) * (A_ - A_.with_rotation(-1)) * active)
+    return exprs
+
+
 def create_proof_engine(eng, params, vk: PV.PinnedKey, fixed, sigma, advice, instances, rng, transcript, zeta: int, delta: int, pk=None) -> None:
     """plonk::create_proof (prover.rs:43-727) on the engine.  `params`: halo2_b200.Params with u; `rng`: scalar() -> int,
     poly(n) -> (n, 32) bytes; `transcript`: tests/prover_replay.Blake2bTranscript (points as (64,) uint8).  Columns are lists of
@@ -392,13 +468,7 @@ def create_proof_engine(eng, params, vk: PV.PinnedKey, fixed, sigma, advice, ins
         for pr in range(num_proofs):
             per = []
             for inp, tab in vk.lookups:
-                def compress(exprs):
-                    acc = Ast.constant_term(0)
-                    for e in exprs:
-                        acc = acc * theta + _to_ast(eng, e, FL, AL[pr], IL[pr])
-                    out = ev_l.evaluate(acc, out=RP(None))
-                    return out
-                ci, ct = compress(inp), compress(tab)
+                ci, ct = (ev_l.evaluate(lookup_compression(eng, exprs, theta, FL, AL[pr], IL[pr]), out=RP(None)) for exprs in (inp, tab))
                 pi, pt = eng.permute_expression_pair_resident(ci, ct, usable, RP(None), RP(None))
                 overwrite_rows(pi, usable, [rng.scalar() for _ in range(bf + 1)])
                 overwrite_rows(pt, usable, [rng.scalar() for _ in range(bf + 1)])
@@ -417,15 +487,10 @@ def create_proof_engine(eng, params, vk: PV.PinnedKey, fixed, sigma, advice, ins
         for pr in range(num_proofs):
             sets, last_z = [], 1
             for ci_ in range(0, len(vk.permutation_columns), chunk_len):
-                cols = vk.permutation_columns[ci_:ci_ + chunk_len]
-                den = None
-                for col, sl in zip(cols, SL[ci_:ci_ + chunk_len]):
-                    term = sl * beta + Ast.constant_term(gamma) + col_leaf(pr, col)
-                    den = term if den is None else den * term
+                cols = [col_leaf(pr, col) for col in vk.permutation_columns[ci_:ci_ + chunk_len]]
+                den = permutation_denominator(eng, cols, SL[ci_:ci_ + chunk_len], beta, gamma)
                 inv_den = eng.batch_invert_resident(ev_l.evaluate(den, out=RP(None)))
-                num = ev_l.register_poly(inv_den)
-                for j, col in enumerate(cols):                      # deltaomega = delta^(global column index) * omega^row
-                    num = num * (Ast.linear_term(pow(delta, ci_ + j, m) * beta % m) + Ast.constant_term(gamma) + col_leaf(pr, col))
+                num = permutation_numerator(eng, ev_l.register_poly(inv_den), cols, ci_, beta, gamma, delta, m)
                 mv = ev_l.evaluate(num, out=RP(None))
                 z = eng.running_product_resident(mv, init=last_z, dst=RP(None))
                 overwrite_rows(z, n - bf, [rng.scalar() for _ in range(bf)])
@@ -439,9 +504,8 @@ def create_proof_engine(eng, params, vk: PV.PinnedKey, fixed, sigma, advice, ins
         for pr in range(num_proofs):
             for lk in lookups[pr]:
                 PI, PT, CI, CT = (ev_l.register_poly(lk[kk]) for kk in ("pi", "pt", "ci", "ct"))
-                den = (PI + Ast.constant_term(beta)) * (PT + Ast.constant_term(gamma))
-                inv_den = eng.batch_invert_resident(ev_l.evaluate(den, out=RP(None)))
-                num = ev_l.register_poly(inv_den) * (CI + Ast.constant_term(beta)) * (CT + Ast.constant_term(gamma))
+                inv_den = eng.batch_invert_resident(ev_l.evaluate(lookup_product_denominator(eng, PI, PT, beta, gamma), out=RP(None)))
+                num = lookup_product_numerator(eng, ev_l.register_poly(inv_den), CI, CT, beta, gamma)
                 z = eng.running_product_resident(ev_l.evaluate(num, out=RP(None)), init=1, dst=RP(None))
                 overwrite_rows(z, n - bf, [rng.scalar() for _ in range(bf)])
                 lk["zb"] = rng.scalar()
@@ -459,40 +523,15 @@ def create_proof_engine(eng, params, vk: PV.PinnedKey, fixed, sigma, advice, ins
         FC = [ev_e.register_poly(p) for p in fixed_c]
         SC = [ev_e.register_poly(p) for p in sigma_c]
         L0, LB, LL = (ev_e.register_poly(p) for p in (l0_c, l_blind_c, l_last_c))
-        one = Ast.constant_term(1)
-        active = one - (LL + LB)
-        last_rot = -(bf + 1)
         exprs = []
         for pr in range(num_proofs):
             AC = [ev_e.register_poly(p) for p in adv_c[pr]]
             IC = [ev_e.register_poly(p) for p in inst_c[pr]]
-            exprs += [_to_ast(eng, gate, FC, AC, IC) for gate in vk.gates]
             ZC = [ev_e.register_poly(s["coset"]) for s in perms[pr]]
-            if ZC:
-                exprs.append((one - ZC[0]) * L0)
-                exprs.append((ZC[-1] * ZC[-1] - ZC[-1]) * LL)
-                for a in range(1, len(ZC)):
-                    exprs.append((ZC[a] - ZC[a - 1].with_rotation(last_rot)) * L0)
-                colc = lambda col: {"Advice": AC, "Fixed": FC, "Instance": IC}[col[0]][col[1]]
-                for a in range(len(ZC)):
-                    cols = vk.permutation_columns[a * chunk_len:(a + 1) * chunk_len]
-                    left = ZC[a].with_rotation(1)
-                    for col, sc in zip(cols, SC[a * chunk_len:(a + 1) * chunk_len]):
-                        left = left * (colc(col) + sc * beta + Ast.constant_term(gamma))
-                    right = ZC[a]
-                    for j, col in enumerate(cols):
-                        right = right * (colc(col) + Ast.linear_term(beta * pow(delta, a * chunk_len + j, m) % m) + Ast.constant_term(gamma))
-                    exprs.append((left - right) * active)
-            for lk in lookups[pr]:
-                Z_, A_, S_ = (ev_e.register_poly(ext(lk[kk])) for kk in ("z_poly", "pi_poly", "pt_poly"))
-                CI_, CT_ = (ev_e.register_poly(ext(coeff(lk[kk]))) for kk in ("ci", "ct"))
-                exprs.append((one - Z_) * L0)
-                exprs.append((Z_ * Z_ - Z_) * LL)
-                left = Z_.with_rotation(1) * (A_ + Ast.constant_term(beta)) * (S_ + Ast.constant_term(gamma))
-                right = Z_ * (CI_ + Ast.constant_term(beta)) * (CT_ + Ast.constant_term(gamma))
-                exprs.append((left - right) * active)
-                exprs.append((A_ - S_) * L0)
-                exprs.append((A_ - S_) * (A_ - A_.with_rotation(-1)) * active)
+            LK = [tuple(ev_e.register_poly(ext(lk[kk])) for kk in ("z_poly", "pi_poly", "pt_poly"))
+                  + tuple(ev_e.register_poly(ext(coeff(lk[kk]))) for kk in ("ci", "ct")) for lk in lookups[pr]]
+            exprs += vanishing_expressions(eng, vk, beta, gamma, delta, FC, SC, (L0, LB, LL), AC, IC, ZC, LK)
+        last_rot = -(bf + 1)
         h_ext = ev_e.evaluate(Ast.distribute_powers(exprs, y), out=RP(None, L))
         D.divide_by_vanishing_poly_resident(h_ext)
         h = D.extended_to_coeff_resident(h_ext, out=RP(None, n * (cs_degree - 1)))
@@ -672,12 +711,7 @@ class CrefProver:
         for pr in range(num_proofs):
             per = []
             for inp, tab in vk.lookups:
-                def compress(exprs):
-                    acc = Ast.constant_term(0)
-                    for e in exprs:
-                        acc = acc * theta + _to_ast(Eng, e, FL, AL[pr], IL[pr])
-                    return run_ast(acc, lag_polys, False)
-                ci, ct = compress(inp), compress(tab)
+                ci, ct = (run_ast(lookup_compression(Eng, exprs, theta, FL, AL[pr], IL[pr]), lag_polys, False) for exprs in (inp, tab))
                 res = cref.permute_expression_pair(ci, ct, usable)
                 assert res is not None, "an input value does not occur in the table"
                 pi = np.concatenate([res[0], cref.ints_to_bytes([rng.scalar() for _ in range(bf + 1)])])
@@ -749,40 +783,15 @@ class CrefProver:
             ext_polys.append(p)
             return AstLeaf(len(ext_polys) - 1)
 
-        one = Ast.constant_term(1)
-        active = one - (LL + LB)
-        last_rot = -(bf + 1)
         exprs = []
         for pr in range(num_proofs):
             AC = [reg(p) for p in adv_c[pr]]
             IC = [reg(p) for p in inst_c[pr]]
-            exprs += [_to_ast(Eng, gate, FC, AC, IC) for gate in vk.gates]
             ZC = [reg(s_["coset"]) for s_ in perms[pr]]
-            if ZC:
-                exprs.append((one - ZC[0]) * L0)
-                exprs.append((ZC[-1] * ZC[-1] - ZC[-1]) * LL)
-                for a in range(1, len(ZC)):
-                    exprs.append((ZC[a] - ZC[a - 1].with_rotation(last_rot)) * L0)
-                colc = lambda col: {"Advice": AC, "Fixed": FC, "Instance": IC}[col[0]][col[1]]
-                for a in range(len(ZC)):
-                    cols = vk.permutation_columns[a * chunk_len:(a + 1) * chunk_len]
-                    left = ZC[a].with_rotation(1)
-                    for col, sc in zip(cols, SC[a * chunk_len:(a + 1) * chunk_len]):
-                        left = left * (colc(col) + sc * beta + Ast.constant_term(gamma))
-                    right = ZC[a]
-                    for j, col in enumerate(cols):
-                        right = right * (colc(col) + Ast.linear_term(beta * pow(delta, a * chunk_len + j, m) % m) + Ast.constant_term(gamma))
-                    exprs.append((left - right) * active)
-            for lk in lookups[pr]:
-                Z_, A_, S_ = (reg(c2e(lk[kk])) for kk in ("z_poly", "pi_poly", "pt_poly"))
-                CI_, CT_ = (reg(c2e(l2c(lk[kk]))) for kk in ("ci", "ct"))
-                exprs.append((one - Z_) * L0)
-                exprs.append((Z_ * Z_ - Z_) * LL)
-                left = Z_.with_rotation(1) * (A_ + Ast.constant_term(beta)) * (S_ + Ast.constant_term(gamma))
-                right = Z_ * (CI_ + Ast.constant_term(beta)) * (CT_ + Ast.constant_term(gamma))
-                exprs.append((left - right) * active)
-                exprs.append((A_ - S_) * L0)
-                exprs.append((A_ - S_) * (A_ - A_.with_rotation(-1)) * active)
+            LK = [tuple(reg(c2e(lk[kk])) for kk in ("z_poly", "pi_poly", "pt_poly")) + tuple(reg(c2e(l2c(lk[kk]))) for kk in ("ci", "ct"))
+                  for lk in lookups[pr]]
+            exprs += vanishing_expressions(Eng, vk, beta, gamma, delta, FC, SC, (L0, LB, LL), AC, IC, ZC, LK)
+        last_rot = -(bf + 1)
         h_ext = run_ast(Ast.distribute_powers(exprs, y), ext_polys, True)
         tev = cref.ints_to_bytes(D.t_evaluations)                  # divide_by_vanishing_poly (domain.rs:329-348) as an elementwise program
         tfull = tev[np.arange(L) % len(D.t_evaluations)]
