@@ -116,6 +116,11 @@ extern "C" {
                                   blinding_factors: u32, repr: c_int) -> c_int;
     pub fn h2_poly_lookup_permuted(out_inputs: *const u64, out_tables: *const u64, count: usize, inputs: *const u64, tables: *const u64, k: u32,
                                    blinding: *const c_void, blinding_factors: u32, repr: c_int) -> c_int;
+    pub fn h2_poly_lagrange_to_coeff_batch(dst: *const u64, src: *const u64, count: usize, k: u32, omega_inv: *const c_void, divisor: *const c_void,
+                                           repr: c_int) -> c_int;
+    pub fn h2_poly_coeff_to_extended_batch(dst: *const u64, src: *const u64, count: usize, k: u32, ext_k: u32, zeta: *const c_void,
+                                           ext_omega: *const c_void, repr: c_int) -> c_int;
+    pub fn h2_poly_set_rows(polys: *const u64, count: usize, start: usize, rows: usize, values: *const c_void, repr: c_int) -> c_int;
 }
 
 fn check(rc: c_int) {

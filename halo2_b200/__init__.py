@@ -10,7 +10,7 @@ from .arithmetic import (best_multiexp, small_multiexp, best_fft, best_fft_curve
                          eval_polynomial, compute_inner_product, kate_division)
 from .poly import (Params, EvaluationDomain, Blind, ResidentPoly, lagrange_generators, compress_points, decompress_points, hash_to_curve,  # noqa: F401
                    eval_polynomial_resident, inner_product_resident, kate_division_resident, batch_invert_resident,
-                   running_product_resident, permute_expression_pair_resident, share_resident)
+                   running_product_resident, permute_expression_pair_resident, share_resident, set_rows_resident)
 
 from .evaluator import Ast, AstLeaf, Evaluator  # noqa: F401
 from .verifier import MSM, Guard, VerifyError, verify_proof, compute_b  # noqa: F401
@@ -18,6 +18,7 @@ from .keygen import (Assembly, CopyConstraints, ProvingKey, build_permutation_po
                      batch_invert_assigned_resident)
 from .products import (permutation_commit, lookup_commit_product, permutation_product_resident, lookup_product_resident,  # noqa: F401
                        lookup_commit_permuted, lookup_permute_resident, Permuted)
+from .columns import instance_commit, advice_commit, InstanceSingle, AdviceSingle, InstanceTooLarge  # noqa: F401
 from . import multiopen, opening  # noqa: F401
 
 __all__ = ["Ast", "AstLeaf", "Evaluator", "Assembly", "CopyConstraints", "ProvingKey", "build_permutation_polys", "keygen_vk", "keygen_pk",
@@ -27,4 +28,5 @@ __all__ = ["Ast", "AstLeaf", "Evaluator", "Assembly", "CopyConstraints", "Provin
            "eval_polynomial", "compute_inner_product", "kate_division", "eval_polynomial_resident", "inner_product_resident",
            "kate_division_resident", "batch_invert_resident", "running_product_resident", "permute_expression_pair_resident",
            "share_resident", "permutation_commit", "lookup_commit_product", "permutation_product_resident", "lookup_product_resident",
-           "lookup_commit_permuted", "lookup_permute_resident", "Permuted"]
+           "lookup_commit_permuted", "lookup_permute_resident", "Permuted", "set_rows_resident", "instance_commit", "advice_commit",
+           "InstanceSingle", "AdviceSingle", "InstanceTooLarge"]

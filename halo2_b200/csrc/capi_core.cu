@@ -439,7 +439,7 @@ static void ctx_destroy(Context &C) {
     DevBuf *all[] = {&C.scal_in, &C.bases_in, &C.bases_phi, &C.glv_parts, &C.scal_canon, &C.counts, &C.cursor, &C.refs, &C.size_hist,
                      &C.items, &C.bucket_sum, &C.pkey, &C.pstart, &C.pend, &C.ppt, &C.ra_t, &C.ra_e,
                      &C.r0, &C.r1, &C.wsum, &C.scan_blocks, &C.result, &C.misc, &C.ntt_io, &C.ntt_out,
-                     &C.ntt_work, &C.pow2, &C.ec_work, &C.ec_io, &C.ec_out, &C.fb_a, &C.fb_b, &C.po_lvl, &C.po_q, &C.po_pts, &C.po_ptrs, &C.ast_code, &C.ast_consts,
+                     &C.ntt_work, &C.ntt_cols, &C.pow2, &C.ec_work, &C.ec_io, &C.ec_out, &C.fb_a, &C.fb_b, &C.po_lvl, &C.po_q, &C.po_pts, &C.po_ptrs, &C.ast_code, &C.ast_consts,
                      &C.multi_parts, &C.ba_lv[0], &C.ba_lv[1], &C.ba_lv[2], &C.lk_keys, &C.lk_aux, &C.lk_u32, &C.kg_tab, &C.kg_map,
                      &C.as_edge, &C.as_cell, &C.as_slot, &C.gp_val, &C.gp_aux};
     for (DevBuf *b : all) b->release();

@@ -39,11 +39,15 @@ struct NttScales {
 };
 
 // d_in: 2^in_log_n elements; d_out: min(out_len, 2^log_n) elements written.  d_out may alias d_in.
+// With in_cols / out_cols (device tables of `count` pointers) the same transform runs on `count` columns, column c from
+// in_cols[c] to out_cols[c] (d_in / d_out unused): every pass is one launch per group of columns (ntt.cuh: ntt_group), so a
+// call whose columns fit in one group issues exactly the launches of one column.  out_cols[c] may alias in_cols[c] only.
 template <class P>
 static int ntt_run(int field, const fe *d_in, uint32_t in_log_n, fe *d_out, uint32_t log_n, const fe &omega_mont, const NttScales &sc,
-                   uint64_t out_len, cudaStream_t s) {
+                   uint64_t out_len, cudaStream_t s, uint64_t count = 1, const fe *const *in_cols = nullptr, fe *const *out_cols = nullptr) {
     Context &X = g_ctx;
     if (log_n > 30) return fail("ntt: log_n > 30 not supported");
+    if (count == 0) return 0;
     uint64_t n = 1ull << log_n;
     const fe *tw = nullptr;
     if (get_twiddles<P>(field, omega_mont, log_n, s, &tw)) return 1;
@@ -52,39 +56,47 @@ static int ntt_run(int field, const fe *d_in, uint32_t in_log_n, fe *d_out, uint
     if (passes == 0) {   // n == 1: the network is empty; only the scalings apply
         sp[0] = 0; logc[0] = 0; passes = 1;
     }
-    if (passes > 1 && X.ntt_work.ensure(n * sizeof(fe))) return 1;
-    uint32_t s0 = 0;
-    for (int i = 0; i < passes; i++) {
-        NttPassArgs A;
-        A.in = i == 0 ? d_in : X.ntt_work.as<fe>();
-        A.out = i == passes - 1 ? d_out : X.ntt_work.as<fe>();
-        A.tw = tw; A.log_n = log_n; A.s0 = s0; A.sp = sp[i]; A.logc = logc[i];
-        A.flags = 0;
-        if (i == 0) A.flags |= NTT_FIRST | (sc.in_scale ? NTT_IN_SCALE : 0u);
-        if (i == passes - 1) A.flags |= NTT_LAST | (sc.out_scale ? NTT_OUT_SCALE : 0u);
-        A.in_log_n = in_log_n; A.out_len = out_len;
-        for (int k = 0; k < 3; k++) { A.in_scale[k] = sc.in_s[k]; A.out_scale[k] = sc.out_s[k]; }
-        uint32_t tiles = (uint32_t)(n >> (sp[i] + logc[i]));
-        uint32_t smem = ntt_smem_bytes(sp[i], logc[i]) + ntt_twc_bytes(sp[i], logc[i], i == passes - 1);
-        static std::atomic<bool> smem_optin{false};   // per instantiation <P>: a single-CTA transform of 2^10 elements wants 64 KiB
-        if (!smem_optin.load()) {
-            CU(cudaFuncSetAttribute(ntt_pass_kernel<P>, cudaFuncAttributeMaxDynamicSharedMemorySize, 100 * 1024));
-            CU(cudaFuncSetAttribute(ntt_pass_tma_kernel<P>, cudaFuncAttributeMaxDynamicSharedMemorySize, 100 * 1024));
-            smem_optin = true;
+    const uint64_t group = ntt_group(log_n, passes, count);
+    if (passes > 1 && X.ntt_work.ensure(group * n * sizeof(fe))) return 1;
+    static std::atomic<bool> smem_optin{false};   // per instantiation <P>: a single-CTA transform of 2^10 elements wants 64 KiB
+    if (!smem_optin.load()) {
+        CU(cudaFuncSetAttribute(ntt_pass_kernel<P>, cudaFuncAttributeMaxDynamicSharedMemorySize, 100 * 1024));
+        CU(cudaFuncSetAttribute(ntt_pass_tma_kernel<P>, cudaFuncAttributeMaxDynamicSharedMemorySize, 100 * 1024));
+        smem_optin = true;
+    }
+    for (uint64_t c0 = 0; c0 < count; c0 += group) {
+        const uint32_t cols = (uint32_t)(count - c0 < group ? count - c0 : group);
+        uint32_t s0 = 0;
+        for (int i = 0; i < passes; i++) {
+            NttPassArgs A;
+            A.in = i == 0 ? d_in : X.ntt_work.as<fe>();
+            A.out = i == passes - 1 ? d_out : X.ntt_work.as<fe>();
+            if (i > 0) A.in_stride = n;
+            if (i < passes - 1) A.out_stride = n;
+            if (i == 0 && in_cols) A.in_cols = in_cols + c0;
+            if (i == passes - 1 && out_cols) A.out_cols = out_cols + c0;
+            A.tw = tw; A.log_n = log_n; A.s0 = s0; A.sp = sp[i]; A.logc = logc[i];
+            A.flags = 0;
+            if (i == 0) A.flags |= NTT_FIRST | (sc.in_scale ? NTT_IN_SCALE : 0u);
+            if (i == passes - 1) A.flags |= NTT_LAST | (sc.out_scale ? NTT_OUT_SCALE : 0u);
+            A.in_log_n = in_log_n; A.out_len = out_len;
+            for (int k = 0; k < 3; k++) { A.in_scale[k] = sc.in_s[k]; A.out_scale[k] = sc.out_s[k]; }
+            uint32_t tiles = (uint32_t)(n >> (sp[i] + logc[i]));
+            uint32_t smem = ntt_smem_bytes(sp[i], logc[i]) + ntt_twc_bytes(sp[i], logc[i], i == passes - 1);
+            prof_begin(PROF_NTT_PASS, s);
+            if (X.ntt_tma && NttDense<P>::supported(A)) {
+                // persistent CTAs (4 per SM by registers), double-buffered tiles on the bulk-copy engine
+                int sms = 132;
+                cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, X.device);
+                // every CTA walks the same number of tiles (+-1): grid = tiles / ceil(tiles / resident CTAs)
+                const uint32_t slots = (uint32_t)sms * 4u, per = (tiles + slots - 1) / slots;
+                const uint32_t grid = (tiles + per - 1) / per;
+                LAUNCH(ntt_pass_tma_kernel<P>, dim3(grid, cols), 128, ntt_tma_smem_bytes(sp[i], logc[i], i == passes - 1), s, A, tiles);
+            } else
+            LAUNCH(ntt_pass_kernel<P>, dim3(tiles, cols), 128, smem, s, A);
+            prof_end(s);
+            s0 += sp[i];
         }
-        prof_begin(PROF_NTT_PASS, s);
-        if (X.ntt_tma && NttDense<P>::supported(A)) {
-            // persistent CTAs (4 per SM by registers), double-buffered tiles on the bulk-copy engine
-            int sms = 132;
-            cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, X.device);
-            // every CTA walks the same number of tiles (+-1): grid = tiles / ceil(tiles / resident CTAs)
-            const uint32_t slots = (uint32_t)sms * 4u, per = (tiles + slots - 1) / slots;
-            const uint32_t grid = (tiles + per - 1) / per;
-            LAUNCH(ntt_pass_tma_kernel<P>, grid, 128, ntt_tma_smem_bytes(sp[i], logc[i], i == passes - 1), s, A, tiles);
-        } else
-        LAUNCH(ntt_pass_kernel<P>, tiles, 128, smem, s, A);
-        prof_end(s);
-        s0 += sp[i];
     }
     return 0;
 }
@@ -342,14 +354,26 @@ extern "C" int h2_poly_download(uint64_t poly, void *dst, size_t len, int repr) 
     if (!b) return 1;
     return h.down(b->field, dst, b->buf.as<fe>(), len, g_ctx.stream);
 }
-// mode as in ntt_host: 1 = inverse transform with divisor, 2 = coeff_to_extended, 3 = extended_to_coeff
+// mode as in ntt_host: 1 = inverse transform with divisor, 2 = coeff_to_extended, 3 = extended_to_coeff.  Column i goes from
+// src[i] to dst[i]; a batch reaches ntt_run through one table of its columns' pointers (ntt_cols: the sources, then the
+// destinations).
 template <class P>
-static int poly_transform(PolyBuf *dst, PolyBuf *src, int mode, uint32_t in_log_n, uint32_t log_n, const void *omega, const void *zeta,
-                          const void *divisor, size_t out_len, const HostArgs &h) {
-    cudaStream_t s = g_ctx.stream;
+static int poly_transform(const std::vector<PolyBuf *> &dst, const std::vector<PolyBuf *> &src, int mode, uint32_t in_log_n, uint32_t log_n,
+                          const void *omega, const void *zeta, const void *divisor, size_t out_len, const HostArgs &h) {
+    Context &X = g_ctx;
+    cudaStream_t s = X.stream;
+    const size_t count = dst.size();
     if (scratch_acquire(s)) return 1;
     const NttScales sc = host_scales<P>(h, false, mode, zeta, divisor);   // resident data: Montgomery in and out
-    if (ntt_run<P>(src->field, src->buf.as<fe>(), in_log_n, dst->buf.as<fe>(), log_n, h.elem<P>(omega), sc, out_len, s)) return 1;
+    if (count == 1) {
+        if (ntt_run<P>(P::ID, src[0]->buf.as<fe>(), in_log_n, dst[0]->buf.as<fe>(), log_n, h.elem<P>(omega), sc, out_len, s)) return 1;
+    } else {
+        std::vector<fe *> tab(2 * count);
+        for (size_t i = 0; i < count; i++) { tab[i] = src[i]->buf.as<fe>(); tab[count + i] = dst[i]->buf.as<fe>(); }
+        if (X.ntt_cols.ensure(tab.size() * sizeof(fe *)) || upload_async(X.ntt_cols.p, tab.data(), tab.size() * sizeof(fe *), s)) return 1;
+        fe *const *cols = X.ntt_cols.as<fe *>();
+        if (ntt_run<P>(P::ID, nullptr, in_log_n, nullptr, log_n, h.elem<P>(omega), sc, out_len, s, count, cols, cols + count)) return 1;
+    }
     return scratch_release(s);       // asynchronous: later calls are ordered behind it on the stream
 }
 static int poly_transform_dispatch(uint64_t dst, uint64_t src, int mode, uint32_t in_log_n, uint32_t log_n, const void *omega, const void *zeta,
@@ -367,7 +391,43 @@ static int poly_transform_dispatch(uint64_t dst, uint64_t src, int mode, uint32_
     if (!a) return 1;
     if (d == a && out_len != ((size_t)1 << log_n)) return fail(std::string(who) + ": in place needs out_len == 2^log_n");
     if (d == a && in_log_n != log_n) return fail(std::string(who) + ": in place needs equal input and output sizes");
-    return by_field(a->field, [&](auto p) { return poly_transform<decltype(p)>(d, a, mode, in_log_n, log_n, omega, zeta, divisor, out_len, h); });
+    return by_field(a->field, [&](auto p) { return poly_transform<decltype(p)>({d}, {a}, mode, in_log_n, log_n, omega, zeta, divisor, out_len, h); });
+}
+// `count` columns of one size and domain, dst[i] = transform(src[i]); every check runs before the first launch.  A destination
+// listed twice, or that is another column's source, would race with that column's launch; dst[i] == src[i] works in place
+// where the sizes are equal, as in the one-column call.  Errors name the first offending index.
+static int poly_transform_batch(const uint64_t *dst, const uint64_t *src, size_t count, int mode, uint32_t in_log_n, uint32_t log_n,
+                                const void *omega, const void *zeta, const void *divisor, const HostArgs &h,
+                                std::initializer_list<HostArgs::Need> needs, const char *in_name, const char *out_name) {
+    const std::string who = h.who;
+    CtxLock lk;
+    if (require_ready() || h.check(needs)) return 1;
+    if (log_n > 30 || in_log_n > log_n) return fail(who + ": bad sizes");
+    if (count == 0) return 0;
+    if (!dst || !src) return fail(who + ": null handle array");
+    const size_t n_in = (size_t)1 << in_log_n, n_out = (size_t)1 << log_n;
+    PolyArgs g(h.who);
+    std::vector<PolyBuf *> d(count), a(count);
+    auto at = [&](const char *role, size_t i) {   // "<who>: <reason>" from PolyArgs -> "<who>: <role>[i]: <reason>"
+        return fail(who + ": " + role + "[" + std::to_string(i) + "]" + last_error_string().substr(who.size()));
+    };
+    for (size_t i = 0; i < count; i++) {
+        if (!(d[i] = g.out(dst[i], n_out, out_name))) return at("dst", i);
+        if (!(a[i] = g.in(src[i], n_in, in_name))) return at("src", i);
+    }
+    std::vector<std::pair<PolyBuf *, size_t>> ds(count), ss(count);
+    for (size_t i = 0; i < count; i++) { ds[i] = {d[i], i}; ss[i] = {a[i], i}; }
+    std::sort(ds.begin(), ds.end());
+    std::sort(ss.begin(), ss.end());
+    for (size_t i = 1; i < count; i++)
+        if (ds[i].first == ds[i - 1].first)
+            return fail(who + ": dst[" + std::to_string(ds[i].second) + "] is also dst[" + std::to_string(ds[i - 1].second) + "]");
+    for (size_t i = 0; i < count; i++) {
+        for (auto it = std::lower_bound(ss.begin(), ss.end(), std::make_pair(d[i], (size_t)0)); it != ss.end() && it->first == d[i]; ++it)
+            if (it->second != i) return fail(who + ": dst[" + std::to_string(i) + "] is also src[" + std::to_string(it->second) + "]");
+        if (d[i] == a[i] && in_log_n != log_n) return fail(who + ": dst[" + std::to_string(i) + "] == src[" + std::to_string(i) + "]: in place needs equal input and output sizes");
+    }
+    return by_field(d[0]->field, [&](auto p) { return poly_transform<decltype(p)>(d, a, mode, in_log_n, log_n, omega, zeta, divisor, n_out, h); });
 }
 extern "C" int h2_poly_lagrange_to_coeff(uint64_t dst, uint64_t src, uint32_t k, const void *omega_inv, const void *divisor, int repr) {
     return poly_transform_dispatch(dst, src, 1, k, k, omega_inv, nullptr, divisor, (size_t)1 << k, {"h2_poly_lagrange_to_coeff", repr},
@@ -381,4 +441,64 @@ extern "C" int h2_poly_extended_to_coeff(uint64_t dst, uint64_t src, uint32_t ex
                                          const void *zeta, size_t out_len, int repr) {
     return poly_transform_dispatch(dst, src, 3, ext_k, ext_k, ext_omega_inv, zeta, ext_divisor, out_len, {"h2_poly_extended_to_coeff", repr},
                                    {{ext_omega_inv, "ext_omega_inv"}, {ext_divisor, "ext_divisor"}, {zeta, "zeta"}}, "2^ext_k", "out_len");
+}
+extern "C" int h2_poly_lagrange_to_coeff_batch(const uint64_t *dst, const uint64_t *src, size_t count, uint32_t k, const void *omega_inv,
+                                               const void *divisor, int repr) {
+    return poly_transform_batch(dst, src, count, 1, k, k, omega_inv, nullptr, divisor, {"h2_poly_lagrange_to_coeff_batch", repr},
+                                {{omega_inv, "omega_inv", count != 0}, {divisor, "divisor", count != 0}}, "2^k", "2^k");
+}
+extern "C" int h2_poly_coeff_to_extended_batch(const uint64_t *dst, const uint64_t *src, size_t count, uint32_t k, uint32_t ext_k, const void *zeta,
+                                               const void *ext_omega, int repr) {
+    return poly_transform_batch(dst, src, count, 2, k, ext_k, ext_omega, zeta, nullptr, {"h2_poly_coeff_to_extended_batch", repr},
+                                {{zeta, "zeta", count != 0}, {ext_omega, "ext_omega", count != 0}}, "2^k", "2^ext_k");
+}
+// rows [start, start + rows) of column c <- vals[c rows ..], from `repr` into Montgomery form on the way
+template <class P> __global__ void set_rows_kernel(fe *const *cols, const fe *vals, uint64_t start, uint64_t rows, uint64_t total, int canon) {
+    const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= total) return;
+    fe x = fe_load(vals + i);
+    if (canon) x = fe_to_mont<P>(x);
+    fe_store(cols[i / rows] + start + i % rows, x);
+}
+extern "C" int h2_poly_set_rows(const uint64_t *polys, size_t count, size_t start, size_t rows, const void *values, int repr) {
+    static const char *who = "h2_poly_set_rows";
+    CtxLock lk;
+    const HostArgs h(who, repr);
+    if (require_ready() || h.check({{values, "values", count != 0 && rows != 0}})) return 1;
+    if (count == 0) return 0;
+    if (!polys) return fail(std::string(who) + ": null handle array");
+    const size_t ptr_fe = (count * sizeof(fe *) + sizeof(fe) - 1) / sizeof(fe);
+    if (rows != 0 && count > ((size_t)-1 / sizeof(fe) - ptr_fe) / rows) return fail(std::string(who) + ": count * rows overflows");
+    PolyArgs g(who);
+    std::vector<std::pair<PolyBuf *, size_t>> ps(count);
+    for (size_t i = 0; i < count; i++) {
+        PolyBuf *b = g.out(polys[i], 0, "0");
+        if (!b) return fail(std::string(who) + ": polys[" + std::to_string(i) + "]" + last_error_string().substr(strlen(who)));
+        if (start > b->len || rows > b->len - start)
+            return fail(std::string(who) + ": polys[" + std::to_string(i) + "]: rows [start, start + rows) exceed the polynomial's length");
+        ps[i] = {b, i};
+    }
+    std::sort(ps.begin(), ps.end());
+    for (size_t i = 1; i < count; i++)
+        if (ps[i].first == ps[i - 1].first)
+            return fail(std::string(who) + ": polys[" + std::to_string(ps[i].second) + "] is also polys[" + std::to_string(ps[i - 1].second) + "]");
+    if (rows == 0) return 0;
+    // one upload: the column pointers, then the values
+    const size_t total = count * rows;
+    std::vector<fe> up(ptr_fe + total);
+    fe **hp = reinterpret_cast<fe **>(up.data());
+    for (auto &p : ps) hp[p.second] = p.first->buf.as<fe>();
+    memcpy(up.data() + ptr_fe, values, total * sizeof(fe));
+    Context &X = g_ctx;
+    cudaStream_t s = X.stream;
+    if (scratch_acquire(s)) return 1;
+    if (X.ntt_cols.ensure(up.size() * sizeof(fe)) || upload_async(X.ntt_cols.p, up.data(), up.size() * sizeof(fe), s)) return 1;
+    const fe *d = X.ntt_cols.as<fe>();
+    if (by_field(ps[0].first->field, [&](auto p) {
+            LAUNCH(set_rows_kernel<decltype(p)>, blocks_for(total, 256), 256, 0, s, reinterpret_cast<fe *const *>(d), d + ptr_fe, (uint64_t)start,
+                   (uint64_t)rows, (uint64_t)total, h.canon() ? 1 : 0);
+            return 0;
+        }))
+        return 1;
+    return scratch_release(s);
 }

@@ -157,8 +157,8 @@ struct Context {
     // MSM scratch
     DevBuf scal_in, bases_in, bases_phi, glv_parts, scal_canon, counts, cursor, refs, size_hist, items, bucket_sum, pkey, pstart, pend, ppt, ra_t, ra_e, r0, r1,
         wsum, scan_blocks, result, misc, ba_lv[3];
-    // NTT scratch
-    DevBuf ntt_io, ntt_out, ntt_work, pow2;
+    // NTT scratch; ntt_cols: the column pointer tables of a batched transform, and the rows of h2_poly_set_rows
+    DevBuf ntt_io, ntt_out, ntt_work, ntt_cols, pow2;
     // EC-FFT / batch-normalise scratch: XYZZ work array (128 B per point), staging for the host forms
     DevBuf ec_work, ec_io, ec_out;
     DevBuf fb_a, fb_b;                       // partial sums of the direct-sum fixed-base MSM (ping-pong)

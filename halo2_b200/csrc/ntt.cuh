@@ -17,6 +17,7 @@
 //       adjacent j (coalesced C*32 B runs); all columns of a tile share their twiddles.
 //   geometry B (last pass): rows = the low sp bits of j (contiguous in memory), columns = C
 //       blocks whose outputs p are adjacent, so the bit-reversed store is coalesced too.
+// Columns: one launch per pass covers every column of a batch (grid.y = column; NttPassArgs::in_cols / out_cols).
 // Fusions: first pass can zero-pad (coeff_to_extended's resize, poly/domain.rs:248) and
 // multiply element j by in_scale[j mod 3] (distribute_powers_zeta, :357-373, and/or the
 // canonical->Montgomery factor); last pass can multiply output p by out_scale[p mod 3]
@@ -41,7 +42,14 @@ struct NttPassArgs {
     uint64_t out_len;    // last pass: outputs with p >= out_len are dropped (truncate)
     fe in_scale[3];
     fe out_scale[3];
+    // A launch covers gridDim.y columns of one size and domain.  Column c reads in_cols[c] when the table is set, else
+    // in + c * in_stride, and writes out_cols[c], else out + c * out_stride.  One column: in / out, no tables.
+    const fe *const *in_cols = nullptr;
+    fe *const *out_cols = nullptr;
+    uint64_t in_stride = 0, out_stride = 0;
 };
+H2_HD const fe *ntt_col_in(const NttPassArgs &A, uint32_t c) { return A.in_cols ? A.in_cols[c] : A.in + c * A.in_stride; }
+H2_HD fe *ntt_col_out(const NttPassArgs &A, uint32_t c) { return A.out_cols ? A.out_cols[c] : A.out + c * A.out_stride; }
 
 H2_HD uint32_t bitrev32(uint32_t x, uint32_t bits) {
     // bits in [0, 32]
@@ -93,8 +101,9 @@ template <class P> struct NttPass {
         return bitrev32(j_high, A.s0);
     }
 
-    static H2_HD void load_phase(const NttPassArgs &A, uint32_t tile, uint32_t tid, uint32_t nthr, uint4 *sm) {
+    static H2_HD void load_phase(const NttPassArgs &A, uint32_t tile, uint32_t tid, uint32_t nthr, uint4 *sm, uint32_t column = 0) {
         const uint32_t R = 1u << A.sp, C = 1u << A.logc, stride = ntt_smem_stride(A.logc), plane = stride << A.sp;
+        const fe *in = ntt_col_in(A, column);
         const bool geomB = (A.flags & NTT_LAST) != 0;
         for (uint32_t e = tid; e < R * C; e += nthr) {
             uint32_t r, col;
@@ -104,7 +113,7 @@ template <class P> struct NttPass {
             if ((A.flags & NTT_FIRST) && (j >> A.in_log_n) != 0) {
                 x = fe_zero();
             } else {
-                x = fe_load(A.in + j);
+                x = fe_load(in + j);
                 if ((A.flags & NTT_FIRST) && (A.flags & NTT_IN_SCALE)) x = fe_mul<P>(x, A.in_scale[j % 3]);
             }
             sm_store(sm, plane, r * stride + col, x);
@@ -219,8 +228,9 @@ template <class P> struct NttPass {
         step_phase_l(A, tile, st, tid, nthr, lay, twc);
     }
 
-    static H2_HD void store_phase(const NttPassArgs &A, uint32_t tile, uint32_t tid, uint32_t nthr, const uint4 *sm) {
+    static H2_HD void store_phase(const NttPassArgs &A, uint32_t tile, uint32_t tid, uint32_t nthr, const uint4 *sm, uint32_t column = 0) {
         const uint32_t R = 1u << A.sp, C = 1u << A.logc, stride = ntt_smem_stride(A.logc), plane = stride << A.sp;
+        fe *out = ntt_col_out(A, column);
         const bool last = (A.flags & NTT_LAST) != 0;
         for (uint32_t e = tid; e < R * C; e += nthr) {
             uint32_t col = e & (C - 1), r = e >> A.logc;
@@ -229,9 +239,9 @@ template <class P> struct NttPass {
                 uint64_t p = ((uint64_t)bitrev32(r, A.sp) << A.s0) | p_low_of(A, tile, col);
                 if (p >= A.out_len) continue;
                 if (A.flags & NTT_OUT_SCALE) x = fe_mul<P>(x, A.out_scale[p % 3]);
-                fe_store(A.out + p, x);
+                fe_store(out + p, x);
             } else {
-                fe_store(A.out + elem_j(A, tile, r, col), x);
+                fe_store(out + elem_j(A, tile, r, col), x);
             }
         }
     }
@@ -260,16 +270,16 @@ template <class P> struct TwiddleGen {
 #if defined(__CUDACC__)
 template <class P> __global__ void __launch_bounds__(128, 4) ntt_pass_kernel(const NttPassArgs A) {
     extern __shared__ uint4 h2_ntt_smem[];
-    const uint32_t tile = blockIdx.x, tid = threadIdx.x, nthr = blockDim.x;
+    const uint32_t tile = blockIdx.x, column = blockIdx.y, tid = threadIdx.x, nthr = blockDim.x;
     uint4 *twc = h2_ntt_smem + (ntt_smem_bytes(A.sp, A.logc) >> 4);
     NttPass<P>::twiddle_phase(A, tile, tid, nthr, twc);
-    NttPass<P>::load_phase(A, tile, tid, nthr, h2_ntt_smem);
+    NttPass<P>::load_phase(A, tile, tid, nthr, h2_ntt_smem, column);
     __syncthreads();
     for (uint32_t st = 0; st < NttPass<P>::num_steps(A.sp); st++) {
         NttPass<P>::step_phase(A, tile, st, tid, nthr, h2_ntt_smem, twc);
         __syncthreads();
     }
-    NttPass<P>::store_phase(A, tile, tid, nthr, h2_ntt_smem);
+    NttPass<P>::store_phase(A, tile, tid, nthr, h2_ntt_smem, column);
 }
 #endif
 // ------------------------------------------------------------------------------------------------------------------
@@ -402,6 +412,8 @@ template <class P> __global__ void __launch_bounds__(128, 4) ntt_pass_tma_kernel
     uint8_t *outst = twc0 + 2 * twb;                                                 // geometry B only
     const uint32_t ntw = NttPass<P>::twc_count(A);
     const uint32_t units_in = NttDense<P>::in_units(A);
+    const fe *in = ntt_col_in(A, blockIdx.y);           // grid.y: the column, as in ntt_pass_kernel
+    fe *out = ntt_col_out(A, blockIdx.y);
     if (tid == 0) {   // one arrival per copy unit: every issuing thread announces its own bytes
         tma::mbar_init(&full[0], units_in);
         tma::mbar_init(&full[1], units_in);
@@ -415,7 +427,7 @@ template <class P> __global__ void __launch_bounds__(128, 4) ntt_pass_tma_kernel
             const auto sp_ = NttDense<P>::in_span(A, tile, u);
             if (sp_.valid) {
                 tma::mbar_expect_tx(&full[b], sp_.bytes);
-                tma::bulk_g2s(buf + sp_.smem_off, A.in + sp_.elem, sp_.bytes, &full[b]);
+                tma::bulk_g2s(buf + sp_.smem_off, in + sp_.elem, sp_.bytes, &full[b]);
             } else {
                 for (uint32_t o = 0; o < sp_.bytes; o += 16) *reinterpret_cast<uint4 *>(buf + sp_.smem_off + o) = make_uint4(0, 0, 0, 0);
                 tma::mbar_expect_tx(&full[b], 0);          // zero padding: arrive without bytes (the release orders the stores above)
@@ -451,7 +463,7 @@ template <class P> __global__ void __launch_bounds__(128, 4) ntt_pass_tma_kernel
         __syncthreads();
         for (uint32_t r = tid; r < R; r += nthr) {
             const auto sp_ = NttDense<P>::out_span(A, cur, r);
-            if (sp_.valid) tma::bulk_s2g(A.out + sp_.elem, lay.out + sp_.smem_off, sp_.bytes);
+            if (sp_.valid) tma::bulk_s2g(out + sp_.elem, lay.out + sp_.smem_off, sp_.bytes);
         }
         tma::bulk_commit();
     }
@@ -494,6 +506,17 @@ inline int ntt_plan(uint32_t log_n, uint32_t sp[8], uint32_t logc[8]) {
         s0 += sp[i];
     }
     return passes;
+}
+// Column batches: each pass of a transform of `count` columns of one size and domain is one launch whose grid.y is the
+// column.  A multi-pass transform keeps its intermediate data in scratch, one 2^log_n-element slot per column: a group
+// takes as many columns as fit in H2_NTT_BATCH_SCRATCH bytes (at least one, at most 65535, the grid.y limit), so the scratch
+// is at most max(32 * 2^log_n, H2_NTT_BATCH_SCRATCH) bytes for any count.  Single-pass transforms need no scratch.
+#define H2_NTT_BATCH_SCRATCH (1ull << 28)
+inline uint64_t ntt_group(uint32_t log_n, int passes, uint64_t count) {
+    uint64_t g = passes > 1 ? H2_NTT_BATCH_SCRATCH / (32ull << log_n) : count;
+    if (g < 1) g = 1;
+    if (g > 65535) g = 65535;
+    return g < count ? g : count;
 }
 
 }  // namespace h2

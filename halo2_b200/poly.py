@@ -394,6 +394,22 @@ def share_resident(polys: Sequence["ResidentPoly"]) -> None:
         p._shared = True
 
 
+def set_rows_resident(polys: Sequence["ResidentPoly"], start: int, values) -> None:
+    """Rows [start, start + rows) of every polynomial <- values[i] (a (count, rows, 32) uint8 array, or one list of ints per
+    polynomial), in one upload and one kernel (h2_poly_set_rows): the blinding rows of resident advice columns."""
+    count = len(polys)
+    if count == 0:
+        return
+    if isinstance(values, np.ndarray):
+        arr = np.ascontiguousarray(values, dtype=np.uint8)
+    else:
+        m = FIELDS[polys[0].field]
+        arr = np.frombuffer(b"".join((int(v) % m).to_bytes(32, "little") for col in values for v in col), dtype=np.uint8)
+    arr = arr.reshape(count, -1, 32) if arr.size else np.zeros((count, 0, 32), dtype=np.uint8)
+    _l.check(_l.init().h2_poly_set_rows(_handles(polys), ctypes.c_size_t(count), ctypes.c_size_t(int(start)), ctypes.c_size_t(arr.shape[1]),
+                                        _l.ptr(arr) if arr.size else None, _l.REPR_CANONICAL))
+
+
 def eval_polynomial_resident(polys: Sequence["ResidentPoly"], points: Sequence[int], n: Optional[int] = None) -> list:
     """[eval_polynomial(p, x)] (arithmetic.rs:297-303) for device-resident coefficient vectors, one launch tree for the batch."""
     batch = len(polys)
@@ -589,4 +605,30 @@ class EvaluationDomain:
                                                      _l.ptr(_l.fe_bytes(self.extended_omega_inv)),
                                                      _l.ptr(_l.fe_bytes(self.extended_ifft_divisor)), _l.ptr(_l.fe_bytes(self.g_coset)),
                                                      ctypes.c_size_t(out_len), _l.REPR_CANONICAL))
+        return out
+
+    def lagrange_to_coeff_batch_resident(self, polys: Sequence["ResidentPoly"], out: Optional[Sequence["ResidentPoly"]] = None) -> list:
+        """lagrange_to_coeff of every column in one call (h2_poly_lagrange_to_coeff_batch): each NTT pass is one launch for all
+        of them.  out=None transforms in place."""
+        out = list(polys) if out is None else list(out)
+        assert len(out) == len(polys)
+        _l.check(_l.init().h2_poly_lagrange_to_coeff_batch(_handles(out), _handles(polys), ctypes.c_size_t(len(polys)), ctypes.c_uint32(self.k),
+                                                           _l.ptr(_l.fe_bytes(self.omega_inv)), _l.ptr(_l.fe_bytes(self.ifft_divisor)),
+                                                           _l.REPR_CANONICAL))
+        return out
+
+    def coeff_to_extended_batch_resident(self, polys: Sequence["ResidentPoly"], out: Optional[Sequence["ResidentPoly"]] = None) -> list:
+        """coeff_to_extended of every column in one call (h2_poly_coeff_to_extended_batch).  out=None allocates the cosets."""
+        fresh = out is None
+        out = [ResidentPoly(self.field, self.extended_len()) for _ in polys] if fresh else list(out)
+        assert len(out) == len(polys)
+        try:
+            _l.check(_l.init().h2_poly_coeff_to_extended_batch(_handles(out), _handles(polys), ctypes.c_size_t(len(polys)), ctypes.c_uint32(self.k),
+                                                               ctypes.c_uint32(self.extended_k), _l.ptr(_l.fe_bytes(self.g_coset)),
+                                                               _l.ptr(_l.fe_bytes(self.extended_omega)), _l.REPR_CANONICAL))
+        except BaseException:
+            if fresh:
+                for p in out:
+                    p.close()
+            raise
         return out

@@ -182,6 +182,23 @@ int h2_poly_lagrange_to_coeff(uint64_t dst, uint64_t src, uint32_t k, const void
 int h2_poly_coeff_to_extended(uint64_t dst, uint64_t src, uint32_t k, uint32_t ext_k, const void *zeta, const void *ext_omega, int repr);
 int h2_poly_extended_to_coeff(uint64_t dst, uint64_t src, uint32_t ext_k, const void *ext_omega_inv, const void *ext_divisor,
                               const void *zeta, size_t out_len, int repr);
+/* The same transforms for `count` columns of one size and domain in one call: dst[i] = lagrange_to_coeff(src[i]) /
+ * coeff_to_extended(src[i]), the instance and advice phases of plonk::create_proof (plonk/prover.rs:79-124, :269-335).  Each
+ * pass is one launch for the whole batch (the launches of one column, while count x 2^log_n x 32 B of scratch stays within
+ * 256 MiB; larger batches run in groups of that size).  Sources are only read and may repeat, so shared polynomials work;
+ * destinations must be the calling context's own, pairwise distinct and none of the other columns' sources.  dst[i] == src[i]
+ * transforms column i in place where the one-column call allows it (equal input and output sizes).  Every check runs before
+ * anything is launched and a failed call changes nothing; messages name the first offending index ("dst[3]").  count == 0
+ * does nothing.  Asynchronous, like the one-column calls. */
+int h2_poly_lagrange_to_coeff_batch(const uint64_t *dst, const uint64_t *src, size_t count, uint32_t k, const void *omega_inv,
+                                    const void *divisor, int repr);
+int h2_poly_coeff_to_extended_batch(const uint64_t *dst, const uint64_t *src, size_t count, uint32_t k, uint32_t ext_k, const void *zeta,
+                                    const void *ext_omega, int repr);
+/* Rows [start, start + rows) of each of `count` resident polynomials <- values (count x rows elements in `repr`, column by
+ * column), one upload and one kernel: the blinding rows of advice columns that are already resident (plonk/prover.rs:276-282).
+ * The polynomials must be the calling context's own and pairwise distinct, each with at least start + rows elements; every
+ * check runs first and a failed call changes nothing.  count == 0 or rows == 0 does nothing.  Asynchronous. */
+int h2_poly_set_rows(const uint64_t *polys, size_t count, size_t start, size_t rows, const void *values, int repr);
 int h2_msm_registered_polys(uint64_t bases_handle, const uint64_t *polys, size_t batch, size_t n, const void *extra_scalars, int repr,
                             void *out_xyz);
 /* The same pass followed by batch_normalize on the device: `batch` affine points (64 B each) -- what the prover writes to
