@@ -91,65 +91,67 @@ extern "C" int h2_bases_release(uint64_t handle) {
 }
 
 std::map<uint64_t, PolyBuf *> g_shared_polys;
-PolyBuf *PolyArgs::fits(PolyBuf *p, uint64_t len, const char *len_name) {
-    if (!field_given && field < 0) field = p->field;
-    if (p->field != field) {
-        fail(who + (field_given ? ": the polynomial is not over the curve's scalar field" : ": the polynomials live in different fields"));
+static std::string arg_label(const char *name, int64_t i) { return i < 0 ? std::string(name) : std::string(name) + "[" + std::to_string(i) + "]"; }
+PolyBuf *PolyArgs::find(bool out, uint64_t h, const char *name, int64_t i, uint64_t off, uint64_t len, const char *len_name) {
+    auto bad = [&](const std::string &reason) -> PolyBuf * {
+        fail(who + ": " + (i < 0 ? "" : arg_label(name, i) + ": ") + reason);
         return nullptr;
-    }
-    if (p->len < len) { fail(who + ": a polynomial holds fewer than " + len_name + " elements"); return nullptr; }
-    return p;
-}
-PolyBuf *PolyArgs::out(uint64_t h, uint64_t len, const char *len_name) {
-    auto it = g_ctx.polys.find(h);
-    if (it == g_ctx.polys.end()) {
-        bool shared;
-        {
-            std::lock_guard<std::mutex> lk(g_reg_mu);
-            shared = g_shared_polys.count(h) != 0;
-        }
-        fail(who + (shared ? ": the polynomial is shared (read-only)" : ": unknown polynomial handle"));
-        return nullptr;
-    }
-    outs.push_back(it->second);
-    return fits(it->second, len, len_name);
-}
-PolyBuf *PolyArgs::in(uint64_t h, uint64_t len, const char *len_name) {
+    };
     auto it = g_ctx.polys.find(h);
     PolyBuf *p = it != g_ctx.polys.end() ? it->second : nullptr;
     if (!p) {
         std::lock_guard<std::mutex> lk(g_reg_mu);
         auto s = g_shared_polys.find(h);
         if (s != g_shared_polys.end()) {
+            if (out) return bad("the polynomial is shared (read-only)");
             p = s->second;
             p->users++;
             held.push_back(p);
         }
     }
-    if (!p) { fail(who + ": unknown polynomial handle"); return nullptr; }
-    ins.push_back(p);
-    return fits(p, len, len_name);
+    if (!p) return bad("unknown polynomial handle");
+    args.push_back({p, out, name, i});
+    if (!field_given && field < 0) field = p->field;
+    if (p->field != field) return bad(field_given ? "the polynomial is not over the curve's scalar field" : "the polynomials live in different fields");
+    if (off > p->len || len > p->len - off) return bad(std::string("a polynomial holds fewer than ") + len_name + " elements");
+    return p;
 }
-int PolyArgs::out(const uint64_t *h, size_t n, uint64_t len, const char *len_name, std::vector<PolyBuf *> &v) {
+int PolyArgs::find(bool out, const uint64_t *h, size_t n, const char *name, uint64_t off, uint64_t len, const char *len_name, std::vector<PolyBuf *> &v) {
     v.resize(n);
     for (size_t i = 0; i < n; i++)
-        if (!(v[i] = out(h[i], len, len_name))) return 1;
-    return 0;
-}
-int PolyArgs::in(const uint64_t *h, size_t n, uint64_t len, const char *len_name, std::vector<PolyBuf *> &v) {
-    v.resize(n);
-    for (size_t i = 0; i < n; i++)
-        if (!(v[i] = in(h[i], len, len_name))) return 1;
+        if (!(v[i] = find(out, h[i], name, (int64_t)i, off, len, len_name))) return 1;
     return 0;
 }
 // Batch slices and product columns run concurrently: an output written twice, or read as another one's input, would race.
-int PolyArgs::distinct(const char *role) {
-    std::vector<PolyBuf *> so(outs), si(ins);
-    std::sort(so.begin(), so.end());
-    std::sort(si.begin(), si.end());
-    if (std::adjacent_find(so.begin(), so.end()) != so.end()) return fail(who + ": " + role + " handle appears twice");
-    for (PolyBuf *p : so)
-        if (std::binary_search(si.begin(), si.end(), p)) return fail(who + ": " + role + " handle is also an input");
+// The arguments are walked in lookup order, and the first one that clashes with an earlier one is reported.
+int PolyArgs::distinct(const char *in_place_out, const char *in_place_in) {
+    auto paired = [&](const Arg &o, const Arg &x) {   // output o and input x are one column of a call that works in place
+        return in_place_out && o.i == x.i && !strcmp(o.name, in_place_out) && !strcmp(x.name, in_place_in);
+    };
+    struct Seen { const Arg *out = nullptr, *in[2] = {}; };   // per polynomial: its output, its first two inputs
+    std::map<PolyBuf *, Seen> seen;
+    for (const Arg &a : args) {
+        Seen &s = seen[a.p];
+        const Arg *o = nullptr, *x = nullptr;
+        if (a.out && s.out) { o = &a; x = s.out; }
+        else if (a.out) { for (const Arg *in : s.in) if (in && !paired(a, *in)) { o = &a; x = in; break; } }
+        else if (s.out && !paired(*s.out, a)) { o = s.out; x = &a; }
+        if (o) return fail(who + ": " + arg_label(o->name, o->i) + " is also " + arg_label(x->name, x->i));
+        if (a.out) s.out = &a;
+        else if (!s.in[0] || !s.in[1]) s.in[s.in[0] ? 1 : 0] = &a;
+    }
+    return 0;
+}
+int col_table(const std::vector<PolyBuf *> &cols, const void *data, size_t bytes, cudaStream_t s, ColTable *t) {
+    Context &X = g_ctx;
+    const size_t at = bytes ? (cols.size() * sizeof(fe *) + sizeof(fe) - 1) / sizeof(fe) * sizeof(fe) : cols.size() * sizeof(fe *);
+    std::vector<uint8_t> up(at + bytes);
+    fe **hp = reinterpret_cast<fe **>(up.data());
+    for (size_t i = 0; i < cols.size(); i++) hp[i] = cols[i] ? cols[i]->buf.as<fe>() : nullptr;
+    if (bytes) memcpy(up.data() + at, data, bytes);
+    if (X.col_tab.ensure(up.size()) || upload_async(X.col_tab.p, up.data(), up.size(), s)) return 1;
+    t->cols = X.col_tab.as<fe *>();
+    t->data = bytes ? reinterpret_cast<fe *>(X.col_tab.as<uint8_t>() + at) : nullptr;
     return 0;
 }
 PolyArgs::~PolyArgs() {
@@ -439,8 +441,8 @@ static void ctx_destroy(Context &C) {
     DevBuf *all[] = {&C.scal_in, &C.bases_in, &C.bases_phi, &C.glv_parts, &C.scal_canon, &C.counts, &C.cursor, &C.refs, &C.size_hist,
                      &C.items, &C.bucket_sum, &C.pkey, &C.pstart, &C.pend, &C.ppt, &C.ra_t, &C.ra_e,
                      &C.r0, &C.r1, &C.wsum, &C.scan_blocks, &C.result, &C.misc, &C.ntt_io, &C.ntt_out,
-                     &C.ntt_work, &C.ntt_cols, &C.pow2, &C.ec_work, &C.ec_io, &C.ec_out, &C.fb_a, &C.fb_b, &C.po_lvl, &C.po_q, &C.po_pts, &C.po_ptrs, &C.ast_code, &C.ast_consts,
-                     &C.multi_parts, &C.ba_lv[0], &C.ba_lv[1], &C.ba_lv[2], &C.lk_keys, &C.lk_aux, &C.lk_u32, &C.kg_tab, &C.kg_map,
+                     &C.ntt_work, &C.pow2, &C.col_tab, &C.ec_work, &C.ec_io, &C.ec_out, &C.fb_a, &C.fb_b, &C.po_lvl, &C.po_q, &C.po_pts, &C.ast_code, &C.ast_consts,
+                     &C.multi_parts, &C.ba_lv[0], &C.ba_lv[1], &C.ba_lv[2], &C.lk_keys, &C.lk_u32, &C.kg_tab, &C.kg_map,
                      &C.as_edge, &C.as_cell, &C.as_slot, &C.gp_val, &C.gp_aux};
     for (DevBuf *b : all) b->release();
     for (auto *t : C.twiddles) { t->buf.release(); delete t; }

@@ -868,7 +868,7 @@ static int ipa_begin_common(uint64_t bases_handle, uint32_t k, const void *p_pri
         using PS = decltype(ps);
         PolyArgs g("h2_ipa_begin_poly", PS::ID);
         PolyBuf *p_poly = nullptr;
-        if (p_poly_handle && !(p_poly = g.in(*p_poly_handle, 1ull << k, "2^k"))) return 1;   // looked up and used under the one lock
+        if (p_poly_handle && !(p_poly = g.in(*p_poly_handle, "p_prime_poly", 1ull << k, "2^k"))) return 1;   // looked up and used under the one lock
         IpaSession *q;
         if (!g_ctx.ipa_pool.empty()) { q = g_ctx.ipa_pool.back(); g_ctx.ipa_pool.pop_back(); }
         else q = new IpaSession();
@@ -1008,7 +1008,7 @@ static int msm_registered_polys_impl(uint64_t bases_handle, const uint64_t *poly
     return by_curve(b->curve, [&](auto, auto ps) {
         PolyArgs g("h2_msm_registered_polys", decltype(ps)::ID);
         std::vector<PolyBuf *> q;
-        if (g.in(polys, batch, n, "n", q)) return 1;
+        if (g.in(polys, batch, "polys", n, "n", q)) return 1;
         Context &X = g_ctx;
         cudaStream_t s = X.stream;
         if (scratch_acquire(s)) return 1;

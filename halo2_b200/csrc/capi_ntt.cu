@@ -306,7 +306,7 @@ extern "C" int h2_poly_upload(uint64_t poly, const void *src, size_t len, int re
     const HostArgs h("h2_poly_upload", repr);
     if (require_ready() || h.check({{src, "src", len != 0}})) return 1;
     PolyArgs g("h2_poly_upload");
-    PolyBuf *b = g.out(poly, len, "len");
+    PolyBuf *b = g.out(poly, "poly", len, "len");
     if (!b) return 1;
     cudaStream_t s = g_ctx.stream;
     if (h.up(b->field, b->buf.as<fe>(), src, len, s)) return 1;
@@ -321,7 +321,7 @@ extern "C" int h2_poly_add_at(uint64_t poly, size_t index, const void *delta, in
     const HostArgs h("h2_poly_add_at", repr);
     if (require_ready() || h.check({{delta, "delta"}})) return 1;
     PolyArgs g("h2_poly_add_at");
-    PolyBuf *b = g.out(poly, 0, "0");
+    PolyBuf *b = g.out(poly, "poly", 0, "0");
     if (!b) return 1;
     if (index >= b->len) return fail("h2_poly_add_at: index out of range");
     cudaStream_t s = g_ctx.stream;
@@ -337,9 +337,9 @@ extern "C" int h2_poly_copy(uint64_t dst, size_t dst_off, uint64_t src, size_t s
     CtxLock lk;
     if (require_ready()) return 1;
     PolyArgs g("h2_poly_copy");
-    PolyBuf *d = g.out(dst, dst_off + len, "dst_off + len");
+    PolyBuf *d = g.out(dst, "dst", dst_off, len, "dst_off + len");
     if (!d) return 1;
-    PolyBuf *a = g.in(src, src_off + len, "src_off + len");
+    PolyBuf *a = g.in(src, "src", src_off, len, "src_off + len");
     if (!a) return 1;
     if (d == a && !(dst_off + len <= src_off || src_off + len <= dst_off)) return fail("h2_poly_copy: overlapping ranges");
     if (len) CU(cudaMemcpyAsync(d->buf.as<fe>() + dst_off, a->buf.as<fe>() + src_off, len * sizeof(fe), cudaMemcpyDeviceToDevice, g_ctx.stream));
@@ -350,13 +350,12 @@ extern "C" int h2_poly_download(uint64_t poly, void *dst, size_t len, int repr) 
     const HostArgs h("h2_poly_download", repr);
     if (require_ready() || h.check({{dst, "dst", len != 0}})) return 1;
     PolyArgs g("h2_poly_download");
-    PolyBuf *b = g.in(poly, len, "len");
+    PolyBuf *b = g.in(poly, "poly", len, "len");
     if (!b) return 1;
     return h.down(b->field, dst, b->buf.as<fe>(), len, g_ctx.stream);
 }
 // mode as in ntt_host: 1 = inverse transform with divisor, 2 = coeff_to_extended, 3 = extended_to_coeff.  Column i goes from
-// src[i] to dst[i]; a batch reaches ntt_run through one table of its columns' pointers (ntt_cols: the sources, then the
-// destinations).
+// src[i] to dst[i]; a batch reaches ntt_run through one table of its columns' pointers (the sources, then the destinations).
 template <class P>
 static int poly_transform(const std::vector<PolyBuf *> &dst, const std::vector<PolyBuf *> &src, int mode, uint32_t in_log_n, uint32_t log_n,
                           const void *omega, const void *zeta, const void *divisor, size_t out_len, const HostArgs &h) {
@@ -368,11 +367,12 @@ static int poly_transform(const std::vector<PolyBuf *> &dst, const std::vector<P
     if (count == 1) {
         if (ntt_run<P>(P::ID, src[0]->buf.as<fe>(), in_log_n, dst[0]->buf.as<fe>(), log_n, h.elem<P>(omega), sc, out_len, s)) return 1;
     } else {
-        std::vector<fe *> tab(2 * count);
-        for (size_t i = 0; i < count; i++) { tab[i] = src[i]->buf.as<fe>(); tab[count + i] = dst[i]->buf.as<fe>(); }
-        if (X.ntt_cols.ensure(tab.size() * sizeof(fe *)) || upload_async(X.ntt_cols.p, tab.data(), tab.size() * sizeof(fe *), s)) return 1;
-        fe *const *cols = X.ntt_cols.as<fe *>();
-        if (ntt_run<P>(P::ID, nullptr, in_log_n, nullptr, log_n, h.elem<P>(omega), sc, out_len, s, count, cols, cols + count)) return 1;
+        std::vector<PolyBuf *> cols(src);
+        cols.insert(cols.end(), dst.begin(), dst.end());
+        ColTable t;
+        if (col_table(cols, nullptr, 0, s, &t) ||
+            ntt_run<P>(P::ID, nullptr, in_log_n, nullptr, log_n, h.elem<P>(omega), sc, out_len, s, count, t.cols, t.cols + count))
+            return 1;
     }
     return scratch_release(s);       // asynchronous: later calls are ordered behind it on the stream
 }
@@ -385,9 +385,9 @@ static int poly_transform_dispatch(uint64_t dst, uint64_t src, int mode, uint32_
     if (log_n > 30 || in_log_n > log_n) return fail("ntt: bad sizes");
     if (out_len > ((size_t)1 << log_n)) out_len = (size_t)1 << log_n;
     PolyArgs g(who);
-    PolyBuf *d = g.out(dst, out_len, out_name);
+    PolyBuf *d = g.out(dst, "dst", out_len, out_name);
     if (!d) return 1;
-    PolyBuf *a = g.in(src, (size_t)1 << in_log_n, in_name);
+    PolyBuf *a = g.in(src, "src", (size_t)1 << in_log_n, in_name);
     if (!a) return 1;
     if (d == a && out_len != ((size_t)1 << log_n)) return fail(std::string(who) + ": in place needs out_len == 2^log_n");
     if (d == a && in_log_n != log_n) return fail(std::string(who) + ": in place needs equal input and output sizes");
@@ -407,26 +407,11 @@ static int poly_transform_batch(const uint64_t *dst, const uint64_t *src, size_t
     if (!dst || !src) return fail(who + ": null handle array");
     const size_t n_in = (size_t)1 << in_log_n, n_out = (size_t)1 << log_n;
     PolyArgs g(h.who);
-    std::vector<PolyBuf *> d(count), a(count);
-    auto at = [&](const char *role, size_t i) {   // "<who>: <reason>" from PolyArgs -> "<who>: <role>[i]: <reason>"
-        return fail(who + ": " + role + "[" + std::to_string(i) + "]" + last_error_string().substr(who.size()));
-    };
-    for (size_t i = 0; i < count; i++) {
-        if (!(d[i] = g.out(dst[i], n_out, out_name))) return at("dst", i);
-        if (!(a[i] = g.in(src[i], n_in, in_name))) return at("src", i);
-    }
-    std::vector<std::pair<PolyBuf *, size_t>> ds(count), ss(count);
-    for (size_t i = 0; i < count; i++) { ds[i] = {d[i], i}; ss[i] = {a[i], i}; }
-    std::sort(ds.begin(), ds.end());
-    std::sort(ss.begin(), ss.end());
-    for (size_t i = 1; i < count; i++)
-        if (ds[i].first == ds[i - 1].first)
-            return fail(who + ": dst[" + std::to_string(ds[i].second) + "] is also dst[" + std::to_string(ds[i - 1].second) + "]");
-    for (size_t i = 0; i < count; i++) {
-        for (auto it = std::lower_bound(ss.begin(), ss.end(), std::make_pair(d[i], (size_t)0)); it != ss.end() && it->first == d[i]; ++it)
-            if (it->second != i) return fail(who + ": dst[" + std::to_string(i) + "] is also src[" + std::to_string(it->second) + "]");
-        if (d[i] == a[i] && in_log_n != log_n) return fail(who + ": dst[" + std::to_string(i) + "] == src[" + std::to_string(i) + "]: in place needs equal input and output sizes");
-    }
+    std::vector<PolyBuf *> d, a;
+    if (g.out(dst, count, "dst", n_out, out_name, d) || g.in(src, count, "src", n_in, in_name, a) || g.distinct("dst", "src")) return 1;
+    for (size_t i = 0; i < count; i++)
+        if (d[i] == a[i] && in_log_n != log_n)
+            return fail(who + ": dst[" + std::to_string(i) + "] == src[" + std::to_string(i) + "]: in place needs equal input and output sizes");
     return by_field(d[0]->field, [&](auto p) { return poly_transform<decltype(p)>(d, a, mode, in_log_n, log_n, omega, zeta, divisor, n_out, h); });
 }
 extern "C" int h2_poly_lagrange_to_coeff(uint64_t dst, uint64_t src, uint32_t k, const void *omega_inv, const void *divisor, int repr) {
@@ -467,36 +452,19 @@ extern "C" int h2_poly_set_rows(const uint64_t *polys, size_t count, size_t star
     if (require_ready() || h.check({{values, "values", count != 0 && rows != 0}})) return 1;
     if (count == 0) return 0;
     if (!polys) return fail(std::string(who) + ": null handle array");
-    const size_t ptr_fe = (count * sizeof(fe *) + sizeof(fe) - 1) / sizeof(fe);
-    if (rows != 0 && count > ((size_t)-1 / sizeof(fe) - ptr_fe) / rows) return fail(std::string(who) + ": count * rows overflows");
+    // the column table, count pointers in (count + 3) / 4 elements and then count x rows values, must fit in size_t
+    if (rows != 0 && count > ((size_t)-1 / sizeof(fe) - (count + 3) / 4) / rows) return fail(std::string(who) + ": count * rows overflows");
     PolyArgs g(who);
-    std::vector<std::pair<PolyBuf *, size_t>> ps(count);
-    for (size_t i = 0; i < count; i++) {
-        PolyBuf *b = g.out(polys[i], 0, "0");
-        if (!b) return fail(std::string(who) + ": polys[" + std::to_string(i) + "]" + last_error_string().substr(strlen(who)));
-        if (start > b->len || rows > b->len - start)
-            return fail(std::string(who) + ": polys[" + std::to_string(i) + "]: rows [start, start + rows) exceed the polynomial's length");
-        ps[i] = {b, i};
-    }
-    std::sort(ps.begin(), ps.end());
-    for (size_t i = 1; i < count; i++)
-        if (ps[i].first == ps[i - 1].first)
-            return fail(std::string(who) + ": polys[" + std::to_string(ps[i].second) + "] is also polys[" + std::to_string(ps[i - 1].second) + "]");
+    std::vector<PolyBuf *> ps;
+    if (g.out(polys, count, "polys", start, rows, "start + rows", ps) || g.distinct()) return 1;
     if (rows == 0) return 0;
-    // one upload: the column pointers, then the values
     const size_t total = count * rows;
-    std::vector<fe> up(ptr_fe + total);
-    fe **hp = reinterpret_cast<fe **>(up.data());
-    for (auto &p : ps) hp[p.second] = p.first->buf.as<fe>();
-    memcpy(up.data() + ptr_fe, values, total * sizeof(fe));
-    Context &X = g_ctx;
-    cudaStream_t s = X.stream;
-    if (scratch_acquire(s)) return 1;
-    if (X.ntt_cols.ensure(up.size() * sizeof(fe)) || upload_async(X.ntt_cols.p, up.data(), up.size() * sizeof(fe), s)) return 1;
-    const fe *d = X.ntt_cols.as<fe>();
-    if (by_field(ps[0].first->field, [&](auto p) {
-            LAUNCH(set_rows_kernel<decltype(p)>, blocks_for(total, 256), 256, 0, s, reinterpret_cast<fe *const *>(d), d + ptr_fe, (uint64_t)start,
-                   (uint64_t)rows, (uint64_t)total, h.canon() ? 1 : 0);
+    cudaStream_t s = g_ctx.stream;
+    ColTable t;
+    if (scratch_acquire(s) || col_table(ps, values, total * sizeof(fe), s, &t)) return 1;
+    if (by_field(ps[0]->field, [&](auto p) {
+            LAUNCH(set_rows_kernel<decltype(p)>, blocks_for(total, 256), 256, 0, s, t.cols, (const fe *)t.data, (uint64_t)start, (uint64_t)rows,
+                   (uint64_t)total, h.canon() ? 1 : 0);
             return 0;
         }))
         return 1;

@@ -28,16 +28,18 @@ static int polyops_run(int mode, const std::vector<PolyBuf *> &a, const std::vec
     const uint64_t lvl_total = off.back() + m.back() * batch + batch;
     if (scratch_acquire(s)) return 1;
     if (X.po_lvl.ensure(lvl_total * sizeof(fe)) || X.po_q.ensure(lvl_total * sizeof(fe)) || X.po_pts.ensure((L + 2) * batch * sizeof(fe)) ||
-        X.po_ptrs.ensure(2 * batch * sizeof(void *)) || X.misc.ensure(batch * sizeof(fe) + 64))
+        X.misc.ensure(batch * sizeof(fe) + 64))
         return 1;
     fe *lvl = X.po_lvl.as<fe>(), *qarr = X.po_q.as<fe>(), *pts = X.po_pts.as<fe>();
     auto level = [&](size_t l) { return lvl + off[l]; };         // values of level l >= 1: [batch][m[l]]
     auto qlevel = [&](size_t l) { return qarr + off[l]; };
-    std::vector<const fe *> hp(2 * batch);
-    for (uint32_t b = 0; b < batch; b++) { hp[b] = a[b]->buf.as<fe>(); hp[batch + b] = c.empty() ? nullptr : c[b]->buf.as<fe>(); }
-    CU(cudaMemcpyAsync(X.po_ptrs.p, hp.data(), 2 * batch * sizeof(void *), cudaMemcpyHostToDevice, s));
-    const fe *const *d_a = X.po_ptrs.as<const fe *>();
-    const fe *const *d_c = d_a + batch;
+    std::vector<PolyBuf *> cols(a);                              // a, then c (null pointers without it)
+    cols.insert(cols.end(), c.begin(), c.end());
+    cols.resize(2 * batch);
+    ColTable t;
+    if (col_table(cols, nullptr, 0, s, &t)) return 1;
+    const fe *const *d_a = t.cols;
+    fe *const *d_c = t.cols + batch;
     // points of level 0 (Montgomery): the caller's, or 1 for the plain sums of the inner product
     if (mode == 1) {
         LAUNCH(fe_fill_kernel<P>, blocks_for(batch, 64), 64, 0, s, pts, batch, fe_one<P>());
@@ -55,7 +57,7 @@ static int polyops_run(int mode, const std::vector<PolyBuf *> &a, const std::vec
             CU(cudaStreamSynchronize(s));
             return 0;
         }
-        LAUNCH(poly_kate_cta_kernel<P>, batch, H2_KATE_CTA, 0, s, d_a, (uint64_t)n, (const fe *)pts, (fe *const *)d_c);
+        LAUNCH(poly_kate_cta_kernel<P>, batch, H2_KATE_CTA, 0, s, d_a, (uint64_t)n, (const fe *)pts, d_c);
         for (uint32_t b = 0; b < batch; b++) CU(cudaMemsetAsync(c[b]->buf.as<fe>() + (n - 1), 0, sizeof(fe), s));
         return scratch_release(s);
     }
@@ -72,7 +74,7 @@ static int polyops_run(int mode, const std::vector<PolyBuf *> &a, const std::vec
     if (mode != 2) {   // the single value of the top level is the result (n == 1: the coefficient itself; n == 0 handled by the caller)
         fe *res = X.misc.as<fe>();
         if (L == 0) {
-            for (uint32_t b = 0; b < batch; b++) CU(cudaMemcpyAsync(res + b, hp[b], sizeof(fe), cudaMemcpyDeviceToDevice, s));
+            for (uint32_t b = 0; b < batch; b++) CU(cudaMemcpyAsync(res + b, a[b]->buf.as<fe>(), sizeof(fe), cudaMemcpyDeviceToDevice, s));
         } else {
             CU(cudaMemcpyAsync(res, level(L), batch * sizeof(fe), cudaMemcpyDeviceToDevice, s));   // m[L] == 1: [batch][1]
         }
@@ -84,12 +86,11 @@ static int polyops_run(int mode, const std::vector<PolyBuf *> &a, const std::vec
     }
     // kate division, downward pass: Q at every position of level l from the carries of level l + 1.  The top level with
     // more than one value (m[L] == 1 always; start from the highest level that has something to walk) needs no carry.
-    fe *const *d_q = (fe *const *)d_c;
     for (size_t l = L; l-- > 0;) {
         const dim3 grid(blocks_for(m[l + 1], 128), batch);
         const fe *carry = (l + 1 < L) ? (const fe *)qlevel(l + 1) : (const fe *)nullptr;   // Q of level l + 1; the top level's Q(1..) are zero
         LAUNCH(poly_kate_down_kernel<P>, grid, 128, 0, s, l == 0 ? d_a : (const fe *const *)nullptr, l == 0 ? (const fe *)nullptr : (const fe *)level(l), m[l],
-               (const fe *)(pts + l * batch), carry, m[l + 1], l == 0 ? (fe *)nullptr : qlevel(l), l == 0 ? d_q : (fe *const *)nullptr);
+               (const fe *)(pts + l * batch), carry, m[l + 1], l == 0 ? (fe *)nullptr : qlevel(l), l == 0 ? d_c : (fe *const *)nullptr);
     }
     // the quotient has n - 1 coefficients; slot n - 1 becomes the zero the reference pushes before committing n of them
     // (poly/multiopen/prover.rs: `kate_division(..); poly.push(ZERO)`)
@@ -107,8 +108,8 @@ static int polyops_dispatch(int mode, const uint64_t *ah, const uint64_t *ch, si
     PolyArgs g(who);
     std::vector<PolyBuf *> a, c;
     if (mode == 2) {   // kate division writes quotients of n - 1 coefficients; the inner product reads both operands
-        if (g.out(ch, batch, n - 1, "n - 1", c) || g.in(ah, batch, n, "n", a) || g.distinct("a quotient")) return 1;
-    } else if (g.in(ah, batch, n, "n", a) || (ch && g.in(ch, batch, n, "n", c))) {
+        if (g.out(ch, batch, "dst", n - 1, "n - 1", c) || g.in(ah, batch, "src", n, "n", a) || g.distinct()) return 1;
+    } else if (g.in(ah, batch, mode == 0 ? "polys" : "a", n, "n", a) || (ch && g.in(ch, batch, "b", n, "n", c))) {
         return 1;
     }
     return by_field(a[0]->field, [&](auto p) { return polyops_run<decltype(p)>(mode, a, c, n, points, h, out); });
@@ -122,15 +123,15 @@ static int ast_run(PolyBuf *out, const std::vector<PolyBuf *> &polys, uint32_t l
     cudaStream_t s = X.stream;
     const uint64_t n = 1ull << log_n;
     if (scratch_acquire(s)) return 1;
-    if (X.ast_code.ensure(n_code * sizeof(AstInstr)) || X.ast_consts.ensure((n_consts + 1) * sizeof(fe)) || X.po_ptrs.ensure((polys.size() + 1) * sizeof(void *)))
-        return 1;
-    std::vector<const fe *> hp(polys.size() + 1, nullptr);
-    for (size_t i = 0; i < polys.size(); i++) hp[i] = polys[i]->buf.as<fe>();
-    CU(cudaMemcpyAsync(X.po_ptrs.p, hp.data(), hp.size() * sizeof(void *), cudaMemcpyHostToDevice, s));
+    if (X.ast_code.ensure(n_code * sizeof(AstInstr)) || X.ast_consts.ensure((n_consts + 1) * sizeof(fe))) return 1;
+    std::vector<PolyBuf *> cols(polys);
+    cols.push_back(nullptr);                                     // a program without operands still gets a table
+    ColTable t;
+    if (col_table(cols, nullptr, 0, s, &t)) return 1;
     CU(cudaMemcpyAsync(X.ast_code.p, code, n_code * sizeof(AstInstr), cudaMemcpyHostToDevice, s));
     if (h.up(P::ID, X.ast_consts.as<fe>(), consts, n_consts, s)) return 1;
     AstArgs A;
-    A.polys = X.po_ptrs.as<const fe *>(); A.code = X.ast_code.as<AstInstr>(); A.n_code = (uint32_t)n_code; A.consts = X.ast_consts.as<fe>();
+    A.polys = t.cols; A.code = X.ast_code.as<AstInstr>(); A.n_code = (uint32_t)n_code; A.consts = X.ast_consts.as<fe>();
     A.tw = nullptr; A.lin_base = fe_one<P>(); A.log_n = log_n; A.out = out->buf.as<fe>();
     if (has_linear) {
         if (get_twiddles_any(out->field, h.elem<P>(omega), log_n, s, &A.tw)) return 1;
@@ -147,8 +148,8 @@ extern "C" int h2_poly_eval_ast(uint64_t out, const uint64_t *polys, size_t n_po
     if (n_code == 0 || n_code > (1u << 20)) return fail("h2_poly_eval_ast: empty or oversized program");
     PolyArgs g("h2_poly_eval_ast");
     std::vector<PolyBuf *> ps;
-    PolyBuf *o = g.out(out, (size_t)1 << log_n, "2^log_n");
-    if (!o || g.in(polys, n_polys, (size_t)1 << log_n, "2^log_n", ps) || g.distinct("an output")) return 1;   // operands are read at other rows
+    PolyBuf *o = g.out(out, "out", (size_t)1 << log_n, "2^log_n");
+    if (!o || g.in(polys, n_polys, "polys", (size_t)1 << log_n, "2^log_n", ps) || g.distinct()) return 1;   // operands are read at other rows
     const AstInstr *prog = reinterpret_cast<const AstInstr *>(code);
     int depth = 0;
     bool has_linear = false;
@@ -175,7 +176,7 @@ extern "C" int h2_poly_batch_invert(uint64_t poly, size_t n) {
     CtxLock lk;
     if (require_ready()) return 1;
     PolyArgs g("h2_poly_batch_invert");
-    PolyBuf *a = g.out(poly, n, "n");
+    PolyBuf *a = g.out(poly, "poly", n, "n");
     if (!a) return 1;
     if (n == 0) return 0;
     cudaStream_t s = g_ctx.stream;
@@ -217,7 +218,7 @@ extern "C" int h2_poly_running_product(uint64_t dst, uint64_t src, size_t n, con
     if (require_ready() || h.check({{init, "init", n != 0}})) return 1;
     PolyArgs g("h2_poly_running_product");
     PolyBuf *d, *a;
-    if (!(d = g.out(dst, n, "n")) || !(a = g.in(src, n, "n")) || g.distinct("a dst")) return 1;
+    if (!(d = g.out(dst, "dst", n, "n")) || !(a = g.in(src, "src", n, "n")) || g.distinct()) return 1;
     if (n == 0) return 0;
     return by_field(a->field, [&](auto p) { return grand_product_run<decltype(p)>(d, a, n, init, h); });
 }
@@ -228,7 +229,7 @@ extern "C" int h2_poly_divide_by_vanishing(uint64_t poly, uint32_t ext_k, const 
     if (require_ready() || h.check({{t_evals, "t_evals"}})) return 1;
     if (ext_k > 30) return fail("h2_poly_divide_by_vanishing: ext_k > 30");
     PolyArgs g("h2_poly_divide_by_vanishing");
-    PolyBuf *a = g.out(poly, (size_t)1 << ext_k, "2^ext_k");
+    PolyBuf *a = g.out(poly, "poly", (size_t)1 << ext_k, "2^ext_k");
     if (!a) return 1;
     if (t_len == 0 || (t_len & (t_len - 1)) || t_len > (1u << ext_k)) return fail("h2_poly_divide_by_vanishing: t_len must be a power of two <= 2^ext_k");
     Context &X = g_ctx;
@@ -296,40 +297,34 @@ template <class P> static int lk_sort(fe *keys, uint64_t N, uint32_t count, cuda
 // The permuted columns of `count` lookups of u usable rows (lookup.cuh), and with `blinding` (count x 2 rows values) the
 // blinding rows [u, u + rows) of every output.  Scratch from the lane's pools, per lookup (N = the power of two >= u, >= 2):
 //   lk_keys  32 N bytes (the sorted table)          lk_u32  4 (3 u + 2) bytes (cnt | unconsumed, scanned in one pass; leftovers)
-//   lk_aux   32 bytes of pointers + 64 rows bytes of blinding values;  plus 4 bytes per 8192 scanned words and the error word.
+//   col_tab  32 bytes of pointers + 64 rows bytes of blinding values;  plus 4 bytes per 8192 scanned words and the error word.
 // `h`: the encoding of the blinding values (nullptr without them).  One synchronisation; *bad = the lowest lookup with an input value
 // its table lacks, H2_LK_NONE when none -- and then every output is as it was (the one writing kernel runs after the miss is known and
 // checks for it first).
 template <class P>
-static int lookup_permuted_run(const std::vector<PolyBuf *> &outs, const std::vector<PolyBuf *> &ins, uint64_t u, uint64_t rows, const void *blinding,
-                               const HostArgs *h, uint32_t *bad) {
+static int lookup_permuted_run(const std::vector<PolyBuf *> &out_in, const std::vector<PolyBuf *> &out_tab, const std::vector<PolyBuf *> &in,
+                               const std::vector<PolyBuf *> &tab, uint64_t u, uint64_t rows, const void *blinding, const HostArgs *h, uint32_t *bad) {
     Context &X = g_ctx;
     cudaStream_t s = X.stream;
-    const uint32_t count = (uint32_t)(ins.size() / 2);
+    const uint32_t count = (uint32_t)in.size();
     uint64_t N = 2;
     while (N < u) N <<= 1;
-    const uint64_t w = u + 1, nblind = blinding ? (uint64_t)count * 2 * rows : 0, ptr_fe = ((uint64_t)count * 4 * sizeof(void *) + sizeof(fe) - 1) / sizeof(fe);
-    std::vector<uint8_t> up((ptr_fe + nblind) * sizeof(fe));
-    const fe **hp = reinterpret_cast<const fe **>(up.data());
-    for (uint32_t b = 0; b < count; b++) {
-        hp[b] = ins[2 * b]->buf.as<fe>();
-        hp[count + b] = ins[2 * b + 1]->buf.as<fe>();
-        hp[2 * count + b] = outs[2 * b]->buf.as<fe>();
-        hp[3 * count + b] = outs[2 * b + 1]->buf.as<fe>();
-    }
-    if (nblind) memcpy(up.data() + ptr_fe * sizeof(fe), blinding, nblind * sizeof(fe));
+    const uint64_t w = u + 1, nblind = blinding ? (uint64_t)count * 2 * rows : 0;
+    std::vector<PolyBuf *> cols(in);                             // LkCols: in, tab, out_in, out_tab
+    for (auto *v : {&tab, &out_in, &out_tab}) cols.insert(cols.end(), v->begin(), v->end());
     if (scratch_acquire(s)) return 1;
-    if (X.lk_keys.ensure(count * N * sizeof(fe)) || X.lk_aux.ensure(up.size()) || X.lk_u32.ensure(((2 * w + u) * count + 4) * sizeof(uint32_t))) return 1;
-    fe *keys = X.lk_keys.as<fe>(), *aux = X.lk_aux.as<fe>();
+    if (X.lk_keys.ensure(count * N * sizeof(fe)) || X.lk_u32.ensure(((2 * w + u) * count + 4) * sizeof(uint32_t))) return 1;
+    fe *keys = X.lk_keys.as<fe>();
     uint32_t *sc = X.lk_u32.as<uint32_t>(), *left = sc + 2 * w * count, *err = left + u * count;
-    CU(cudaMemcpyAsync(aux, up.data(), up.size(), cudaMemcpyHostToDevice, s));
+    ColTable t;
+    if (col_table(cols, blinding, nblind * sizeof(fe), s, &t)) return 1;
     LkCols c;
-    c.in = reinterpret_cast<const fe *const *>(aux);
+    c.in = t.cols;
     c.tab = c.in + count;
-    c.out_in = reinterpret_cast<fe *const *>(aux) + 2 * count;
+    c.out_in = t.cols + 2 * count;
     c.out_tab = c.out_in + count;
-    c.blind = nblind ? aux + ptr_fe : nullptr;
-    if (nblind && h->to_mont(P::ID, aux + ptr_fe, nblind, s)) return 1;
+    c.blind = t.data;
+    if (nblind && h->to_mont(P::ID, t.data, nblind, s)) return 1;
     CU(cudaMemsetAsync(sc, 0, w * count * sizeof(uint32_t), s));
     CU(cudaMemsetAsync(err, 0xFF, sizeof(uint32_t), s));
     LAUNCH(lk_load_kernel<P>, dim3(blocks_for(N, 256), count), 256, 0, s, c, u, keys, N);
@@ -350,14 +345,15 @@ extern "C" int h2_poly_lookup_permute(uint64_t input, uint64_t table, size_t usa
     static const char *who = "h2_poly_lookup_permute";
     CtxLock lk;
     if (require_ready()) return 1;
-    const uint64_t oh[2] = {out_input, out_table}, ih[2] = {input, table};
     PolyArgs g(who);
-    std::vector<PolyBuf *> outs, ins;
-    if (g.out(oh, 2, usable_rows, "usable_rows", outs) || g.in(ih, 2, usable_rows, "usable_rows", ins) || g.distinct("an output")) return 1;
+    PolyBuf *oi, *ot, *i, *t;
+    if (!(oi = g.out(out_input, "out_input", usable_rows, "usable_rows")) || !(ot = g.out(out_table, "out_table", usable_rows, "usable_rows")) ||
+        !(i = g.in(input, "input", usable_rows, "usable_rows")) || !(t = g.in(table, "table", usable_rows, "usable_rows")) || g.distinct())
+        return 1;
     if (usable_rows >= (1ull << 31)) return fail("h2_poly_lookup_permute: usable_rows >= 2^31");
     if (usable_rows == 0) return 0;
     uint32_t bad = H2_LK_NONE;
-    if (by_field(outs[0]->field, [&](auto p) { return lookup_permuted_run<decltype(p)>(outs, ins, usable_rows, 0, nullptr, nullptr, &bad); }))
+    if (by_field(oi->field, [&](auto p) { return lookup_permuted_run<decltype(p)>({oi}, {ot}, {i}, {t}, usable_rows, 0, nullptr, nullptr, &bad); }))
         return 1;
     if (bad != H2_LK_NONE) return fail(std::string(who) + ": " + lk_miss);
     return 0;
@@ -373,17 +369,14 @@ extern "C" int h2_poly_lookup_permuted(const uint64_t *out_inputs, const uint64_
     if (count == 0) return 0;
     if (!out_inputs || !out_tables || !inputs || !tables) return fail(std::string(who) + ": null argument");
     if (count > 65535) return fail(std::string(who) + ": more than 65535 lookups");
-    std::vector<uint64_t> oh, ih;
-    for (size_t b = 0; b < count; b++) {
-        oh.insert(oh.end(), {out_inputs[b], out_tables[b]});
-        ih.insert(ih.end(), {inputs[b], tables[b]});
-    }
     const uint64_t n = 1ull << k, rows = (uint64_t)blinding_factors + 1;
     PolyArgs g(who);
-    std::vector<PolyBuf *> outs, ins;
-    if (g.out(oh.data(), 2 * count, n, "2^k", outs) || g.in(ih.data(), 2 * count, n, "2^k", ins) || g.distinct("an output")) return 1;
+    std::vector<PolyBuf *> oi, ot, i, t;
+    if (g.out(out_inputs, count, "out_inputs", n, "2^k", oi) || g.out(out_tables, count, "out_tables", n, "2^k", ot) ||
+        g.in(inputs, count, "inputs", n, "2^k", i) || g.in(tables, count, "tables", n, "2^k", t) || g.distinct())
+        return 1;
     uint32_t bad = H2_LK_NONE;
-    if (by_field(outs[0]->field, [&](auto p) { return lookup_permuted_run<decltype(p)>(outs, ins, n - rows, rows, blinding, &h, &bad); })) return 1;
+    if (by_field(oi[0]->field, [&](auto p) { return lookup_permuted_run<decltype(p)>(oi, ot, i, t, n - rows, rows, blinding, &h, &bad); })) return 1;
     if (bad != H2_LK_NONE) return fail(std::string(who) + ": lookup " + std::to_string(bad) + ": " + lk_miss);
     return 0;
 }
@@ -412,7 +405,7 @@ extern "C" int h2_poly_compute_s(uint64_t dst, const void *u, uint32_t k, const 
     if (k == 0) return fail("h2_poly_compute_s: no challenges (assert!(!u.is_empty()), poly/commitment/verifier.rs:157)");
     if (k > 30) return fail("h2_poly_compute_s: k > 30");
     PolyArgs g("h2_poly_compute_s");
-    PolyBuf *d = g.out(dst, (size_t)1 << k, "2^k");
+    PolyBuf *d = g.out(dst, "dst", (size_t)1 << k, "2^k");
     if (!d) return 1;
     return by_field(d->field, [&](auto p) { return compute_s_run<decltype(p)>(d, u, k, init, accumulate, h); });
 }
@@ -423,8 +416,8 @@ extern "C" int h2_poly_scale_add(uint64_t dst, const void *a, uint64_t src, cons
     const HostArgs h("h2_poly_scale_add", repr);
     if (require_ready() || h.check({{a, "a"}, {b, "b", src != 0}})) return 1;
     PolyArgs g("h2_poly_scale_add");
-    PolyBuf *d = g.out(dst, n, "n"), *x = nullptr;
-    if (!d || (src && !(x = g.in(src, n, "n"))) || g.distinct("a dst")) return 1;
+    PolyBuf *d = g.out(dst, "dst", n, "n"), *x = nullptr;
+    if (!d || (src && !(x = g.in(src, "src", n, "n"))) || g.distinct()) return 1;
     if (n == 0) return 0;
     cudaStream_t s = g_ctx.stream;
     const fe *sp = x ? x->buf.as<fe>() : nullptr;
@@ -501,7 +494,7 @@ extern "C" int h2_poly_permutation_sigma(const uint64_t *dst, size_t cols, uint3
     if (!dst || !mapping) return fail("h2_poly_permutation_sigma: null argument");
     PolyArgs g("h2_poly_permutation_sigma");
     std::vector<PolyBuf *> d;
-    if (g.out(dst, cols, (size_t)1 << k, "2^k", d) || g.distinct("a dst")) return 1;
+    if (g.out(dst, cols, "dst", (size_t)1 << k, "2^k", d) || g.distinct()) return 1;
     return by_field(d[0]->field, [&](auto p) { return permutation_sigma_run<decltype(p)>(d, k, mapping, omega, delta, h); });
 }
 
@@ -627,7 +620,7 @@ extern "C" int h2_poly_permutation_sigma_copies(const uint64_t *dst, size_t cols
     if ((uint64_t)m >= (1ull << 32)) return fail("h2_poly_permutation_sigma_copies: m >= 2^32 copies");
     PolyArgs g("h2_poly_permutation_sigma_copies");
     std::vector<PolyBuf *> d;
-    if (g.out(dst, cols, (size_t)1 << k, "2^k", d) || g.distinct("a dst")) return 1;
+    if (g.out(dst, cols, "dst", (size_t)1 << k, "2^k", d) || g.distinct()) return 1;
     return by_field(d[0]->field, [&](auto p) { return permutation_sigma_copies_run<decltype(p)>(d, k, copies, m, omega, delta, h); });
 }
 
@@ -636,8 +629,8 @@ extern "C" int h2_poly_permutation_sigma_copies(const uint64_t *dst, size_t cols
 // the permutation and lookup arguments' product columns, every column of every proof in one call (grandproduct.cuh)
 // ------------------------------------------------------------------------------------------------
 // `ins`: the permutation's proofs x cols column pointers then its cols sigma pointers, or 4 pointers per lookup column.
-// Scratch: gp_val [count][n] (den, den^-1, mv), po_lvl / po_q the tree's levels and exclusive products, gp_aux one upload of
-// the pointer arrays and the blinding values, then the power tables and the carries.
+// Scratch: gp_val [count][n] (den, den^-1, mv), po_lvl / po_q the tree's levels and exclusive products, col_tab one upload of
+// the pointer arrays (z, then ins) and the blinding values, gp_aux the power tables and the carries.
 template <class P>
 static int product_run(bool perm, const std::vector<PolyBuf *> &z, const std::vector<PolyBuf *> &ins, uint32_t ncols, uint32_t chunk_len,
                        uint32_t sets, uint32_t k, const void *beta, const void *gamma, const void *omega, const void *delta, const void *blinding,
@@ -649,23 +642,18 @@ static int product_run(bool perm, const std::vector<PolyBuf *> &z, const std::ve
     G.m[0] = n; G.m[1] = (n + H2_POLY_CHUNK - 1) / H2_POLY_CHUNK; G.L = 1;
     while (G.m[G.L] > H2_POLY_CHUNK) { G.off[G.L + 1] = G.off[G.L] + G.m[G.L] * count; G.m[G.L + 1] = (G.m[G.L] + H2_POLY_CHUNK - 1) / H2_POLY_CHUNK; G.L++; }
     const uint64_t total = G.off[G.L] + G.m[G.L] * count;
-    const uint64_t nptr = count + ins.size(), ptr_fe = (nptr * sizeof(void *) + sizeof(fe) - 1) / sizeof(fe);
     const uint64_t tlen = perm ? KeygenOps<P>::table_len(k, ncols) : 0, nblind = count * bf;
-    std::vector<uint8_t> up((ptr_fe + nblind) * sizeof(fe));
-    const fe **hp = reinterpret_cast<const fe **>(up.data());
-    for (uint64_t b = 0; b < count; b++) hp[b] = z[b]->buf.as<fe>();
-    for (size_t i = 0; i < ins.size(); i++) hp[count + i] = ins[i]->buf.as<fe>();
-    if (nblind) memcpy(up.data() + ptr_fe * sizeof(fe), blinding, nblind * sizeof(fe));
+    std::vector<PolyBuf *> cols(z);
+    cols.insert(cols.end(), ins.begin(), ins.end());
     if (scratch_acquire(s)) return 1;
     if (X.gp_val.ensure(count * n * sizeof(fe)) || X.po_lvl.ensure(total * sizeof(fe)) || X.po_q.ensure(total * sizeof(fe)) ||
-        X.gp_aux.ensure((ptr_fe + nblind + tlen + count) * sizeof(fe)))
+        X.gp_aux.ensure((tlen + count) * sizeof(fe)))
         return 1;
-    fe *val = X.gp_val.as<fe>(), *lvl = X.po_lvl.as<fe>(), *ex = X.po_q.as<fe>();
-    fe *aux = X.gp_aux.as<fe>(), *blind = aux + ptr_fe, *tab = blind + nblind, *init = tab + tlen;
-    fe *const *zp = reinterpret_cast<fe *const *>(aux);
-    const fe *const *ip = reinterpret_cast<const fe *const *>(aux) + count;
-    CU(cudaMemcpyAsync(aux, up.data(), up.size(), cudaMemcpyHostToDevice, s));
-    if (h.to_mont(P::ID, blind, nblind, s)) return 1;
+    fe *val = X.gp_val.as<fe>(), *lvl = X.po_lvl.as<fe>(), *ex = X.po_q.as<fe>(), *tab = X.gp_aux.as<fe>(), *init = tab + tlen;
+    ColTable t;
+    if (col_table(cols, blinding, nblind * sizeof(fe), s, &t) || h.to_mont(P::ID, t.data, nblind, s)) return 1;
+    fe *const *zp = t.cols;
+    const fe *const *ip = t.cols + count;
     const fe b_m = h.elem<P>(beta), g_m = h.elem<P>(gamma);
     if (perm) {
         LAUNCH(keygen_tables_kernel<P>, blocks_for(tlen, 128), 128, 0, s, tab, h.elem<P>(omega), h.elem<P>(delta), k, ncols);
@@ -685,7 +673,7 @@ static int product_run(bool perm, const std::vector<PolyBuf *> &z, const std::ve
                l == G.L ? (const fe *)nullptr : (const fe *)(ex + G.off[l + 1]), (const fe *)init, l == 0 ? (fe *)nullptr : ex + G.off[l],
                l == 0 ? zp : (fe *const *)nullptr, chunks);
     }
-    if (bf) LAUNCH(gp_blind_kernel<P>, blocks_for(nblind, 256), 256, 0, s, zp, n, bf, (const fe *)blind, count);
+    if (bf) LAUNCH(gp_blind_kernel<P>, blocks_for(nblind, 256), 256, 0, s, zp, n, bf, (const fe *)t.data, count);
     return scratch_release(s);
 }
 static int product_scalars(const char *who, uint32_t k, uint32_t bf) {
@@ -709,11 +697,12 @@ extern "C" int h2_poly_permutation_product(const uint64_t *z_out, size_t proofs,
     if (!z_out || !columns || !sigmas) return fail(std::string(who) + ": null argument");
     const uint64_t sets = (cols + chunk_len - 1) / chunk_len;
     if (cols >= (1ull << 20) || proofs >= (1ull << 16) || proofs * sets > 65535) return fail(std::string(who) + ": more than 65535 product columns");
-    std::vector<uint64_t> ih(columns, columns + proofs * cols);
-    ih.insert(ih.end(), sigmas, sigmas + cols);
     PolyArgs g(who);
-    std::vector<PolyBuf *> z, ins;
-    if (g.out(z_out, proofs * sets, 1ull << k, "2^k", z) || g.in(ih.data(), ih.size(), 1ull << k, "2^k", ins) || g.distinct("a z_out")) return 1;
+    std::vector<PolyBuf *> z, ins, sig;
+    if (g.out(z_out, proofs * sets, "z_out", 1ull << k, "2^k", z) || g.in(columns, proofs * cols, "columns", 1ull << k, "2^k", ins) ||
+        g.in(sigmas, cols, "sigmas", 1ull << k, "2^k", sig) || g.distinct())
+        return 1;
+    ins.insert(ins.end(), sig.begin(), sig.end());
     return by_field(z[0]->field, [&](auto p) {
         return product_run<decltype(p)>(true, z, ins, (uint32_t)cols, chunk_len, (uint32_t)sets, k, beta, gamma, omega, delta, blinding, blinding_factors, h);
     });
@@ -730,10 +719,13 @@ extern "C" int h2_poly_lookup_product(const uint64_t *z_out, size_t count, const
     if (count == 0) return 0;
     if (!z_out || !inputs || !tables || !permuted_inputs || !permuted_tables) return fail(std::string(who) + ": null argument");
     if (count > 65535) return fail(std::string(who) + ": more than 65535 product columns");
-    std::vector<uint64_t> ih;
-    for (size_t b = 0; b < count; b++) ih.insert(ih.end(), {inputs[b], tables[b], permuted_inputs[b], permuted_tables[b]});
+    const uint64_t n = 1ull << k;
     PolyArgs g(who);
-    std::vector<PolyBuf *> z, ins;
-    if (g.out(z_out, count, 1ull << k, "2^k", z) || g.in(ih.data(), ih.size(), 1ull << k, "2^k", ins) || g.distinct("a z_out")) return 1;
+    std::vector<PolyBuf *> z, in, tab, pin, ptab;
+    if (g.out(z_out, count, "z_out", n, "2^k", z) || g.in(inputs, count, "inputs", n, "2^k", in) || g.in(tables, count, "tables", n, "2^k", tab) ||
+        g.in(permuted_inputs, count, "permuted_inputs", n, "2^k", pin) || g.in(permuted_tables, count, "permuted_tables", n, "2^k", ptab) || g.distinct())
+        return 1;
+    std::vector<PolyBuf *> ins;                                  // gp_lookup_factors_kernel: 4 per column
+    for (size_t b = 0; b < count; b++) ins.insert(ins.end(), {in[b], tab[b], pin[b], ptab[b]});
     return by_field(z[0]->field, [&](auto p) { return product_run<decltype(p)>(false, z, ins, 0, 1, 1, k, beta, gamma, nullptr, nullptr, blinding, blinding_factors, h); });
 }

@@ -157,19 +157,20 @@ struct Context {
     // MSM scratch
     DevBuf scal_in, bases_in, bases_phi, glv_parts, scal_canon, counts, cursor, refs, size_hist, items, bucket_sum, pkey, pstart, pend, ppt, ra_t, ra_e, r0, r1,
         wsum, scan_blocks, result, misc, ba_lv[3];
-    // NTT scratch; ntt_cols: the column pointer tables of a batched transform, and the rows of h2_poly_set_rows
-    DevBuf ntt_io, ntt_out, ntt_work, ntt_cols, pow2;
+    // NTT scratch
+    DevBuf ntt_io, ntt_out, ntt_work, pow2;
+    DevBuf col_tab;                          // the column table of the call in flight (col_table)
     // EC-FFT / batch-normalise scratch: XYZZ work array (128 B per point), staging for the host forms
     DevBuf ec_work, ec_io, ec_out;
     DevBuf fb_a, fb_b;                       // partial sums of the direct-sum fixed-base MSM (ping-pong)
     DevBuf multi_parts;                      // primary device: the per-GPU partial results of a multi-GPU MSM (peer-written)
     StageRing stage;
     DevBuf ast_code, ast_consts;             // asteval.cuh: the postfix program and its constants
-    DevBuf po_lvl, po_q, po_pts, po_ptrs;    // polyops.cuh: level arrays, kate carries, per-level points, pointer arrays
-    DevBuf lk_keys, lk_aux, lk_u32;          // lookup.cuh: sorted tables, column pointers + blinding values, histogram / scan / leftover arrays
+    DevBuf po_lvl, po_q, po_pts;             // polyops.cuh: level arrays, kate carries, per-level points
+    DevBuf lk_keys, lk_u32;                  // lookup.cuh: sorted tables, histogram / scan / leftover arrays
     DevBuf kg_tab, kg_map;                   // keygen.cuh: power tables + error word, one piece of the copy-constraint mapping (all of it for assembly.cuh)
     DevBuf as_edge, as_cell, as_slot;        // assembly.cuh: per-copy, per-cell and per-slot u32 arrays
-    DevBuf gp_val, gp_aux;                   // grandproduct.cuh: denominators / mv of every column, pointers + tables + carries + blinding values
+    DevBuf gp_val, gp_aux;                   // grandproduct.cuh: denominators / mv of every column, power tables + carries
     std::vector<TwiddleEntry *> twiddles;
     uint64_t tw_stamp = 0;
     std::map<uint64_t, BaseSet *> shards;    // this device's shards of multi-GPU base sets (h2_multi_bases_register)
@@ -294,33 +295,53 @@ struct HostArgs {
 // Shared polynomials (h2_poly_share): read-only from then on, and readable from every context.  Sharing moves them out of
 // their owner's `polys` into this registry with unchanged handles; they never go into a poly_pool.
 extern std::map<uint64_t, PolyBuf *> g_shared_polys;
-// The resident-polynomial arguments of one entry point `who`, all checked before it launches anything:
-//   - an output is a polynomial of the calling context; a shared one fails with "<who>: the polynomial is shared (read-only)";
+// The resident-polynomial arguments of one entry point `who`, all checked before it launches anything.  `name` is the
+// parameter's name as the header spells it; an element of a handle array is "<name>[i]".
+//   - an output is a polynomial of the calling context; a shared one fails with "the polynomial is shared (read-only)";
 //   - an input is the calling context's or a shared one, and a shared input counts the call as a user until the PolyArgs is
 //     dropped, so h2_poly_free cannot free it meanwhile.  Declared after the call's CtxLock, so it is dropped before the
 //     context's mutex;
 //   - every polynomial is over one field (`field`, the curve's scalar field for the MSM-side calls, or else the first
-//     polynomial's) and holds at least the `len` elements its lookup asks for, named `len_name` in the message;
-//   - with distinct(), no output is listed twice or is also an input; calls that work in place do not ask for it.
-// Every failure sets "<who>: <reason>"; a lookup then gives nullptr, the other members 1.
+//     polynomial's) and holds the elements [off, off + len) its lookup asks for (off = 0 unless given), else "a polynomial
+//     holds fewer than <len_name> elements".  off + len is never formed, so it cannot wrap;
+//   - with distinct(), no output is listed twice or is also an input: "<a> is also <b>", the output first ("dst[2] is also
+//     dst[0]", "dst is also src").  A call that works in place names its index-paired output and input arrays, and then
+//     out[i] == in[i] is allowed.
+// A failed lookup sets "<who>: <reason>" for a single handle, "<who>: <name>[i]: <reason>" for an element of an array; a
+// lookup then gives nullptr, the other members 1.
 struct PolyArgs {
     explicit PolyArgs(const char *who, int field = -1) : who(who), field(field), field_given(field >= 0) {}
     ~PolyArgs();
-    PolyBuf *out(uint64_t h, uint64_t len, const char *len_name);
-    PolyBuf *in(uint64_t h, uint64_t len, const char *len_name);
-    int out(const uint64_t *h, size_t n, uint64_t len, const char *len_name, std::vector<PolyBuf *> &v);
-    int in(const uint64_t *h, size_t n, uint64_t len, const char *len_name, std::vector<PolyBuf *> &v);
-    int distinct(const char *role);          // role with its article: "<who>: a dst handle appears twice"
+    PolyBuf *out(uint64_t h, const char *name, uint64_t off, uint64_t len, const char *len_name) { return find(true, h, name, -1, off, len, len_name); }
+    PolyBuf *in(uint64_t h, const char *name, uint64_t off, uint64_t len, const char *len_name) { return find(false, h, name, -1, off, len, len_name); }
+    PolyBuf *out(uint64_t h, const char *name, uint64_t len, const char *len_name) { return out(h, name, 0, len, len_name); }
+    PolyBuf *in(uint64_t h, const char *name, uint64_t len, const char *len_name) { return in(h, name, 0, len, len_name); }
+    using Polys = std::vector<PolyBuf *>;    // handle arrays: h[0 .. n) into v
+    int out(const uint64_t *h, size_t n, const char *name, uint64_t off, uint64_t len, const char *len_name, Polys &v) { return find(true, h, n, name, off, len, len_name, v); }
+    int out(const uint64_t *h, size_t n, const char *name, uint64_t len, const char *len_name, Polys &v) { return find(true, h, n, name, 0, len, len_name, v); }
+    int in(const uint64_t *h, size_t n, const char *name, uint64_t len, const char *len_name, Polys &v) { return find(false, h, n, name, 0, len, len_name, v); }
+    int distinct(const char *in_place_out = nullptr, const char *in_place_in = nullptr);
     PolyArgs(const PolyArgs &) = delete;
     PolyArgs &operator=(const PolyArgs &) = delete;
 
   private:
+    struct Arg { PolyBuf *p; bool out; const char *name; int64_t i; };   // i < 0: a single handle
     std::string who;
     int field;
     bool field_given;
-    std::vector<PolyBuf *> outs, ins, held;  // held: the shared polynomials this call is a user of
-    PolyBuf *fits(PolyBuf *p, uint64_t len, const char *len_name);
+    std::vector<Arg> args;                   // every polynomial looked up, in order
+    std::vector<PolyBuf *> held;             // the shared polynomials this call is a user of
+    PolyBuf *find(bool out, uint64_t h, const char *name, int64_t i, uint64_t off, uint64_t len, const char *len_name);
+    int find(bool out, const uint64_t *h, size_t n, const char *name, uint64_t off, uint64_t len, const char *len_name, Polys &v);
 };
+// One upload of a kernel's column table into the context's table buffer (col_tab), on `s` after scratch_acquire: the device
+// pointers of `cols` in the order the kernel reads them (a null PolyBuf gives a null pointer), then `bytes` host bytes from
+// `data` at the next 32-byte boundary.  The table is scratch: it holds until the call's scratch_release.
+struct ColTable {
+    fe *const *cols;                         // the pointers on the device
+    fe *data;                                // the bytes on the device; nullptr without any
+};
+int col_table(const std::vector<PolyBuf *> &cols, const void *data, size_t bytes, cudaStream_t s, ColTable *t);
 int shared_poly_free(uint64_t h);            // h2_poly_free of a handle that is not the calling context's
 // f(FpParams{}) or f(FqParams{}) for a field id; any other id fails
 template <class F> static int by_field(int field, F &&f) {

@@ -167,7 +167,9 @@ int h2_poly_free(uint64_t poly);
  * has landed.  Handles do not change.  A shared handle is accepted wherever a polynomial is only read (downloads, the
  * sources of copies, transforms, running products, Kate divisions and scale_add, the operands of eval_ast / eval /
  * inner_product, the inputs of lookup_permute and of the product columns, h2_msm_registered_polys*, h2_ipa_begin_poly); every call that would write
- * one fails with "<entry point>: the polynomial is shared (read-only)" and changes nothing.  h2_lane_destroy of the lane
+ * one fails with "<entry point>: the polynomial is shared (read-only)" and changes nothing.  Every rejected polynomial
+ * handle is reported this way, "<entry point>: <reason>"; an element of a handle array as "<entry point>: <name>[i]:
+ * <reason>", and an output that another argument also names as "<entry point>: dst[2] is also dst[0]".  h2_lane_destroy of the lane
  * that shared it leaves it alive; h2_shutdown frees every shared polynomial.  n == 0 does nothing; fails before h2_init. */
 int h2_poly_share(const uint64_t *polys, size_t n);
 int h2_poly_upload(uint64_t poly, const void *src, size_t len, int repr);

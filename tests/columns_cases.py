@@ -124,10 +124,9 @@ class ColumnsFake(fake_engine.FakeLib):
         if count == 0:
             return 0
         d, s = [int(dst[i]) for i in range(count)], [int(src[i]) for i in range(count)]
-        if len(set(d)) != count:
-            return self._fail(f"{who}: a dst handle appears twice")
-        if any(s[j] == h for i, h in enumerate(d) for j in range(count) if j != i):
-            return self._fail(f"{who}: a dst handle is another column's source")
+        c = fake_engine.clash(fake_engine.args("dst", d, True) + fake_engine.args("src", s, False), in_place=("dst", "src"))
+        if c:
+            return self._fail(f"{who}: {c}")
         f = self.polys[s[0]][0]
         in_log, log_n = fake_engine._v(in_log), fake_engine._v(log_n)
         rd = fake_engine._rd
@@ -152,10 +151,12 @@ class ColumnsFake(fake_engine.FakeLib):
         if count == 0 or rows == 0:
             return 0
         hs = [int(polys[i]) for i in range(count)]
-        if len(set(hs)) != count:
-            return self._fail("h2_poly_set_rows: a polynomial appears twice")
-        if any(start + rows > self.polys[h][1].shape[0] for h in hs):
-            return self._fail("h2_poly_set_rows: rows [start, start + rows) exceed the polynomial's length")
+        short = [i for i, h in enumerate(hs) if start + rows > self.polys[h][1].shape[0]]
+        if short:
+            return self._fail(f"h2_poly_set_rows: polys[{short[0]}]: a polynomial holds fewer than start + rows elements")
+        c = fake_engine.clash(fake_engine.args("polys", hs, True))
+        if c:
+            return self._fail(f"h2_poly_set_rows: {c}")
         vals = fake_engine._rd(values, 32 * count * rows).reshape(count, rows, 32)
         for i, h in enumerate(hs):
             self.polys[h][1][start:start + rows] = vals[i]

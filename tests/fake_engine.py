@@ -32,6 +32,33 @@ def _v(x) -> int:
     return int(x.value) if hasattr(x, "value") else int(x)
 
 
+def args(name: str, handles, out: bool) -> list:
+    """The elements of one handle array as clash() takes them."""
+    return [(f"{name}[{i}]", int(h), out) for i, h in enumerate(handles)]
+
+
+def clash(looked_up, in_place=None):
+    """The library's aliasing rule (PolyArgs::distinct, capi_core.cu) on (label, handle, is_output) in lookup order: the
+    first argument that clashes with an earlier one, as "<a> is also <b>" with the output first, or None.  in_place:
+    the (output, input) array names whose elements of one index may be the same polynomial."""
+    paired = lambda o, x: in_place is not None and o[0] == in_place[0] + x[0][len(in_place[1]):] and x[0].startswith(in_place[1] + "[")
+    seen = {}
+    for a in looked_up:
+        out, ins = seen.setdefault(a[1], [None, []])
+        if a[2] and out:
+            return f"{a[0]} is also {out[0]}"
+        x = next((x for x in ins if not paired(a, x)), None) if a[2] else None
+        if x:
+            return f"{a[0]} is also {x[0]}"
+        if not a[2] and out and not paired(out, a):
+            return f"{out[0]} is also {a[0]}"
+        if a[2]:
+            seen[a[1]][0] = a
+        else:
+            ins.append(a)
+    return None
+
+
 def _jac_bytes(xy: np.ndarray) -> np.ndarray:
     out = np.zeros(96, dtype=np.uint8)
     if xy.any():
@@ -127,7 +154,7 @@ class FakeLib:
         self._log("h2_poly_scale_add")
         n = _v(n)
         if _v(src) and _v(src) == _v(dst):
-            return self._fail("h2_poly_scale_add: a dst handle is also an input")
+            return self._fail("h2_poly_scale_add: dst is also src")
         f, d = self.polys[_v(dst)]
         buf = np.ascontiguousarray(d[:n])
         sb = np.ascontiguousarray(self.polys[_v(src)][1][:n]) if _v(src) else None
@@ -211,9 +238,10 @@ class FakeLib:
         self._log("h2_poly_kate_division")
         n, batch = _v(n), _v(batch)
         pts = _rd(points, 32 * batch).reshape(-1, 32)
+        c = clash(args("dst", dst[:batch], True) + args("src", src[:batch], False))
+        if c:
+            return self._fail(f"h2_poly_kate_division: {c}")
         for i in range(batch):
-            if int(dst[i]) == int(src[i]):
-                return self._fail("h2_poly_kate_division: a quotient handle is also an input")
             f, a = self.polys[int(src[i])]
             q = cref.kate_division(f, a[:n], int.from_bytes(pts[i].tobytes(), "little"))
             d = self.polys[int(dst[i])][1]
@@ -273,11 +301,15 @@ class FakeLib:
                 return self._fail("h2_poly_eval_ast: operand stack out of range")
         if depth != 1:
             return self._fail("h2_poly_eval_ast: the program leaves more than one value")
-        if _v(out) in [int(polys[i]) for i in range(n_polys)]:
-            return self._fail("h2_poly_eval_ast: an output handle is also an input")
-        f = self.polys[_v(out)][0]
-        if self.polys[_v(out)][1].shape[0] < n or any(self.polys[int(polys[i])][1].shape[0] < n for i in range(n_polys)):
+        if self.polys[_v(out)][1].shape[0] < n:
             return self._fail("h2_poly_eval_ast: a polynomial holds fewer than 2^log_n elements")
+        short = [i for i in range(n_polys) if self.polys[int(polys[i])][1].shape[0] < n]
+        if short:
+            return self._fail(f"h2_poly_eval_ast: polys[{short[0]}]: a polynomial holds fewer than 2^log_n elements")
+        c = clash([("out", _v(out), True)] + args("polys", polys[:n_polys], False))
+        if c:
+            return self._fail(f"h2_poly_eval_ast: {c}")
+        f = self.polys[_v(out)][0]
         stack = np.ascontiguousarray(np.stack([self.polys[int(polys[i])][1][:n] for i in range(n_polys)])) if n_polys else np.zeros((1, n, 32), dtype=np.uint8)
         cs = _rd(consts, 32 * n_consts) if n_consts else np.zeros(32, dtype=np.uint8)
         res = np.zeros((n, 32), dtype=np.uint8)
@@ -298,7 +330,7 @@ class FakeLib:
     def h2_poly_running_product(self, dst, src, n, init, repr_):
         self._log("h2_poly_running_product")
         if _v(dst) == _v(src):
-            return self._fail("h2_poly_running_product: a dst handle is also an input")
+            return self._fail("h2_poly_running_product: dst is also src")
         f, a = self.polys[_v(src)]
         n = _v(n)
         res = np.zeros((n, 32), dtype=np.uint8)

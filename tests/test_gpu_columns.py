@@ -124,7 +124,7 @@ def _call(name, dst, src, k, ext_k=None):
 
 
 @pytest.mark.parametrize("on_lane", [False, True])
-def test_argument_errors_launch_nothing_and_change_nothing(on_lane):
+def test_argument_errors_name_the_column_launch_nothing_and_change_nothing(on_lane):
     lane = L.Lane().bind() if on_lane else None
     try:
         k, n = 8, 256
@@ -143,7 +143,7 @@ def test_argument_errors_launch_nothing_and_change_nothing(on_lane):
             ("l2c", [d[0], 987654321], [a[0], a[1]], k, None, "dst\\[1\\]: unknown polynomial handle"),
             ("l2c", [d[0], d[1]], [a[0], 987654321], k, None, "src\\[1\\]: unknown polynomial handle"),
             ("l2c", [d[0], shared[0]], [a[0], a[1]], k, None, "dst\\[1\\]: the polynomial is shared"),
-            ("l2c", [d[0], d[1]], [a[0], other], k, None, "different fields"),
+            ("l2c", [d[0], d[1]], [a[0], other], k, None, "src\\[1\\]: the polynomials live in different fields"),
             ("c2e", [d[0], d[1]], [a[0], d[1]], k, k + 2, "dst\\[1\\] == src\\[1\\]: in place needs equal input and output sizes"),
         ]
         for name, dst, src, kk, ext_k, msg in cases:
@@ -157,7 +157,8 @@ def test_argument_errors_launch_nothing_and_change_nothing(on_lane):
         assert L.launch_count() == before
         # set_rows: a repeated polynomial or rows past the end fail before the upload and change nothing
         vals = np.stack([cref.gen_scalars("fp", 3, 6)] * 2)
-        for polys, start, msg in (([a[0], a[0]], 10, "polys\\[1\\] is also polys\\[0\\]"), ([a[0], short], n // 2 - 3, "polys\\[1\\]: rows"),
+        for polys, start, msg in (([a[0], a[0]], 10, "polys\\[1\\] is also polys\\[0\\]"),
+                                  ([a[0], short], n // 2 - 3, "polys\\[1\\]: a polynomial holds fewer than start \\+ rows elements"),
                                   ([a[0], shared[0]], 0, "polys\\[1\\]: the polynomial is shared")):
             before = L.launch_count()
             with pytest.raises(L.H2Error, match=msg):

@@ -408,17 +408,21 @@ def _error_cases(eng):
 
     try:
         cases = [
-            (lambda: perm(zs=[z[0], 0xDEADBEEF]), "unknown"), (lambda: perm(zs=[z[0], gone_h]), "unknown"),
-            (lambda: perm(cs=[cols[0], cols[1], 0xDEADBEEF]), "unknown"), (lambda: perm(ss=[sig[0], sig[1], fq]), "different fields"),
-            (lambda: perm(zs=[z[0], fq]), "different fields"), (lambda: perm(cs=[cols[0], short, cols[2]]), "fewer than 2^k"),
-            (lambda: perm(zs=[z[0], short]), "fewer than 2^k"), (lambda: perm(zs=[z[0], sh]), "shared (read-only)"),
-            (lambda: perm(zs=[z[0], z[0]]), "appears twice"), (lambda: perm(zs=[z[0], cols[1]]), "also an input"),
-            (lambda: perm(zs=[sig[2], z[1]]), "also an input"), (lambda: perm(chunk=0), "chunk_len == 0"),
+            (lambda: perm(zs=[z[0], 0xDEADBEEF]), "z_out[1]: unknown polynomial handle"), (lambda: perm(zs=[z[0], gone_h]), "z_out[1]: unknown polynomial handle"),
+            (lambda: perm(cs=[cols[0], cols[1], 0xDEADBEEF]), "columns[2]: unknown polynomial handle"),
+            (lambda: perm(ss=[sig[0], sig[1], fq]), "sigmas[2]: the polynomials live in different fields"),
+            (lambda: perm(zs=[z[0], fq]), "z_out[1]: the polynomials live in different fields"),
+            (lambda: perm(cs=[cols[0], short, cols[2]]), "columns[1]: a polynomial holds fewer than 2^k elements"),
+            (lambda: perm(zs=[z[0], short]), "z_out[1]: a polynomial holds fewer than 2^k elements"),
+            (lambda: perm(zs=[z[0], sh]), "z_out[1]: the polynomial is shared (read-only)"),
+            (lambda: perm(zs=[z[0], z[0]]), "z_out[1] is also z_out[0]"), (lambda: perm(zs=[z[0], cols[1]]), "z_out[1] is also columns[1]"),
+            (lambda: perm(zs=[sig[2], z[1]]), "z_out[0] is also sigmas[2]"), (lambda: perm(chunk=0), "chunk_len == 0"),
             (lambda: perm(bf=n - 1), "blinding_factors + 1 >= n"), (lambda: perm(kk=31), "k > 30"),
-            (lambda: look(zs=[z[0], 0xDEADBEEF]), "unknown"), (lambda: look(zs=[z[0], sh]), "shared (read-only)"),
-            (lambda: look(zs=[z[0], z[0]]), "appears twice"), (lambda: look(zs=[z[0], cols[2]]), "also an input"),
-            (lambda: look(ins=[cols[0], cols[1], fq, sig[0], sig[1], sig[2], sh, cols[0]]), "different fields"),
-            (lambda: look(ins=[cols[0], cols[1], cols[2], short, sig[1], sig[2], sh, cols[0]]), "fewer than 2^k"),
+            (lambda: look(zs=[z[0], 0xDEADBEEF]), "z_out[1]: unknown polynomial handle"),
+            (lambda: look(zs=[z[0], sh]), "z_out[1]: the polynomial is shared (read-only)"),
+            (lambda: look(zs=[z[0], z[0]]), "z_out[1] is also z_out[0]"), (lambda: look(zs=[z[0], cols[2]]), "z_out[1] is also permuted_inputs[0]"),
+            (lambda: look(ins=[cols[0], cols[1], fq, sig[0], sig[1], sig[2], sh, cols[0]]), "permuted_inputs[0]: the polynomials live in different fields"),
+            (lambda: look(ins=[cols[0], cols[1], cols[2], short, sig[1], sig[2], sh, cols[0]]), "permuted_tables[0]: a polynomial holds fewer than 2^k elements"),
             (lambda: look(bf=n - 1), "blinding_factors + 1 >= n"), (lambda: look(kk=31), "k > 30"),
         ]
         for i, (call, msg) in enumerate(cases):
@@ -432,11 +436,11 @@ def _error_cases(eng):
         _close(cols, sig, z, [fq, short, sh])
 
 
-def test_errors_on_the_primary_context(eng):
+def test_errors_name_the_argument_on_the_primary_context(eng):
     _error_cases(eng)
 
 
-def test_errors_on_a_lane(eng):
+def test_errors_name_the_argument_on_a_lane(eng):
     def go():
         with eng.Lane():
             _error_cases(eng)

@@ -185,8 +185,9 @@ def _error_cases(eng):
             mp[where] = bad
             assert _sigma_call([a, b], k, mp, omega, delta) != 0 and "mapping entry" in _err()
             works()
-        cases = (([a, 0xDEADBEEF], "unknown"), ([a, gone_h], "unknown"), ([a, fq], "different fields"), ([short, a], "fewer than 2^k"),
-                 ([a, a], "appears twice"))
+        cases = (([a, 0xDEADBEEF], "dst[1]: unknown polynomial handle"), ([a, gone_h], "dst[1]: unknown polynomial handle"),
+                 ([a, fq], "dst[1]: the polynomials live in different fields"), ([short, a], "dst[0]: a polynomial holds fewer than 2^k elements"),
+                 ([a, a], "dst[1] is also dst[0]"))
         for polys, msg in cases:
             assert _sigma_call(polys, k, ident, omega, delta) != 0 and msg in _err(), (polys, _err())
             works()
@@ -199,11 +200,11 @@ def _error_cases(eng):
             p.close()
 
 
-def test_errors_on_the_primary_context(eng):
+def test_errors_name_the_argument_on_the_primary_context(eng):
     _error_cases(eng)
 
 
-def test_errors_on_a_lane(eng):
+def test_errors_name_the_argument_on_a_lane(eng):
     def go():
         with eng.Lane():
             _error_cases(eng)

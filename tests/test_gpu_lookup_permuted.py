@@ -166,12 +166,16 @@ def _error_cases(eng):
 
     try:
         cases = [
-            (lambda: call(o=[outs[0], 0xDEADBEEF, outs[2], outs[3]]), "unknown"), (lambda: call(o=[outs[0], outs[1], gone_h, outs[3]]), "unknown"),
-            (lambda: call(i=[ins[0], ins[1], 0xDEADBEEF, ins[3]]), "unknown"),
-            (lambda: call(i=[ins[0], fq, ins[2], ins[3]]), "different fields"), (lambda: call(o=[outs[0], outs[1], fq, outs[3]]), "different fields"),
-            (lambda: call(i=[ins[0], ins[1], short, ins[3]]), "fewer than 2^k"), (lambda: call(o=[outs[0], short, outs[2], outs[3]]), "fewer than 2^k"),
-            (lambda: call(o=[outs[0], outs[1], sh, outs[3]]), "shared (read-only)"),
-            (lambda: call(o=[outs[0], outs[1], outs[0], outs[3]]), "appears twice"), (lambda: call(o=[outs[0], ins[3], outs[2], outs[3]]), "also an input"),
+            (lambda: call(o=[outs[0], 0xDEADBEEF, outs[2], outs[3]]), "out_tables[0]: unknown polynomial handle"),
+            (lambda: call(o=[outs[0], outs[1], gone_h, outs[3]]), "out_inputs[1]: unknown polynomial handle"),
+            (lambda: call(i=[ins[0], ins[1], 0xDEADBEEF, ins[3]]), "inputs[1]: unknown polynomial handle"),
+            (lambda: call(i=[ins[0], fq, ins[2], ins[3]]), "tables[0]: the polynomials live in different fields"),
+            (lambda: call(o=[outs[0], outs[1], fq, outs[3]]), "out_inputs[1]: the polynomials live in different fields"),
+            (lambda: call(i=[ins[0], ins[1], short, ins[3]]), "inputs[1]: a polynomial holds fewer than 2^k elements"),
+            (lambda: call(o=[outs[0], short, outs[2], outs[3]]), "out_tables[0]: a polynomial holds fewer than 2^k elements"),
+            (lambda: call(o=[outs[0], outs[1], sh, outs[3]]), "out_inputs[1]: the polynomial is shared (read-only)"),
+            (lambda: call(o=[outs[0], outs[1], outs[0], outs[3]]), "out_inputs[1] is also out_inputs[0]"),
+            (lambda: call(o=[outs[0], ins[3], outs[2], outs[3]]), "out_tables[0] is also tables[1]"),
             (lambda: call(b=n - 1), "blinding_factors + 1 >= n"), (lambda: call(kk=31), "k > 30"),
             (lambda: call(count=65536), "more than 65535"),
             (lambda: call(i=[ins[0], ins[1], miss, ins[3]]), "lookup 1: an input value does not occur"),
@@ -188,11 +192,11 @@ def _error_cases(eng):
         _close(ins, outs, [fq, short, sh, miss])
 
 
-def test_errors_on_the_primary_context(eng):
+def test_errors_name_the_argument_on_the_primary_context(eng):
     _error_cases(eng)
 
 
-def test_errors_on_a_lane(eng):
+def test_errors_name_the_argument_on_a_lane(eng):
     def go():
         with eng.Lane():
             _error_cases(eng)

@@ -250,10 +250,12 @@ class KeygenFakeLib(fake_engine.FakeLib):
         if cols == 0:
             return 0
         hs = [int(dst[i]) for i in range(cols)]
-        if any(h not in self.polys for h in hs):
-            return self._fail("h2_poly_permutation_sigma: unknown polynomial handle")
-        if len(set(hs)) != cols:
-            return self._fail("h2_poly_permutation_sigma: a dst handle appears twice")
+        unknown = [i for i, h in enumerate(hs) if h not in self.polys]
+        if unknown:
+            return self._fail(f"h2_poly_permutation_sigma: dst[{unknown[0]}]: unknown polynomial handle")
+        c = fake_engine.clash(fake_engine.args("dst", hs, True))
+        if c:
+            return self._fail(f"h2_poly_permutation_sigma: {c}")
         field = self.polys[hs[0]][0]
         n = 1 << k
         if any(self.polys[h][0] != field or self.polys[h][1].shape[0] < n for h in hs):

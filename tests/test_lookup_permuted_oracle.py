@@ -148,8 +148,10 @@ class PermutedFake(fake_engine.FakeLib):
         n, rows = 1 << k, bf + 1
         outs = [int(out_inputs[b]) for b in range(count)] + [int(out_tables[b]) for b in range(count)]
         ins = [int(inputs[b]) for b in range(count)] + [int(tables[b]) for b in range(count)]
-        if len(set(outs)) != len(outs) or set(outs) & set(ins):
-            return self._fail("h2_poly_lookup_permuted: an output handle appears twice or is also an input")
+        c = fake_engine.clash(fake_engine.args("out_inputs", outs[:count], True) + fake_engine.args("out_tables", outs[count:], True) +
+                              fake_engine.args("inputs", ins[:count], False) + fake_engine.args("tables", ins[count:], False))
+        if c:
+            return self._fail(f"h2_poly_lookup_permuted: {c}")
         f = self.polys[ins[0]][0]
         col = lambda hs: np.ascontiguousarray(np.concatenate([self.polys[h][1][:n] for h in hs]))
         oa, ot = col(outs[:count]), col(outs[count:])
