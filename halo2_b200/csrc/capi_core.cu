@@ -174,10 +174,10 @@ int HostArgs::from_mont(int field, fe *d, size_t n, cudaStream_t s) const { retu
 int HostArgs::down(int field, void *h, const fe *d, size_t n, cudaStream_t s) const {
     if (mont()) return download_sync(h, d, n * sizeof(fe), s);
     Context &X = g_ctx;
-    if (scratch_acquire(s) || X.ntt_out.ensure(n * sizeof(fe))) return 1;
+    if (X.ntt_out.ensure(n * sizeof(fe))) return 1;
     CU(cudaMemcpyAsync(X.ntt_out.p, d, n * sizeof(fe), cudaMemcpyDeviceToDevice, s));
-    if (from_mont(field, X.ntt_out.as<fe>(), n, s) || download_sync(h, X.ntt_out.p, n * sizeof(fe), s)) return 1;
-    return scratch_release(s);
+    if (from_mont(field, X.ntt_out.as<fe>(), n, s)) return 1;
+    return download_sync(h, X.ntt_out.p, n * sizeof(fe), s);
 }
 // From any thread and any context: the caller holds no Context mutex.
 int shared_poly_free(uint64_t h) {
@@ -399,14 +399,15 @@ int require_ready() {
     CU(cudaSetDevice(g_ctx.device));
     return 0;
 }
-int scratch_acquire(cudaStream_t s) {
-    if (g_ctx.have_last) CU(cudaStreamWaitEvent(s, g_ctx.last_use, 0));
-    return 0;
+StreamSplice::StreamSplice(cudaStream_t s) : X(g_ctx), s(s) {
+    cudaError_t e = cudaEventRecord(X.ev_splice, X.stream);
+    if (e == cudaSuccess) e = cudaStreamWaitEvent(s, X.ev_splice, 0);
+    if (e != cudaSuccess) failed = fail(std::string("stream splice: ") + cudaGetErrorString(e));
 }
-int scratch_release(cudaStream_t s) {
-    CU(cudaEventRecord(g_ctx.last_use, s));
-    g_ctx.have_last = true;
-    return 0;
+// A failure here can only be a sticky device error, which every later CUDA call, and so the context's next call, reports.
+StreamSplice::~StreamSplice() {
+    cudaEventRecord(X.ev_splice, s);
+    cudaStreamWaitEvent(X.stream, X.ev_splice, 0);
 }
 
 extern "C" const char *h2_last_error(void) { return g_err.c_str(); }
@@ -423,7 +424,7 @@ static int ctx_create(Context &C, int device) {
     CU(cudaGetDeviceProperties(&prop, device));
     if (prop.major != 9 || prop.minor != 0) return fail("h2_init: this library is built for sm_90a (H100) only");
     CU(cudaStreamCreateWithFlags(&C.stream, cudaStreamNonBlocking));
-    CU(cudaEventCreateWithFlags(&C.last_use, cudaEventDisableTiming));
+    CU(cudaEventCreateWithFlags(&C.ev_splice, cudaEventDisableTiming));
     CU(cudaStreamCreateWithFlags(&C.copy_stream, cudaStreamNonBlocking));
     CU(cudaEventCreateWithFlags(&C.ev_scalars_up, cudaEventDisableTiming));
     for (int j = 0; j < H2_MAX_UPLOAD_CHUNKS; j++) {
@@ -468,7 +469,7 @@ static void ctx_destroy(Context &C) {
     cudaEventDestroy(C.ev_scalars_up);
     for (int j = 0; j < H2_MAX_UPLOAD_CHUNKS; j++) { cudaEventDestroy(C.ev_bases_up[j]); cudaEventDestroy(C.ev_scal_up[j]); }
     cudaStreamDestroy(C.copy_stream);
-    cudaEventDestroy(C.last_use);
+    cudaEventDestroy(C.ev_splice);
     cudaStreamDestroy(C.stream);
     C = Context();
 }
@@ -743,7 +744,6 @@ extern "C" int h2_test_field_op(int field, int op, const void *a, const void *b,
     if (require_ready()) return 1;
     Context &X = g_ctx;
     cudaStream_t s = X.stream;
-    if (scratch_acquire(s)) return 1;
     if (X.misc.ensure(3 * n * sizeof(fe) + 64)) return 1;
     fe *da = X.misc.as<fe>(), *db = da + n, *dout = db + n;
     CU(cudaMemcpyAsync(da, a, n * sizeof(fe), cudaMemcpyHostToDevice, s));
@@ -754,7 +754,6 @@ extern "C" int h2_test_field_op(int field, int op, const void *a, const void *b,
         }))
         return 1;
     CU(cudaMemcpyAsync(out, dout, n * sizeof(fe), cudaMemcpyDeviceToHost, s));
-    if (scratch_release(s)) return 1;
     CU(cudaStreamSynchronize(s));
     return 0;
 }
@@ -767,7 +766,6 @@ extern "C" int h2_test_curve_op(int curve, int op, const void *a_xy, const void 
     if (require_ready()) return 1;
     Context &X = g_ctx;
     cudaStream_t s = X.stream;
-    if (scratch_acquire(s)) return 1;
     if (X.misc.ensure(3 * n * sizeof(affine) + 64)) return 1;
     affine *da = X.misc.as<affine>(), *db = da + n, *dout = db + n;
     CU(cudaMemcpyAsync(da, a_xy, n * sizeof(affine), cudaMemcpyHostToDevice, s));
@@ -779,7 +777,6 @@ extern "C" int h2_test_curve_op(int curve, int op, const void *a_xy, const void 
         }))
         return 1;
     CU(cudaMemcpyAsync(out_xy, dout, n * sizeof(affine), cudaMemcpyDeviceToHost, s));
-    if (scratch_release(s)) return 1;
     CU(cudaStreamSynchronize(s));
     return 0;
 }
@@ -788,7 +785,6 @@ extern "C" int h2_bench_field_mul(int field, uint32_t threads_per_block, uint32_
     if (require_ready()) return 1;
     Context &X = g_ctx;
     cudaStream_t s = X.stream;
-    if (scratch_acquire(s)) return 1;
     size_t threads = (size_t)threads_per_block * blocks;
     if (X.misc.ensure(threads * 4 * sizeof(fe))) return 1;
     CU(cudaMemsetAsync(X.misc.p, 0x11, threads * 4 * sizeof(fe), s));
@@ -806,7 +802,7 @@ extern "C" int h2_bench_field_mul(int field, uint32_t threads_per_block, uint32_
     }
     CU(cudaEventElapsedTime(ms, e0, e1));
     cudaEventDestroy(e0); cudaEventDestroy(e1);
-    return scratch_release(s);
+    return 0;
 }
 
 // mode: 0 dependent mul chain, 1 two chains, 2 four chains, 3 xyzz_double, 4 xyzz_add, 5 xyzz_add_mixed;
@@ -816,7 +812,6 @@ extern "C" int h2_bench_latency(int mode, uint32_t iters, float *ms) {
     if (require_ready()) return 1;
     Context &X = g_ctx;
     cudaStream_t s = X.stream;
-    if (scratch_acquire(s)) return 1;
     if (X.misc.ensure(32 * 4 * sizeof(fe))) return 1;
     CU(cudaMemsetAsync(X.misc.p, 0x11, 32 * 4 * sizeof(fe), s));
     cudaEvent_t e0, e1;
@@ -829,7 +824,7 @@ extern "C" int h2_bench_latency(int mode, uint32_t iters, float *ms) {
     }
     CU(cudaEventElapsedTime(ms, e0, e1));
     cudaEventDestroy(e0); cudaEventDestroy(e1);
-    return scratch_release(s);
+    return 0;
 }
 
 // ------------------------------------------------------------------------------------------------

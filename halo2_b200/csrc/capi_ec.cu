@@ -30,7 +30,7 @@ static int ecfft_stages(xyzz *work, uint32_t log_n, const fe &omega_mont, const 
     return 0;
 }
 // mode 0: Jacobian in -> Jacobian out (h2_ec_fft); mode 1: affine in -> scaled, normalised affine out (h2_params_lagrange)
-// `in` == nullptr: the input is already in X.ec_io on the device (h2_params_new), scratch acquired by the caller
+// `in` == nullptr: the input is already in X.ec_io on the device (h2_params_new)
 template <class P, class PS>
 static int ecfft_host(int mode, const void *in, uint32_t log_n, const void *omega, const void *scale, const HostArgs &h, void *out) {
     Context &X = g_ctx;
@@ -39,7 +39,6 @@ static int ecfft_host(int mode, const void *in, uint32_t log_n, const void *omeg
     const int canon = h.canon();
     const size_t in_sz = mode == 0 ? sizeof(jacobian) : sizeof(affine);
     if (in) {
-        if (scratch_acquire(s)) return 1;
         if (X.ec_io.ensure(n * sizeof(jacobian))) return 1;
         if (upload_async(X.ec_io.p, in, n * in_sz, s)) return 1;
     }
@@ -68,7 +67,6 @@ static int ecfft_host(int mode, const void *in, uint32_t log_n, const void *omeg
                X.ec_out.as<affine>(), canon, n);
         CU(cudaMemcpyAsync(out, X.ec_out.p, n * sizeof(affine), cudaMemcpyDeviceToHost, s));
     }
-    if (scratch_release(s)) return 1;
     CU(cudaStreamSynchronize(s));
     return 0;
 }
@@ -91,7 +89,7 @@ extern "C" int h2_params_lagrange(int curve, const void *g_xy, uint32_t k, const
 // ------------------------------------------------------------------------------------------------
 // hash_to_curve (h2c.cuh) and Params::new (poly/commitment.rs:38-114)
 // ------------------------------------------------------------------------------------------------
-// n messages -> n affine points in X.ec_io (device, `repr`); scratch held by the caller.  msgs == nullptr: generator
+// n messages -> n affine points in X.ec_io (device, `repr`).  msgs == nullptr: generator
 // messages 0 || (first + i) as u32 LE
 template <class P>
 static int h2c_issue(const H2cConst &K, const void *msgs, size_t msg_len, uint64_t first, size_t n, const HostArgs &h, affine *d_out, cudaStream_t s) {
@@ -112,11 +110,9 @@ static int hash_to_curve_host(const char *domain_prefix, const void *msgs, size_
     cudaStream_t s = X.stream;
     const H2cConst K = make_h2c_const<P>(domain_prefix);
     if (!K.ok) return fail("h2_hash_to_curve: domain prefix too long (DST must be < 256 bytes)");
-    if (scratch_acquire(s)) return 1;
     if (X.ec_io.ensure(n * sizeof(affine))) return 1;
     if (h2c_issue<P>(K, msgs, msg_len, 0, n, h, X.ec_io.as<affine>(), s)) return 1;
     CU(cudaMemcpyAsync(out_xy, X.ec_io.p, n * sizeof(affine), cudaMemcpyDeviceToHost, s));
-    if (scratch_release(s)) return 1;
     CU(cudaStreamSynchronize(s));
     return 0;
 }
@@ -148,7 +144,6 @@ static int params_new_host(uint32_t k, const HostArgs &h, void *g_xy, void *gl_x
     fe minv = fe_one<PS>();
     for (uint32_t i = 0; i < k; i++) minv = fe_mul<PS>(minv, two_inv);
     if (h.canon()) { alpha_inv = fe_from_mont<PS>(alpha_inv); minv = fe_from_mont<PS>(minv); }   // ecfft_host reads them in repr
-    if (scratch_acquire(s)) return 1;
     if (X.ec_io.ensure((n + 2) * sizeof(jacobian))) return 1;
     affine *d_g = X.ec_io.as<affine>();
     static const uint8_t wu[2] = {1, 2};
@@ -157,7 +152,7 @@ static int params_new_host(uint32_t k, const HostArgs &h, void *g_xy, void *gl_x
     CU(cudaMemcpyAsync(g_xy, d_g, n * sizeof(affine), cudaMemcpyDeviceToHost, s));
     CU(cudaMemcpyAsync(w_xy, d_g + n, sizeof(affine), cudaMemcpyDeviceToHost, s));
     CU(cudaMemcpyAsync(u_xy, d_g + n + 1, sizeof(affine), cudaMemcpyDeviceToHost, s));
-    return ecfft_host<P, PS>(1, nullptr, k, alpha_inv.v, minv.v, h, gl_xy);   // releases the scratch, synchronises
+    return ecfft_host<P, PS>(1, nullptr, k, alpha_inv.v, minv.v, h, gl_xy);   // synchronises
 }
 extern "C" int h2_params_new(int curve, uint32_t k, int repr, void *out_g_xy, void *out_g_lagrange_xy, void *out_w_xy, void *out_u_xy) {
     CtxLock lk;
@@ -176,7 +171,6 @@ extern "C" int h2_batch_normalize(int curve, const void *points_xyz, size_t n, i
     Context &X = g_ctx;
     cudaStream_t s = X.stream;
     const int canon = h.canon();
-    if (scratch_acquire(s)) return 1;
     if (X.ec_io.ensure(n * sizeof(jacobian)) || X.ec_out.ensure(n * sizeof(affine))) return 1;
     CU(cudaMemcpyAsync(X.ec_io.p, points_xyz, n * sizeof(jacobian), cudaMemcpyHostToDevice, s));
     const uint32_t nb = blocks_for((n + H2_NORM_CHUNK - 1) / H2_NORM_CHUNK, 64);
@@ -186,7 +180,6 @@ extern "C" int h2_batch_normalize(int curve, const void *points_xyz, size_t n, i
         }))
         return 1;
     CU(cudaMemcpyAsync(out_xy, X.ec_out.p, n * sizeof(affine), cudaMemcpyDeviceToHost, s));
-    if (scratch_release(s)) return 1;
     CU(cudaStreamSynchronize(s));
     return 0;
 }
@@ -199,7 +192,6 @@ template <class P> static int points_codec(int decompress, const void *in, size_
     Context &X = g_ctx;
     cudaStream_t s = X.stream;
     const int mont = h.mont();
-    if (scratch_acquire(s)) return 1;
     if (X.ec_io.ensure(n * sizeof(affine)) || X.ec_out.ensure(n * sizeof(affine)) || X.misc.ensure(64)) return 1;
     uint32_t bad = 0xffffffffu;
     if (!decompress) {
@@ -214,7 +206,6 @@ template <class P> static int points_codec(int decompress, const void *in, size_
         CU(cudaMemcpyAsync(out, X.ec_out.p, n * sizeof(affine), cudaMemcpyDeviceToHost, s));
         CU(cudaMemcpyAsync(&bad, X.misc.p, 4, cudaMemcpyDeviceToHost, s));
     }
-    if (scratch_release(s)) return 1;
     CU(cudaStreamSynchronize(s));
     if (bad != 0xffffffffu) return fail("h2_points_decompress: invalid point encoding at index " + std::to_string(bad));
     return 0;

@@ -357,10 +357,10 @@ static int msm_dispatch(int curve, const fe *d_scalars, int scalars_mont, const 
 // Where the result of an msm_pass goes: `sets` Jacobian points to host memory, or (affine) as many affine points after
 // batch_normalize on the device, or one Jacobian point to `peer` on device `peer_dev` (a multi-GPU worker's partial sum).
 struct PassOut { void *host; bool affine = false; void *peer = nullptr; int peer_dev = -1; };
-// One MSM pass whose result leaves the device, with the scratch acquired by the caller: issued, normalised (to.affine), copied out,
-// the scratch released and the stream synchronised.  A pass over a window table runs fast first (MsmPlan::fast) unless fast passes
-// are off (h2_test_set_fast_fixed) or its bases arrive in chunks; if either device flag comes back set -- a bin overflowed or a
-// bucket was split -- its result is not valid and the pass runs again, in full.  `issued`, if given, runs after each issue with the
+// One MSM pass whose result leaves the device, on the context's stream: issued, normalised (to.affine), copied out and the
+// stream synchronised.  A pass over a window table runs fast first (MsmPlan::fast) unless fast passes are off
+// (h2_test_set_fast_fixed) or its bases arrive in chunks; if either device flag comes back set -- a bin overflowed or a bucket
+// was split -- its result is not valid and the pass runs again, in full.  `issued`, if given, runs after each issue with the
 // issue's return code and returns the code to go on with.
 static int msm_pass(int curve, const fe *d_scalars, int scalars_mont, const PassBases &B, size_t n, uint32_t sets, jacobian *d_result,
                     int canon, const PassOut &to, const BasesChunks *bc = nullptr, const std::function<int(int)> &issued = nullptr) {
@@ -390,10 +390,8 @@ static int msm_pass(int curve, const fe *d_scalars, int scalars_mont, const Pass
             if (!X.h_flags) CU(cudaHostAlloc((void **)&X.h_flags, 2 * sizeof(uint32_t), cudaHostAllocDefault));
             CU(cudaMemcpyAsync(X.h_flags, X.last_flags, 2 * sizeof(uint32_t), cudaMemcpyDeviceToHost, s));
         }
-        if (scratch_release(s)) return 1;
         CU(cudaStreamSynchronize(s));
         if (!fast || (X.h_flags[0] == 0 && X.h_flags[1] == 0)) break;
-        if (scratch_acquire(s)) return 1;
     }
     return 0;
 }
@@ -454,11 +452,10 @@ extern "C" int h2_msm_dev(int curve, const void *d_scalars, int scalars_repr, co
     const HostArgs h("h2_msm_dev", scalars_repr);
     if (require_ready() || h.check()) return 1;
     cudaStream_t s = (cudaStream_t)stream;
-    if (scratch_acquire(s)) return 1;
-    int rc = msm_dispatch(curve, (const fe *)d_scalars, h.mont(), PassBases{(const affine *)d_bases, window_bits}, n,
-                          (jacobian *)d_out_xyz, 0, s, nullptr, 1);
-    if (rc) return rc;
-    return scratch_release(s);
+    StreamSplice splice(s);   // the MSM scratch is the context's
+    if (splice.failed) return 1;
+    return msm_dispatch(curve, (const fe *)d_scalars, h.mont(), PassBases{(const affine *)d_bases, window_bits}, n, (jacobian *)d_out_xyz, 0, s,
+                        nullptr, 1);
 }
 
 // host_bases != nullptr: one-shot MSM -- the bases are uploaded (and converted) on the copy stream AFTER the
@@ -467,7 +464,6 @@ static int msm_host_common(int curve, const void *scalars, size_t n_scalars, con
                            size_t n_total, const HostArgs &h, const PassOut &to, const void *host_bases = nullptr) {
     Context &X = g_ctx;
     cudaStream_t s = X.stream;
-    if (scratch_acquire(s)) return 1;
     if (X.scal_in.ensure((n_total + 1) * sizeof(fe)) || X.result.ensure(sizeof(jacobian))) return 1;
     BasesChunks bc;
     std::atomic<uint32_t> recorded{0};
@@ -531,7 +527,6 @@ extern "C" int h2_msm(int curve, const void *scalars, const void *bases_xy, size
     if (require_ready() || check_curve(curve) || h.check({{scalars, "scalars", n != 0}, {bases_xy, "bases_xy", n != 0}, {out_xyz, "out_xyz"}})) return 1;
     Context &X = g_ctx;
     cudaStream_t s = X.stream;
-    if (scratch_acquire(s)) return 1;
     if (X.bases_in.ensure((n + 1) * sizeof(affine))) return 1;
     return msm_host_common(curve, scalars, n, nullptr, {X.bases_in.as<affine>()}, n, h, {out_xyz}, bases_xy);
 }
@@ -606,7 +601,6 @@ static int msm_registered_batch_impl(uint64_t handle, const void *scalars, size_
     if (total > b->n) return fail("h2_msm_registered_batch: more scalars than registered bases");
     Context &X = g_ctx;
     cudaStream_t s = X.stream;
-    if (scratch_acquire(s)) return 1;
     if (X.scal_in.ensure(batch * total * sizeof(fe)) || X.result.ensure(batch * sizeof(jacobian))) return 1;
     fe *d = X.scal_in.as<fe>();
     if (!extra_scalars) {
@@ -624,7 +618,6 @@ extern "C" int h2_point_sum(int curve, const void *points_xyz, size_t g, int rep
     if (require_ready() || h.check({{points_xyz, "points_xyz", g != 0}, {out_xyz, "out_xyz"}})) return 1;
     Context &X = g_ctx;
     cudaStream_t s = X.stream;
-    if (scratch_acquire(s)) return 1;
     if (X.misc.ensure((g + 1) * sizeof(jacobian)) || X.result.ensure(sizeof(jacobian))) return 1;
     if (g) CU(cudaMemcpyAsync(X.misc.p, points_xyz, g * sizeof(jacobian), cudaMemcpyHostToDevice, s));
     const int canon = h.canon();
@@ -634,7 +627,6 @@ extern "C" int h2_point_sum(int curve, const void *points_xyz, size_t g, int rep
         }))
         return 1;
     CU(cudaMemcpyAsync(out_xyz, X.result.p, sizeof(jacobian), cudaMemcpyDeviceToHost, s));
-    if (scratch_release(s)) return 1;
     CU(cudaStreamSynchronize(s));
     return 0;
 }
@@ -717,7 +709,6 @@ extern "C" int h2_msm_multi_gpu(int curve, const void *scalars, const void *base
         Context &X = g_ctx;
         size_t lo, hi;
         shard_range(n, g, G, &lo, &hi);
-        if (scratch_acquire(X.stream)) return 1;
         if (X.bases_in.ensure((hi - lo + 1) * sizeof(affine))) return 1;
         return msm_host_common(curve, (const fe *)scalars + lo, hi - lo, nullptr, {X.bases_in.as<affine>()}, hi - lo, h,
                                {nullptr, false, parts + g, prim}, (const affine *)bases_xy + lo);
@@ -874,9 +865,7 @@ static int ipa_begin_common(uint64_t bases_handle, uint32_t k, const void *p_pri
         else q = new IpaSession();
         q->bases = bases_handle; q->k = k; q->round = 0; q->folded = 1;
         cudaStream_t s = g_ctx.stream;
-        if (scratch_acquire(s)) { ipa_free(q); return 1; }   // pow2 is shared scratch
         if (ipa_begin_impl<PS>(q, p_prime, p_poly, x3, h, s)) { ipa_free(q); return 1; }
-        if (scratch_release(s)) { ipa_free(q); return 1; }
         cudaError_t e = cudaStreamSynchronize(s);   // p_prime may be pageable host memory
         if (e != cudaSuccess) { ipa_free(q); return fail(std::string("h2_ipa_begin: ") + cudaGetErrorString(e)); }
         uint64_t id = new_handle();
@@ -907,7 +896,6 @@ static int ipa_round_common(uint64_t session, const void *z, const void *l_rand,
     if (!q->folded) return fail("h2_ipa_round: h2_ipa_fold must follow each round");
     BaseSet *b = ref.b;
     cudaStream_t s = g_ctx.stream;
-    if (scratch_acquire(s)) return 1;
     const uint64_t n = 1ull << q->k;
     const IpaState S = ipa_state(q);
     // S.scal from p, b and s: a re-run of the pass reads them again, as no MSM kernel writes its scalars
@@ -1011,7 +999,6 @@ static int msm_registered_polys_impl(uint64_t bases_handle, const uint64_t *poly
         if (g.in(polys, batch, "polys", n, "n", q)) return 1;
         Context &X = g_ctx;
         cudaStream_t s = X.stream;
-        if (scratch_acquire(s)) return 1;
         if (X.scal_in.ensure(batch * total * sizeof(fe)) || X.result.ensure(batch * sizeof(jacobian)) || X.misc.ensure(batch * sizeof(fe) + 64)) return 1;
         fe *d = X.scal_in.as<fe>();
         if (extra_scalars && h.up(decltype(ps)::ID, X.misc.as<fe>(), extra_scalars, batch, s)) return 1;   // the blinds: Montgomery form like the resident data

@@ -136,15 +136,13 @@ static int ntt_host(int field, int mode, const void *a_in, uint32_t in_log_n, ui
                     const void *divisor, size_t out_len, void *out, const HostArgs &h) {
     Context &X = g_ctx;
     cudaStream_t s = X.stream;
-    if (scratch_acquire(s)) return 1;
     uint64_t n = 1ull << log_n, n_in = 1ull << in_log_n;
     if (out_len > n) out_len = n;
     if (X.ntt_io.ensure(n_in * sizeof(fe)) || X.ntt_out.ensure(n * sizeof(fe))) return 1;
     const NttScales sc = host_scales<P>(h, h.canon(), mode, zeta, divisor);
     if (upload_async(X.ntt_io.p, a_in, n_in * sizeof(fe), s)) return 1;
     if (ntt_run<P>(field, X.ntt_io.as<fe>(), in_log_n, X.ntt_out.as<fe>(), log_n, h.elem<P>(omega), sc, out_len, s)) return 1;
-    if (download_sync(out, X.ntt_out.p, out_len * sizeof(fe), s)) return 1;
-    return scratch_release(s);
+    return download_sync(out, X.ntt_out.p, out_len * sizeof(fe), s);
 }
 static int ntt_host_dispatch(int field, int mode, const void *a_in, uint32_t in_log_n, uint32_t log_n, const void *omega, const void *zeta,
                              const void *divisor, size_t out_len, void *out, const HostArgs &h, std::initializer_list<HostArgs::Need> needs) {
@@ -175,14 +173,13 @@ extern "C" int h2_ntt_dev(int field, const void *d_in, void *d_out, const void *
     const HostArgs h("h2_ntt_dev", omega_repr);
     if (require_ready() || h.check({{omega, "omega"}})) return 1;
     cudaStream_t s = (cudaStream_t)stream;
-    if (scratch_acquire(s)) return 1;
+    StreamSplice splice(s);   // the twiddle cache, pow2 and the NTT scratch are the context's
+    if (splice.failed) return 1;
     NttScales sc;   // Montgomery in, Montgomery out, no scaling
-    if (by_field(field, [&](auto p) {
-            using P = decltype(p);
-            return ntt_run<P>(field, (const fe *)d_in, log_n, (fe *)d_out, log_n, h.elem<P>(omega), sc, 1ull << log_n, s);
-        }))
-        return 1;
-    return scratch_release(s);
+    return by_field(field, [&](auto p) {
+        using P = decltype(p);
+        return ntt_run<P>(field, (const fe *)d_in, log_n, (fe *)d_out, log_n, h.elem<P>(omega), sc, 1ull << log_n, s);
+    });
 }
 // test / bench hook: 1 = the bulk-copy (TMA) persistent pass kernel where it applies, 0 = the classic kernel (default; ctx.cuh)
 extern "C" int h2_test_set_ntt_tma(int on) {
@@ -362,7 +359,6 @@ static int poly_transform(const std::vector<PolyBuf *> &dst, const std::vector<P
     Context &X = g_ctx;
     cudaStream_t s = X.stream;
     const size_t count = dst.size();
-    if (scratch_acquire(s)) return 1;
     const NttScales sc = host_scales<P>(h, false, mode, zeta, divisor);   // resident data: Montgomery in and out
     if (count == 1) {
         if (ntt_run<P>(P::ID, src[0]->buf.as<fe>(), in_log_n, dst[0]->buf.as<fe>(), log_n, h.elem<P>(omega), sc, out_len, s)) return 1;
@@ -374,7 +370,7 @@ static int poly_transform(const std::vector<PolyBuf *> &dst, const std::vector<P
             ntt_run<P>(P::ID, nullptr, in_log_n, nullptr, log_n, h.elem<P>(omega), sc, out_len, s, count, t.cols, t.cols + count))
             return 1;
     }
-    return scratch_release(s);       // asynchronous: later calls are ordered behind it on the stream
+    return 0;   // asynchronous: later calls are ordered behind it on the stream
 }
 static int poly_transform_dispatch(uint64_t dst, uint64_t src, int mode, uint32_t in_log_n, uint32_t log_n, const void *omega, const void *zeta,
                                    const void *divisor, size_t out_len, const HostArgs &h, std::initializer_list<HostArgs::Need> needs,
@@ -461,12 +457,10 @@ extern "C" int h2_poly_set_rows(const uint64_t *polys, size_t count, size_t star
     const size_t total = count * rows;
     cudaStream_t s = g_ctx.stream;
     ColTable t;
-    if (scratch_acquire(s) || col_table(ps, values, total * sizeof(fe), s, &t)) return 1;
-    if (by_field(ps[0]->field, [&](auto p) {
-            LAUNCH(set_rows_kernel<decltype(p)>, blocks_for(total, 256), 256, 0, s, t.cols, (const fe *)t.data, (uint64_t)start, (uint64_t)rows,
-                   (uint64_t)total, h.canon() ? 1 : 0);
-            return 0;
-        }))
-        return 1;
-    return scratch_release(s);
+    if (col_table(ps, values, total * sizeof(fe), s, &t)) return 1;
+    return by_field(ps[0]->field, [&](auto p) {
+        LAUNCH(set_rows_kernel<decltype(p)>, blocks_for(total, 256), 256, 0, s, t.cols, (const fe *)t.data, (uint64_t)start, (uint64_t)rows,
+               (uint64_t)total, h.canon() ? 1 : 0);
+        return 0;
+    });
 }

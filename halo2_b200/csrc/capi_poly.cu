@@ -26,7 +26,6 @@ static int polyops_run(int mode, const std::vector<PolyBuf *> &a, const std::vec
     if (mode == 1 && m.size() == 1) { off.push_back(0); m.push_back(1); }   // a length-1 inner product still needs its product level
     const size_t L = m.size() - 1;                               // levels above the polynomial itself
     const uint64_t lvl_total = off.back() + m.back() * batch + batch;
-    if (scratch_acquire(s)) return 1;
     if (X.po_lvl.ensure(lvl_total * sizeof(fe)) || X.po_q.ensure(lvl_total * sizeof(fe)) || X.po_pts.ensure((L + 2) * batch * sizeof(fe)) ||
         X.misc.ensure(batch * sizeof(fe) + 64))
         return 1;
@@ -53,13 +52,12 @@ static int polyops_run(int mode, const std::vector<PolyBuf *> &a, const std::vec
             LAUNCH(poly_eval_cta_kernel<P>, batch, H2_POLY_CTA, 0, s, d_a, (uint64_t)n, (const fe *)pts, res);
             if (h.from_mont(P::ID, res, batch, s)) return 1;
             CU(cudaMemcpyAsync(out, res, batch * sizeof(fe), cudaMemcpyDeviceToHost, s));
-            if (scratch_release(s)) return 1;
             CU(cudaStreamSynchronize(s));
             return 0;
         }
         LAUNCH(poly_kate_cta_kernel<P>, batch, H2_KATE_CTA, 0, s, d_a, (uint64_t)n, (const fe *)pts, d_c);
         for (uint32_t b = 0; b < batch; b++) CU(cudaMemsetAsync(c[b]->buf.as<fe>() + (n - 1), 0, sizeof(fe), s));
-        return scratch_release(s);
+        return 0;
     }
     // upward pass: level l + 1 from level l at the point x^(CHUNK^l)
     for (size_t l = 0; l < L; l++) {
@@ -80,7 +78,6 @@ static int polyops_run(int mode, const std::vector<PolyBuf *> &a, const std::vec
         }
         if (h.from_mont(P::ID, res, batch, s)) return 1;
         CU(cudaMemcpyAsync(out, res, batch * sizeof(fe), cudaMemcpyDeviceToHost, s));
-        if (scratch_release(s)) return 1;
         CU(cudaStreamSynchronize(s));
         return 0;
     }
@@ -95,7 +92,7 @@ static int polyops_run(int mode, const std::vector<PolyBuf *> &a, const std::vec
     // the quotient has n - 1 coefficients; slot n - 1 becomes the zero the reference pushes before committing n of them
     // (poly/multiopen/prover.rs: `kate_division(..); poly.push(ZERO)`)
     for (uint32_t b = 0; b < batch; b++) CU(cudaMemsetAsync(c[b]->buf.as<fe>() + (n - 1), 0, sizeof(fe), s));
-    return scratch_release(s);
+    return 0;
 }
 // h: checked by the caller
 static int polyops_dispatch(int mode, const uint64_t *ah, const uint64_t *ch, size_t batch, size_t n, const void *points, const HostArgs &h, void *out) {
@@ -122,7 +119,6 @@ static int ast_run(PolyBuf *out, const std::vector<PolyBuf *> &polys, uint32_t l
     Context &X = g_ctx;
     cudaStream_t s = X.stream;
     const uint64_t n = 1ull << log_n;
-    if (scratch_acquire(s)) return 1;
     if (X.ast_code.ensure(n_code * sizeof(AstInstr)) || X.ast_consts.ensure((n_consts + 1) * sizeof(fe))) return 1;
     std::vector<PolyBuf *> cols(polys);
     cols.push_back(nullptr);                                     // a program without operands still gets a table
@@ -138,7 +134,7 @@ static int ast_run(PolyBuf *out, const std::vector<PolyBuf *> &polys, uint32_t l
         A.lin_base = h.elem<P>(lin_base);
     }
     LAUNCH(ast_eval_kernel<P>, blocks_for(n, 128), 128, 0, s, A);
-    return scratch_release(s);
+    return 0;
 }
 extern "C" int h2_poly_eval_ast(uint64_t out, const uint64_t *polys, size_t n_polys, uint32_t log_n, const uint32_t *code, size_t n_code,
                                 const void *consts, size_t n_consts, const void *omega, const void *lin_base, int repr) {
@@ -180,14 +176,11 @@ extern "C" int h2_poly_batch_invert(uint64_t poly, size_t n) {
     if (!a) return 1;
     if (n == 0) return 0;
     cudaStream_t s = g_ctx.stream;
-    if (scratch_acquire(s)) return 1;
     const uint32_t nb = blocks_for((n + 15) / 16, 64);
-    if (by_field(a->field, [&](auto p) {
-            LAUNCH(poly_batch_invert_kernel<decltype(p)>, nb, 64, 0, s, a->buf.as<fe>(), (uint64_t)n);
-            return 0;
-        }))
-        return 1;
-    return scratch_release(s);
+    return by_field(a->field, [&](auto p) {
+        LAUNCH(poly_batch_invert_kernel<decltype(p)>, nb, 64, 0, s, a->buf.as<fe>(), (uint64_t)n);
+        return 0;
+    });
 }
 // dst[0] = init, dst[i] = dst[i - 1] * src[i - 1] for i < n: the running product of plonk/permutation/prover.rs:150-156
 template <class P> static int grand_product_run(PolyBuf *d, PolyBuf *a, size_t n, const void *init, const HostArgs &h) {
@@ -198,7 +191,6 @@ template <class P> static int grand_product_run(PolyBuf *d, PolyBuf *a, size_t n
     const size_t L = m.size() - 1;
     uint64_t total = 1;
     for (size_t l = 1; l <= L; l++) total += m[l];
-    if (scratch_acquire(s)) return 1;
     if (X.po_lvl.ensure(total * sizeof(fe)) || X.po_q.ensure(total * sizeof(fe))) return 1;
     fe *lvl = X.po_lvl.as<fe>(), *ex = X.po_q.as<fe>();
     const fe *src = a->buf.as<fe>();
@@ -210,7 +202,7 @@ template <class P> static int grand_product_run(PolyBuf *d, PolyBuf *a, size_t n
         LAUNCH(poly_product_down_kernel<P>, blocks_for(chunks, 128), 128, 0, s, l == 0 ? src : (const fe *)(lvl + off[l]), m[l],
                l == L ? (const fe *)nullptr : (const fe *)(ex + off[l + 1]), in0, l == 0 ? d->buf.as<fe>() : ex + off[l], chunks);
     }
-    return scratch_release(s);
+    return 0;
 }
 extern "C" int h2_poly_running_product(uint64_t dst, uint64_t src, size_t n, const void *init, int repr) {
     CtxLock lk;
@@ -234,16 +226,13 @@ extern "C" int h2_poly_divide_by_vanishing(uint64_t poly, uint32_t ext_k, const 
     if (t_len == 0 || (t_len & (t_len - 1)) || t_len > (1u << ext_k)) return fail("h2_poly_divide_by_vanishing: t_len must be a power of two <= 2^ext_k");
     Context &X = g_ctx;
     cudaStream_t s = X.stream;
-    if (scratch_acquire(s)) return 1;
     if (X.po_pts.ensure((size_t)t_len * sizeof(fe))) return 1;
     if (h.up(a->field, X.po_pts.as<fe>(), t_evals, t_len, s)) return 1;
     const uint64_t n = 1ull << ext_k;
-    if (by_field(a->field, [&](auto p) {
-            LAUNCH(poly_vanish_div_kernel<decltype(p)>, blocks_for(n, 256), 256, 0, s, a->buf.as<fe>(), n, (const fe *)X.po_pts.as<fe>(), t_len - 1);
-            return 0;
-        }))
-        return 1;
-    return scratch_release(s);
+    return by_field(a->field, [&](auto p) {
+        LAUNCH(poly_vanish_div_kernel<decltype(p)>, blocks_for(n, 256), 256, 0, s, a->buf.as<fe>(), n, (const fe *)X.po_pts.as<fe>(), t_len - 1);
+        return 0;
+    });
 }
 extern "C" int h2_poly_eval(const uint64_t *polys, size_t batch, size_t n, const void *points, int repr, void *out) {
     const HostArgs h("h2_poly_eval", repr);
@@ -312,7 +301,6 @@ static int lookup_permuted_run(const std::vector<PolyBuf *> &out_in, const std::
     const uint64_t w = u + 1, nblind = blinding ? (uint64_t)count * 2 * rows : 0;
     std::vector<PolyBuf *> cols(in);                             // LkCols: in, tab, out_in, out_tab
     for (auto *v : {&tab, &out_in, &out_tab}) cols.insert(cols.end(), v->begin(), v->end());
-    if (scratch_acquire(s)) return 1;
     if (X.lk_keys.ensure(count * N * sizeof(fe)) || X.lk_u32.ensure(((2 * w + u) * count + 4) * sizeof(uint32_t))) return 1;
     fe *keys = X.lk_keys.as<fe>();
     uint32_t *sc = X.lk_u32.as<uint32_t>(), *left = sc + 2 * w * count, *err = left + u * count;
@@ -336,7 +324,6 @@ static int lookup_permuted_run(const std::vector<PolyBuf *> &out_in, const std::
     LAUNCH(lk_fill_kernel<P>, dim3(blocks_for(u + (nblind ? rows : 0), 256), count), 256, 0, s, c, (const fe *)keys, N, u, rows, (const uint32_t *)sc, count,
            (const uint32_t *)left, (const uint32_t *)err);
     CU(cudaMemcpyAsync(bad, err, sizeof *bad, cudaMemcpyDeviceToHost, s));
-    if (scratch_release(s)) return 1;
     CU(cudaStreamSynchronize(s));
     return 0;
 }
@@ -390,13 +377,12 @@ extern "C" int h2_poly_lookup_permuted(const uint64_t *out_inputs, const uint64_
 template <class P> static int compute_s_run(PolyBuf *d, const void *u, uint32_t k, const void *init, int accumulate, const HostArgs &h) {
     Context &X = g_ctx;
     cudaStream_t s = X.stream;
-    if (scratch_acquire(s)) return 1;
     if (X.po_pts.ensure((size_t)k * sizeof(fe))) return 1;
     fe *du = X.po_pts.as<fe>();
     if (h.up(P::ID, du, u, k, s)) return 1;
     const uint64_t groups = 1ull << (k - (k < 2 ? k : 2));
     LAUNCH(verifier_compute_s_kernel<P>, blocks_for(groups, 128), 128, 0, s, d->buf.as<fe>(), (const fe *)du, k, h.elem<P>(init), accumulate);
-    return scratch_release(s);
+    return 0;
 }
 extern "C" int h2_poly_compute_s(uint64_t dst, const void *u, uint32_t k, const void *init, int accumulate, int repr) {
     CtxLock lk;
@@ -436,7 +422,7 @@ extern "C" int h2_poly_scale_add(uint64_t dst, const void *a, uint64_t src, cons
 // the circuit's size; every piece is ordered on the context's stream behind the kernel that read the previous one.
 #define H2_KEYGEN_CHUNK (1ull << 22)
 // The launches both entry points share: the power tables, then one sigma launch per (column, piece) of the mapping, then
-// the error word back.  sigma_tables is called after scratch_acquire; sigma_finish releases the scratch and synchronises.
+// the error word back.  sigma_finish synchronises.
 template <class P>
 static int sigma_tables(uint32_t k, uint64_t cols, const void *omega, const void *delta, const HostArgs &h, fe **tab, uint32_t **err) {
     Context &X = g_ctx;
@@ -458,7 +444,6 @@ static int sigma_finish(uint32_t *err, const char *who) {
     cudaStream_t s = g_ctx.stream;
     uint32_t h_err = 0;
     CU(cudaMemcpyAsync(&h_err, err, sizeof h_err, cudaMemcpyDeviceToHost, s));
-    if (scratch_release(s)) return 1;
     CU(cudaStreamSynchronize(s));
     if (h_err) return fail(std::string(who) + ": a mapping entry is outside the permutation's columns or the domain's rows");
     return 0;
@@ -472,7 +457,6 @@ static int permutation_sigma_run(const std::vector<PolyBuf *> &dst, uint32_t k, 
     const uint64_t piece = n < H2_KEYGEN_CHUNK ? n : H2_KEYGEN_CHUNK;
     fe *tab;
     uint32_t *err;
-    if (scratch_acquire(s)) return 1;
     if (X.kg_map.ensure(piece * sizeof(uint2)) || sigma_tables<P>(k, cols, omega, delta, h, &tab, &err)) return 1;
     uint2 *map = X.kg_map.as<uint2>();
     for (uint64_t i = 0; i < cols; i++)
@@ -592,10 +576,8 @@ static int permutation_sigma_copies_run(const std::vector<PolyBuf *> &dst, uint3
     cudaStream_t s = X.stream;
     const uint64_t n = 1ull << k, cols = dst.size();
     unsigned long long bad = ~0ull;
-    if (scratch_acquire(s)) return 1;
     if (assembly_run((uint32_t)cols, k, copies, m, &bad)) return 1;
     if (bad != ~0ull) {
-        if (scratch_release(s)) return 1;
         return fail("h2_poly_permutation_sigma_copies: copy " + std::to_string(bad >> 1) +
                     ((bad & 1) ? ": a row is outside the domain (Error::BoundsFailure)" : ": a column is outside the permutation (Error::ColumnNotInPermutation)"));
     }
@@ -645,7 +627,6 @@ static int product_run(bool perm, const std::vector<PolyBuf *> &z, const std::ve
     const uint64_t tlen = perm ? KeygenOps<P>::table_len(k, ncols) : 0, nblind = count * bf;
     std::vector<PolyBuf *> cols(z);
     cols.insert(cols.end(), ins.begin(), ins.end());
-    if (scratch_acquire(s)) return 1;
     if (X.gp_val.ensure(count * n * sizeof(fe)) || X.po_lvl.ensure(total * sizeof(fe)) || X.po_q.ensure(total * sizeof(fe)) ||
         X.gp_aux.ensure((tlen + count) * sizeof(fe)))
         return 1;
@@ -674,7 +655,7 @@ static int product_run(bool perm, const std::vector<PolyBuf *> &z, const std::ve
                l == 0 ? zp : (fe *const *)nullptr, chunks);
     }
     if (bf) LAUNCH(gp_blind_kernel<P>, blocks_for(nblind, 256), 256, 0, s, zp, n, bf, (const fe *)t.data, count);
-    return scratch_release(s);
+    return 0;
 }
 static int product_scalars(const char *who, uint32_t k, uint32_t bf) {
     if (k > 30) return fail(std::string(who) + ": k > 30");

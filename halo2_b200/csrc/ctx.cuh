@@ -116,12 +116,15 @@ struct Context {
     CtxMutex mu;                             // held for a whole call on this context (CtxLock)
     bool ready = false;
     int device = -1;
+    // Every call's work, in call order.  The context's device state (scratch, caches, tables, graphs, resident polynomials, IPA
+    // sessions) is touched only on this stream, on copy_stream under its events (msm_host_common), by a multi-GPU worker's peer
+    // copy into the primary's multi_parts (synchronised in msm_pass before the worker returns), or on a caller's stream inside a
+    // StreamSplice.  A new entry point that takes a caller's stream and touches context state must use the splice.
     cudaStream_t stream = nullptr;
     cudaStream_t copy_stream = nullptr;      // uploads that may overlap compute (bases of a one-shot MSM)
     cudaEvent_t ev_scalars_up = nullptr, ev_bases_up[H2_MAX_UPLOAD_CHUNKS] = {}, ev_scal_up[H2_MAX_UPLOAD_CHUNKS] = {};
     uint32_t chunk_min_log = 19;             // one-shot MSMs of >= 2^19 points upload their bases in chunks
-    cudaEvent_t last_use = nullptr;
-    bool have_last = false;
+    cudaEvent_t ev_splice = nullptr;         // StreamSplice
     uint32_t window_override = 0;
     const uint32_t *last_flags = nullptr;    // device flags of the most recent MSM (test hook; the fast fixed-base pass's validity check)
     uint32_t fast_on = 1;                    // fixed-base passes over resident tables first run WITHOUT the fallback kernels (exact sort: histogram, 3 scan
@@ -262,12 +265,24 @@ int upload_async(void *d_dst, const void *h_src, size_t bytes, cudaStream_t s);
 int download_sync(void *h_dst, const void *d_src, size_t bytes, cudaStream_t s);
 void h2_set_staging(int on);             // test / bench hook: 0 = always plain cudaMemcpyAsync
 int require_ready();
-int scratch_acquire(cudaStream_t s);     // make `s` wait for whatever last used the shared scratch
-int scratch_release(cudaStream_t s);
+// One call on a caller's stream `s` that uses the calling context's state (scratch, the twiddle cache, pow2) while its kernels
+// stay on `s`: on construction `s` waits for the work queued so far on the context's stream, and on destruction, whichever
+// way the call returns, the context's stream waits for what the call queued on `s`.  One event serves both waits, as a wait
+// takes the event's state when it is issued and the context's mutex keeps other calls from recording it in between.
+// `failed`: the entry wait could not be issued (the error is set), and the call returns without using `s`.
+struct StreamSplice {
+    explicit StreamSplice(cudaStream_t s);
+    ~StreamSplice();
+    StreamSplice(const StreamSplice &) = delete;
+    StreamSplice &operator=(const StreamSplice &) = delete;
+    Context &X;
+    cudaStream_t s;
+    int failed = 0;
+};
 static inline uint32_t blocks_for(uint64_t n, uint32_t bs) { return (uint32_t)((n + bs - 1) / bs); }
 
 // The host-side field elements and points of one entry point `who`, in the encoding `repr` (include/halo2_b200.h).
-// check() runs before the call acquires scratch, copies or launches anything:
+// check() runs before the call copies or launches anything:
 //   - repr is H2_REPR_CANONICAL or H2_REPR_MONTGOMERY, else "<who>: unknown repr";
 //   - every required host pointer is set, else "<who>: null <name>" (name as in the header); a Need whose `required` is
 //     false (an optional pointer, or an array of no elements) is not checked.
@@ -334,9 +349,9 @@ struct PolyArgs {
     PolyBuf *find(bool out, uint64_t h, const char *name, int64_t i, uint64_t off, uint64_t len, const char *len_name);
     int find(bool out, const uint64_t *h, size_t n, const char *name, uint64_t off, uint64_t len, const char *len_name, Polys &v);
 };
-// One upload of a kernel's column table into the context's table buffer (col_tab), on `s` after scratch_acquire: the device
+// One upload of a kernel's column table into the context's table buffer (col_tab), on `s`: the device
 // pointers of `cols` in the order the kernel reads them (a null PolyBuf gives a null pointer), then `bytes` host bytes from
-// `data` at the next 32-byte boundary.  The table is scratch: it holds until the call's scratch_release.
+// `data` at the next 32-byte boundary.  The table is scratch: it holds for the kernels the call queues on `s` after it.
 struct ColTable {
     fe *const *cols;                         // the pointers on the device
     fe *data;                                // the bytes on the device; nullptr without any

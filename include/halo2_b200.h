@@ -327,7 +327,9 @@ int h2_set_sort_mode(int exact_only);
 int h2_set_glv(int on);
 
 /* Device-resident MSM: d_scalars (n x 32 B, `scalars_repr`), d_bases (n x 64 B, Montgomery),
- * d_out_xyz (96 B, Montgomery).  window_bits 0 = automatic. */
+ * d_out_xyz (96 B, Montgomery).  window_bits 0 = automatic.  Asynchronous on `stream`: the MSM runs after the caller's
+ * earlier work on `stream` and after the calling context's earlier calls, and the context's later calls run after it.
+ * Other lanes are unaffected. */
 int h2_msm_dev(int curve, const void *d_scalars, int scalars_repr, const void *d_bases, size_t n,
                uint32_t window_bits, void *d_out_xyz, void *stream);
 
@@ -370,7 +372,9 @@ int h2_extended_to_coeff(int field, const void *a, uint32_t ext_k, const void *e
                          const void *ext_divisor, const void *zeta, size_t out_len, void *out, int repr);
 
 /* Device-resident NTT on Montgomery data; omega is a HOST pointer in `omega_repr`.
- * d_out may equal d_in.  mode: 0 = plain, see the host variants for the scaled forms. */
+ * d_out may equal d_in.  mode: 0 = plain, see the host variants for the scaled forms.  Asynchronous on `stream`: the
+ * transform runs after the caller's earlier work on `stream` and after the calling context's earlier calls, and the
+ * context's later calls run after it.  Other lanes are unaffected. */
 int h2_ntt_dev(int field, const void *d_in, void *d_out, const void *omega, int omega_repr, uint32_t log_n,
                void *stream);
 /* Drops cached twiddle tables (the next call rebuilds them: "cold" timing). */
