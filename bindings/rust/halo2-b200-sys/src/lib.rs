@@ -74,6 +74,9 @@ extern "C" {
     pub fn h2_poly_permutation_sigma_copies(dst: *const u64, cols: usize, k: u32, copies: *const u32, m: usize, omega: *const c_void,
                                             delta: *const c_void, repr: c_int) -> c_int;
     pub fn h2_poly_divide_by_vanishing(poly: u64, ext_k: u32, t_evals: *const c_void, t_len: u32, repr: c_int) -> c_int;
+    // h(X) divided, transformed back and split into `count` pieces of 2^k coefficients in one call (plonk/vanishing/prover.rs:84-100)
+    pub fn h2_poly_vanishing_quotient(pieces: *const u64, count: usize, src: u64, k: u32, ext_k: u32, ext_omega_inv: *const c_void,
+                                      ext_divisor: *const c_void, zeta: *const c_void, t_evals: *const c_void, t_len: u32, repr: c_int) -> c_int;
     pub fn h2_poly_eval(polys: *const u64, batch: usize, n: usize, points: *const c_void, repr: c_int, out: *mut c_void) -> c_int;
     pub fn h2_poly_inner_product(a: *const u64, b: *const u64, batch: usize, n: usize, repr: c_int, out: *mut c_void) -> c_int;
     pub fn h2_poly_kate_division(dst: *const u64, src: *const u64, batch: usize, n: usize, points: *const c_void, repr: c_int) -> c_int;

@@ -19,6 +19,7 @@ from .keygen import (Assembly, CopyConstraints, ProvingKey, build_permutation_po
 from .products import (permutation_commit, lookup_commit_product, permutation_product_resident, lookup_product_resident,  # noqa: F401
                        lookup_commit_permuted, lookup_permute_resident, Permuted)
 from .columns import instance_commit, advice_commit, InstanceSingle, AdviceSingle, InstanceTooLarge  # noqa: F401
+from .vanishing import vanishing_commit, vanishing_quotient_resident, Committed, Constructed, Evaluated  # noqa: F401
 from . import multiopen, opening  # noqa: F401
 
 __all__ = ["Ast", "AstLeaf", "Evaluator", "Assembly", "CopyConstraints", "ProvingKey", "build_permutation_polys", "keygen_vk", "keygen_pk",
@@ -29,4 +30,5 @@ __all__ = ["Ast", "AstLeaf", "Evaluator", "Assembly", "CopyConstraints", "Provin
            "kate_division_resident", "batch_invert_resident", "running_product_resident", "permute_expression_pair_resident",
            "share_resident", "permutation_commit", "lookup_commit_product", "permutation_product_resident", "lookup_product_resident",
            "lookup_commit_permuted", "lookup_permute_resident", "Permuted", "set_rows_resident", "instance_commit", "advice_commit",
-           "InstanceSingle", "AdviceSingle", "InstanceTooLarge"]
+           "InstanceSingle", "AdviceSingle", "InstanceTooLarge",
+           "vanishing_commit", "vanishing_quotient_resident", "Committed", "Constructed", "Evaluated"]

@@ -36,6 +36,10 @@ template <class P> static int get_twiddles(int field, const fe &omega_mont, uint
 struct NttScales {
     bool in_scale = false, out_scale = false;
     fe in_s[3], out_s[3];
+    const fe *in_table = nullptr;   // device table: the first pass multiplies element j by in_table[j & in_mask] (NTT_IN_TABLE)
+    uint32_t in_mask = 0;
+    bool pieces = false;            // the last pass writes output p to out_cols[p >> piece_log] (NTT_OUT_PIECES; one column)
+    uint32_t piece_log = 0;
 };
 
 // d_in: 2^in_log_n elements; d_out: min(out_len, 2^log_n) elements written.  d_out may alias d_in.
@@ -77,8 +81,9 @@ static int ntt_run(int field, const fe *d_in, uint32_t in_log_n, fe *d_out, uint
             if (i == passes - 1 && out_cols) A.out_cols = out_cols + c0;
             A.tw = tw; A.log_n = log_n; A.s0 = s0; A.sp = sp[i]; A.logc = logc[i];
             A.flags = 0;
-            if (i == 0) A.flags |= NTT_FIRST | (sc.in_scale ? NTT_IN_SCALE : 0u);
-            if (i == passes - 1) A.flags |= NTT_LAST | (sc.out_scale ? NTT_OUT_SCALE : 0u);
+            if (i == 0) A.flags |= NTT_FIRST | (sc.in_scale ? NTT_IN_SCALE : 0u) | (sc.in_table ? NTT_IN_TABLE : 0u);
+            if (i == passes - 1) A.flags |= NTT_LAST | (sc.out_scale ? NTT_OUT_SCALE : 0u) | (sc.pieces ? NTT_OUT_PIECES : 0u);
+            A.in_table = sc.in_table; A.in_mask = sc.in_mask; A.piece_log = sc.piece_log;
             A.in_log_n = in_log_n; A.out_len = out_len;
             for (int k = 0; k < 3; k++) { A.in_scale[k] = sc.in_s[k]; A.out_scale[k] = sc.out_s[k]; }
             uint32_t tiles = (uint32_t)(n >> (sp[i] + logc[i]));
@@ -462,5 +467,35 @@ extern "C" int h2_poly_set_rows(const uint64_t *polys, size_t count, size_t star
         LAUNCH(set_rows_kernel<decltype(p)>, blocks_for(total, 256), 256, 0, s, t.cols, (const fe *)t.data, (uint64_t)start, (uint64_t)rows,
                (uint64_t)total, h.canon() ? 1 : 0);
         return 0;
+    });
+}
+// The vanishing argument's quotient (plonk/vanishing/prover.rs:84-100, K24): pieces[i] = coefficients [i n, (i + 1) n) of
+// extended_to_coeff(divide_by_vanishing_poly(src)), in one transform.  The division rides on the first pass's loads
+// (NTT_IN_TABLE, t_evals after the column table in one upload), the ζ un-shift, 1 / 2^ext_k and the split on the last
+// pass's stores (NTT_OUT_PIECES); src is only read.
+extern "C" int h2_poly_vanishing_quotient(const uint64_t *pieces, size_t count, uint64_t src, uint32_t k, uint32_t ext_k,
+                                          const void *ext_omega_inv, const void *ext_divisor, const void *zeta, const void *t_evals,
+                                          uint32_t t_len, int repr) {
+    static const char *who = "h2_poly_vanishing_quotient";
+    CtxLock lk;
+    const HostArgs h(who, repr);
+    if (require_ready() || h.check({{ext_omega_inv, "ext_omega_inv"}, {ext_divisor, "ext_divisor"}, {zeta, "zeta"}, {t_evals, "t_evals"}}))
+        return 1;
+    if (const char *why = vanishing_quotient_sizes(k, ext_k, count, t_len)) return fail(std::string(who) + ": " + why);
+    if (!pieces) return fail(std::string(who) + ": null handle array");
+    PolyArgs g(who);
+    std::vector<PolyBuf *> d;
+    PolyBuf *a = nullptr;
+    if (g.out(pieces, count, "pieces", (size_t)1 << k, "2^k", d) || !(a = g.in(src, "src", (size_t)1 << ext_k, "2^ext_k")) || g.distinct())
+        return 1;
+    cudaStream_t s = g_ctx.stream;
+    ColTable t;
+    if (col_table(d, t_evals, (size_t)t_len * sizeof(fe), s, &t) || h.to_mont(a->field, t.data, t_len, s)) return 1;
+    return by_field(a->field, [&](auto p) {
+        using P = decltype(p);
+        NttScales sc = host_scales<P>(h, false, 3, zeta, ext_divisor);   // extended_to_coeff's: Montgomery in and out
+        sc.in_table = t.data; sc.in_mask = t_len - 1;
+        sc.pieces = true; sc.piece_log = k;
+        return ntt_run<P>(P::ID, a->buf.as<fe>(), ext_k, nullptr, ext_k, h.elem<P>(ext_omega_inv), sc, (uint64_t)count << k, s, 1, nullptr, t.cols);
     });
 }

@@ -22,12 +22,15 @@
 // multiply element j by in_scale[j mod 3] (distribute_powers_zeta, :357-373, and/or the
 // canonical->Montgomery factor); last pass can multiply output p by out_scale[p mod 3]
 // (ifft divisor :375-383, coset un-scale :303-325, and/or Montgomery->canonical).
+// The vanishing argument's quotient (K24) adds two more: the first pass can multiply element j by in_table[j & in_mask]
+// (divide_by_vanishing_poly, :329-348), and the last pass can scatter output p into pieces of 2^piece_log coefficients,
+// out_cols[p >> piece_log] + (p mod 2^piece_log) (h_poly.chunks_exact(n), plonk/vanishing/prover.rs:95-100).
 #pragma once
 #include "field.cuh"
 
 namespace h2 {
 
-enum : uint32_t { NTT_FIRST = 1u, NTT_LAST = 2u, NTT_IN_SCALE = 4u, NTT_OUT_SCALE = 8u };
+enum : uint32_t { NTT_FIRST = 1u, NTT_LAST = 2u, NTT_IN_SCALE = 4u, NTT_OUT_SCALE = 8u, NTT_IN_TABLE = 16u, NTT_OUT_PIECES = 32u };
 
 struct NttPassArgs {
     const fe *in;
@@ -47,6 +50,10 @@ struct NttPassArgs {
     const fe *const *in_cols = nullptr;
     fe *const *out_cols = nullptr;
     uint64_t in_stride = 0, out_stride = 0;
+    // NTT_IN_TABLE (first pass): element j is multiplied by in_table[j & in_mask] as it is loaded.  NTT_OUT_PIECES (last pass,
+    // one column): output p goes to out_cols[p >> piece_log] + (p & (2^piece_log - 1)); out_len drops the tail as usual.
+    const fe *in_table = nullptr;
+    uint32_t in_mask = 0, piece_log = 0;
 };
 H2_HD const fe *ntt_col_in(const NttPassArgs &A, uint32_t c) { return A.in_cols ? A.in_cols[c] : A.in + c * A.in_stride; }
 H2_HD fe *ntt_col_out(const NttPassArgs &A, uint32_t c) { return A.out_cols ? A.out_cols[c] : A.out + c * A.out_stride; }
@@ -114,6 +121,7 @@ template <class P> struct NttPass {
                 x = fe_zero();
             } else {
                 x = fe_load(in + j);
+                if ((A.flags & NTT_FIRST) && (A.flags & NTT_IN_TABLE)) x = fe_mul<P>(x, fe_load(A.in_table + (j & A.in_mask)));
                 if ((A.flags & NTT_FIRST) && (A.flags & NTT_IN_SCALE)) x = fe_mul<P>(x, A.in_scale[j % 3]);
             }
             sm_store(sm, plane, r * stride + col, x);
@@ -239,7 +247,8 @@ template <class P> struct NttPass {
                 uint64_t p = ((uint64_t)bitrev32(r, A.sp) << A.s0) | p_low_of(A, tile, col);
                 if (p >= A.out_len) continue;
                 if (A.flags & NTT_OUT_SCALE) x = fe_mul<P>(x, A.out_scale[p % 3]);
-                fe_store(out + p, x);
+                if (A.flags & NTT_OUT_PIECES) fe_store(A.out_cols[p >> A.piece_log] + (p & ((1ull << A.piece_log) - 1)), x);
+                else fe_store(out + p, x);
             } else {
                 fe_store(out + elem_j(A, tile, r, col), x);
             }
@@ -363,6 +372,7 @@ template <class P> struct NttDense {
     static H2_HD bool supported(const NttPassArgs &A) {
         if ((A.flags & NTT_LAST) && (A.out_len & ((1ull << A.logc) - 1))) return false;      // whole rows only on the way out
         if ((A.flags & NTT_FIRST) && (A.flags & NTT_LAST)) return false;                      // single-pass transforms: classic kernel
+        if (A.flags & (NTT_IN_TABLE | NTT_OUT_PIECES)) return false;                          // the vanishing quotient's fusions: classic kernel
         return true;
     }
 };
@@ -517,6 +527,15 @@ inline uint64_t ntt_group(uint32_t log_n, int passes, uint64_t count) {
     if (g < 1) g = 1;
     if (g > 65535) g = 65535;
     return g < count ? g : count;
+}
+// The size arguments of h2_poly_vanishing_quotient (K24): `count` pieces of 2^k coefficients out of an extended domain of
+// 2^ext_k points, t_len inverses of t(X) = X^n - 1 repeated over it.  The reason they are rejected, or nullptr.
+inline const char *vanishing_quotient_sizes(uint32_t k, uint32_t ext_k, uint64_t count, uint32_t t_len) {
+    if (ext_k > 30) return "ext_k > 30";
+    if (ext_k < k) return "ext_k < k";
+    if (count == 0 || count > (1ull << (ext_k - k))) return "count must be at least 1 and count * 2^k at most 2^ext_k";
+    if (t_len == 0 || (t_len & (t_len - 1)) || t_len > (1u << ext_k)) return "t_len must be a power of two <= 2^ext_k";
+    return nullptr;
 }
 
 }  // namespace h2

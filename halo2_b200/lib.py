@@ -23,7 +23,7 @@ BASE_FIELD = {"pallas": "fp", "vesta": "fq"}
 SYMBOLS = [
     "h2_init", "h2_shutdown", "h2_last_error", "h2_device_count", "h2_abi_version", "h2_msm", "h2_bases_register", "h2_bases_register_ex",
     "h2_bases_release", "h2_msm_registered", "h2_msm_registered_batch", "h2_msm_registered_batch_affine", "h2_ipa_begin", "h2_ipa_round", "h2_ipa_fold", "h2_ipa_finish", "h2_poly_alloc", "h2_poly_free", "h2_poly_share", "h2_poly_upload", "h2_poly_download", "h2_poly_lagrange_to_coeff",
-    "h2_poly_coeff_to_extended", "h2_poly_extended_to_coeff", "h2_msm_registered_polys", "h2_msm_registered_polys_affine", "h2_ipa_begin_poly", "h2_ipa_round_affine", "h2_poly_add_at", "h2_poly_copy", "h2_poly_eval", "h2_poly_inner_product", "h2_poly_kate_division", "h2_poly_divide_by_vanishing", "h2_poly_eval_ast", "h2_poly_batch_invert", "h2_poly_lookup_permute", "h2_poly_running_product", "h2_poly_compute_s", "h2_poly_scale_add", "h2_poly_permutation_sigma", "h2_poly_permutation_sigma_copies", "h2_poly_permutation_product", "h2_poly_lookup_product", "h2_poly_lookup_permuted", "h2_poly_lagrange_to_coeff_batch", "h2_poly_coeff_to_extended_batch", "h2_poly_set_rows", "h2_set_window_bits", "h2_set_glv", "h2_set_sort_mode", "h2_msm_dev", "h2_point_sum", "h2_point_sum_dev", "h2_multi_init", "h2_multi_count", "h2_msm_multi_gpu", "h2_multi_bases_register", "h2_multi_bases_release", "h2_msm_multi_registered", "h2_test_set_staging", "h2_test_set_copy_threads", "h2_test_set_batched_affine", "h2_test_set_ntt_tma", "h2_ntt",
+    "h2_poly_coeff_to_extended", "h2_poly_extended_to_coeff", "h2_msm_registered_polys", "h2_msm_registered_polys_affine", "h2_ipa_begin_poly", "h2_ipa_round_affine", "h2_poly_add_at", "h2_poly_copy", "h2_poly_eval", "h2_poly_inner_product", "h2_poly_kate_division", "h2_poly_divide_by_vanishing", "h2_poly_eval_ast", "h2_poly_batch_invert", "h2_poly_lookup_permute", "h2_poly_running_product", "h2_poly_compute_s", "h2_poly_scale_add", "h2_poly_permutation_sigma", "h2_poly_permutation_sigma_copies", "h2_poly_permutation_product", "h2_poly_lookup_product", "h2_poly_lookup_permuted", "h2_poly_lagrange_to_coeff_batch", "h2_poly_coeff_to_extended_batch", "h2_poly_set_rows", "h2_poly_vanishing_quotient", "h2_set_window_bits", "h2_set_glv", "h2_set_sort_mode", "h2_msm_dev", "h2_point_sum", "h2_point_sum_dev", "h2_multi_init", "h2_multi_count", "h2_msm_multi_gpu", "h2_multi_bases_register", "h2_multi_bases_release", "h2_msm_multi_registered", "h2_test_set_staging", "h2_test_set_copy_threads", "h2_test_set_batched_affine", "h2_test_set_ntt_tma", "h2_ntt",
     "h2_intt_scaled", "h2_coeff_to_extended", "h2_extended_to_coeff", "h2_ntt_dev", "h2_ntt_clear_cache",
     "h2_ec_fft", "h2_batch_normalize", "h2_params_lagrange", "h2_hash_to_curve", "h2_params_new", "h2_points_compress", "h2_points_decompress",
     "h2_dev_gen_points", "h2_dev_convert", "h2_test_last_msm_flags", "h2_test_last_msm_plan", "h2_test_set_chunk_threshold", "h2_test_set_chunk_cuts", "h2_test_set_graphs", "h2_test_set_poly_cta", "h2_test_set_fast_fixed", "h2_test_set_ecfft_quad", "h2_test_set_accum_ways", "h2_test_field_op", "h2_test_curve_op", "h2_bench_field_mul", "h2_bench_latency",

@@ -250,6 +250,16 @@ int h2_poly_lookup_permuted(const uint64_t *out_inputs, const uint64_t *out_tabl
 /* EvaluationDomain::divide_by_vanishing_poly (poly/domain.rs:329-348) in place on a resident extended-domain polynomial:
  * h[i] *= t_evals[i mod t_len]; t_evals = the domain's t_evaluations (domain.rs:86-128), t_len = 2^(ext_k - k).  Asynchronous. */
 int h2_poly_divide_by_vanishing(uint64_t poly, uint32_t ext_k, const void *t_evals, uint32_t t_len, int repr);
+/* The vanishing argument's quotient h(X) in pieces (plonk/vanishing/prover.rs:84-100): pieces[i] <- coefficients
+ * [i 2^k, (i + 1) 2^k) of extended_to_coeff(divide_by_vanishing_poly(src)), i < count, in one transform of 2^ext_k points.
+ * The division by t(X) = X^n - 1 is fused into the first NTT pass, the zeta un-shift, the 1 / 2^ext_k scaling and the split
+ * into the last; the bytes equal h2_poly_divide_by_vanishing + h2_poly_extended_to_coeff + count h2_poly_copy calls.  src
+ * (2^ext_k extended-domain evaluations) is only read and may be shared; the pieces must be the calling context's own, hold
+ * 2^k elements each, be pairwise distinct and not src.  Requires k <= ext_k <= 30, 1 <= count <= 2^(ext_k - k) and t_len a
+ * power of two <= 2^ext_k (t_evals as for h2_poly_divide_by_vanishing).  Every check runs before anything is launched, a
+ * failed call changes nothing, and messages name the argument and index ("pieces[2]").  Asynchronous. */
+int h2_poly_vanishing_quotient(const uint64_t *pieces, size_t count, uint64_t src, uint32_t k, uint32_t ext_k, const void *ext_omega_inv,
+                               const void *ext_divisor, const void *zeta, const void *t_evals, uint32_t t_len, int repr);
 /* compute_inner_product (arithmetic.rs:308-319): out[i] = sum_j a[i][j] * b[i][j]. */
 int h2_poly_inner_product(const uint64_t *a, const uint64_t *b, size_t batch, size_t n, int repr, void *out);
 /* kate_division (arithmetic.rs:322-341): dst[i] <- the n - 1 coefficients of (src[i] - src[i](points[i])) / (X - points[i]);
