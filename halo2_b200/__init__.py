@@ -20,6 +20,8 @@ from .products import (permutation_commit, lookup_commit_product, permutation_pr
                        lookup_commit_permuted, lookup_permute_resident, Permuted)
 from .columns import instance_commit, advice_commit, InstanceSingle, AdviceSingle, InstanceTooLarge  # noqa: F401
 from .vanishing import vanishing_commit, vanishing_quotient_resident, Committed, Constructed, Evaluated  # noqa: F401
+from .arguments import (PermutationCommitted, PermutationConstructed, PermutationEvaluated, permutation_key_evaluate,  # noqa: F401
+                        permutation_key_open, LookupCommitted, LookupConstructed, LookupEvaluated, evaluate_columns, open_columns)
 from . import multiopen, opening  # noqa: F401
 
 __all__ = ["Ast", "AstLeaf", "Evaluator", "Assembly", "CopyConstraints", "ProvingKey", "build_permutation_polys", "keygen_vk", "keygen_pk",
@@ -31,4 +33,6 @@ __all__ = ["Ast", "AstLeaf", "Evaluator", "Assembly", "CopyConstraints", "Provin
            "share_resident", "permutation_commit", "lookup_commit_product", "permutation_product_resident", "lookup_product_resident",
            "lookup_commit_permuted", "lookup_permute_resident", "Permuted", "set_rows_resident", "instance_commit", "advice_commit",
            "InstanceSingle", "AdviceSingle", "InstanceTooLarge",
-           "vanishing_commit", "vanishing_quotient_resident", "Committed", "Constructed", "Evaluated"]
+           "vanishing_commit", "vanishing_quotient_resident", "Committed", "Constructed", "Evaluated",
+           "PermutationCommitted", "PermutationConstructed", "PermutationEvaluated", "permutation_key_evaluate", "permutation_key_open",
+           "LookupCommitted", "LookupConstructed", "LookupEvaluated", "evaluate_columns", "open_columns"]
