@@ -5,21 +5,14 @@ reference's write order, the opens, and multiopen.create_proof.  Also:
 
 - a proving key built from Lagrange columns with the same transforms create_proof_engine uses;
 - a circuit whose lookup is not linear in the columns (a selector-gated input and table over two rows) with a pinned key,
-  so that compressing on the coset and extending the compressed Lagrange column give different polynomials;
-- the ABI stand-in with every entry point the composition reaches.
+  so that compressing on the coset and extending the compressed Lagrange column give different polynomials.
 """
 from __future__ import annotations
-
-import contextlib
 
 import numpy as np
 
 from oracle import cref, pasta
-from tests import columns_cases as CC
-from tests import fake_engine
 from tests import plonk_prover as PP
-from tests import vanishing_cases as VC
-from tests.test_lookup_permuted_oracle import PermutedFake
 
 
 # ---- the proving key ---------------------------------------------------------------------------------------------------
@@ -290,62 +283,6 @@ def coset_compression_differs(h2, D):
                     for p in (co, interpolated, on_coset):
                         p.close()
     return seen, hook
-
-
-# ---- the ABI stand-in --------------------------------------------------------------------------------------------------
-class ArgumentsFake(CC.ColumnsFake, VC.VanishingFake, PermutedFake):
-    """The ABI stand-in with every entry point a package-composed proof reaches: the column-batched transforms and
-    h2_poly_set_rows, the vanishing quotient, the lookup permutation, and the two product columns (the device bodies on the
-    host emulation, emul_grandproduct.cpp)."""
-
-    def h2_poly_permutation_product(self, z_out, proofs, columns, sigmas, cols, chunk_len, k, beta, gamma, omega, delta, blinding, bf, repr_):
-        self._log("h2_poly_permutation_product")
-        v = fake_engine._v
-        proofs, cols, chunk_len, k, bf = v(proofs), v(cols), v(chunk_len), v(k), v(bf)
-        n, sets = 1 << k, -(-cols // chunk_len)
-        col = lambda h: self.polys[int(h)][1][:n]                  # noqa: E731
-        f = self.polys[int(sigmas[0])][0]
-        data = np.ascontiguousarray(np.concatenate([col(columns[i]) for i in range(proofs * cols)] + [col(sigmas[i]) for i in range(cols)]))
-        out = np.zeros((proofs * sets * n, 32), dtype=np.uint8)
-        rd = fake_engine._rd
-        bl = rd(blinding, 32 * proofs * sets * bf) if bf else None
-        self.emu.emu_permutation_product(cref.FIELD_ID[f], cref._p(data), proofs, cols, chunk_len, k, cref._p(rd(beta, 32)), cref._p(rd(gamma, 32)),
-                                         cref._p(rd(omega, 32)), cref._p(rd(delta, 32)), cref._p(bl) if bf else None, bf, cref._p(out))
-        for i in range(proofs * sets):
-            self.polys[int(z_out[i])][1][:n] = out[i * n:(i + 1) * n]
-        return 0
-
-    def h2_poly_lookup_product(self, z_out, count, inputs, tables, permuted_inputs, permuted_tables, k, beta, gamma, blinding, bf, repr_):
-        self._log("h2_poly_lookup_product")
-        v = fake_engine._v
-        count, k, bf = v(count), v(k), v(bf)
-        if count == 0:
-            return 0
-        n = 1 << k
-        col = lambda h: self.polys[int(h)][1][:n]                  # noqa: E731
-        f = self.polys[int(inputs[0])][0]
-        data = np.ascontiguousarray(np.concatenate([col(arr[b]) for b in range(count) for arr in (inputs, tables, permuted_inputs, permuted_tables)]))
-        out = np.zeros((count * n, 32), dtype=np.uint8)
-        rd = fake_engine._rd
-        bl = rd(blinding, 32 * count * bf) if bf else None
-        self.emu.emu_lookup_product(cref.FIELD_ID[f], cref._p(data), count, k, cref._p(rd(beta, 32)), cref._p(rd(gamma, 32)),
-                                    cref._p(bl) if bf else None, bf, cref._p(out))
-        for b in range(count):
-            self.polys[int(z_out[b])][1][:n] = out[b * n:(b + 1) * n]
-        return 0
-
-
-@contextlib.contextmanager
-def installed():
-    """halo2_b200.lib bound to an ArgumentsFake for the duration of the block (and back to whatever it was afterwards)."""
-    from halo2_b200 import lib as L
-    saved = (L._lib, L._inited_device)
-    fake = ArgumentsFake()
-    L._lib, L._inited_device = fake, 0
-    try:
-        yield fake
-    finally:
-        L._lib, L._inited_device = saved
 
 
 def params_for(h2, k: int, seed: int = 99):

@@ -3,8 +3,12 @@ a, b, c under one permutation, four fixed columns sm, sa, sb, sc, one gate a*sa 
 given k it fills 2^k - 6 rows -- every usable row -- with (2^(k-1) - 3) multiply / add pairs and two copy constraints per pair),
 rebuilt from its source as columns, permutation polynomials, a witness and a PINNED KEY TEXT in the format of
 `format!("{:#?}", vk.pinned())`, so that tests/plonk_prover.py and tests/plonk_verifier.py can prove and verify it.  Test
-infrastructure; pure integer bookkeeping (the commitments in the key text are supplied by the caller's keygen)."""
+infrastructure; the columns and the key text are pure integer bookkeeping (the commitments in the key text are supplied by the
+caller's keygen).  Below them: the circuit's copy constraints, and its seeded generators and columns as the tests set them up."""
 from __future__ import annotations
+
+from oracle import cref, pasta
+from tests import plonk_api_circuit as circ
 
 BLINDING_FACTORS = 5                                               # max(3, 1 query per advice column) + 2, plonk/circuit.rs:1435-1460
 DEGREE = 5                                                         # set_minimum_degree(5), benches/plonk.rs:183
@@ -87,3 +91,40 @@ def pinned_key_text(k: int, extended_k: int, base_modulus: int, scalar_modulus: 
         "fixed_commitments: [", pts(fixed_commitments), "],",
         "permutation: VerifyingKey {", "commitments: [", pts(permutation_commitments), "],", "},",
         "}"])
+
+
+def bench_copies(k: int):
+    """The copy constraints (benches/plonk.rs:226-241): copy(a0, a1) and copy(b1, c0) per multiply / add pair."""
+    for it in range((1 << (k - 1)) - 3):
+        rm, ra = 2 * it, 2 * it + 1
+        yield 0, rm, 0, ra
+        yield 1, ra, 2, rm
+
+
+def _bench_setup(k: int):
+    """(curve, modulus, (g, g_lagrange, w, u) of seeded generators, fixed, sigma, advice, copies) at k."""
+    c = pasta.VESTA
+    m = pasta.P_MOD
+    n = 1 << k
+    pts = cref.gen_points("vesta", 99, n + 2)
+    gens = (pts[:n], cref.params_lagrange("vesta", pts[:n], k, pasta.inv(pasta.omega_for_k("fp", k), m), pow(pasta.inv(2, m), k, m)),
+            pts[n:n + 1], pts[n + 1:n + 2])
+    omega = pasta.omega_for_k("fp", k)
+    fixed, sigma, adv = columns(k, m, omega, circ.DELTA, circ.A_SMALL * circ.ZETA % m)
+    asm_copies = list(bench_copies(k))
+    return c, m, gens, fixed, sigma, adv, asm_copies
+
+
+def _bench_params(eng, k: int):
+    """eng.Params over the seeded generators of _bench_setup, g_lagrange derived on the device."""
+    n = 1 << k
+    pts = cref.gen_points("vesta", 99, n + 2)
+    g, w, u = pts[:n], pts[n:n + 1], pts[n + 1:n + 2]
+    return eng.Params("vesta", k, g, eng.lagrange_generators("vesta", k, g), w, u=u)
+
+
+def _bench_assembly(eng, k: int):
+    asm = eng.Assembly(1 << k, 3)
+    for cp in bench_copies(k):
+        asm.copy(*cp)
+    return asm

@@ -3,13 +3,9 @@ composition (run up to its first challenge) and halo2_b200.instance_commit / adv
 the points in transcript order and the bytes of every column's values, coefficient form and coset."""
 from __future__ import annotations
 
-import contextlib
-import ctypes
-
 import numpy as np
 
 from oracle import cref, pasta
-from tests import fake_engine
 from tests import multiopen_cases as MC
 from tests import plonk_prover as PP
 from tests import prover_replay as R
@@ -112,65 +108,3 @@ def assert_same(want: dict, got: dict) -> None:
 
 def random_columns(field: str, seed: int, proofs: int, columns: int, n: int):
     return [[cref.gen_scalars(field, seed + 100 * p + c, n) for c in range(columns)] for p in range(proofs)]
-
-
-class ColumnsFake(fake_engine.FakeLib):
-    """The ABI stand-in with the column-batched transforms (the batched pass bodies on the host emulation,
-    emul_ntt_batch.cpp) and h2_poly_set_rows, with the library's checks that the host mirror can reach."""
-
-    def _transform_batch(self, who, mode, dst, src, count, in_log, log_n, omega, zeta, divisor):
-        self._log(who)
-        count = fake_engine._v(count)
-        if count == 0:
-            return 0
-        d, s = [int(dst[i]) for i in range(count)], [int(src[i]) for i in range(count)]
-        c = fake_engine.clash(fake_engine.args("dst", d, True) + fake_engine.args("src", s, False), in_place=("dst", "src"))
-        if c:
-            return self._fail(f"{who}: {c}")
-        f = self.polys[s[0]][0]
-        in_log, log_n = fake_engine._v(in_log), fake_engine._v(log_n)
-        rd = fake_engine._rd
-        stack = np.ascontiguousarray(np.stack([self.polys[h][1][:1 << in_log] for h in s]))
-        out = np.zeros((count, 1 << log_n, 32), dtype=np.uint8)
-        self.emu.emu_ntt_batch(cref.FIELD_ID[f], mode, cref._p(stack), ctypes.c_uint64(count), in_log, log_n, cref._p(rd(omega, 32)),
-                               cref._p(rd(zeta, 32)) if zeta is not None else None, cref._p(rd(divisor, 32)) if divisor is not None else None,
-                               cref._p(out), ctypes.c_uint64(0), 0, 64)
-        for i, h in enumerate(d):
-            self.polys[h][1][:1 << log_n] = out[i]
-        return 0
-
-    def h2_poly_lagrange_to_coeff_batch(self, dst, src, count, k, omega_inv, divisor, repr_):
-        return self._transform_batch("h2_poly_lagrange_to_coeff_batch", 1, dst, src, count, k, k, omega_inv, None, divisor)
-
-    def h2_poly_coeff_to_extended_batch(self, dst, src, count, k, ext_k, zeta, ext_omega, repr_):
-        return self._transform_batch("h2_poly_coeff_to_extended_batch", 2, dst, src, count, k, ext_k, ext_omega, zeta, None)
-
-    def h2_poly_set_rows(self, polys, count, start, rows, values, repr_):
-        self._log("h2_poly_set_rows")
-        count, start, rows = fake_engine._v(count), fake_engine._v(start), fake_engine._v(rows)
-        if count == 0 or rows == 0:
-            return 0
-        hs = [int(polys[i]) for i in range(count)]
-        short = [i for i, h in enumerate(hs) if start + rows > self.polys[h][1].shape[0]]
-        if short:
-            return self._fail(f"h2_poly_set_rows: polys[{short[0]}]: a polynomial holds fewer than start + rows elements")
-        c = fake_engine.clash(fake_engine.args("polys", hs, True))
-        if c:
-            return self._fail(f"h2_poly_set_rows: {c}")
-        vals = fake_engine._rd(values, 32 * count * rows).reshape(count, rows, 32)
-        for i, h in enumerate(hs):
-            self.polys[h][1][start:start + rows] = vals[i]
-        return 0
-
-
-@contextlib.contextmanager
-def installed():
-    """halo2_b200.lib bound to a ColumnsFake for the duration of the block (and back to whatever it was afterwards)."""
-    from halo2_b200 import lib as L
-    saved = (L._lib, L._inited_device)
-    fake = ColumnsFake()
-    L._lib, L._inited_device = fake, 0
-    try:
-        yield fake
-    finally:
-        L._lib, L._inited_device = saved

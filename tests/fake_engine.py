@@ -1,9 +1,10 @@
-"""TEST-ONLY stand-in for the CUDA library's ctypes handle, so that the HOST LOGIC of halo2_b200.verifier (the mirror of
-poly/commitment/msm.rs and verifier.rs: term merging, the order of calls, what goes to which entry point) runs in the
-`-m "not gpu"` suite.  It implements just the C-ABI entry points that mirror touches, with the ABI's own calling convention
-(ctypes values, pointers and out-parameters exactly as halo2_b200/lib.py passes them): the two verifier kernels run as the
-device bodies on the host emulation (tests/kernel_emul), the group operations through the oracle.  It is never importable from
-the package: a test installs it with `installed()` and removes it again; the product has no CPU fallback."""
+"""TEST-ONLY stand-in for the CUDA library's ctypes handle, so that the HOST LOGIC of the package (the verifier's mirror of
+poly/commitment/msm.rs and verifier.rs, the prover's phases, key generation: the order of calls, what goes to which entry
+point) runs in the `-m "not gpu"` suite.  It implements the C-ABI entry points that logic touches, with the ABI's own calling
+convention (ctypes values, pointers and out-parameters exactly as halo2_b200/lib.py passes them): the kernels run as the device
+bodies on the host emulation (tests/kernel_emul), the transforms and group operations through the oracle.  Each call that a
+test may count is logged in `calls`.  It is never importable from the package: a test installs it with `installed()` and
+removes it again; the product has no CPU fallback."""
 from __future__ import annotations
 
 import contextlib
@@ -16,6 +17,8 @@ from tests.kernel_emul import build as emul_build
 
 _CURVES = {0: "pallas", 1: "vesta"}
 _FIELDS = {0: "fp", 1: "fq"}
+KEYGEN_CHUNK = 1 << 22                                             # rows per launch in capi_poly.cu (H2_KEYGEN_CHUNK)
+NONE = 0xFFFFFFFF                                                  # emu_lookup_permuted's status when no lookup misses
 
 
 def _rd(p, nbytes: int) -> np.ndarray:
@@ -59,6 +62,16 @@ def clash(looked_up, in_place=None):
     return None
 
 
+def emu_assembly(emu, copies, cols: int, k: int):
+    """The copy-cycle bodies on the host emulation: (rc, mapping (cols, 2^k, 2), first-bad code, Borůvka rounds, |F|)."""
+    cp = np.ascontiguousarray(np.asarray(copies, dtype=np.uint32).reshape(-1, 4))
+    out = np.zeros((cols, 1 << k, 2), dtype=np.uint32)
+    bad, rounds, forest = ctypes.c_ulonglong(), ctypes.c_uint32(), ctypes.c_uint32()
+    rc = emu.emu_assembly(cp.ctypes.data_as(ctypes.c_void_p), ctypes.c_uint64(cp.shape[0]), ctypes.c_uint32(cols), ctypes.c_uint32(k),
+                          out.ctypes.data_as(ctypes.c_void_p), ctypes.byref(bad), ctypes.byref(rounds), ctypes.byref(forest))
+    return rc, out, bad.value, rounds.value, forest.value
+
+
 def _jac_bytes(xy: np.ndarray) -> np.ndarray:
     out = np.zeros(96, dtype=np.uint8)
     if xy.any():
@@ -70,9 +83,11 @@ def _jac_bytes(xy: np.ndarray) -> np.ndarray:
 class FakeLib:
     def __init__(self):
         self.emu = ctypes.CDLL(emul_build.build())
+        self.emu.emu_lookup_permuted.restype = ctypes.c_uint32
         self.polys, self.bases, self.next = {}, {}, 1
         self.err = b""
         self.calls = []
+        self.shared, self.share_calls, self.freed = set(), [], []       # h2_poly_share's handles, each call's, every h2_poly_free's
 
     def _fail(self, msg: str) -> int:
         self.err = msg.encode()
@@ -112,7 +127,18 @@ class FakeLib:
         return 0
 
     def h2_poly_free(self, h):
+        self.freed.append(_v(h))
+        self.shared.discard(_v(h))
         self.polys.pop(_v(h), None)
+        return 0
+
+    def h2_poly_share(self, polys, n):
+        """The library's all-or-nothing rule: the calling context's or already shared handles only."""
+        hs = [int(x) for x in polys[:_v(n)]]
+        self.share_calls.append(hs)
+        if any(h not in self.polys for h in hs):
+            return self._fail("h2_poly_share: unknown polynomial handle")
+        self.shared.update(hs)
         return 0
 
     def h2_poly_upload(self, h, src, length, repr_):
@@ -349,6 +375,187 @@ class FakeLib:
         if rc != 0:
             return self._fail("h2_poly_lookup_permute: an input value does not occur in the table")
         self.polys[_v(out_in)][1][:n], self.polys[_v(out_tab)][1][:n] = oa, ot
+        return 0
+
+    # ---- the prover phases' batched calls (the device bodies on the host emulation, after the library's checks the host
+    # mirror can reach) ----
+    def _transform_batch(self, who, mode, dst, src, count, in_log, log_n, omega, zeta, divisor):
+        self._log(who)
+        count = _v(count)
+        if count == 0:
+            return 0
+        d, s = [int(dst[i]) for i in range(count)], [int(src[i]) for i in range(count)]
+        c = clash(args("dst", d, True) + args("src", s, False), in_place=("dst", "src"))
+        if c:
+            return self._fail(f"{who}: {c}")
+        f = self.polys[s[0]][0]
+        in_log, log_n = _v(in_log), _v(log_n)
+        stack = np.ascontiguousarray(np.stack([self.polys[h][1][:1 << in_log] for h in s]))
+        out = np.zeros((count, 1 << log_n, 32), dtype=np.uint8)
+        self.emu.emu_ntt_batch(cref.FIELD_ID[f], mode, cref._p(stack), ctypes.c_uint64(count), in_log, log_n, cref._p(_rd(omega, 32)),
+                               cref._p(_rd(zeta, 32)) if zeta is not None else None, cref._p(_rd(divisor, 32)) if divisor is not None else None,
+                               cref._p(out), ctypes.c_uint64(0), 0, 64)
+        for i, h in enumerate(d):
+            self.polys[h][1][:1 << log_n] = out[i]
+        return 0
+
+    def h2_poly_lagrange_to_coeff_batch(self, dst, src, count, k, omega_inv, divisor, repr_):
+        return self._transform_batch("h2_poly_lagrange_to_coeff_batch", 1, dst, src, count, k, k, omega_inv, None, divisor)
+
+    def h2_poly_coeff_to_extended_batch(self, dst, src, count, k, ext_k, zeta, ext_omega, repr_):
+        return self._transform_batch("h2_poly_coeff_to_extended_batch", 2, dst, src, count, k, ext_k, ext_omega, zeta, None)
+
+    def h2_poly_set_rows(self, polys, count, start, rows, values, repr_):
+        self._log("h2_poly_set_rows")
+        count, start, rows = _v(count), _v(start), _v(rows)
+        if count == 0 or rows == 0:
+            return 0
+        hs = [int(polys[i]) for i in range(count)]
+        short = [i for i, h in enumerate(hs) if start + rows > self.polys[h][1].shape[0]]
+        if short:
+            return self._fail(f"h2_poly_set_rows: polys[{short[0]}]: a polynomial holds fewer than start + rows elements")
+        c = clash(args("polys", hs, True))
+        if c:
+            return self._fail(f"h2_poly_set_rows: {c}")
+        vals = _rd(values, 32 * count * rows).reshape(count, rows, 32)
+        for i, h in enumerate(hs):
+            self.polys[h][1][start:start + rows] = vals[i]
+        return 0
+
+    def h2_poly_lookup_permuted(self, out_inputs, out_tables, count, inputs, tables, k, blinding, bf, repr_):
+        self._log("h2_poly_lookup_permuted")
+        count, k, bf = _v(count), _v(k), _v(bf)
+        n, rows = 1 << k, bf + 1
+        outs = [int(out_inputs[b]) for b in range(count)] + [int(out_tables[b]) for b in range(count)]
+        ins = [int(inputs[b]) for b in range(count)] + [int(tables[b]) for b in range(count)]
+        c = clash(args("out_inputs", outs[:count], True) + args("out_tables", outs[count:], True) +
+                  args("inputs", ins[:count], False) + args("tables", ins[count:], False))
+        if c:
+            return self._fail(f"h2_poly_lookup_permuted: {c}")
+        f = self.polys[ins[0]][0]
+        col = lambda hs: np.ascontiguousarray(np.concatenate([self.polys[h][1][:n] for h in hs]))  # noqa: E731
+        oa, ot = col(outs[:count]), col(outs[count:])
+        bl = _rd(blinding, 32 * count * 2 * rows)
+        rc = self.emu.emu_lookup_permuted(cref.FIELD_ID[f], cref._p(col(ins[:count])), cref._p(col(ins[count:])), ctypes.c_uint32(count), ctypes.c_size_t(n),
+                                          ctypes.c_size_t(n - rows), cref._p(bl), ctypes.c_size_t(rows), cref._p(oa), cref._p(ot))
+        if rc != NONE:
+            return self._fail(f"h2_poly_lookup_permuted: lookup {rc}: an input value does not occur in the table")
+        for b in range(count):
+            self.polys[outs[b]][1][:n] = oa[b * n:(b + 1) * n]
+            self.polys[outs[count + b]][1][:n] = ot[b * n:(b + 1) * n]
+        return 0
+
+    def h2_poly_permutation_product(self, z_out, proofs, columns, sigmas, cols, chunk_len, k, beta, gamma, omega, delta, blinding, bf, repr_):
+        self._log("h2_poly_permutation_product")
+        proofs, cols, chunk_len, k, bf = _v(proofs), _v(cols), _v(chunk_len), _v(k), _v(bf)
+        n, sets = 1 << k, -(-cols // chunk_len)
+        col = lambda h: self.polys[int(h)][1][:n]                  # noqa: E731
+        f = self.polys[int(sigmas[0])][0]
+        data = np.ascontiguousarray(np.concatenate([col(columns[i]) for i in range(proofs * cols)] + [col(sigmas[i]) for i in range(cols)]))
+        out = np.zeros((proofs * sets * n, 32), dtype=np.uint8)
+        bl = _rd(blinding, 32 * proofs * sets * bf) if bf else None
+        self.emu.emu_permutation_product(cref.FIELD_ID[f], cref._p(data), proofs, cols, chunk_len, k, cref._p(_rd(beta, 32)), cref._p(_rd(gamma, 32)),
+                                         cref._p(_rd(omega, 32)), cref._p(_rd(delta, 32)), cref._p(bl) if bf else None, bf, cref._p(out))
+        for i in range(proofs * sets):
+            self.polys[int(z_out[i])][1][:n] = out[i * n:(i + 1) * n]
+        return 0
+
+    def h2_poly_lookup_product(self, z_out, count, inputs, tables, permuted_inputs, permuted_tables, k, beta, gamma, blinding, bf, repr_):
+        self._log("h2_poly_lookup_product")
+        count, k, bf = _v(count), _v(k), _v(bf)
+        if count == 0:
+            return 0
+        n = 1 << k
+        col = lambda h: self.polys[int(h)][1][:n]                  # noqa: E731
+        f = self.polys[int(inputs[0])][0]
+        data = np.ascontiguousarray(np.concatenate([col(arr[b]) for b in range(count) for arr in (inputs, tables, permuted_inputs, permuted_tables)]))
+        out = np.zeros((count * n, 32), dtype=np.uint8)
+        bl = _rd(blinding, 32 * count * bf) if bf else None
+        self.emu.emu_lookup_product(cref.FIELD_ID[f], cref._p(data), count, k, cref._p(_rd(beta, 32)), cref._p(_rd(gamma, 32)),
+                                    cref._p(bl) if bf else None, bf, cref._p(out))
+        for b in range(count):
+            self.polys[int(z_out[b])][1][:n] = out[b * n:(b + 1) * n]
+        return 0
+
+    def h2_poly_vanishing_quotient(self, pieces, count, src, k, ext_k, ext_omega_inv, ext_divisor, zeta, t_evals, t_len, repr_):
+        who = "h2_poly_vanishing_quotient"
+        self._log(who)
+        count, src, k, ext_k, t_len = (_v(x) for x in (count, src, k, ext_k, t_len))
+        why = self.emu.emu_vanishing_quotient_sizes(k, ext_k, ctypes.c_uint64(count), t_len)
+        if why:
+            return self._fail(f"{who}: {ctypes.string_at(why).decode()}")
+        hs = [int(pieces[i]) for i in range(count)]
+        short = [i for i, h in enumerate(hs) if self.polys[h][1].shape[0] < 1 << k]
+        if short:
+            return self._fail(f"{who}: pieces[{short[0]}]: a polynomial holds fewer than 2^k elements")
+        c = clash(args("pieces", hs, True) + [("src", src, False)])
+        if c:
+            return self._fail(f"{who}: {c}")
+        f, a = self.polys[src]
+        out = np.zeros((count, 1 << k, 32), dtype=np.uint8)
+        rc = self.emu.emu_vanishing_quotient(cref.FIELD_ID[f], cref._p(np.ascontiguousarray(a[:1 << ext_k])), k, ext_k, ctypes.c_uint64(count),
+                                             cref._p(_rd(ext_omega_inv, 32)), cref._p(_rd(ext_divisor, 32)), cref._p(_rd(zeta, 32)),
+                                             cref._p(_rd(t_evals, 32 * t_len)), t_len, cref._p(out), 0, 64)
+        assert rc > 0, rc
+        for i, h in enumerate(hs):
+            self.polys[h][1][:1 << k] = out[i]
+        return 0
+
+    # ---- key generation: the sigma bodies, and the copy-cycle bodies before them, on the host emulation ----
+    def h2_poly_permutation_sigma(self, dst, cols, k, mapping, omega, delta, repr_):
+        self._log("h2_poly_permutation_sigma")
+        cols, k = _v(cols), _v(k)
+        if k > 30:
+            return self._fail("h2_poly_permutation_sigma: k > 30")
+        if cols == 0:
+            return 0
+        hs = [int(dst[i]) for i in range(cols)]
+        unknown = [i for i, h in enumerate(hs) if h not in self.polys]
+        if unknown:
+            return self._fail(f"h2_poly_permutation_sigma: dst[{unknown[0]}]: unknown polynomial handle")
+        c = clash(args("dst", hs, True))
+        if c:
+            return self._fail(f"h2_poly_permutation_sigma: {c}")
+        field = self.polys[hs[0]][0]
+        n = 1 << k
+        if any(self.polys[h][0] != field or self.polys[h][1].shape[0] < n for h in hs):
+            return self._fail("h2_poly_permutation_sigma: a polynomial of another field or shorter than 2^k")
+        mp = np.frombuffer(ctypes.string_at(_v(mapping), 8 * cols * n), dtype=np.uint32).copy()
+        out = np.zeros((cols * n, 32), dtype=np.uint8)
+        rc = self.emu.emu_permutation_sigma(cref.FIELD_ID[field], mp.ctypes.data_as(ctypes.c_void_p), cols, k, cref._p(_rd(omega, 32)),
+                                            cref._p(_rd(delta, 32)), ctypes.c_uint64(KEYGEN_CHUNK), cref._p(out))
+        if rc:
+            return self._fail("h2_poly_permutation_sigma: a mapping entry is outside the permutation's columns or the domain's rows")
+        for i, h in enumerate(hs):
+            self.polys[h][1][:n] = out[i * n:(i + 1) * n]
+        return 0
+
+    def h2_poly_permutation_sigma_copies(self, dst, cols, k, copies, m, omega, delta, repr_):
+        self._log("h2_poly_permutation_sigma_copies")
+        cols, k, m = _v(cols), _v(k), _v(m)
+        if k > 30:
+            return self._fail("h2_poly_permutation_sigma_copies: k > 30")
+        if cols == 0:
+            return 0
+        if (cols << k) >= 1 << 32 or m >= 1 << 32:
+            return self._fail("h2_poly_permutation_sigma_copies: too many cells or copies")
+        hs = [int(dst[i]) for i in range(cols)]
+        if any(h not in self.polys for h in hs) or len(set(hs)) != cols:
+            return self._fail("h2_poly_permutation_sigma_copies: unknown or repeated polynomial handle")
+        field = self.polys[hs[0]][0]
+        n = 1 << k
+        if any(self.polys[h][0] != field or self.polys[h][1].shape[0] < n for h in hs):
+            return self._fail("h2_poly_permutation_sigma_copies: a polynomial of another field or shorter than 2^k")
+        cp = np.frombuffer(ctypes.string_at(_v(copies), 16 * m), dtype=np.uint32).reshape(-1, 4) if m else np.zeros((0, 4), np.uint32)
+        rc, mapping, bad, _, _ = emu_assembly(self.emu, cp, cols, k)
+        if rc:
+            return self._fail(f"h2_poly_permutation_sigma_copies: copy {bad >> 1}: a {'row' if bad & 1 else 'column'} is out of range")
+        out = np.zeros((cols * n, 32), dtype=np.uint8)
+        rc = self.emu.emu_permutation_sigma(cref.FIELD_ID[field], mapping.ctypes.data_as(ctypes.c_void_p), cols, k, cref._p(_rd(omega, 32)),
+                                            cref._p(_rd(delta, 32)), ctypes.c_uint64(KEYGEN_CHUNK), cref._p(out))
+        assert rc == 0
+        for i, h in enumerate(hs):
+            self.polys[h][1][:n] = out[i * n:(i + 1) * n]
         return 0
 
     # ---- the opening's round loop: the reference's own folding loop, one round per call (poly/commitment/prover.rs:100-142) ----

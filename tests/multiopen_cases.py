@@ -4,6 +4,7 @@ driver that runs prover and verifier through either the oracle or the engine's h
 from __future__ import annotations
 
 import numpy as np
+import pytest
 
 from oracle import cref, pasta
 from tests import prover_replay as R
@@ -26,6 +27,31 @@ class SeededRng:
         self.i += 1
         b = cref.gen_scalars(self.field, self.seed + self.i, n)
         return b if self.as_bytes else cref.bytes_to_ints(b)
+
+
+class RecordingRng:
+    """Passes every draw through and keeps the scalars drawn."""
+
+    def __init__(self, inner):
+        self.inner, self.draws = inner, []
+
+    def scalar(self):
+        x = self.inner.scalar()
+        self.draws.append(x)
+        return x
+
+    def poly(self, n):
+        return self.inner.poly(n)
+
+
+class ReplayRng:
+    """Gives back recorded scalar draws in order."""
+
+    def __init__(self, draws):
+        self.draws = list(draws)
+
+    def scalar(self):
+        return self.draws.pop(0)
 
 
 def reference_roundtrip_polys(n: int):
@@ -59,8 +85,7 @@ class OracleSide:
         return pasta.to_affine(self.c, pasta.best_multiexp(self.c, list(poly) + [blind], self.g + [self.w]))
 
     def prove(self, polys, blinds, plan, rng_seed) -> bytes:
-        from tests.test_verifier_oracle import _WriteT
-        W = _WriteT(self.c.r)
+        W = R._WriteT(self.c.r)
         qs = [pasta.ProverQuery(pt, polys[i], blinds[i]) for i, pt in plan]
         pasta.multiopen_create_proof(self.c, self.g, self.w, self.u, SeededRng(self.c.scalar, rng_seed, False), W, qs)
         return bytes(W.T.proof)
@@ -122,3 +147,24 @@ class EngineSide:
 def evals_for(field: str, polys, plan):
     m = pasta.FIELDS[field]
     return [(i, pt, pasta.eval_polynomial_mod(m, polys[i], pt)) for i, pt in plan]
+
+
+def roundtrip(side, field):
+    """multiopen.rs:278-373 and :375-481 on `side`."""
+    m = pasta.FIELDS[field]
+    n = 1 << side.k
+    ax, bx, cx = reference_roundtrip_polys(n)
+    blind, x, y, bvx_bad = cref.bytes_to_ints(cref.gen_scalars(field, SEED + 20, 4))
+    a, b, c = (side.commit(p, blind) for p in (ax, bx, cx))
+    avx, bvx, cvy = (pasta.eval_polynomial_mod(m, p, pt) for p, pt in ((ax, x), (bx, x), (cx, y)))
+    polys = [ax, bx, cx]
+    proof = side.prove(polys, [blind] * 3, [(0, x), (1, x), (2, y)], SEED + 30)
+    assert not side.verify(proof, [a, b, c], [(0, x, avx), (1, x, avx), (2, y, cvy)])        # "NB: wrong!" (:347): should fail
+    assert side.verify(proof, [a, b, c], [(0, x, avx), (1, x, bvx), (2, y, cvy)])            # should succeed (:360-371)
+    # test_identical_queries (:464-479): the same commitment at the same point with two different evaluations
+    VerifyError = pasta.VerifyError if isinstance(side, OracleSide) else side.eng.VerifyError
+    with pytest.raises(VerifyError):
+        side.verify(proof, [a, b, c], [(0, x, avx), (1, x, bvx_bad), (1, x, bvx), (2, y, cvy)])
+    # bx and cx have the same coefficients but are different polynomials (different pointers): b == c as points, two queries
+    assert np.array_equal(np.asarray(b), np.asarray(c)) if not isinstance(b, tuple) else b == c
+    return proof

@@ -595,6 +595,19 @@ def create_proof_engine(eng, params, vk: PV.PinnedKey, fixed, sigma, advice, ins
             close_proving_key(pk)
 
 
+def prover_pk_dict(pk):
+    """A halo2_b200.ProvingKey in the shape create_proof_engine(pk=...) keeps it."""
+    P = pk.permutation
+    return {"fixed_l": pk.fixed_values, "fixed_p": pk.fixed_polys, "fixed_c": pk.fixed_cosets, "sigma_l": P.permutations,
+            "sigma_p": P.polys, "sigma_c": P.cosets, "l": [pk.l0, pk.l_blind, pk.l_last]}
+
+
+def prover_pk_bytes(pk) -> list:
+    """The bytes of every polynomial of a halo2_b200.ProvingKey, in prover_pk_dict's order."""
+    d = prover_pk_dict(pk)
+    return [p.download().tobytes() for key in ("fixed_l", "fixed_p", "fixed_c", "sigma_l", "sigma_p", "sigma_c", "l") for p in d[key]]
+
+
 def close_proving_key(pk) -> None:
     for key in ("fixed_l", "fixed_p", "fixed_c", "sigma_l", "sigma_p", "sigma_c", "l", "tmp"):
         for p in pk.pop(key, []):

@@ -73,6 +73,37 @@ class Blake2bTranscript:
         return int.from_bytes(self.state.copy().digest(), "little") % self.modulus
 
 
+class _WriteT:
+    """Blake2bTranscript on affine tuples (what the oracle speaks)."""
+
+    def __init__(self, modulus):
+        from oracle import cref
+        self.T, self._bytes = Blake2bTranscript(modulus), lambda pt: cref.affines_to_bytes([pt])[0]
+
+    def write_point(self, pt):
+        self.T.write_point(self._bytes(pt))
+
+    def write_scalar(self, s):
+        self.T.write_scalar(s)
+
+    def common_point(self, pt):
+        self.T.common_point(self._bytes(pt))
+
+    def common_scalar(self, s):
+        self.T.common_scalar(s)
+
+    def squeeze_challenge(self):
+        return self.T.squeeze_challenge()
+
+
+def _encode(points, m) -> bytes:
+    """The proof bytes of `points` written to a fresh transcript."""
+    T = Blake2bTranscript(m)
+    for p in points:
+        T.write_point(p)
+    return bytes(T.proof)
+
+
 class Blake2bRead:
     """transcript.rs:66-158 (Blake2bRead) with Challenge255: the verifier's view of the same transcript.  `decompress`:
     32 proof bytes -> (64,) uint8 affine x||y, raising on an invalid encoding (C::from_bytes, :91-100) -- the engine's

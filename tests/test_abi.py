@@ -6,14 +6,9 @@ import re
 import numpy as np
 import pytest
 
+from tests.abi_cases import _header_symbols
+
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-
-
-def _header_symbols():
-    with open(os.path.join(ROOT, "include", "halo2_b200.h")) as f:
-        text = f.read()
-    text = re.sub(r"/\*.*?\*/", "", text, flags=re.S)
-    return sorted(set(re.findall(r"\b(h2_[a-z0-9_]+)\s*\(", text)))
 
 
 def test_library_exports_every_declared_symbol():

@@ -15,11 +15,12 @@ from halo2_b200 import arguments as A
 from halo2_b200 import lib as L
 from oracle import cref, pasta
 from tests import arguments_cases as AC
+from tests import fake_engine
 from tests import multiopen_cases as MC
+from tests import plonk_api_circuit as circ
 from tests import plonk_prover as PP
 from tests import plonk_verifier as PV
 from tests import prover_replay as R
-from tests import test_real_proof as TR
 
 
 def _gens(prm_gens):
@@ -29,24 +30,23 @@ def _gens(prm_gens):
 def test_plonk_api_proof_from_package_calls_is_byte_identical():
     """Under the golden key and one seeded rng, the package composition writes the oracle prover's proof and
     create_proof_engine's, and frees every polynomial it made; the golden-pinned verifier accepts the proof."""
-    from tests import plonk_api_circuit as circ
     c = pasta.VESTA
     P = pasta.Params.new(c, 5)
-    vk = PV.PinnedKey(TR.CASE["key_text"])
-    fixed, sigma = circ.fixed_columns(TR.M, TR.ZETA), circ.permutation_columns(TR.M, vk.omega, TR.DELTA)
+    vk = PV.PinnedKey(circ.CASE["key_text"])
+    fixed, sigma = circ.fixed_columns(circ.M, circ.ZETA), circ.permutation_columns(circ.M, vk.omega, circ.DELTA)
     gens = (cref.affines_to_bytes(P.g), cref.affines_to_bytes(P.g_lagrange), cref.affines_to_bytes([P.w]), cref.affines_to_bytes([P.u]))
     inst = [[[2]], [[2]]]
-    oracle = TR.prove((c, P, vk, fixed, sigma, gens), [TR.witness(), TR.witness()], inst, 777)
-    with AC.installed() as fake:
+    oracle = circ.prove((c, P, vk, fixed, sigma, gens), [circ.witness(), circ.witness()], inst, 777)
+    with fake_engine.installed() as fake:
         prm = halo2_b200.Params("vesta", 5, gens[0], gens[1], gens[2], u=gens[3])
-        D = halo2_b200.EvaluationDomain("fp", vk.degree(), vk.k, TR.ZETA)
-        T = R.Blake2bTranscript(TR.M)
-        PP.create_proof_engine(halo2_b200, prm, vk, fixed, sigma, [TR.witness(), TR.witness()], inst, MC.SeededRng("fp", 777, True), T, TR.ZETA, TR.DELTA)
+        D = halo2_b200.EvaluationDomain("fp", vk.degree(), vk.k, circ.ZETA)
+        T = R.Blake2bTranscript(circ.M)
+        PP.create_proof_engine(halo2_b200, prm, vk, fixed, sigma, [circ.witness(), circ.witness()], inst, MC.SeededRng("fp", 777, True), T, circ.ZETA, circ.DELTA)
         engine = bytes(T.proof)
         pk = AC.proving_key(halo2_b200, D, fixed, sigma, vk.blinding_factors())
         held, calls = set(fake.polys), len(fake.calls)
-        T = R.Blake2bTranscript(TR.M)
-        AC.create_proof_package(halo2_b200, prm, D, pk, vk, [TR.witness(), TR.witness()], inst, MC.SeededRng("fp", 777, True), T, TR.DELTA)
+        T = R.Blake2bTranscript(circ.M)
+        AC.create_proof_package(halo2_b200, prm, D, pk, vk, [circ.witness(), circ.witness()], inst, MC.SeededRng("fp", 777, True), T, circ.DELTA)
         got = bytes(T.proof)
         assert set(fake.polys) == held                             # the composition freed everything it made
         mine = fake.calls[calls:]
@@ -56,17 +56,17 @@ def test_plonk_api_proof_from_package_calls_is_byte_identical():
         prm.close()
         assert not fake.polys
     assert len(got) == 4160 and got == engine == oracle
-    assert PV.verify_proof(PV.OracleArm("vesta", 5, *gens), vk, got, inst, TR.DELTA)
+    assert PV.verify_proof(PV.OracleArm("vesta", 5, *gens), vk, got, inst, circ.DELTA)
 
 
 def _nonlinear_proof(k, seed=11, instance=None, hook=None):
     prm, commit, gens = AC.params_for(halo2_b200, k)
-    vk, D, fixed, sigma, advice, inst = AC.nonlinear_case(halo2_b200, k, commit, TR.ZETA, TR.DELTA)
+    vk, D, fixed, sigma, advice, inst = AC.nonlinear_case(halo2_b200, k, commit, circ.ZETA, circ.DELTA)
     pk = AC.proving_key(halo2_b200, D, fixed, sigma, vk.blinding_factors())
     insts = [inst, inst] if instance is None else instance
     try:
-        T = R.Blake2bTranscript(TR.M)
-        AC.create_proof_package(halo2_b200, prm, D, pk, vk, [advice, advice], insts, MC.SeededRng("fp", seed, True), T, TR.DELTA,
+        T = R.Blake2bTranscript(circ.M)
+        AC.create_proof_package(halo2_b200, prm, D, pk, vk, [advice, advice], insts, MC.SeededRng("fp", seed, True), T, circ.DELTA,
                                 on_construct=hook(D) if hook else None)
     finally:
         pk.close()
@@ -76,7 +76,7 @@ def _nonlinear_proof(k, seed=11, instance=None, hook=None):
 
 @pytest.mark.parametrize("k", [4, 5, 6])
 def test_nonlinear_lookup_circuit_verifies(k):
-    with AC.installed() as fake:
+    with fake_engine.installed() as fake:
         seen = []
 
         def hook(D):
@@ -88,24 +88,24 @@ def test_nonlinear_lookup_circuit_verifies(k):
     assert len(vk.permutation_columns) == 10 and vk.degree() - 2 == 4          # three sets
     assert seen[0] == [True] * 4                                   # input and table of both proofs
     arm = PV.OracleArm("vesta", k, *_gens(gens))
-    assert PV.verify_proof(arm, vk, proof, [inst, inst], TR.DELTA)
+    assert PV.verify_proof(arm, vk, proof, [inst, inst], circ.DELTA)
     bad = bytearray(proof)
     bad[len(proof) // 2] ^= 1
-    assert not PV.verify_proof(arm, vk, bytes(bad), [inst, inst], TR.DELTA)
+    assert not PV.verify_proof(arm, vk, bytes(bad), [inst, inst], circ.DELTA)
     wrong = [[[inst[0][0] + 1]], inst]
-    assert not PV.verify_proof(arm, vk, proof, wrong, TR.DELTA)
+    assert not PV.verify_proof(arm, vk, proof, wrong, circ.DELTA)
 
 
 def test_nonlinear_lookup_circuit_with_the_wrong_public_input_is_rejected():
     """A proof made for another public input than the copy constraint ties to the witness fails verification."""
-    with AC.installed():
+    with fake_engine.installed():
         vk, proof, inst, gens = _nonlinear_proof(4, instance=[[[5]], [[5]]])
-    assert not PV.verify_proof(PV.OracleArm("vesta", 4, *_gens(gens)), vk, proof, [[[5]], [[5]]], TR.DELTA)
+    assert not PV.verify_proof(PV.OracleArm("vesta", 4, *_gens(gens)), vk, proof, [[[5]], [[5]]], circ.DELTA)
 
 
 # ---- argument errors ---------------------------------------------------------------------------------------------------
 def _setup(fake, k=4, sets=3, lookups=2):
-    D = halo2_b200.EvaluationDomain("fp", 6, k, TR.ZETA)
+    D = halo2_b200.EvaluationDomain("fp", 6, k, circ.ZETA)
     n, N = D.n, D.extended_len()
     rp = lambda length: halo2_b200.ResidentPoly("fp", length)     # noqa: E731
     from halo2_b200.keygen import PermutationProvingKey
@@ -128,7 +128,7 @@ def _expect(fake, msg, fn):
 
 
 def test_argument_errors_raise_before_any_launch():
-    with AC.installed() as fake:
+    with fake_engine.installed() as fake:
         D, pk, perm, look, ev, (l0, lb, ll), cols = _setup(fake)
         registered = len(ev.polys)
         c = lambda committed, **kw: committed.construct(ev, pk, kw.get("cols", cols), l0, lb, ll, 2, 3, 5, kw.get("chunk", 4), 5)  # noqa: E731
@@ -169,7 +169,7 @@ def test_argument_errors_raise_before_any_launch():
 def test_objects_free_what_they_allocated_on_every_path(monkeypatch):
     """construct of the lookups makes the product cosets and frees them when the batched transform fails; each object's
     close frees its polynomials and those of what it was made from; evaluations allocate nothing."""
-    with AC.installed() as fake:
+    with fake_engine.installed() as fake:
         D, pk, perm, look, ev, (l0, lb, ll), cols = _setup(fake)
         a, b = cols[0], cols[1]
         exprs = [([a * b], [b]), ([a], [b + a])]

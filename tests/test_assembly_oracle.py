@@ -9,7 +9,6 @@ orc_assembly, halo2_b200.CopyConstraints) against the restated reference Assembl
 - the device bodies on the host emulation, in the host driver's order, give the same mapping for k = 1 ... 12 and 1 to 8
   columns, including a list that needs every one of the floor(log2 cells) Borůvka rounds, and name the same first bad copy;
 - keygen_vk / keygen_pk from CopyConstraints over an ABI stand-in reproduce the test prover's key values."""
-import contextlib
 import ctypes
 import random
 
@@ -19,10 +18,15 @@ import pytest
 from oracle import assembly as orc
 from oracle import cref, pasta
 from tests import bench_circuit as BC
+from tests import fake_engine
 from tests import plonk_api_circuit as circ
-from tests.test_keygen_oracle import (KeygenFakeLib, _bench_setup, bench_copies, delta_of, oracle_assembly, oracle_copy, oracle_sigma,
-                                      plonk_api_copies, prover_pk_dict, KEYGEN_CHUNK, ZETA)
+from tests.bench_circuit import _bench_setup, bench_copies
+from tests.fake_engine import emu_assembly
+from tests.keygen_cases import oracle_assembly, oracle_copy, oracle_sigma
 from tests.kernel_emul import build as emul_build
+from tests.plonk_api_circuit import ZETA, plonk_api_copies
+from tests.plonk_prover import prover_pk_dict
+from tests.plonk_verifier import scalar_delta
 
 
 # ---- copy lists --------------------------------------------------------------------------------------------------------
@@ -95,7 +99,7 @@ def copy_lists(rng, cols: int, k: int):
 
 
 def restated_mapping(n: int, cols: int, copies):
-    """The sequential loop (test_keygen_oracle.oracle_copy) as a (cols, n, 2) uint32 array."""
+    """The sequential loop (tests/keygen_cases.oracle_copy) as a (cols, n, 2) uint32 array."""
     asm = oracle_assembly(n, cols)
     for c in copies:
         oracle_copy(asm, *c)
@@ -174,7 +178,7 @@ def test_orc_assembly_on_the_test_circuits():
         omega = pasta.omega_for_k("fp", k)
         got, err = orc.assembly(list(bench_copies(k)), 3, k)
         assert err is None
-        assert oracle_sigma(got, n, omega, delta_of(m), m) == BC.columns(k, m, omega, delta_of(m), 7)[1]
+        assert oracle_sigma(got, n, omega, scalar_delta(m), m) == BC.columns(k, m, omega, scalar_delta(m), 7)[1]
 
 
 def _bad_lists(cols: int, n: int):
@@ -209,16 +213,6 @@ def test_orc_assembly_first_bad_copy():
 @pytest.fixture(scope="module")
 def emu():
     return ctypes.CDLL(emul_build.build())
-
-
-def emu_assembly(emu, copies, cols: int, k: int):
-    """(rc, mapping (cols, 2^k, 2), first-bad code, Borůvka rounds, |F|)."""
-    cp = np.ascontiguousarray(np.asarray(copies, dtype=np.uint32).reshape(-1, 4))
-    out = np.zeros((cols, 1 << k, 2), dtype=np.uint32)
-    bad, rounds, forest = ctypes.c_ulonglong(), ctypes.c_uint32(), ctypes.c_uint32()
-    rc = emu.emu_assembly(cp.ctypes.data_as(ctypes.c_void_p), ctypes.c_uint64(cp.shape[0]), ctypes.c_uint32(cols), ctypes.c_uint32(k),
-                          out.ctypes.data_as(ctypes.c_void_p), ctypes.byref(bad), ctypes.byref(rounds), ctypes.byref(forest))
-    return rc, out, bad.value, rounds.value, forest.value
 
 
 @pytest.mark.parametrize("k", range(1, 13))
@@ -292,52 +286,6 @@ def test_copy_constraints_checks_and_records():
     assert cc.copies.tolist() == [[0, 7, 2, 0], [1, 2, 1, 3], [2, 5, 0, 0], [1, 1, 1, 1]] and cc.copies.dtype == np.uint32
 
 
-class AssemblyFakeLib(KeygenFakeLib):
-    """The keygen ABI stand-in plus h2_poly_permutation_sigma_copies: the copy-cycle bodies and the sigma bodies on the
-    host emulation, with the library's argument checks."""
-
-    def h2_poly_permutation_sigma_copies(self, dst, cols, k, copies, m, omega, delta, repr_):
-        from tests import fake_engine as FE
-        self._log("h2_poly_permutation_sigma_copies")
-        cols, k, m = FE._v(cols), FE._v(k), FE._v(m)
-        if k > 30:
-            return self._fail("h2_poly_permutation_sigma_copies: k > 30")
-        if cols == 0:
-            return 0
-        if (cols << k) >= 1 << 32 or m >= 1 << 32:
-            return self._fail("h2_poly_permutation_sigma_copies: too many cells or copies")
-        hs = [int(dst[i]) for i in range(cols)]
-        if any(h not in self.polys for h in hs) or len(set(hs)) != cols:
-            return self._fail("h2_poly_permutation_sigma_copies: unknown or repeated polynomial handle")
-        field = self.polys[hs[0]][0]
-        n = 1 << k
-        if any(self.polys[h][0] != field or self.polys[h][1].shape[0] < n for h in hs):
-            return self._fail("h2_poly_permutation_sigma_copies: a polynomial of another field or shorter than 2^k")
-        cp = np.frombuffer(ctypes.string_at(FE._v(copies), 16 * m), dtype=np.uint32).reshape(-1, 4) if m else np.zeros((0, 4), np.uint32)
-        rc, mapping, bad, _, _ = emu_assembly(self.emu, cp, cols, k)
-        if rc:
-            return self._fail(f"h2_poly_permutation_sigma_copies: copy {bad >> 1}: a {'row' if bad & 1 else 'column'} is out of range")
-        out = np.zeros((cols * n, 32), dtype=np.uint8)
-        rc = self.emu.emu_permutation_sigma(cref.FIELD_ID[field], mapping.ctypes.data_as(ctypes.c_void_p), cols, k, cref._p(FE._rd(omega, 32)),
-                                            cref._p(FE._rd(delta, 32)), ctypes.c_uint64(KEYGEN_CHUNK), cref._p(out))
-        assert rc == 0
-        for i, h in enumerate(hs):
-            self.polys[h][1][:n] = out[i * n:(i + 1) * n]
-        return 0
-
-
-@contextlib.contextmanager
-def installed():
-    from halo2_b200 import lib as L
-    saved = (L._lib, L._inited_device)
-    fake = AssemblyFakeLib()
-    L._lib, L._inited_device = fake, 0
-    try:
-        yield fake
-    finally:
-        L._lib, L._inited_device = saved
-
-
 def test_keygen_from_copy_constraints_reproduces_the_test_provers_key():
     """keygen_vk / keygen_pk given CopyConstraints at k = 5: the same commitments and key values as from the Assembly
     (which test_keygen_oracle ties to the test prover's own key), through one copies call each, and the same proof bytes."""
@@ -349,8 +297,8 @@ def test_keygen_from_copy_constraints_reproduces_the_test_provers_key():
     k = 5
     c, m, gens, fixed, sigma, adv, copies = _bench_setup(k)
     n = 1 << k
-    delta = delta_of(m)
-    with installed() as fake:
+    delta = scalar_delta(m)
+    with fake_engine.installed() as fake:
         prm = h2.Params("vesta", k, *gens[:3], u=gens[3])
         D = h2.EvaluationDomain("fp", BC.DEGREE, k, ZETA)
         cc = h2.CopyConstraints(n, 3)
@@ -398,8 +346,8 @@ def test_plonk_api_copies_through_copy_constraints():
     """The plonk_api circuit's copies give the sigma columns the test circuit pins (the golden commitments on the GPU)."""
     import halo2_b200 as h2
     m = pasta.P_MOD
-    omega, delta = pasta.omega_for_k("fp", circ.K), delta_of(m)
-    with installed():
+    omega, delta = pasta.omega_for_k("fp", circ.K), scalar_delta(m)
+    with fake_engine.installed():
         D = h2.EvaluationDomain("fp", 4, circ.K, ZETA)
         assert D.omega == omega
         cc = h2.CopyConstraints(circ.N, 12)

@@ -1,6 +1,6 @@
 """CPU checks of the column-batched transforms and of instance_commit / advice_commit: the batched NTT pass bodies on the
-host emulation against the oracle's transforms, h2_poly_set_rows on the ABI stand-in (tests/columns_cases.ColumnsFake: the
-stand-in with the new entry points) against per-column copies, and the two phases over the stand-in against
+host emulation against the oracle's transforms, h2_poly_set_rows on the ABI stand-in (tests/fake_engine.py) against
+per-column copies, and the two phases over the stand-in against
 create_proof_engine's per-column composition on the plonk_api circuit."""
 import ctypes
 
@@ -9,6 +9,8 @@ import pytest
 
 from oracle import cref, pasta
 from tests import columns_cases as CC
+from tests import fake_engine
+from tests import plonk_api_circuit as circ
 from tests.kernel_emul import build as emul_build
 
 
@@ -75,7 +77,7 @@ def _gens():
 
 def test_set_rows_equals_per_column_copies():
     import halo2_b200
-    with CC.installed() as fake:
+    with fake_engine.installed() as fake:
         n, start, rows = 32, 26, 6
         cols = [cref.gen_scalars("fp", 5 + c, n) for c in range(4)]
         vals = [cref.gen_scalars("fp", 50 + c, rows) for c in range(4)]
@@ -91,26 +93,20 @@ def test_set_rows_equals_per_column_copies():
             halo2_b200.set_rows_resident([a[0], a[0]], start, np.stack(vals[:2]))
 
 
-def _plonk_api():
-    from tests import plonk_verifier as PV
-    from tests import test_real_proof as TR
-    return PV.PinnedKey(TR.CASE["key_text"]), TR
-
-
 def test_phases_of_the_plonk_api_circuit():
     """instance_commit and advice_commit over the stand-in equal create_proof_engine's instance and advice phases on the
     plonk_api circuit (k = 5, 5 advice columns, two proofs) under the same rng: the commitments in transcript order and the
     bytes of every column's values, polynomial and coset.  advice_commit makes one set_rows call, and the two phases one
     batched call per transform each."""
     import halo2_b200
-    vk, TR = _plonk_api()
-    with CC.installed() as fake:
+    vk = circ.plonk_api_key()
+    with fake_engine.installed() as fake:
         g, gl, w, u = _gens()
         prm = halo2_b200.Params("vesta", 5, g, gl, w, u=u)
-        advice, instances = [TR.witness(), TR.witness()], [[[2]], [[2]]]
-        want = CC.engine_phases(halo2_b200, prm, vk, advice, instances, 777, TR.ZETA)
+        advice, instances = [circ.witness(), circ.witness()], [[[2]], [[2]]]
+        want = CC.engine_phases(halo2_b200, prm, vk, advice, instances, 777, circ.ZETA)
         fake.calls.clear()
-        got = CC.batched_phases(halo2_b200, prm, vk, advice, instances, 777, TR.ZETA)
+        got = CC.batched_phases(halo2_b200, prm, vk, advice, instances, 777, circ.ZETA)
         for name in ("h2_poly_set_rows", "h2_poly_lagrange_to_coeff_batch", "h2_poly_coeff_to_extended_batch"):
             assert fake.calls.count(name) == (1 if name == "h2_poly_set_rows" else 2), name
         assert fake.calls.count("h2_msm_registered_polys_affine") == 2
@@ -121,11 +117,11 @@ def test_phases_of_the_plonk_api_circuit():
 
 def test_instance_too_large():
     import halo2_b200
-    vk, TR = _plonk_api()
-    with CC.installed():
+    vk = circ.plonk_api_key()
+    with fake_engine.installed():
         g, gl, w, u = _gens()
         prm = halo2_b200.Params("vesta", 5, g, gl, w, u=u)
-        D = halo2_b200.EvaluationDomain("fp", vk.degree(), vk.k, TR.ZETA)
+        D = halo2_b200.EvaluationDomain("fp", vk.degree(), vk.k, circ.ZETA)
         bf = vk.blinding_factors()
         ok = halo2_b200.instance_commit(prm, D, [[[1] * (D.n - bf - 1)]], bf)
         for p in ok[0].values + ok[0].polys + ok[0].cosets:

@@ -12,41 +12,40 @@ from halo2_b200 import poly as P
 from oracle import cref, pasta
 from tests import arguments_cases as AC
 from tests import multiopen_cases as MC
+from tests import plonk_api_circuit as circ
 from tests import plonk_prover as PP
 from tests import plonk_verifier as PV
 from tests import prover_replay as R
-from tests import test_real_proof as TR
 
 pytestmark = pytest.mark.gpu
 
 
 def _engine_proof(prm, vk, fixed, sigma, advice, inst, seed, pk=None):
-    T = R.Blake2bTranscript(TR.M)
-    PP.create_proof_engine(halo2_b200, prm, vk, fixed, sigma, advice, inst, MC.SeededRng("fp", seed, True), T, TR.ZETA, TR.DELTA, pk=pk)
+    T = R.Blake2bTranscript(circ.M)
+    PP.create_proof_engine(halo2_b200, prm, vk, fixed, sigma, advice, inst, MC.SeededRng("fp", seed, True), T, circ.ZETA, circ.DELTA, pk=pk)
     return bytes(T.proof)
 
 
 def _package_proof(prm, D, pk, vk, advice, inst, seed, hook=None):
-    T = R.Blake2bTranscript(TR.M)
-    AC.create_proof_package(halo2_b200, prm, D, pk, vk, advice, inst, MC.SeededRng("fp", seed, True), T, TR.DELTA, on_construct=hook)
+    T = R.Blake2bTranscript(circ.M)
+    AC.create_proof_package(halo2_b200, prm, D, pk, vk, advice, inst, MC.SeededRng("fp", seed, True), T, circ.DELTA, on_construct=hook)
     return bytes(T.proof)
 
 
 def test_plonk_api_circuit_equals_create_proof_engine():
-    from tests import plonk_api_circuit as circ
-    vk = PV.PinnedKey(TR.CASE["key_text"])
-    fixed, sigma = circ.fixed_columns(TR.M, TR.ZETA), circ.permutation_columns(TR.M, vk.omega, TR.DELTA)
+    vk = PV.PinnedKey(circ.CASE["key_text"])
+    fixed, sigma = circ.fixed_columns(circ.M, circ.ZETA), circ.permutation_columns(circ.M, vk.omega, circ.DELTA)
     inst = [[[2]], [[2]]]
     prm = halo2_b200.Params.new("vesta", 5)
-    D = halo2_b200.EvaluationDomain("fp", vk.degree(), vk.k, TR.ZETA)
+    D = halo2_b200.EvaluationDomain("fp", vk.degree(), vk.k, circ.ZETA)
     pk = AC.proving_key(halo2_b200, D, fixed, sigma, vk.blinding_factors())
     try:
-        want = _engine_proof(prm, vk, fixed, sigma, [TR.witness(), TR.witness()], inst, 777)
-        got = _package_proof(prm, D, pk, vk, [TR.witness(), TR.witness()], inst, 777)
+        want = _engine_proof(prm, vk, fixed, sigma, [circ.witness(), circ.witness()], inst, 777)
+        got = _package_proof(prm, D, pk, vk, [circ.witness(), circ.witness()], inst, 777)
         assert len(got) == 4160 and got == want
         earm = PV.EngineArm(halo2_b200, "vesta", 5, params=prm)
-        assert PV.verify_proof(earm, vk, got, inst, TR.DELTA)
-        assert PV.verify_proof(PV.OracleArm("vesta", 5, prm.g, prm.g_lagrange, prm.w, prm.u), vk, got, inst, TR.DELTA)
+        assert PV.verify_proof(earm, vk, got, inst, circ.DELTA)
+        assert PV.verify_proof(PV.OracleArm("vesta", 5, prm.g, prm.g_lagrange, prm.w, prm.u), vk, got, inst, circ.DELTA)
     finally:
         pk.close()
         prm.close()
@@ -54,11 +53,10 @@ def test_plonk_api_circuit_equals_create_proof_engine():
 
 def test_benchmark_circuit_k14_equals_create_proof_engine():
     from tests import bench_circuit as BC
-    from tests import plonk_api_circuit as circ
-    k, m = 14, TR.M
+    k, m = 14, circ.M
     prm = halo2_b200.Params.new("vesta", k)
-    D = halo2_b200.EvaluationDomain("fp", BC.DEGREE, k, TR.ZETA)
-    fixed, sigma, adv = BC.columns(k, m, D.omega, TR.DELTA, circ.A_SMALL * TR.ZETA % m)
+    D = halo2_b200.EvaluationDomain("fp", BC.DEGREE, k, circ.ZETA)
+    fixed, sigma, adv = BC.columns(k, m, D.omega, circ.DELTA, circ.A_SMALL * circ.ZETA % m)
     fb, sb, ab = ([cref.ints_to_bytes(c_) for c_ in cols] for cols in (fixed, sigma, adv))
     vk = PV.PinnedKey(BC.pinned_key_text(k, D.extended_k, pasta.Q_MOD, m, D.omega, [_commit(prm, c_) for c_ in fb], [_commit(prm, c_) for c_ in sb]))
     pk = AC.proving_key(halo2_b200, D, fb, sb, vk.blinding_factors())
@@ -66,7 +64,7 @@ def test_benchmark_circuit_k14_equals_create_proof_engine():
         want = _engine_proof(prm, vk, fb, sb, [ab], [[]], 5)
         got = _package_proof(prm, D, pk, vk, [ab], [[]], 5)
         assert got == want
-        assert PV.verify_proof(PV.EngineArm(halo2_b200, "vesta", k, params=prm), vk, got, [[]], TR.DELTA)
+        assert PV.verify_proof(PV.EngineArm(halo2_b200, "vesta", k, params=prm), vk, got, [[]], circ.DELTA)
     finally:
         pk.close()
         prm.close()
@@ -80,7 +78,7 @@ def _commit(prm, values):
 
 def _nonlinear(k):
     prm = halo2_b200.Params.new("vesta", k)
-    vk, D, fixed, sigma, advice, inst = AC.nonlinear_case(halo2_b200, k, lambda c: _commit(prm, c), TR.ZETA, TR.DELTA)
+    vk, D, fixed, sigma, advice, inst = AC.nonlinear_case(halo2_b200, k, lambda c: _commit(prm, c), circ.ZETA, circ.DELTA)
     adv = [cref.ints_to_bytes(c) for c in advice]
     return prm, vk, D, AC.proving_key(halo2_b200, D, fixed, sigma, vk.blinding_factors()), adv, inst
 
@@ -102,9 +100,9 @@ def test_nonlinear_lookup_circuit(k):
         bad = bytearray(proof)
         bad[len(proof) // 3] ^= 1
         for arm in arms:
-            assert PV.verify_proof(arm, vk, proof, [inst, inst], TR.DELTA), arm.name
-            assert not PV.verify_proof(arm, vk, bytes(bad), [inst, inst], TR.DELTA), arm.name
-            assert not PV.verify_proof(arm, vk, proof, [inst, [[inst[0][0] + 1]]], TR.DELTA), arm.name
+            assert PV.verify_proof(arm, vk, proof, [inst, inst], circ.DELTA), arm.name
+            assert not PV.verify_proof(arm, vk, bytes(bad), [inst, inst], circ.DELTA), arm.name
+            assert not PV.verify_proof(arm, vk, proof, [inst, [[inst[0][0] + 1]]], circ.DELTA), arm.name
     finally:
         pk.close()
         prm.close()
@@ -119,7 +117,7 @@ def test_on_a_lane_with_a_shared_key():
         with L.Lane():
             got = _package_proof(prm, D, pk, vk, [adv, adv], [inst, inst], 3)
         assert got == want
-        assert PV.verify_proof(PV.EngineArm(halo2_b200, "vesta", 12, params=prm), vk, got, [inst, inst], TR.DELTA)
+        assert PV.verify_proof(PV.EngineArm(halo2_b200, "vesta", 12, params=prm), vk, got, [inst, inst], circ.DELTA)
     finally:
         pk.close()
         prm.close()
@@ -143,7 +141,7 @@ def test_failing_construct_and_evaluate_leave_nothing_allocated(monkeypatch):
     refused permutation construct allocates nothing."""
     monkeypatch.setattr(P, "ResidentPoly", _Counting)
     k = 6
-    D = halo2_b200.EvaluationDomain("fp", 6, k, TR.ZETA)
+    D = halo2_b200.EvaluationDomain("fp", 6, k, circ.ZETA)
     n, N = D.n, D.extended_len()
     rp = lambda length, s: halo2_b200.ResidentPoly("fp", length, cref.gen_scalars("fp", s, length))   # noqa: E731
     permuted = [halo2_b200.Permuted(*[rp(n, 10 * i + j) for j in range(6)], rp(N, 10 * i + 6), rp(N, 10 * i + 7), 3, 4) for i in range(2)]

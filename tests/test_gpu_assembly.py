@@ -22,10 +22,12 @@ from oracle import assembly as orc  # noqa: E402
 from oracle import cref, pasta  # noqa: E402
 from tests import bench_circuit as BC  # noqa: E402
 from tests import plonk_api_circuit as circ  # noqa: E402
-from tests.test_gpu_keygen import _bench_assembly, _bench_params, _dump, _err, _lib, _sigma_call  # noqa: E402
-from tests.test_gpu_lanes import _run_parallel  # noqa: E402
-from tests.test_keygen_oracle import ZETA, bench_copies, delta_of, oracle_sigma, plonk_api_copies, prover_pk_dict  # noqa: E402
-from tests.test_oracle_golden import golden_columns  # noqa: E402
+from tests.abi_cases import _err, _lib, _run_parallel, _sigma_call  # noqa: E402
+from tests.bench_circuit import _bench_assembly, _bench_params, bench_copies  # noqa: E402
+from tests.keygen_cases import oracle_sigma  # noqa: E402
+from tests.plonk_api_circuit import ZETA, golden_columns, plonk_api_copies  # noqa: E402
+from tests.plonk_prover import prover_pk_bytes, prover_pk_dict  # noqa: E402
+from tests.plonk_verifier import scalar_delta  # noqa: E402
 
 SEED = 0x41534D42
 
@@ -54,7 +56,7 @@ def _sigma_pair(eng, field: str, cols: int, k: int, copies, mapping, mont: bool)
     """The sigma columns from the copies and from the mapping, downloaded."""
     m = pasta.FIELDS[field]
     conv = (lambda x: (x << 256) % m) if mont else (lambda x: x)
-    w, d = conv(pasta.omega_for_k(field, k)), conv(delta_of(m))
+    w, d = conv(pasta.omega_for_k(field, k)), conv(scalar_delta(m))
     a = [eng.ResidentPoly(field, 1 << k) for _ in range(cols)]
     b = [eng.ResidentPoly(field, 1 << k) for _ in range(cols)]
     try:
@@ -111,7 +113,7 @@ def test_keygen_vk_from_copies_reproduces_the_golden_commitments(eng, goldens):
         cc = eng.CopyConstraints(circ.N, 12)
         for cp in plonk_api_copies():
             cc.copy(*cp)
-        fc, pc = eng.keygen_vk(prm, D, circ.fixed_columns(m, ZETA), cc, delta_of(m))
+        fc, pc = eng.keygen_vk(prm, D, circ.fixed_columns(m, ZETA), cc, scalar_delta(m))
         assert [cref.bytes_to_affine(x) for x in np.concatenate([fc, pc])] == want
     finally:
         prm.close()
@@ -160,7 +162,7 @@ def test_sigma_from_copies_large(eng, field):
 def _error_cases(eng):
     field, k, n = "fp", 4, 16
     m = pasta.P_MOD
-    omega, delta = pasta.omega_for_k(field, k), delta_of(m)
+    omega, delta = pasta.omega_for_k(field, k), scalar_delta(m)
     ident = np.stack(np.meshgrid(np.arange(2), np.arange(n), indexing="ij"), axis=-1).astype(np.uint32)
     good = [(0, 1, 1, 2), (1, 2, 0, 5), (0, 5, 0, 5)]
     want = [cref.ints_to_bytes(col) for col in oracle_sigma(orc.assembly(good, 2, k)[0], n, omega, delta, m)]
@@ -232,7 +234,7 @@ def test_benchmark_circuit_proof_from_copies_k14(eng):
     from tests import prover_replay as R
     k = 14
     m = pasta.P_MOD
-    delta = delta_of(m)
+    delta = scalar_delta(m)
     prm = _bench_params(eng, k)
     keys = []
     try:
@@ -251,7 +253,7 @@ def test_benchmark_circuit_proof_from_copies_k14(eng):
             T = R.Blake2bTranscript(m)
             PP.create_proof_engine(eng, prm, vk, None, None, [ab], [[]], MC.SeededRng("fp", 5, True), T, ZETA, delta, pk=prover_pk_dict(keys[-1]))
             proofs.append(bytes(T.proof))
-        assert _dump(keys[0]) == _dump(keys[1])
+        assert prover_pk_bytes(keys[0]) == prover_pk_bytes(keys[1])
         assert proofs[0] == proofs[1]
         arm = PV.EngineArm(eng, "vesta", k, params=prm)
         try:
@@ -271,7 +273,7 @@ def test_benchmark_circuit_proof_from_copies_k14(eng):
 def test_keygen_from_copies_on_two_lanes(eng):
     k = 12
     m = pasta.P_MOD
-    delta = delta_of(m)
+    delta = scalar_delta(m)
     prm = _bench_params(eng, k)
     D = eng.EvaluationDomain("fp", BC.DEGREE, k, ZETA)
     fixed = BC.columns(k, m, D.omega, delta, 7)[0]
@@ -279,7 +281,7 @@ def test_keygen_from_copies_on_two_lanes(eng):
     lib = _lib()
     pk0 = eng.keygen_pk(prm, D, fixed, _bench_assembly(eng, k), delta, BC.BLINDING_FACTORS)
     try:
-        want = _dump(pk0)
+        want = prover_pk_bytes(pk0)
         handles = {}
         meet = threading.Barrier(2, timeout=300)
 
@@ -288,7 +290,7 @@ def test_keygen_from_copies_on_two_lanes(eng):
                 with eng.Lane():
                     pk = eng.keygen_pk(prm, D, fixed, cc, delta, BC.BLINDING_FACTORS)
                     try:
-                        got = _dump(pk)
+                        got = prover_pk_bytes(pk)
                         handles[i] = pk.permutation.permutations[0]._h.value
                         meet.wait()
                         foreign = [lib.h2_poly_download(ctypes.c_uint64(h), None, ctypes.c_size_t(0), 0) != 0 and "unknown" in _err()

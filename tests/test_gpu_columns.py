@@ -192,12 +192,12 @@ def _params(curve, k):
 
 def test_phases_of_the_plonk_api_circuit():
     from tests import plonk_verifier as PV
-    from tests import test_real_proof as TR
-    vk = PV.PinnedKey(TR.CASE["key_text"])
+    from tests import plonk_api_circuit as circ
+    vk = PV.PinnedKey(circ.CASE["key_text"])
     prm = _params("vesta", vk.k)
-    advice, instances = [TR.witness(), TR.witness()], [[[2]], [[2]]]
-    want = CC.engine_phases(halo2_b200, prm, vk, advice, instances, 777, TR.ZETA)
-    CC.assert_same(want, CC.batched_phases(halo2_b200, prm, vk, advice, instances, 777, TR.ZETA))
+    advice, instances = [circ.witness(), circ.witness()], [[[2]], [[2]]]
+    want = CC.engine_phases(halo2_b200, prm, vk, advice, instances, 777, circ.ZETA)
+    CC.assert_same(want, CC.batched_phases(halo2_b200, prm, vk, advice, instances, 777, circ.ZETA))
     prm.close()
 
 

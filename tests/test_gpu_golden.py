@@ -9,7 +9,7 @@ import pytest
 pytestmark = pytest.mark.gpu
 
 from oracle import cref, pasta  # noqa: E402
-from tests.test_oracle_golden import golden_columns  # noqa: E402
+from tests.plonk_api_circuit import golden_columns  # noqa: E402
 
 
 @pytest.fixture(scope="module")

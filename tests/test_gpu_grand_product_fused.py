@@ -1,7 +1,7 @@
 """GPU tests of the product columns in one call per argument (h2_poly_permutation_product, h2_poly_lookup_product;
 halo2_b200.permutation_commit / lookup_commit_product):
 
-- the products equal the reference's loops restated with big integers (tests/test_grand_product_oracle.py) element for
+- the products equal the reference's loops restated with big integers (tests/grand_product_cases.py) element for
   element, both fields, k = 1, 4, 8, 11, several proofs, sets and lookups per call;
 - at k = 14, 16, 18 and 20 the z columns and their commitments are byte-identical to the composition the engine-API prover
   uses (Ast programs, batch_invert, running_product, the host's last_z);
@@ -20,9 +20,13 @@ pytestmark = pytest.mark.gpu
 from oracle import cref, pasta  # noqa: E402
 from tests import bench_circuit as BC  # noqa: E402
 from tests import plonk_api_circuit as circ  # noqa: E402
-from tests.test_gpu_lanes import _run_parallel  # noqa: E402
-from tests.test_grand_product_oracle import delta_of, oracle_lookup_product, oracle_permutation_product  # noqa: E402
-from tests.test_keygen_oracle import ZETA, bench_copies, prover_pk_dict  # noqa: E402
+from tests.abi_cases import _err, _run_parallel  # noqa: E402
+from tests.bench_circuit import _bench_params, bench_copies  # noqa: E402
+from tests.grand_product_cases import (_close, composition_lookup, composition_permutation, oracle_lookup_product,  # noqa: E402
+                                       oracle_permutation_product)
+from tests.plonk_api_circuit import ZETA  # noqa: E402
+from tests.plonk_prover import prover_pk_dict  # noqa: E402
+from tests.plonk_verifier import scalar_delta  # noqa: E402
 
 SEED = 0x46555345
 
@@ -33,77 +37,6 @@ def eng():
     from halo2_b200 import lib as L
     L.init()
     return halo2_b200
-
-
-def _err() -> str:
-    from halo2_b200 import lib as L
-    return L.load().h2_last_error().decode()
-
-
-def _params(eng, k: int):
-    n = 1 << k
-    pts = cref.gen_points("vesta", 99, n + 2)
-    return eng.Params("vesta", k, pts[:n], eng.lagrange_generators("vesta", k, pts[:n]), pts[n:n + 1], u=pts[n + 1:n + 2])
-
-
-def _close(*groups):
-    for g in groups:
-        for p in g:
-            p.close()
-
-
-# ---- the existing composition (tests/plonk_prover.create_proof_engine, the permutation and lookup product steps) ---------
-def composition_permutation(eng, D, columns, sigmas, beta, gamma, delta, chunk_len, bf, blinding):
-    """Per proof, per set: the Ast denominators, batch_invert, the Ast numerators, running_product from last_z, the blinding
-    rows written, last_z read back.  Returns z[p][a] (resident)."""
-    Ast, m, n = eng.Ast, D.m, D.n
-    ev = eng.Evaluator(D, "lagrange")
-    SL = [ev.register_poly(s) for s in sigmas]
-    out, at, tmp = [], 0, []
-    for cols in columns:
-        CL = [ev.register_poly(c) for c in cols]
-        sets, last_z = [], 1
-        for c0 in range(0, len(sigmas), chunk_len):
-            den = None
-            for cl, sl in zip(CL[c0:c0 + chunk_len], SL[c0:c0 + chunk_len]):
-                term = sl * beta + Ast.constant_term(gamma) + cl
-                den = term if den is None else den * term
-            inv_den = eng.batch_invert_resident(ev.evaluate(den, out=eng.ResidentPoly(D.field, n)))
-            num = ev.register_poly(inv_den)
-            for j, cl in enumerate(CL[c0:c0 + chunk_len]):
-                num = num * (Ast.linear_term(pow(delta, c0 + j, m) * beta % m) + Ast.constant_term(gamma) + cl)
-            mv = ev.evaluate(num, out=eng.ResidentPoly(D.field, n))
-            z = eng.running_product_resident(mv, init=last_z, dst=eng.ResidentPoly(D.field, n))
-            if bf:
-                z.copy_from(eng.ResidentPoly(D.field, bf, cref.ints_to_bytes(blinding[at:at + bf])), bf, dst_off=n - bf)
-            at += bf
-            one = eng.ResidentPoly(D.field, 1).copy_from(z, 1, src_off=n - bf - 1)     # last_z: one element back to the host
-            last_z = int.from_bytes(one.download(1)[0].tobytes(), "little")
-            tmp += [inv_den, mv, one]
-            sets.append(z)
-        out.append(sets)
-    _close(tmp)
-    ev.close()
-    return out
-
-
-def composition_lookup(eng, D, lookups, beta, gamma, bf, blinding):
-    Ast, n = eng.Ast, D.n
-    ev = eng.Evaluator(D, "lagrange")
-    out, tmp = [], []
-    for b, (ci, ct, pi, pt) in enumerate(lookups):
-        CI, CT, PI, PT = (ev.register_poly(p) for p in (ci, ct, pi, pt))
-        inv_den = eng.batch_invert_resident(ev.evaluate((PI + Ast.constant_term(beta)) * (PT + Ast.constant_term(gamma)), out=eng.ResidentPoly(D.field, n)))
-        num = ev.register_poly(inv_den) * (CI + Ast.constant_term(beta)) * (CT + Ast.constant_term(gamma))
-        mv = ev.evaluate(num, out=eng.ResidentPoly(D.field, n))
-        z = eng.running_product_resident(mv, init=1, dst=eng.ResidentPoly(D.field, n))
-        if bf:
-            z.copy_from(eng.ResidentPoly(D.field, bf, cref.ints_to_bytes(blinding[b * bf:(b + 1) * bf])), bf, dst_off=n - bf)
-        tmp += [inv_den, mv]
-        out.append(z)
-    _close(tmp)
-    ev.close()
-    return out
 
 
 # ---- 1. against the restatement ----------------------------------------------------------------------------------------
@@ -121,10 +54,10 @@ def test_permutation_product_against_the_restatement(eng, field, k):
             val[-1][0][n // 2] = (-(beta * sig[0][n // 2] + gamma)) % m          # a zero denominator
         sets = -(-cols // chunk_len)
         blinding = pasta.gen_scalars(field, seed + 9, proofs * sets * bf) if bf else []
-        want = oracle_permutation_product(val, sig, beta, gamma, D.omega, delta_of(m), chunk_len, bf, blinding, m)
+        want = oracle_permutation_product(val, sig, beta, gamma, D.omega, scalar_delta(m), chunk_len, bf, blinding, m)
         S = [eng.ResidentPoly(field, n, cref.ints_to_bytes(s)) for s in sig]
         C = [[eng.ResidentPoly(field, n, cref.ints_to_bytes(v)) for v in per] for per in val]
-        z = eng.permutation_product_resident(D, C, S, beta, gamma, delta_of(m), chunk_len, bf, blinding)
+        z = eng.permutation_product_resident(D, C, S, beta, gamma, scalar_delta(m), chunk_len, bf, blinding)
         got = [[cref.bytes_to_ints(q.download()) for q in per] for per in z]
         _close(S, *C, *z)
         assert got == want, (proofs, cols, chunk_len, bf)
@@ -161,8 +94,8 @@ SHAPES = {"benchmark": (3, 3), "wide": (16, 3)}                             # (c
 def test_same_bytes_as_the_composition(eng, k):
     field, m, n, bf = "fp", pasta.P_MOD, 1 << k, BC.BLINDING_FACTORS
     D = eng.EvaluationDomain(field, BC.DEGREE, k, ZETA)
-    prm = _params(eng, k)
-    delta = delta_of(m)
+    prm = _bench_params(eng, k)
+    delta = scalar_delta(m)
     beta, gamma = pasta.gen_scalars(field, SEED + k, 2)
     try:
         for name, (cols, chunk_len) in SHAPES.items():
@@ -195,27 +128,6 @@ def test_same_bytes_as_the_composition(eng, k):
 
 
 # ---- 3. real proofs -----------------------------------------------------------------------------------------------------
-class RecordingRng:
-    def __init__(self, inner):
-        self.inner, self.draws = inner, []
-
-    def scalar(self):
-        x = self.inner.scalar()
-        self.draws.append(x)
-        return x
-
-    def poly(self, n):
-        return self.inner.poly(n)
-
-
-class ReplayRng:
-    def __init__(self, draws):
-        self.draws = list(draws)
-
-    def scalar(self):
-        return self.draws.pop(0)
-
-
 class RecordingTranscript:
     """Passes every call through; records the challenges and, on every point written, calls on_point(index)."""
     def __init__(self, inner, on_point=None):
@@ -236,22 +148,14 @@ class RecordingTranscript:
         return getattr(self.inner, name)
 
 
-def _encode(points, m) -> bytes:
-    from tests import prover_replay as R
-    T = R.Blake2bTranscript(m)
-    for p in points:
-        T.write_point(p)
-    return bytes(T.proof)
-
-
 def test_benchmark_proof_k14_contains_the_permutation_commitments(eng):
     from tests import multiopen_cases as MC
     from tests import plonk_prover as PP
     from tests import plonk_verifier as PV
     from tests import prover_replay as R
     k, m = 14, pasta.P_MOD
-    n, delta = 1 << k, delta_of(m)
-    prm = _params(eng, k)
+    n, delta = 1 << k, scalar_delta(m)
+    prm = _bench_params(eng, k)
     pk = None
     try:
         D = eng.EvaluationDomain("fp", BC.DEGREE, k, ZETA)
@@ -262,7 +166,7 @@ def test_benchmark_proof_k14_contains_the_permutation_commitments(eng):
         A = cref.bytes_to_affine
         vk = PV.PinnedKey(BC.pinned_key_text(k, D.extended_k, pasta.Q_MOD, m, D.omega, [A(x) for x in fc], [A(x) for x in pc]))
         pk = eng.keygen_pk(prm, D, fixed, cc, delta, BC.BLINDING_FACTORS)
-        rng = RecordingRng(MC.SeededRng("fp", 11, True))
+        rng = MC.RecordingRng(MC.SeededRng("fp", 11, True))
         T = RecordingTranscript(R.Blake2bTranscript(m))
         ab = [cref.ints_to_bytes(c) for c in adv]
         PP.create_proof_engine(eng, prm, vk, None, None, [ab], [[]], rng, T, ZETA, delta, pk=prover_pk_dict(pk))
@@ -275,9 +179,9 @@ def test_benchmark_proof_k14_contains_the_permutation_commitments(eng):
         cols = [{"Advice": adv_l, "Fixed": pk.fixed_values}[t][i] for t, i in vk.permutation_columns]
         beta, gamma = T.challenges[1], T.challenges[2]                          # theta, beta, gamma
         chunk_len = vk.degree() - 2
-        sets, cm = eng.permutation_commit(prm, D, pk, [cols], beta, gamma, delta, chunk_len, bf, ReplayRng(rng.draws[nadv * (n - usable) + nadv:]))
+        sets, cm = eng.permutation_commit(prm, D, pk, [cols], beta, gamma, delta, chunk_len, bf, MC.ReplayRng(rng.draws[nadv * (n - usable) + nadv:]))
         at = 32 * nadv                                                          # the advice commitments come first
-        assert proof[at:at + 32 * len(cm)] == _encode(cm, m)
+        assert proof[at:at + 32 * len(cm)] == R._encode(cm, m)
         assert len(sets) == 1 and len(sets[0]) == len(cm) == -(-len(vk.permutation_columns) // chunk_len)
         _close(adv_l, [q for s in sets[0] for q in s[:2]])
     finally:
@@ -291,9 +195,8 @@ def test_plonk_api_lookup_products_equal_the_provers(eng):
     from tests import plonk_prover as PP
     from tests import plonk_verifier as PV
     from tests import prover_replay as R
-    from tests import test_real_proof as TR
-    vk = PV.PinnedKey(TR.CASE["key_text"])
-    k, n, M = 5, 32, TR.M
+    vk = PV.PinnedKey(circ.CASE["key_text"])
+    k, n, M = 5, 32, circ.M
     bf = vk.blinding_factors()
     prm = eng.Params.new("vesta", k)
     seen = {"perm": [], "z": []}
@@ -315,7 +218,7 @@ def test_plonk_api_lookup_products_equal_the_provers(eng):
             return z
 
     snaps = []
-    rng = RecordingRng(MC.SeededRng("fp", 777, True))
+    rng = MC.RecordingRng(MC.SeededRng("fp", 777, True))
     nsets = -(-len(vk.permutation_columns) // (vk.degree() - 2))
 
     def on_point(i):                                            # a product column's commitment: snapshot it and its inputs
@@ -325,10 +228,10 @@ def test_plonk_api_lookup_products_equal_the_provers(eng):
     T = RecordingTranscript(R.Blake2bTranscript(M), on_point)
     try:
         inst = [[[2]], [[2]]]
-        PP.create_proof_engine(Eng(), prm, vk, circ.fixed_columns(M, TR.ZETA), circ.permutation_columns(M, vk.omega, TR.DELTA),
-                               [TR.witness(), TR.witness()], inst, rng, T, TR.ZETA, TR.DELTA)
+        PP.create_proof_engine(Eng(), prm, vk, circ.fixed_columns(M, circ.ZETA), circ.permutation_columns(M, vk.omega, circ.DELTA),
+                               [circ.witness(), circ.witness()], inst, rng, T, circ.ZETA, circ.DELTA)
         assert len(vk.lookups) >= 1 and len(snaps) == 2 * len(vk.lookups)
-        D = eng.EvaluationDomain("fp", vk.degree(), k, TR.ZETA)
+        D = eng.EvaluationDomain("fp", vk.degree(), k, circ.ZETA)
         beta, gamma = T.challenges[1], T.challenges[2]
         cols = [tuple(eng.ResidentPoly("fp", n, c) for c in s[1]) for s in snaps]
         z = eng.lookup_product_resident(D, [cols[:len(vk.lookups)], cols[len(vk.lookups):]], beta, gamma, bf, [x for s in snaps for x in s[2]])
@@ -343,8 +246,8 @@ def test_plonk_api_lookup_products_equal_the_provers(eng):
 def test_shared_key_sigma_on_a_lane(eng):
     from halo2_b200 import lib as L
     k, m = 10, pasta.P_MOD
-    n, delta = 1 << k, delta_of(m)
-    prm = _params(eng, k)
+    n, delta = 1 << k, scalar_delta(m)
+    prm = _bench_params(eng, k)
     D = eng.EvaluationDomain("fp", BC.DEGREE, k, ZETA)
     cc = eng.CopyConstraints(n, 3)
     cc.extend(np.array(list(bench_copies(k)), dtype=np.uint32))

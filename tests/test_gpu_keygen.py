@@ -20,10 +20,12 @@ pytestmark = pytest.mark.gpu
 from oracle import cref, pasta  # noqa: E402
 from tests import bench_circuit as BC  # noqa: E402
 from tests import plonk_api_circuit as circ  # noqa: E402
-from tests.test_gpu_lanes import _run_parallel  # noqa: E402
-from tests.test_keygen_oracle import (ZETA, bench_copies, delta_of, oracle_sigma, plonk_api_copies, prover_pk_dict,  # noqa: E402
-                                      random_mapping)
-from tests.test_oracle_golden import golden_columns  # noqa: E402
+from tests.abi_cases import _err, _lib, _run_parallel, _sigma_call  # noqa: E402
+from tests.bench_circuit import _bench_assembly, _bench_params  # noqa: E402
+from tests.keygen_cases import oracle_sigma, random_mapping  # noqa: E402
+from tests.plonk_api_circuit import ZETA, golden_columns, plonk_api_copies  # noqa: E402
+from tests.plonk_prover import prover_pk_bytes, prover_pk_dict  # noqa: E402
+from tests.plonk_verifier import scalar_delta  # noqa: E402
 
 SEED = 0x4B455947
 
@@ -36,51 +38,12 @@ def eng():
     return halo2_b200
 
 
-def _lib():
-    from halo2_b200 import lib as L
-    return L.load()
-
-
-def _err() -> str:
-    return _lib().h2_last_error().decode()
-
-
-def _sigma_call(polys, k: int, mapping, omega: int, delta: int, repr_: int = 0, cols=None) -> int:
-    """h2_poly_permutation_sigma on raw handles / mapping; omega and delta as given (already in `repr_`)."""
-    from halo2_b200 import lib as L
-    hs = [p if isinstance(p, int) else p._h.value for p in polys]
-    arr = (ctypes.c_uint64 * max(len(hs), 1))(*hs)
-    mp = None if mapping is None else np.ascontiguousarray(mapping, dtype=np.uint32)
-    return _lib().h2_poly_permutation_sigma(arr if hs else None, ctypes.c_size_t(len(hs) if cols is None else cols), ctypes.c_uint32(k),
-                                            None if mp is None else mp.ctypes.data_as(ctypes.c_void_p), L.ptr(L.fe_bytes(omega)),
-                                            L.ptr(L.fe_bytes(delta)), repr_)
-
-
 def _device_sigma(eng, field: str, mapping, k: int, omega: int, delta: int, mont: bool):
     m = pasta.FIELDS[field]
     conv = (lambda x: (x << 256) % m) if mont else (lambda x: x)
     polys = [eng.ResidentPoly(field, 1 << k) for _ in range(mapping.shape[0])]
     assert _sigma_call(polys, k, mapping, conv(omega), conv(delta), 1 if mont else 0) == 0, _err()
     return polys
-
-
-def _bench_params(eng, k: int):
-    n = 1 << k
-    pts = cref.gen_points("vesta", 99, n + 2)
-    g, w, u = pts[:n], pts[n:n + 1], pts[n + 1:n + 2]
-    return eng.Params("vesta", k, g, eng.lagrange_generators("vesta", k, g), w, u=u)
-
-
-def _bench_assembly(eng, k: int):
-    asm = eng.Assembly(1 << k, 3)
-    for cp in bench_copies(k):
-        asm.copy(*cp)
-    return asm
-
-
-def _dump(pk) -> list:
-    d = prover_pk_dict(pk)
-    return [p.download().tobytes() for key in ("fixed_l", "fixed_p", "fixed_c", "sigma_l", "sigma_p", "sigma_c", "l") for p in d[key]]
 
 
 # ---- the reference's golden verifying key -------------------------------------------------------------------------------
@@ -94,7 +57,7 @@ def test_keygen_vk_reproduces_the_golden_commitments(eng, goldens):
         asm = eng.Assembly(circ.N, 12)
         for cp in plonk_api_copies():
             asm.copy(*cp)
-        fc, pc = eng.keygen_vk(prm, D, circ.fixed_columns(m, ZETA), asm, delta_of(m))
+        fc, pc = eng.keygen_vk(prm, D, circ.fixed_columns(m, ZETA), asm, scalar_delta(m))
         assert fc.shape == (7, 64) and pc.shape == (12, 64)
         assert [cref.bytes_to_affine(x) for x in np.concatenate([fc, pc])] == want
     finally:
@@ -106,7 +69,7 @@ def test_keygen_vk_reproduces_the_golden_commitments(eng, goldens):
 def test_sigma_every_element(eng, field):
     m = pasta.FIELDS[field]
     rng = np.random.default_rng(SEED)
-    delta = delta_of(m)
+    delta = scalar_delta(m)
     for k in range(1, 17):
         n = 1 << k
         omega = pasta.omega_for_k(field, k)
@@ -134,7 +97,7 @@ def test_sigma_every_element(eng, field):
 def _sampled(eng, field, k, cols, rng, mont, samples=4096):
     m = pasta.FIELDS[field]
     n = 1 << k
-    omega, delta = pasta.omega_for_k(field, k), delta_of(m)
+    omega, delta = pasta.omega_for_k(field, k), scalar_delta(m)
     perm = rng.permutation(cols * n)
     mp = np.stack([perm // n, perm % n], axis=-1).astype(np.uint32).reshape(cols, n, 2)
     polys = _device_sigma(eng, field, mp, k, omega, delta, mont)
@@ -164,7 +127,7 @@ def test_sigma_several_launches_per_column(eng):
 def _error_cases(eng):
     field, k, n = "fp", 4, 16
     m = pasta.P_MOD
-    omega, delta = pasta.omega_for_k(field, k), delta_of(m)
+    omega, delta = pasta.omega_for_k(field, k), scalar_delta(m)
     ident = np.stack(np.meshgrid(np.arange(2), np.arange(n), indexing="ij"), axis=-1).astype(np.uint32)
     want = [cref.ints_to_bytes(col) for col in oracle_sigma(ident, n, omega, delta, m)]
     a, b = eng.ResidentPoly(field, n), eng.ResidentPoly(field, n)
@@ -219,7 +182,7 @@ def test_benchmark_circuit_key_and_proof_k14(eng):
     from tests import prover_replay as R
     k = 14
     m = pasta.P_MOD
-    delta = delta_of(m)
+    delta = scalar_delta(m)
     prm = _bench_params(eng, k)
     pk = None
     try:
@@ -258,7 +221,7 @@ def test_benchmark_circuit_key_and_proof_k14(eng):
 def test_keygen_pk_on_two_lanes(eng):
     k = 12
     m = pasta.P_MOD
-    delta = delta_of(m)
+    delta = scalar_delta(m)
     prm = _bench_params(eng, k)
     D = eng.EvaluationDomain("fp", BC.DEGREE, k, ZETA)
     fixed = BC.columns(k, m, D.omega, delta, 7)[0]
@@ -266,7 +229,7 @@ def test_keygen_pk_on_two_lanes(eng):
     lib = _lib()
     pk0 = eng.keygen_pk(prm, D, fixed, asm, delta, BC.BLINDING_FACTORS)
     try:
-        want = _dump(pk0)
+        want = prover_pk_bytes(pk0)
         handles = {}
         meet = threading.Barrier(2, timeout=300)
 
@@ -275,7 +238,7 @@ def test_keygen_pk_on_two_lanes(eng):
                 with eng.Lane():
                     pk = eng.keygen_pk(prm, D, fixed, asm, delta, BC.BLINDING_FACTORS)
                     try:
-                        got = _dump(pk)
+                        got = prover_pk_bytes(pk)
                         handles[i] = pk.permutation.cosets[0]._h.value
                         meet.wait()                                     # both keys exist
                         foreign = [lib.h2_poly_download(ctypes.c_uint64(h), None, ctypes.c_size_t(0), 0) != 0 and "unknown" in _err()

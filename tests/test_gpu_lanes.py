@@ -14,6 +14,7 @@ pytestmark = pytest.mark.gpu
 
 from oracle import cref, pasta  # noqa: E402
 from tests import prover_replay as R  # noqa: E402
+from tests.abi_cases import _bind, _create, _destroy, _err, _lib, _run_parallel  # noqa: E402
 
 SEED = 0x4C414E4553
 MAX_LANES = 16          # include/halo2_b200.h
@@ -27,32 +28,9 @@ def eng():
     return halo2_b200
 
 
-def _lib():
-    from halo2_b200 import lib as L
-    return L.load()
-
-
-def _err() -> str:
-    return _lib().h2_last_error().decode()
-
-
 def _device() -> int:
     from halo2_b200 import lib as L
     return L._inited_device
-
-
-def _create() -> int:
-    h = ctypes.c_uint64(0)
-    assert _lib().h2_lane_create(ctypes.byref(h)) == 0, _err()
-    return h.value
-
-
-def _bind(h: int) -> int:
-    return _lib().h2_lane_bind(ctypes.c_uint64(h))
-
-
-def _destroy(h: int) -> int:
-    return _lib().h2_lane_destroy(ctypes.c_uint64(h))
 
 
 def _plan():
@@ -80,27 +58,6 @@ def _in_thread(fn):
     if "e" in box:
         raise box["e"]
     return box.get("r")
-
-
-def _run_parallel(fns):
-    """Runs every fn on its own host thread at once; returns the results in order, or raises the first exception."""
-    res, errs = [None] * len(fns), []
-    start = threading.Barrier(len(fns))
-
-    def run(i):
-        try:
-            start.wait()
-            res[i] = fns[i]()
-        except BaseException as e:  # noqa: BLE001
-            errs.append(e)
-    th = [threading.Thread(target=run, args=(i,)) for i in range(len(fns))]
-    for t in th:
-        t.start()
-    for t in th:
-        t.join()
-    if errs:
-        raise errs[0]
-    return res
 
 
 # ---- lifecycle and errors ---------------------------------------------------------------------------------------------

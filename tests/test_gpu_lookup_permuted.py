@@ -15,7 +15,8 @@ import pytest
 pytestmark = pytest.mark.gpu
 
 from oracle import cref, pasta  # noqa: E402
-from tests.test_gpu_lanes import _run_parallel  # noqa: E402
+from tests.abi_cases import _err, _run_parallel  # noqa: E402
+from tests.lookup_permuted_cases import columns, composition  # noqa: E402
 
 SEED = 0x4C4B5032
 
@@ -28,43 +29,10 @@ def eng():
     return halo2_b200
 
 
-def _err() -> str:
-    from halo2_b200 import lib as L
-    return L.load().h2_last_error().decode()
-
-
 def _close(*groups):
     for g in groups:
         for p in g:
             p.close()
-
-
-def columns(field, n, u, seed, hot):
-    """(input, table) as (n, 32) canonical bytes: a full-width table, the input drawn from its usable rows (hot: 90 % of
-    the rows on its first value), random rows past u."""
-    rnd = np.random.default_rng(seed)
-    tab = cref.gen_scalars(field, seed, n)
-    pick = rnd.integers(0, u, size=n)
-    if hot:
-        pick[rnd.random(n) < 0.9] = 0
-    inp = tab[pick].copy()
-    inp[u:] = cref.gen_scalars(field, seed + 1, n - u)
-    return np.ascontiguousarray(inp), np.ascontiguousarray(tab)
-
-
-def composition(eng, D, pairs, bf, blinding):
-    """What tests/plonk_prover.create_proof_engine does per lookup: h2_poly_lookup_permute over the usable rows, then the
-    blinding rows uploaded into rows [u, n)."""
-    rows, n = bf + 1, D.n
-    out = []
-    for b, (a, t) in enumerate(pairs):
-        pi, pt = eng.permute_expression_pair_resident(a, t, n - rows, eng.ResidentPoly(D.field, n), eng.ResidentPoly(D.field, n))
-        for q, vals in ((pi, blinding[2 * rows * b:2 * rows * b + rows]), (pt, blinding[2 * rows * b + rows:2 * rows * (b + 1)])):
-            tmp = eng.ResidentPoly(D.field, rows, cref.ints_to_bytes(vals))
-            q.copy_from(tmp, rows, src_off=0, dst_off=n - rows)
-            tmp.close()
-        out.append((pi, pt))
-    return out
 
 
 CASES = [(k, (1, 3, 16)[k % 3]) for k in range(4, 21)] + [(20, 16), (14, 1), (11, 3)]
@@ -113,23 +81,24 @@ def test_plonk_api_proof(eng):
     """The plonk_api circuit (k = 5, two proofs, lookups): lookup_commit_permuted, fed the recorded theta and draws, gives the
     permuted commitments at their offsets in the proof bytes, and lookup_commit_product, given its result as it is and the
     recorded beta, gamma and draws, gives the lookup product commitments."""
-    from tests.test_gpu_grand_product_fused import ReplayRng, _encode, _params
-    from tests.test_lookup_permuted_oracle import plonk_api_key, plonk_api_lookups, plonk_api_proof
-    from tests import test_real_proof as TR
-    vk = plonk_api_key()
+    from tests import bench_circuit as BC
+    from tests import multiopen_cases as MC
+    from tests import plonk_api_circuit as circ
+    from tests import prover_replay as R
+    vk = circ.plonk_api_key()
     bf, L = vk.blinding_factors(), len(vk.lookups)
-    prm = _params(eng, 5)
+    prm = BC._bench_params(eng, 5)
     try:
-        proof, seen = plonk_api_proof(eng, prm)
-        D, ev, lookups = plonk_api_lookups(eng, seen)
-        perm, cm = eng.lookup_commit_permuted(prm, D, ev, lookups, seen["theta"], bf, ReplayRng(seen["draws"][seen["draws_at_theta"]:]))
+        proof, seen = circ.plonk_api_proof(eng, prm)
+        D, ev, lookups = circ.plonk_api_lookups(eng, seen)
+        perm, cm = eng.lookup_commit_permuted(prm, D, ev, lookups, seen["theta"], bf, MC.ReplayRng(seen["draws"][seen["draws_at_theta"]:]))
         at = seen["points_at_theta"]
-        assert len(cm) == 2 * 2 * L and proof[32 * at:32 * (at + len(cm))] == _encode(cm, TR.M)
+        assert len(cm) == 2 * 2 * L and proof[32 * at:32 * (at + len(cm))] == R._encode(cm, circ.M)
         nsets = -(-len(vk.permutation_columns) // (vk.degree() - 2))
         first = at + len(cm) + 2 * nsets                            # the lookup products follow the permutation products
         beta, gamma = seen["challenges"][1], seen["challenges"][2]
-        z, zcm = eng.lookup_commit_product(prm, D, perm, beta, gamma, bf, ReplayRng(seen["draws"][seen["point_draws"][first - 1]:]))
-        assert len(zcm) == 2 * L and proof[32 * first:32 * (first + len(zcm))] == _encode(zcm, TR.M)
+        z, zcm = eng.lookup_commit_product(prm, D, perm, beta, gamma, bf, MC.ReplayRng(seen["draws"][seen["point_draws"][first - 1]:]))
+        assert len(zcm) == 2 * L and proof[32 * first:32 * (first + len(zcm))] == R._encode(zcm, circ.M)
         _close([p for per in perm for q in per for p in q[:8]], ev.polys, [q[0] for per in z for q in per])
     finally:
         prm.close()

@@ -25,14 +25,13 @@ def eng():
 
 def test_roundtrip_and_identical_queries_device(eng):
     """multiopen.rs:278-373, :375-481 with Params::<EqAffine>::new(4) derived on the device."""
-    from tests.test_multiopen_oracle import _roundtrip
     prm = eng.Params.new("vesta", 4)
     g, gl, w, u = prm.g, prm.g_lagrange, prm.w, prm.u
     prm.close()
     side = MC.EngineSide(eng, "vesta", 4, g, w, u, g_lagrange=gl)
     try:
-        got = _roundtrip(side, "fp")
-        want = _roundtrip(MC.OracleSide("vesta", 4, g, w, u), "fp")
+        got = MC.roundtrip(side, "fp")
+        want = MC.roundtrip(MC.OracleSide("vesta", 4, g, w, u), "fp")
         assert got == want
         p = eng.ResidentPoly("fp", 16, cref.ints_to_bytes(list(range(16))))
         with pytest.raises(ValueError):

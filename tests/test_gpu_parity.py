@@ -9,6 +9,7 @@ import pytest
 pytestmark = pytest.mark.gpu
 
 from oracle import cref, pasta  # noqa: E402
+from tests.ast_cases import _ast_tuple  # noqa: E402
 from tests.poseidon_kat import permute  # noqa: E402
 
 SEED = 0x48414C4F32
@@ -867,19 +868,6 @@ def test_poly_reductions(eng, field):
 
 
 # ------------------------------------------------------------------------------------------ K15
-def _ast_tuple(node):
-    k, a = node.kind, node.args
-    if k == "poly":
-        return ("poly", a[0], a[1])
-    if k in ("add", "mul"):
-        return (k, _ast_tuple(a[0]), _ast_tuple(a[1]))
-    if k == "scale":
-        return ("scale", _ast_tuple(a[0]), a[1])
-    if k == "dp":
-        return ("dp", [_ast_tuple(t) for t in a[0]], a[1])
-    return (k, a[0])
-
-
 @pytest.mark.parametrize("field", ["fp", "fq"])
 def test_ast_evaluator_and_quotient_pipeline(eng, field):
     """Evaluator::evaluate (poly/evaluator.rs:129-228) on the device against the restated tree walk, in both bases; then the

@@ -19,7 +19,7 @@ import pytest
 pytestmark = pytest.mark.gpu
 
 from oracle import cref  # noqa: E402
-from tests.test_gpu_lanes import _bind, _create, _destroy, _err, _lib  # noqa: E402
+from tests.abi_cases import _bind, _create, _destroy, _err, _lib  # noqa: E402
 
 SEED = 0x41524753
 K, N = 6, 1 << 6

@@ -16,6 +16,7 @@ import pytest
 pytestmark = pytest.mark.gpu
 
 from oracle import cref, pasta  # noqa: E402
+from tests.abi_cases import _err  # noqa: E402
 
 SEED = 0x52455052
 K, N = 4, 1 << 4
@@ -521,11 +522,6 @@ ENTRY_POINTS = [
     "h2_poly_running_product", "h2_poly_divide_by_vanishing", "h2_poly_lookup_permuted", "h2_poly_compute_s", "h2_poly_scale_add",
     "h2_poly_permutation_sigma", "h2_poly_permutation_sigma_copies", "h2_poly_permutation_product", "h2_poly_lookup_product",
 ]
-
-
-def _err():
-    from halo2_b200 import lib as L
-    return L.load().h2_last_error().decode()
 
 
 def _snapshot(torch, outs):

@@ -21,8 +21,11 @@ pytestmark = pytest.mark.gpu
 from oracle import cref, pasta  # noqa: E402
 from tests import bench_circuit as BC  # noqa: E402
 from tests import plonk_api_circuit as circ  # noqa: E402
-from tests.test_gpu_lanes import _bind, _create, _destroy, _err, _lib, _run_parallel  # noqa: E402
-from tests.test_keygen_oracle import ZETA, bench_copies, delta_of, prover_pk_dict  # noqa: E402
+from tests.abi_cases import _bind, _create, _destroy, _err, _lib, _run_parallel  # noqa: E402
+from tests.bench_circuit import bench_copies  # noqa: E402
+from tests.plonk_api_circuit import ZETA  # noqa: E402
+from tests.plonk_prover import prover_pk_bytes, prover_pk_dict  # noqa: E402
+from tests.plonk_verifier import scalar_delta  # noqa: E402
 
 SEED = 0x5348415245
 K, N = 10, 1 << 10
@@ -191,10 +194,10 @@ def _write_calls(eng, S, P):
         ("h2_poly_lookup_permute", lambda: lib.h2_poly_lookup_permute(P["input"]._h, P["table"]._h, ctypes.c_size_t(N - 7), s_lag._h, P["coeff"]._h)),
         ("h2_poly_lookup_permute", lambda: lib.h2_poly_lookup_permute(P["input"]._h, P["table"]._h, ctypes.c_size_t(N - 7), P["coeff"]._h, s_lag._h)),
         ("h2_poly_permutation_sigma", lambda: lib.h2_poly_permutation_sigma(arr(s_lag), ctypes.c_size_t(1), ctypes.c_uint32(K),
-                                                                             ident.ctypes.data_as(ctypes.c_void_p), _fe(dom.omega), _fe(delta_of(M)), 0)),
+                                                                             ident.ctypes.data_as(ctypes.c_void_p), _fe(dom.omega), _fe(scalar_delta(M)), 0)),
         ("h2_poly_permutation_sigma_copies", lambda: lib.h2_poly_permutation_sigma_copies(arr(s_lag), ctypes.c_size_t(1), ctypes.c_uint32(K),
                                                                                            copies.ctypes.data_as(ctypes.c_void_p), ctypes.c_size_t(1),
-                                                                                           _fe(dom.omega), _fe(delta_of(M)), 0)),
+                                                                                           _fe(dom.omega), _fe(scalar_delta(M)), 0)),
     ]
 
 
@@ -372,11 +375,6 @@ def test_shutdown_frees_shared(eng):
 
 
 # ---- 5. end to end ------------------------------------------------------------------------------------------------------
-def _dump(pk) -> list:
-    d = prover_pk_dict(pk)
-    return [p.download().tobytes() for key in ("fixed_l", "fixed_p", "fixed_c", "sigma_l", "sigma_p", "sigma_c", "l") for p in d[key]]
-
-
 def test_shared_key_proves_on_four_lanes_k14(eng):
     from tests import multiopen_cases as MC
     from tests import plonk_prover as PP
@@ -384,7 +382,7 @@ def test_shared_key_proves_on_four_lanes_k14(eng):
     from tests import prover_replay as R
     k = 14
     n = 1 << k
-    delta = delta_of(M)
+    delta = scalar_delta(M)
     pts = cref.gen_points("vesta", 99, n + 2)
     g, w, u = pts[:n], pts[n:n + 1], pts[n + 1:n + 2]
     prm14 = eng.Params("vesta", k, g, eng.lagrange_generators("vesta", k, g), w, u=u)
@@ -416,13 +414,13 @@ def test_shared_key_proves_on_four_lanes_k14(eng):
         keys.append(private)
         want = [[prove(private, s) for s in ss] for ss in seeds]          # serially, private key, primary context
         assert len({p for ps in want for p in ps}) == 8
-        key_bytes = _dump(private)
+        key_bytes = prover_pk_bytes(private)
         # the key built on the primary context and shared
         pk = eng.keygen_pk(prm14, D, fixed, cc, delta, BC.BLINDING_FACTORS)
         keys.append(pk)
         assert pk.share() is pk and all(p.shared for p in pk._all())
         assert on_lanes(pk) == want
-        assert _dump(pk) == key_bytes
+        assert prover_pk_bytes(pk) == key_bytes
         arm = PV.EngineArm(eng, "vesta", k, params=prm14)
         try:
             assert all(PV.verify_proof(arm, vk, p, [[]], delta) for ps in want for p in ps)
@@ -441,7 +439,7 @@ def test_shared_key_proves_on_four_lanes_k14(eng):
             assert _bind(0) == 0
             assert _destroy(lane) == 0, _err()
         assert on_lanes(pk2) == want
-        assert _dump(pk2) == key_bytes
+        assert prover_pk_bytes(pk2) == key_bytes
     finally:
         for key in keys:
             key.close()

@@ -1,6 +1,6 @@
 """GPU checks of h2_poly_vanishing_quotient and halo2_b200.vanishing: the fused call against the existing path
-(divide_by_vanishing_poly + extended_to_coeff + one copy per piece), the module against create_proof_engine's vanishing lines,
-a whole proof composed with the module, the argument checks, cleanup on failure, and a run on a lane over a shared key."""
+(divide_by_vanishing_poly + extended_to_coeff + one copy per piece), a proof composed with the module against
+create_proof_engine, the argument checks, cleanup on failure, and a run on a lane over a shared key."""
 import ctypes
 
 import numpy as np
@@ -10,7 +10,9 @@ import halo2_b200
 from halo2_b200 import lib as L
 from halo2_b200 import vanishing as V
 from oracle import cref, pasta
+from tests import arguments_cases as AC
 from tests import multiopen_cases as MC
+from tests import plonk_api_circuit as circ
 from tests import plonk_prover as PP
 from tests import vanishing_cases as VC
 
@@ -86,11 +88,8 @@ def test_the_bulk_copy_setting_changes_nothing():
 
 
 def _plonk_api():
-    from tests import plonk_api_circuit as circ
-    from tests import plonk_verifier as PV
-    from tests import test_real_proof as TR
-    vk = PV.PinnedKey(TR.CASE["key_text"])
-    return vk, circ.fixed_columns(TR.M, TR.ZETA), circ.permutation_columns(TR.M, vk.omega, TR.DELTA), TR
+    vk = circ.plonk_api_key()
+    return vk, circ.fixed_columns(circ.M, circ.ZETA), circ.permutation_columns(circ.M, vk.omega, circ.DELTA)
 
 
 def _assert_same(want, got):
@@ -102,59 +101,69 @@ def _assert_same(want, got):
     assert want["proof"] == got["proof"]
 
 
+def _engine_and_package(prm, D, vk, fixed, sigma, advice, instances, seed):
+    """VC.record of create_proof_engine and of create_proof_package (over a key from arguments_cases.proving_key) on the same
+    inputs and seeded rng."""
+    engine_pk, pk = {}, AC.proving_key(halo2_b200, D, fixed, sigma, vk.blinding_factors())
+    try:
+        want = VC.record(halo2_b200, circ.M, lambda eng, t: PP.create_proof_engine(eng, prm, vk, fixed, sigma, advice, instances,
+                                                                                  MC.SeededRng("fp", seed, True), t, circ.ZETA, circ.DELTA, pk=engine_pk))
+        got = VC.record(halo2_b200, circ.M, lambda eng, t: AC.create_proof_package(eng, prm, D, pk, vk, advice, instances,
+                                                                                  MC.SeededRng("fp", seed, True), t, circ.DELTA))
+    finally:
+        PP.close_proving_key(engine_pk)
+        pk.close()
+    return want, got
+
+
 def test_the_module_equals_create_proof_engine_on_the_plonk_api_circuit():
-    """Under the golden key and one seeded rng: the random commitment, the h piece commitments (every point written), random_eval
-    (every scalar written), h_poly / h_blind and random_poly / random_blind (the last two queries) and the proof bytes, which
-    the engine's verifier and the restated reference verifier accept."""
+    """Under the golden key and one seeded rng, a proof whose vanishing argument comes from the module (create_proof_package)
+    and create_proof_engine's: the random commitment, the h piece commitments (every point written), random_eval (every scalar
+    written), h_poly / h_blind and random_poly / random_blind (the last two queries) and the proof bytes, which the engine's
+    verifier and the restated reference verifier accept."""
     from tests import plonk_verifier as PV
-    vk, fixed, sigma, TR = _plonk_api()
+    vk, fixed, sigma = _plonk_api()
     prm = halo2_b200.Params.new("vesta", 5)
     try:
         inst = [[[2]], [[2]]]
-        run = lambda prover: VC.record(halo2_b200, prover, prm, vk, fixed, sigma, [TR.witness(), TR.witness()], inst,  # noqa: E731
-                                       MC.SeededRng("fp", 777, True), TR.ZETA, TR.DELTA)
-        want, got = run(PP.create_proof_engine), run(VC.create_proof_module)
+        D = halo2_b200.EvaluationDomain("fp", vk.degree(), vk.k, circ.ZETA)
+        want, got = _engine_and_package(prm, D, vk, fixed, sigma, [circ.witness(), circ.witness()], inst, 777)
         _assert_same(want, got)
         assert len(got["proof"]) == 4160
         gens = (prm.g, prm.g_lagrange, prm.w, prm.u)
         earm = PV.EngineArm(halo2_b200, "vesta", 5, *gens)
         try:
-            assert PV.verify_proof(earm, vk, got["proof"], inst, TR.DELTA)
+            assert PV.verify_proof(earm, vk, got["proof"], inst, circ.DELTA)
         finally:
             earm.close()
-        assert PV.verify_proof(PV.OracleArm("vesta", 5, *gens), vk, got["proof"], inst, TR.DELTA)
+        assert PV.verify_proof(PV.OracleArm("vesta", 5, *gens), vk, got["proof"], inst, circ.DELTA)
     finally:
         prm.close()
 
 
 def test_the_module_equals_create_proof_engine_on_the_benchmark_circuit_k14():
     """The benchmark circuit (benches/plonk.rs, degree 5: four pieces of a 4n extended domain) at k = 14, key built as
-    tests/test_gpu_zz_real_proof.py builds it, two proofs sharing the resident proving key."""
+    tests/test_gpu_zz_real_proof.py builds it; create_proof_engine keeps its own resident key, the package proves over
+    arguments_cases.proving_key's."""
     from tests import bench_circuit as BC
-    from tests import plonk_api_circuit as circ
     from tests import plonk_verifier as PV
-    from tests import test_real_proof as TR
-    k, m = 14, TR.M
+    k, m = 14, circ.M
     n = 1 << k
     pts = cref.gen_points("vesta", 77, n + 2)
     g, w, u = pts[:n], pts[n:n + 1], pts[n + 1:n + 2]
     prm = halo2_b200.Params("vesta", k, g, halo2_b200.lagrange_generators("vesta", k, g), w, u=u)
-    pk = {}
     try:
-        D = halo2_b200.EvaluationDomain("fp", BC.DEGREE, k, TR.ZETA)
+        D = halo2_b200.EvaluationDomain("fp", BC.DEGREE, k, circ.ZETA)
         assert D.quotient_poly_degree == 4 and D.extended_k == k + 2
-        fixed, sigma, adv = BC.columns(k, m, D.omega, TR.DELTA, circ.A_SMALL * TR.ZETA % m)
+        fixed, sigma, adv = BC.columns(k, m, D.omega, circ.DELTA, circ.A_SMALL * circ.ZETA % m)
         fb, sb, ab = ([cref.ints_to_bytes(c_) for c_ in cols] for cols in (fixed, sigma, adv))
         xy = lambda col: cref.bytes_to_affine(halo2_b200.batch_normalize(prm.commit_lagrange(col, halo2_b200.Blind(1)).reshape(1, 96), "vesta")[0])  # noqa: E731
         vk = PV.PinnedKey(BC.pinned_key_text(k, D.extended_k, pasta.Q_MOD, m, D.omega, [xy(c_) for c_ in fb], [xy(c_) for c_ in sb]))
-        run = lambda prover: VC.record(halo2_b200, prover, prm, vk, fb, sb, [ab], [[]], MC.SeededRng("fp", 5, True), TR.ZETA, TR.DELTA,  # noqa: E731
-                                       pk=pk)
-        want, got = run(PP.create_proof_engine), run(VC.create_proof_module)
+        want, got = _engine_and_package(prm, D, vk, fb, sb, [ab], [[]], 5)
         _assert_same(want, got)
         arm = PV.EngineArm(halo2_b200, "vesta", k, params=prm)
-        assert PV.verify_proof(arm, vk, got["proof"], [[]], TR.DELTA)
+        assert PV.verify_proof(arm, vk, got["proof"], [[]], circ.DELTA)
     finally:
-        PP.close_proving_key(pk)
         prm.close()
 
 

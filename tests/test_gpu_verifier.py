@@ -212,8 +212,7 @@ def test_opening_proof_device(eng, curve, k):
         ch_prover = W.squeeze_challenge()
         proof = bytes(W.proof)
         if k <= 4:                                                # the oracle's prover writes the same bytes
-            from tests.test_verifier_oracle import _WriteT
-            OW = _WriteT(r)
+            OW = R._WriteT(r)
             gt = [cref.bytes_to_affine(x_) for x_ in prm.g]
             OW.write_point(cref.bytes_to_affine(p))
             assert OW.squeeze_challenge() == x

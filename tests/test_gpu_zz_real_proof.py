@@ -17,7 +17,6 @@ from tests import plonk_api_circuit as circ  # noqa: E402
 from tests import plonk_prover as PP  # noqa: E402
 from tests import plonk_verifier as PV  # noqa: E402
 from tests import prover_replay as R  # noqa: E402
-from tests import test_real_proof as TR  # noqa: E402
 
 
 def test_real_proof_on_the_device():
@@ -25,33 +24,33 @@ def test_real_proof_on_the_device():
     from halo2_b200 import lib as L
     L.init()
     c = pasta.VESTA
-    vk = PV.PinnedKey(TR.CASE["key_text"])
+    vk = PV.PinnedKey(circ.CASE["key_text"])
     prm = halo2_b200.Params.new("vesta", 5)                          # Params::<EqAffine>::new(5) on the device
     try:
         gens = (prm.g, prm.g_lagrange, prm.w, prm.u)
         P = pasta.Params.from_generators(c, 5, [cref.bytes_to_affine(x) for x in prm.g], cref.bytes_to_affine(prm.w[0]), cref.bytes_to_affine(prm.u[0]))
-        fixed = circ.fixed_columns(TR.M, TR.ZETA)
-        sigma = circ.permutation_columns(TR.M, vk.omega, TR.DELTA)
+        fixed = circ.fixed_columns(circ.M, circ.ZETA)
+        sigma = circ.permutation_columns(circ.M, vk.omega, circ.DELTA)
         inst = [[[2]], [[2]]]
-        want = TR.prove((c, P, vk, fixed, sigma, gens), [TR.witness(), TR.witness()], inst, 777)
-        T = R.Blake2bTranscript(TR.M)
-        PP.create_proof_engine(halo2_b200, prm, vk, fixed, sigma, [TR.witness(), TR.witness()], inst, MC.SeededRng("fp", 777, True), T, TR.ZETA, TR.DELTA)
+        want = circ.prove((c, P, vk, fixed, sigma, gens), [circ.witness(), circ.witness()], inst, 777)
+        T = R.Blake2bTranscript(circ.M)
+        PP.create_proof_engine(halo2_b200, prm, vk, fixed, sigma, [circ.witness(), circ.witness()], inst, MC.SeededRng("fp", 777, True), T, circ.ZETA, circ.DELTA)
         got = bytes(T.proof)
         assert len(got) == 4160
         assert got == want                                           # bit-identical to the oracle's proof
         earm = PV.EngineArm(halo2_b200, "vesta", 5, *gens)
         try:
-            assert PV.verify_proof(earm, vk, got, inst, TR.DELTA)
+            assert PV.verify_proof(earm, vk, got, inst, circ.DELTA)
             bad = bytearray(got)
             bad[2000] ^= 1
-            assert not PV.verify_proof(earm, vk, bytes(bad), inst, TR.DELTA)
+            assert not PV.verify_proof(earm, vk, bytes(bad), inst, circ.DELTA)
         finally:
             earm.close()
-        assert PV.verify_proof(PV.OracleArm("vesta", 5, *gens), vk, got, inst, TR.DELTA)
+        assert PV.verify_proof(PV.OracleArm("vesta", 5, *gens), vk, got, inst, circ.DELTA)
         # a witness that breaks a gate: the device prover still runs, the verifier rejects
-        T2 = R.Blake2bTranscript(TR.M)
-        PP.create_proof_engine(halo2_b200, prm, vk, fixed, sigma, [TR.witness(break_row=5)], [[[2]]], MC.SeededRng("fp", 901, True), T2, TR.ZETA, TR.DELTA)
-        assert not PV.verify_proof(PV.OracleArm("vesta", 5, *gens), vk, bytes(T2.proof), [[[2]]], TR.DELTA)
+        T2 = R.Blake2bTranscript(circ.M)
+        PP.create_proof_engine(halo2_b200, prm, vk, fixed, sigma, [circ.witness(break_row=5)], [[[2]]], MC.SeededRng("fp", 901, True), T2, circ.ZETA, circ.DELTA)
+        assert not PV.verify_proof(PV.OracleArm("vesta", 5, *gens), vk, bytes(T2.proof), [[[2]]], circ.DELTA)
     finally:
         prm.close()
 
@@ -67,32 +66,32 @@ def test_benchmark_circuit_real_proof_on_the_device():
     L.init()
     k = 8
     n = 1 << k
-    m = TR.M
+    m = circ.M
     pts = cref.gen_points("vesta", 99, n + 2)
     g, w, u = pts[:n], pts[n:n + 1], pts[n + 1:n + 2]
     gl = h2.lagrange_generators("vesta", k, g)
     prm = h2.Params("vesta", k, g, gl, w, u=u)
     pk = {}
     try:
-        D = h2.EvaluationDomain("fp", BC.DEGREE, k, TR.ZETA)
-        fixed, sigma, adv = BC.columns(k, m, D.omega, TR.DELTA, circ.A_SMALL * TR.ZETA % m)
+        D = h2.EvaluationDomain("fp", BC.DEGREE, k, circ.ZETA)
+        fixed, sigma, adv = BC.columns(k, m, D.omega, circ.DELTA, circ.A_SMALL * circ.ZETA % m)
         fb, sb, ab = ([cref.ints_to_bytes(c_) for c_ in cols] for cols in (fixed, sigma, adv))
         xy = lambda col: cref.bytes_to_affine(h2.batch_normalize(prm.commit_lagrange(col, h2.Blind(1)).reshape(1, 96), "vesta")[0])
         vk = PV.PinnedKey(BC.pinned_key_text(k, D.extended_k, pasta.Q_MOD, m, D.omega, [xy(c_) for c_ in fb], [xy(c_) for c_ in sb]))
         proofs = []
         for seed in (5, 6):
             T = R.Blake2bTranscript(m)
-            PP.create_proof_engine(h2, prm, vk, fb, sb, [ab], [[]], MC.SeededRng("fp", seed, True), T, TR.ZETA, TR.DELTA, pk=pk)
+            PP.create_proof_engine(h2, prm, vk, fb, sb, [ab], [[]], MC.SeededRng("fp", seed, True), T, circ.ZETA, circ.DELTA, pk=pk)
             proofs.append(bytes(T.proof))
         cp = PP.CrefProver(cref, "vesta", "fp", g, gl, w, u, 8)
         Tc = R.Blake2bTranscript(m)
-        cp.create_proof(vk, fb, sb, [ab], [[]], MC.SeededRng("fp", 6, True), Tc, TR.ZETA, TR.DELTA)
+        cp.create_proof(vk, fb, sb, [ab], [[]], MC.SeededRng("fp", 6, True), Tc, circ.ZETA, circ.DELTA)
         assert proofs[1] == bytes(Tc.proof) and proofs[0] != proofs[1]
         arm = PV.EngineArm(h2, "vesta", k, params=prm)
-        assert PV.verify_proof(arm, vk, proofs[0], [[]], TR.DELTA) and PV.verify_proof(arm, vk, proofs[1], [[]], TR.DELTA)
+        assert PV.verify_proof(arm, vk, proofs[0], [[]], circ.DELTA) and PV.verify_proof(arm, vk, proofs[1], [[]], circ.DELTA)
         bad = bytearray(proofs[1])
         bad[len(bad) // 3] ^= 8
-        assert not PV.verify_proof(arm, vk, bytes(bad), [[]], TR.DELTA)
+        assert not PV.verify_proof(arm, vk, bytes(bad), [[]], circ.DELTA)
     finally:
         PP.close_proving_key(pk)
         prm.close()

@@ -6,63 +6,19 @@ schedule, against the reference's loops restated with big integers:
 - lookup::Permuted::commit_product (plonk/lookup/prover.rs:279-337).
 
 Both fields, k = 1 ... 10, partial last sets and chunk_len = 1, several proofs per call, rows whose denominator is exactly
-zero, bf = 0 and bf = n - 2.  The restatements are also what tests/test_gpu_grand_product_fused.py checks the device against."""
+zero, bf = 0 and bf = n - 2.  The restatements (tests/grand_product_cases.py) are also what tests/test_gpu_grand_product_fused.py checks the device
+against."""
 import ctypes
 
 import numpy as np
 import pytest
 
 from oracle import cref, pasta
+from tests.grand_product_cases import oracle_lookup_product, oracle_permutation_product
 from tests.kernel_emul import build as emul_build
+from tests.plonk_verifier import scalar_delta
 
 SEED = 0x4B3231
-
-
-def delta_of(m: int) -> int:
-    return pow(pasta.MULT_GEN, 1 << pasta.S_2ADICITY, m)          # F::DELTA
-
-
-# ---- the reference, restated -------------------------------------------------------------------------------------------
-def oracle_permutation_product(columns, sigmas, beta, gamma, omega, delta, chunk_len, bf, blinding, m):
-    """permutation/prover.rs:81-168 for every proof: columns[p][c] and sigmas[c] are lists of n ints, blinding the
-    proofs x sets x bf values in the rng's order.  Returns z[p][a] (lists of n ints)."""
-    n = len(sigmas[0])
-    out, at = [], 0
-    for cols in columns:
-        last_z, deltaomega, sets = 1, 1, []
-        for c0 in range(0, len(sigmas), chunk_len):
-            mv = [1] * n
-            for v, s in zip(cols[c0:c0 + chunk_len], sigmas[c0:c0 + chunk_len]):           # :101-116
-                mv = [x * ((beta * s_i + gamma + v_i) % m) % m for x, s_i, v_i in zip(mv, s, v)]
-            mv = [pasta.inv(x, m) if x else 0 for x in mv]                                   # :120 batch_invert
-            for v in cols[c0:c0 + chunk_len]:                                                # :124-143
-                cur = deltaomega
-                for i in range(n):
-                    mv[i] = mv[i] * ((cur * beta + gamma + v[i]) % m) % m
-                    cur = cur * omega % m
-                deltaomega = deltaomega * delta % m
-            z = [last_z]
-            for row in range(1, n):                                                          # :150-156
-                z.append(z[row - 1] * mv[row - 1] % m)
-            z[n - bf:] = blinding[at:at + bf]                                                # :158-161
-            at += bf
-            last_z = z[n - (bf + 1)]                                                         # :163
-            sets.append(z)
-        out.append(sets)
-    return out
-
-
-def oracle_lookup_product(a, s, a_perm, s_perm, beta, gamma, bf, blinding, m):
-    """lookup/prover.rs:279-321 for one lookup: compressed input / table a, s and permuted a', s' (lists of n ints)."""
-    n = len(a)
-    lp = [(beta + x) * (gamma + y) % m for x, y in zip(a_perm, s_perm)]                     # :281-291
-    lp = [pasta.inv(x, m) if x else 0 for x in lp]                                           # :295
-    lp = [p * ((x + beta) % m) % m * ((y + gamma) % m) % m for p, x, y in zip(lp, a, s)]    # :299-309
-    z, state = [], 1
-    for cur in [1] + lp:                                                                     # :311-318
-        state = state * cur % m
-        z.append(state)
-    return z[:n - bf] + list(blinding)                                                       # :319-321
 
 
 # ---- the emulated kernels ----------------------------------------------------------------------------------------------
@@ -124,7 +80,7 @@ def test_emul_permutation_product(emu, field, k, proofs, cols, chunk_len, bf):
     seed = SEED + 1000 * k + 10 * cols + chunk_len
     zero_rows = [(proofs - 1, cols - 1, n // 2)] if n > 2 else []
     m, beta, gamma, sigmas, columns = permutation_case(field, k, proofs, cols, bf, seed, zero_rows)
-    omega, delta = pasta.omega_for_k(field, k), delta_of(m)
+    omega, delta = pasta.omega_for_k(field, k), scalar_delta(m)
     sets = -(-cols // chunk_len)
     blinding = pasta.gen_scalars(field, seed + 7, proofs * sets * bf) if bf else []
     want = oracle_permutation_product(columns, sigmas, beta, gamma, omega, delta, chunk_len, bf, blinding, m)
@@ -144,7 +100,7 @@ def test_emul_permutation_carries_across_sets(emu, field):
     k, cols, chunk_len, bf = 6, 11, 3, 5
     n = 1 << k
     m, beta, gamma, sigmas, columns = permutation_case(field, k, 1, cols, bf, SEED + 77)
-    omega, delta = pasta.omega_for_k(field, k), delta_of(m)
+    omega, delta = pasta.omega_for_k(field, k), scalar_delta(m)
     blinding = pasta.gen_scalars(field, SEED + 78, 4 * bf)
     got = emu_permutation_product(emu, field, columns, sigmas, beta, gamma, omega, delta, chunk_len, k, bf, blinding)[0]
     assert len(got) == 4

@@ -9,6 +9,7 @@ import numpy as np
 import pytest
 
 from oracle import cref, pasta
+from tests.ast_cases import _ast_tuple, _quotient_like_ast
 from tests.kernel_emul import build as emul_build
 
 SEED = 0x48414C4F32
@@ -569,31 +570,6 @@ def test_emul_polyops(emu, field, n):
 
 
 # ---- K15: Evaluator::evaluate over an Ast (poly/evaluator.rs:129-228) as one postfix program ----------------------------
-def _ast_tuple(node):
-    """halo2_b200.evaluator.Ast -> the oracle's nested-tuple form."""
-    k, a = node.kind, node.args
-    if k == "poly":
-        return ("poly", a[0], a[1])
-    if k in ("add", "mul"):
-        return (k, _ast_tuple(a[0]), _ast_tuple(a[1]))
-    if k == "scale":
-        return ("scale", _ast_tuple(a[0]), a[1])
-    if k == "dp":
-        return ("dp", [_ast_tuple(t) for t in a[0]], a[1])
-    return (k, a[0])
-
-
-def _quotient_like_ast(ev_leaves, y, theta):
-    """An h(X)-shaped expression: gates folded by powers of y (DistributePowers), products of rotated columns, a scaled
-    selector, the identity term of the permutation argument (LinearTerm) and a constant."""
-    from halo2_b200.evaluator import Ast
-    a, b, c, q = ev_leaves
-    gate0 = (a * b - c) * q
-    gate1 = (a.with_rotation(1) - a) * (b.with_rotation(-1) + Ast.constant_term(7)) * 3
-    perm = (c + Ast.linear_term(theta) + Ast.constant_term(11)) * (a.with_rotation(-2) + b * theta)
-    return Ast.distribute_powers([gate0, gate1, -perm, q.with_rotation(3)], y) + Ast.constant_term(0) * 5
-
-
 @pytest.mark.parametrize("basis,j,k", [("extended", 3, 4), ("extended", 5, 3), ("lagrange", 2, 5), ("lagrange", 2, 0)])
 def test_emul_ast_evaluator(emu, basis, j, k):
     from halo2_b200.evaluator import AstLeaf, compile_ast

@@ -7,7 +7,6 @@
   omega-power loop and deltaomega gather;
 - keygen_pk / keygen_vk / batch_invert_assigned_resident run their calls, in their order, over an ABI stand-in (the
   sigma kernel on the emulation), and reproduce the test prover's proving-key values."""
-import contextlib
 import ctypes
 import random
 
@@ -18,99 +17,26 @@ from oracle import cref, pasta
 from tests import bench_circuit as BC
 from tests import fake_engine
 from tests import plonk_api_circuit as circ
+from tests.bench_circuit import _bench_setup, bench_copies
+from tests.fake_engine import KEYGEN_CHUNK
+from tests.keygen_cases import oracle_assembly, oracle_copy, oracle_sigma, random_mapping
 from tests.kernel_emul import build as emul_build
-from tests.test_oracle_golden import FP_ZETA_INDEX
-
-KEYGEN_CHUNK = 1 << 22                                             # rows per launch in capi_poly.cu (H2_KEYGEN_CHUNK)
-ZETA = pasta.zeta_candidates("fp")[FP_ZETA_INDEX]
+from tests.plonk_api_circuit import ZETA, plonk_api_copies
+from tests.plonk_prover import prover_pk_dict
+from tests.plonk_verifier import scalar_delta
 
 
 # ---- the reference, restated -------------------------------------------------------------------------------------------
-def oracle_assembly(n: int, num_columns: int):
-    """Assembly::new (permutation/keygen.rs:25-43): (mapping, aux, sizes) as lists of lists of (column, row) tuples."""
-    mapping = [[(i, j) for j in range(n)] for i in range(num_columns)]
-    aux = [[(i, j) for j in range(n)] for i in range(num_columns)]
-    sizes = [[1] * n for _ in range(num_columns)]
-    return mapping, aux, sizes
-
-
-def oracle_copy(asm, left_column: int, left_row: int, right_column: int, right_row: int) -> None:
-    """Assembly::copy (permutation/keygen.rs:45-100); IndexError for Error::BoundsFailure."""
-    mapping, aux, sizes = asm
-    if left_row >= len(mapping[left_column]) or right_row >= len(mapping[right_column]):
-        raise IndexError("BoundsFailure")
-    left_cycle = aux[left_column][left_row]
-    right_cycle = aux[right_column][right_row]
-    if left_cycle == right_cycle:
-        return
-    if sizes[left_cycle[0]][left_cycle[1]] < sizes[right_cycle[0]][right_cycle[1]]:
-        left_cycle, right_cycle = right_cycle, left_cycle
-    sizes[left_cycle[0]][left_cycle[1]] += sizes[right_cycle[0]][right_cycle[1]]
-    i = right_cycle
-    while True:
-        aux[i[0]][i[1]] = left_cycle
-        i = mapping[i[0]][i[1]]
-        if i == right_cycle:
-            break
-    tmp = mapping[left_column][left_row]
-    mapping[left_column][left_row] = mapping[right_column][right_row]
-    mapping[right_column][right_row] = tmp
-
-
-def oracle_sigma(mapping, n: int, omega: int, delta: int, m: int):
-    """build_vk / build_pk's permutation polynomials (permutation/keygen.rs:108-143): the serial omega-power loop, the
-    deltaomega table, the gather.  `mapping[i][j]` = (column, row)."""
-    omega_powers = []
-    cur = 1
-    for _ in range(n):
-        omega_powers.append(cur)
-        cur = cur * omega % m
-    deltaomega = []
-    cur = 1
-    for _ in range(len(mapping)):
-        deltaomega.append([o * cur % m for o in omega_powers])
-        cur = cur * delta % m
-    return [[deltaomega[int(c)][int(r)] for c, r in mapping[i]] for i in range(len(mapping))]
-
-
 def oracle_batch_invert_assigned(numerators, denominators, m: int):
     """batch_invert_assigned (poly.rs:135-180): numerator * denominator^-1, with BatchInvert leaving a zero denominator 0."""
     return [[a * (pow(d, -1, m) if d % m else 0) % m for a, d in zip(nums, dens)] for nums, dens in zip(numerators, denominators)]
-
-
-def plonk_api_copies():
-    """The plonk_api circuit's copy constraints in the order synthesis makes them (tests/plonk_api.rs:399-400, each twice by
-    StandardCs::copy, :216-217): columns a = 0, b = 1, c = 2 of the permutation."""
-    for it in range(10):
-        rm, ra = 1 + 2 * it, 2 + 2 * it
-        yield from [(0, rm, 0, ra)] * 2
-        yield from [(1, ra, 2, rm)] * 2
-
-
-def bench_copies(k: int):
-    """The benchmark circuit's (benches/plonk.rs:226-241): copy(a0, a1) and copy(b1, c0) per multiply / add pair."""
-    for it in range((1 << (k - 1)) - 3):
-        rm, ra = 2 * it, 2 * it + 1
-        yield 0, rm, 0, ra
-        yield 1, ra, 2, rm
-
-
-def delta_of(m: int) -> int:
-    return pow(pasta.MULT_GEN, 1 << pasta.S_2ADICITY, m)          # F::DELTA
-
-
-def prover_pk_dict(pk):
-    """The proving key in the shape tests/plonk_prover.create_proof_engine(pk=...) keeps it."""
-    P = pk.permutation
-    return {"fixed_l": pk.fixed_values, "fixed_p": pk.fixed_polys, "fixed_c": pk.fixed_cosets, "sigma_l": P.permutations,
-            "sigma_p": P.polys, "sigma_c": P.cosets, "l": [pk.l0, pk.l_blind, pk.l_last]}
 
 
 # ---- 1. the mirror's Assembly ------------------------------------------------------------------------------------------
 def test_assembly_plonk_api_circuit():
     import halo2_b200 as h2
     m = pasta.P_MOD
-    omega, delta = pasta.omega_for_k("fp", circ.K), delta_of(m)
+    omega, delta = pasta.omega_for_k("fp", circ.K), scalar_delta(m)
     asm = h2.Assembly(circ.N, 12)
     ref = oracle_assembly(circ.N, 12)
     for cp in plonk_api_copies():
@@ -127,7 +53,7 @@ def test_assembly_bench_circuit(k):
     import halo2_b200 as h2
     m = pasta.P_MOD
     n = 1 << k
-    omega, delta = pasta.omega_for_k("fp", k), delta_of(m)
+    omega, delta = pasta.omega_for_k("fp", k), scalar_delta(m)
     assert omega == h2.EvaluationDomain("fp", BC.DEGREE, k, ZETA).omega
     asm = h2.Assembly(n, 3)
     for cp in bench_copies(k):
@@ -159,17 +85,6 @@ def emu():
     return ctypes.CDLL(emul_build.build())
 
 
-def random_mapping(rng, cols: int, n: int) -> np.ndarray:
-    """Random in-range (column, row) entries, with rows 0 and n - 1 and every column present."""
-    mp = np.empty((cols, n, 2), dtype=np.uint32)
-    mp[..., 0] = rng.integers(0, cols, size=(cols, n))
-    mp[..., 1] = rng.integers(0, n, size=(cols, n))
-    mp[0, 0] = (cols - 1, n - 1)
-    mp[cols - 1, n - 1] = (0, 0)
-    mp[:, 0, 0] = np.arange(cols)
-    return mp
-
-
 def emu_sigma(emu, field: str, mapping: np.ndarray, k: int, omega: int, delta: int, piece: int = KEYGEN_CHUNK):
     cols = mapping.shape[0]
     mp = np.ascontiguousarray(mapping, dtype=np.uint32)
@@ -184,7 +99,7 @@ def test_emul_tables(emu, field):
     m = pasta.FIELDS[field]
     emu.emu_keygen_tables.restype = ctypes.c_uint64
     for k in range(0, 13):
-        omega, delta = pasta.omega_for_k(field, k), delta_of(m)
+        omega, delta = pasta.omega_for_k(field, k), scalar_delta(m)
         h = emu.emu_keygen_split(k)
         assert h == (k + 1) // 2 and h + (k - h) == k and (k % 2 == 0 or h == k - h + 1)
         for cols in (1, 3, 12):
@@ -201,7 +116,7 @@ def test_emul_tables(emu, field):
 def test_emul_sigma_matches_oracle(emu, field):
     m = pasta.FIELDS[field]
     rng = np.random.default_rng(19)
-    delta = delta_of(m)
+    delta = scalar_delta(m)
     for k in range(1, 13):
         n = 1 << k
         omega = pasta.omega_for_k(field, k)
@@ -231,72 +146,13 @@ def test_emul_sigma_rejects_out_of_range_entries(emu, field):
     for where, bad in (((0, 0), (cols, 0)), ((2, 15), (0, n)), ((1, 7), (0xFFFFFFFF, 0xFFFFFFFF))):
         mp = random_mapping(rng, cols, n)
         mp[where] = bad
-        rc, _ = emu_sigma(emu, field, mp, k, omega, delta_of(m))
+        rc, _ = emu_sigma(emu, field, mp, k, omega, scalar_delta(m))
         assert rc == 1
-    rc, _ = emu_sigma(emu, field, random_mapping(rng, cols, n), k, omega, delta_of(m))
+    rc, _ = emu_sigma(emu, field, random_mapping(rng, cols, n), k, omega, scalar_delta(m))
     assert rc == 0
 
 
 # ---- 3. keygen.py over an ABI stand-in ---------------------------------------------------------------------------------
-class KeygenFakeLib(fake_engine.FakeLib):
-    """tests/fake_engine.FakeLib plus h2_poly_permutation_sigma, whose kernel bodies run on the host emulation with the
-    library's argument checks."""
-
-    def h2_poly_permutation_sigma(self, dst, cols, k, mapping, omega, delta, repr_):
-        self._log("h2_poly_permutation_sigma")
-        cols, k = fake_engine._v(cols), fake_engine._v(k)
-        if k > 30:
-            return self._fail("h2_poly_permutation_sigma: k > 30")
-        if cols == 0:
-            return 0
-        hs = [int(dst[i]) for i in range(cols)]
-        unknown = [i for i, h in enumerate(hs) if h not in self.polys]
-        if unknown:
-            return self._fail(f"h2_poly_permutation_sigma: dst[{unknown[0]}]: unknown polynomial handle")
-        c = fake_engine.clash(fake_engine.args("dst", hs, True))
-        if c:
-            return self._fail(f"h2_poly_permutation_sigma: {c}")
-        field = self.polys[hs[0]][0]
-        n = 1 << k
-        if any(self.polys[h][0] != field or self.polys[h][1].shape[0] < n for h in hs):
-            return self._fail("h2_poly_permutation_sigma: a polynomial of another field or shorter than 2^k")
-        mp = np.frombuffer(ctypes.string_at(fake_engine._v(mapping), 8 * cols * n), dtype=np.uint32).copy()
-        out = np.zeros((cols * n, 32), dtype=np.uint8)
-        rc = self.emu.emu_permutation_sigma(cref.FIELD_ID[field], mp.ctypes.data_as(ctypes.c_void_p), cols, k,
-                                            cref._p(fake_engine._rd(omega, 32)), cref._p(fake_engine._rd(delta, 32)), ctypes.c_uint64(KEYGEN_CHUNK),
-                                            cref._p(out))
-        if rc:
-            return self._fail("h2_poly_permutation_sigma: a mapping entry is outside the permutation's columns or the domain's rows")
-        for i, h in enumerate(hs):
-            self.polys[h][1][:n] = out[i * n:(i + 1) * n]
-        return 0
-
-
-@contextlib.contextmanager
-def installed():
-    from halo2_b200 import lib as L
-    saved = (L._lib, L._inited_device)
-    fake = KeygenFakeLib()
-    L._lib, L._inited_device = fake, 0
-    try:
-        yield fake
-    finally:
-        L._lib, L._inited_device = saved
-
-
-def _bench_setup(k: int):
-    c = pasta.VESTA
-    m = pasta.P_MOD
-    n = 1 << k
-    pts = cref.gen_points("vesta", 99, n + 2)
-    gens = (pts[:n], cref.params_lagrange("vesta", pts[:n], k, pasta.inv(pasta.omega_for_k("fp", k), m), pow(pasta.inv(2, m), k, m)),
-            pts[n:n + 1], pts[n + 1:n + 2])
-    omega = pasta.omega_for_k("fp", k)
-    fixed, sigma, adv = BC.columns(k, m, omega, delta_of(m), circ.A_SMALL * ZETA % m)
-    asm_copies = list(bench_copies(k))
-    return c, m, gens, fixed, sigma, adv, asm_copies
-
-
 def test_keygen_pk_reproduces_the_test_provers_key():
     """keygen_pk's resident key at k = 5 holds exactly the values create_proof_engine's own keygen part computes, and a proof
     made with it is the proof made with the host-built sigma."""
@@ -308,8 +164,8 @@ def test_keygen_pk_reproduces_the_test_provers_key():
     k = 5
     c, m, gens, fixed, sigma, adv, copies = _bench_setup(k)
     n = 1 << k
-    delta = delta_of(m)
-    with installed() as fake:
+    delta = scalar_delta(m)
+    with fake_engine.installed() as fake:
         prm = h2.Params("vesta", k, *gens[:3], u=gens[3])
         D = h2.EvaluationDomain("fp", BC.DEGREE, k, ZETA)
         asm = h2.Assembly(n, 3)
@@ -352,7 +208,7 @@ def test_keygen_accepts_assigned_fixed_columns():
     n = 1 << k
     m = pasta.P_MOD
     pts = cref.gen_points("vesta", 7, n + 2)
-    with installed() as fake:
+    with fake_engine.installed() as fake:
         prm = h2.Params("vesta", k, pts[:n], pts[:n], pts[n:n + 1], u=pts[n + 1:])
         D = h2.EvaluationDomain("fp", 3, k, ZETA)
         num = pasta.gen_scalars("fp", 1, n)
@@ -360,11 +216,11 @@ def test_keygen_accepts_assigned_fixed_columns():
         quot = oracle_batch_invert_assigned([num], [den], m)[0]
         asm = h2.Assembly(n, 2)
         asm.copy(0, 1, 1, 6)
-        got = h2.keygen_vk(prm, D, [(num, den), quot], asm, delta_of(m))
+        got = h2.keygen_vk(prm, D, [(num, den), quot], asm, scalar_delta(m))
         assert (got[0][0] == got[0][1]).all() and got[1].shape == (2, 64)
-        pk = h2.keygen_pk(prm, D, [(num, den)], asm, delta_of(m), 2)
+        pk = h2.keygen_pk(prm, D, [(num, den)], asm, scalar_delta(m), 2)
         assert cref.bytes_to_ints(pk.fixed_values[0].download()) == quot
-        assert [cref.bytes_to_ints(p.download()) for p in pk.permutation.permutations] == oracle_sigma(asm.mapping, n, D.omega, delta_of(m), m)
+        assert [cref.bytes_to_ints(p.download()) for p in pk.permutation.permutations] == oracle_sigma(asm.mapping, n, D.omega, scalar_delta(m), m)
         l_vals = []
         for p in (pk.l0, pk.l_blind, pk.l_last):                   # back to Lagrange values: extended_to_coeff, then the forward NTT
             co = D.extended_to_coeff_resident(p)
@@ -390,7 +246,7 @@ def test_batch_invert_assigned_resident(field):
             [rnd.choice([0, 1, rnd.randrange(m)]) for _ in range(n)]]
     nums[2][3] = 0
     want = oracle_batch_invert_assigned(nums, dens, m)
-    with installed() as fake:
+    with fake_engine.installed() as fake:
         rn = [h2.ResidentPoly(field, n, cref.ints_to_bytes(v)) for v in nums]
         rd = [h2.ResidentPoly(field, n, cref.ints_to_bytes(v)) for v in dens]
         out = h2.batch_invert_assigned_resident(rn, rd)

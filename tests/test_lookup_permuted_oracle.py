@@ -6,14 +6,15 @@ stand-in on the reference's plonk_api circuit and gives the permuted commitments
 import ctypes
 import random
 
-import numpy as np
 import pytest
 
 from oracle import cref, pasta
 from tests import fake_engine
+from tests import multiopen_cases as MC
+from tests import plonk_api_circuit as circ
+from tests import prover_replay as R
+from tests.fake_engine import NONE
 from tests.kernel_emul import build as emul_build
-
-NONE = 0xFFFFFFFF
 
 
 @pytest.fixture(scope="module")
@@ -134,130 +135,27 @@ def test_rank_form_equals_the_two_sort_form(emu, field):
             assert (rc2 == 1) == (rc1 == 0) == (missing not in set(tab[:u]))
 
 
-class PermutedFake(fake_engine.FakeLib):
-    """The ABI stand-in with h2_poly_lookup_permuted: the emulated bodies, and the library's checks that the orchestration
-    can reach."""
-
-    def __init__(self):
-        super().__init__()
-        self.emu.emu_lookup_permuted.restype = ctypes.c_uint32
-
-    def h2_poly_lookup_permuted(self, out_inputs, out_tables, count, inputs, tables, k, blinding, bf, repr_):
-        self._log("h2_poly_lookup_permuted")
-        count, k, bf = fake_engine._v(count), fake_engine._v(k), fake_engine._v(bf)
-        n, rows = 1 << k, bf + 1
-        outs = [int(out_inputs[b]) for b in range(count)] + [int(out_tables[b]) for b in range(count)]
-        ins = [int(inputs[b]) for b in range(count)] + [int(tables[b]) for b in range(count)]
-        c = fake_engine.clash(fake_engine.args("out_inputs", outs[:count], True) + fake_engine.args("out_tables", outs[count:], True) +
-                              fake_engine.args("inputs", ins[:count], False) + fake_engine.args("tables", ins[count:], False))
-        if c:
-            return self._fail(f"h2_poly_lookup_permuted: {c}")
-        f = self.polys[ins[0]][0]
-        col = lambda hs: np.ascontiguousarray(np.concatenate([self.polys[h][1][:n] for h in hs]))
-        oa, ot = col(outs[:count]), col(outs[count:])
-        bl = fake_engine._rd(blinding, 32 * count * 2 * rows)
-        rc = self.emu.emu_lookup_permuted(cref.FIELD_ID[f], cref._p(col(ins[:count])), cref._p(col(ins[count:])), ctypes.c_uint32(count), ctypes.c_size_t(n),
-                                          ctypes.c_size_t(n - rows), cref._p(bl), ctypes.c_size_t(rows), cref._p(oa), cref._p(ot))
-        if rc != NONE:
-            return self._fail(f"h2_poly_lookup_permuted: lookup {rc}: an input value does not occur in the table")
-        for b in range(count):
-            self.polys[outs[b]][1][:n] = oa[b * n:(b + 1) * n]
-            self.polys[outs[count + b]][1][:n] = ot[b * n:(b + 1) * n]
-        return 0
-
-
-def plonk_api_proof(h2, prm):
-    """create_proof_engine on the plonk_api circuit (k = 5, two proofs, seed 777) through `h2`, recording what the permuted
-    and product commitments need.  Returns (proof bytes, record): record["theta"], the Lagrange columns registered by then
-    ("cols"), the rng's draws ("draws", "draws_at_theta") and, per point written, the number of draws made before it."""
-    from tests import multiopen_cases as MC
-    from tests import plonk_api_circuit as circ
-    from tests import plonk_prover as PP
-    from tests import prover_replay as R
-    from tests import test_real_proof as TR
-    from tests.test_gpu_grand_product_fused import RecordingRng
-    vk = plonk_api_key()
-    seen = {"point_draws": [], "challenges": []}
-    rng = RecordingRng(MC.SeededRng("fp", 777, True))
-
-    class Eng:                                                     # the package, keeping the Lagrange-basis evaluator
-        def __getattr__(self, name):
-            return getattr(h2, name)
-
-        def Evaluator(self, D, basis="extended"):
-            ev = h2.Evaluator(D, basis)
-            seen.setdefault(basis, ev)
-            return ev
-
-    class T(R.Blake2bTranscript):
-        def squeeze_challenge(self):
-            c = super().squeeze_challenge()
-            seen["challenges"].append(c)
-            if "theta" not in seen:
-                seen.update(theta=c, draws_at_theta=len(rng.draws), points_at_theta=len(self.proof) // 32,
-                            cols=[p.download() for p in seen["lagrange"].polys])
-            return c
-
-        def write_point(self, xy):
-            seen["point_draws"].append(len(rng.draws))
-            super().write_point(xy)
-
-    tr = T(TR.M)
-    PP.create_proof_engine(Eng(), prm, vk, circ.fixed_columns(TR.M, TR.ZETA), circ.permutation_columns(TR.M, vk.omega, TR.DELTA),
-                           [TR.witness(), TR.witness()], [[[2]], [[2]]], rng, tr, TR.ZETA, TR.DELTA)
-    seen["draws"] = rng.draws
-    return bytes(tr.proof), seen
-
-
-def plonk_api_key():
-    from tests import plonk_verifier as PV
-    from tests import test_real_proof as TR
-    return PV.PinnedKey(TR.CASE["key_text"])
-
-
-def plonk_api_lookups(h2, seen):
-    """The recorded Lagrange columns registered again in the prover's order (fixed, sigma, advice per proof, instance per
-    proof) on a new evaluator, and the key's lookup expressions over it: (domain, evaluator, lookups[proof])."""
-    from tests import plonk_api_circuit as circ
-    from tests import plonk_prover as PP
-    from tests import test_real_proof as TR
-    vk = plonk_api_key()
-    D = h2.EvaluationDomain("fp", vk.degree(), vk.k, TR.ZETA)
-    ev = h2.Evaluator(D, "lagrange")
-    leaves = [ev.register_poly(h2.ResidentPoly("fp", D.n, c)) for c in seen["cols"]]
-    nf, ns, na = len(circ.fixed_columns(TR.M, TR.ZETA)), len(vk.permutation_columns), 5
-    FL, AL = leaves[:nf], [leaves[nf + ns + p * na:nf + ns + (p + 1) * na] for p in range(2)]
-    IL = [leaves[nf + ns + 2 * na + p:nf + ns + 2 * na + p + 1] for p in range(2)]
-    ast = lambda e, p: PP._to_ast(h2, e, FL, AL[p], IL[p])
-    return D, ev, [[([ast(e, p) for e in inp], [ast(e, p) for e in tab]) for inp, tab in vk.lookups] for p in range(2)]
-
-
 def test_commit_permuted_of_the_plonk_api_proof():
     """create_proof_engine (its per-lookup composition) proves the plonk_api circuit (k = 5, two proofs, one lookup each) over
     the stand-in while the Lagrange columns, theta and the rng's draws are recorded.  lookup_commit_permuted, fed the same,
     makes one permute call and gives the four permuted commitments the proof holds at their offsets, and draws as many values."""
     import halo2_b200
-    from halo2_b200 import lib as L
-    from tests import test_real_proof as TR
-    from tests.test_gpu_grand_product_fused import ReplayRng, _encode
-    vk = plonk_api_key()
+    vk = circ.plonk_api_key()
     bf = vk.blinding_factors()
-    saved = (L._lib, L._inited_device)
-    fake = PermutedFake()
-    L._lib, L._inited_device = fake, 0
-    try:
+    with fake_engine.installed() as fake:
         g, gl, w, u = _gens()
         prm = halo2_b200.Params("vesta", 5, g, gl, w, u=u)
-        proof, seen = plonk_api_proof(halo2_b200, prm)
+        proof, seen = circ.plonk_api_proof(halo2_b200, prm)
         assert fake.calls.count("h2_poly_lookup_permute") == 2 and len(vk.lookups) == 1
-        D, ev, lookups = plonk_api_lookups(halo2_b200, seen)
-        replay = ReplayRng(seen["draws"][seen["draws_at_theta"]:])
+        assert "h2_poly_lookup_permuted" not in fake.calls
+        D, ev, lookups = circ.plonk_api_lookups(halo2_b200, seen)
+        replay = MC.ReplayRng(seen["draws"][seen["draws_at_theta"]:])
         before = len(replay.draws)
         perm, cm = halo2_b200.lookup_commit_permuted(prm, D, ev, lookups, seen["theta"], bf, replay)
         assert fake.calls.count("h2_poly_lookup_permuted") == 1
         assert before - len(replay.draws) == 2 * (2 * (bf + 1) + 2)
         at = 32 * seen["points_at_theta"]
-        assert len(cm) == 4 and proof[at:at + 32 * len(cm)] == _encode(cm, TR.M)
+        assert len(cm) == 4 and proof[at:at + 32 * len(cm)] == R._encode(cm, circ.M)
         assert [len(per) for per in perm] == [1, 1] and isinstance(perm[0][0], halo2_b200.Permuted)
         for per in perm:
             for q in per:
@@ -266,8 +164,6 @@ def test_commit_permuted_of_the_plonk_api_proof():
         for p in ev.polys:
             p.close()
         prm.close()
-    finally:
-        L._lib, L._inited_device = saved
 
 
 def _gens():

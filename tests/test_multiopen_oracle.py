@@ -32,37 +32,16 @@ def eng():
         del halo2_b200._fake
 
 
-def _roundtrip(side, field):
-    """multiopen.rs:278-373 and :375-481 on `side`."""
-    m = pasta.FIELDS[field]
-    n = 1 << side.k
-    ax, bx, cx = MC.reference_roundtrip_polys(n)
-    blind, x, y, bvx_bad = cref.bytes_to_ints(cref.gen_scalars(field, SEED + 20, 4))
-    a, b, c = (side.commit(p, blind) for p in (ax, bx, cx))
-    avx, bvx, cvy = (pasta.eval_polynomial_mod(m, p, pt) for p, pt in ((ax, x), (bx, x), (cx, y)))
-    polys = [ax, bx, cx]
-    proof = side.prove(polys, [blind] * 3, [(0, x), (1, x), (2, y)], SEED + 30)
-    assert not side.verify(proof, [a, b, c], [(0, x, avx), (1, x, avx), (2, y, cvy)])        # "NB: wrong!" (:347): should fail
-    assert side.verify(proof, [a, b, c], [(0, x, avx), (1, x, bvx), (2, y, cvy)])            # should succeed (:360-371)
-    # test_identical_queries (:464-479): the same commitment at the same point with two different evaluations
-    VerifyError = pasta.VerifyError if isinstance(side, MC.OracleSide) else side.eng.VerifyError
-    with pytest.raises(VerifyError):
-        side.verify(proof, [a, b, c], [(0, x, avx), (1, x, bvx_bad), (1, x, bvx), (2, y, cvy)])
-    # bx and cx have the same coefficients but are different polynomials (different pointers): b == c as points, two queries
-    assert np.array_equal(np.asarray(b), np.asarray(c)) if not isinstance(b, tuple) else b == c
-    return proof
-
-
 def test_roundtrip_and_identical_queries_oracle():
     g, w, u = _gens("vesta", 4, real=True)                          # Params::<EqAffine>::new(4)
-    _roundtrip(MC.OracleSide("vesta", 4, g, w, u), "fp")
+    MC.roundtrip(MC.OracleSide("vesta", 4, g, w, u), "fp")
 
 
 def test_roundtrip_host_mirror_matches_oracle(eng):
     g, w, u = _gens("vesta", 3, real=False)
-    want = _roundtrip(MC.OracleSide("vesta", 3, g, w, u), "fp")
+    want = MC.roundtrip(MC.OracleSide("vesta", 3, g, w, u), "fp")
     side = MC.EngineSide(eng, "vesta", 3, g, w, u)
-    got = _roundtrip(side, "fp")
+    got = MC.roundtrip(side, "fp")
     assert got == want
     # a repeated (polynomial, point) query: the reference's prover returns io::Error InvalidInput (prover.rs:41-46)
     p = eng.ResidentPoly("fp", 8, cref.ints_to_bytes(list(range(8))))

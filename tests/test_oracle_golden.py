@@ -4,6 +4,7 @@ import numpy as np
 import pytest
 
 from oracle import cref, pasta
+from tests.plonk_api_circuit import FP_ZETA_INDEX, golden_columns
 from tests.poseidon_kat import permute
 
 
@@ -114,19 +115,6 @@ def test_point_compression_on_golden_commitments(goldens):
 # the others are MSMs over g_lagrange = 2^-5 * EC-iFFT(32 hashed generators) -- so they pin hash_to_curve, the EC-FFT
 # (best_fft at G = curve point) and best_multiexp together.  tests/plonk_api_circuit.py rebuilds the columns.
 # ------------------------------------------------------------------------------------------------------------------
-FP_ZETA_INDEX = 1          # which primitive cube root pasta calls Fp::ZETA -- pinned by fixed_commitments[6]
-
-
-def golden_columns(goldens):
-    from tests import plonk_api_circuit as circ
-    vk = goldens["vk_plonk_api_k5"]
-    m = pasta.P_MOD
-    omega = int(vk["omega"], 16)
-    delta = pow(pasta.MULT_GEN, 1 << pasta.S_2ADICITY, m)     # F::DELTA = g^(2^S) (plonk/permutation/keygen.rs:131)
-    cols = circ.fixed_columns(m, pasta.zeta_candidates("fp")[FP_ZETA_INDEX]) + circ.permutation_columns(m, omega, delta)
-    want = [(int(x, 16), int(y, 16)) for x, y in vk["fixed_commitments"] + vk["permutation_commitments"]]
-    assert len(cols) == len(want) == 19
-    return cols, want
 
 
 def test_hash_to_curve_w_is_golden(goldens):

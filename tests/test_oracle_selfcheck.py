@@ -167,7 +167,7 @@ def test_ast_evaluate_restatements_agree():
     """Evaluator::evaluate (poly/evaluator.rs:129-228): the recursive big-int walk and the C interpreter of the flattened program
     agree in both bases, for any thread count (chunk boundaries, evaluator.rs:16-32)."""
     from halo2_b200.evaluator import Ast, AstLeaf, compile_ast     # the flattening only: no GPU, no engine call
-    from tests.test_kernel_emul import _ast_tuple, _quotient_like_ast
+    from tests.ast_cases import _ast_tuple, _quotient_like_ast
     field = "fq"
     for basis, j, k in (("extended", 3, 3), ("lagrange", 2, 6), ("extended", 5, 2)):
         d = pasta.EvaluationDomain(field, j, k, pasta.zeta_candidates(field)[1])

@@ -13,13 +13,13 @@ from tests import multiopen_cases as MC
 from tests import plonk_api_circuit as circ
 from tests import plonk_prover as PP
 from tests import plonk_verifier as PV
-from tests.test_oracle_golden import FP_ZETA_INDEX
-from tests.test_verifier_oracle import _WriteT
+from tests import prover_replay as R
+from tests.plonk_api_circuit import CASE, DELTA, M, ZETA, prove, witness
 
-CASE = PV.load_golden_proofs()[0]
-M = pasta.P_MOD
-DELTA = PV.scalar_delta(M)
-ZETA = pasta.zeta_candidates("fp")[FP_ZETA_INDEX]                  # Fp::ZETA (pinned by the golden key's table-column commitment)
+# the entry points of the prover phases and of key generation, which create_proof_engine composes from finer calls
+PHASE_CALLS = {"h2_poly_lagrange_to_coeff_batch", "h2_poly_coeff_to_extended_batch", "h2_poly_set_rows", "h2_poly_lookup_permuted",
+               "h2_poly_permutation_product", "h2_poly_lookup_product", "h2_poly_vanishing_quotient", "h2_poly_permutation_sigma",
+               "h2_poly_permutation_sigma_copies"}
 
 
 @pytest.fixture(scope="module")
@@ -31,31 +31,6 @@ def setup():
     sigma = circ.permutation_columns(M, vk.omega, DELTA)           # their commitments ARE the golden key's (tests/test_oracle_golden.py)
     gens = (cref.affines_to_bytes(P.g), cref.affines_to_bytes(P.g_lagrange), cref.affines_to_bytes([P.w]), cref.affines_to_bytes([P.u]))
     return c, P, vk, fixed, sigma, gens
-
-
-def witness(break_row=None):
-    """MyCircuit::synthesize (tests/plonk_api.rs:371-395) with a = 2834758237 * ZETA: row 0 the public input, then ten times a
-    raw_multiply row (a, a, a^2; d = a^4, e = a^4) and a raw_add row (a, a^2, a^2 + a; d = a^4, e = a^8).  Advice columns in
-    creation order: e, a, b, c, d (the permutation argument's column list, :880-930 of the pinned key)."""
-    n = circ.N
-    a = circ.A_SMALL * ZETA % M
-    a2 = a * a % M
-    col = {name: [0] * n for name in "abcde"}
-    col["a"][0] = 2
-    for it in range(10):
-        rm, ra = 1 + 2 * it, 2 + 2 * it
-        col["a"][rm], col["b"][rm], col["c"][rm], col["d"][rm], col["e"][rm] = a, a, a2, pow(a, 4, M), pow(a, 4, M)
-        col["a"][ra], col["b"][ra], col["c"][ra], col["d"][ra], col["e"][ra] = a, a2, (a2 + a) % M, pow(a, 4, M), pow(a2, 4, M)
-    if break_row is not None:
-        col["c"][break_row] = (col["c"][break_row] + 1) % M
-    return [col["e"], col["a"], col["b"], col["c"], col["d"]]
-
-
-def prove(setup, advice, instances, seed):
-    c, P, vk, fixed, sigma, _ = setup
-    W = _WriteT(M)
-    PP.create_proof(c, P.g, P.g_lagrange, P.w, P.u, vk, fixed, sigma, advice, instances, MC.SeededRng("fp", seed, False), W, ZETA, DELTA)
-    return bytes(W.T.proof)
 
 
 def test_real_proof_of_the_reference_circuit_verifies(setup):
@@ -109,7 +84,6 @@ def test_real_proof_through_the_engine_api(setup):
     BODIES: with the same seeded randomness it writes THE SAME 4 160 BYTES as the oracle's prover, and the golden-proof-pinned
     verifier accepts them."""
     import halo2_b200
-    from tests import prover_replay as R
     c, P, vk, fixed, sigma, gens = setup
     inst = [[[2]], [[2]]]
     want = prove(setup, [witness(), witness()], inst, 777)
@@ -120,6 +94,7 @@ def test_real_proof_through_the_engine_api(setup):
         got = bytes(T.proof)
         assert got == want
         assert fake.calls.count("h2_poly_eval_ast") > 20 and fake.calls.count("h2_poly_lookup_permute") == 2
+        assert not PHASE_CALLS & set(fake.calls)
         assert not fake.polys                                      # every resident polynomial the prover allocated is released
         earm = PV.EngineArm(halo2_b200, "vesta", 5, *gens)
         assert PV.verify_proof(earm, vk, got, inst, DELTA)
@@ -136,7 +111,6 @@ def test_benchmark_circuit_real_proof(k):
     `bench.py`'s `extra.create_proof_k14_real` times on the GPU at k = 14."""
     import halo2_b200
     from tests import bench_circuit as BC
-    from tests import prover_replay as R
     c = pasta.VESTA
     n = 1 << k
     pts = cref.gen_points("vesta", 99, n + 2)
@@ -147,7 +121,7 @@ def test_benchmark_circuit_real_proof(k):
     cl = lambda v: pasta.to_affine(c, pasta.best_multiexp(c, list(v) + [1], P.g_lagrange + [P.w]))
     vk = PV.PinnedKey(BC.pinned_key_text(k, D.extended_k, c.p, M, D.omega, [cl(f) for f in fixed], [cl(s_) for s_ in sigma]))
     assert (vk.degree(), vk.blinding_factors(), vk.extended_k) == (5, BC.BLINDING_FACTORS, k + 2)
-    W = _WriteT(M)
+    W = R._WriteT(M)
     PP.create_proof(c, P.g, P.g_lagrange, P.w, P.u, vk, fixed, sigma, [adv], [[]], MC.SeededRng("fp", 5, False), W, ZETA, DELTA)
     want = bytes(W.T.proof)
     # 3 advice + 1 permutation product + random + 4 h pieces + f + s + 2k rounds; 3 + 4 + 1 + 3 + 2 evaluations + the q's + c, f
@@ -162,6 +136,7 @@ def test_benchmark_circuit_real_proof(k):
             PP.create_proof_engine(halo2_b200, prm, vk, fixed, sigma, [adv_bytes], [[]], MC.SeededRng("fp", seed, True), T, ZETA, DELTA, pk=pk)
             got = bytes(T.proof)
             assert expect is None or got == expect
+            assert not PHASE_CALLS & set(fake.calls)
             earm = PV.EngineArm(halo2_b200, "vesta", k, params=prm)
             assert PV.verify_proof(earm, vk, got, [[]], DELTA)
             earm.close()
@@ -179,7 +154,6 @@ def test_benchmark_circuit_real_proof(k):
 def test_cref_prover_matches_the_oracle_on_the_reference_circuit(setup):
     """PP.CrefProver (the C restatement's hot calls under the same control flow: the timed CPU arm for real proofs) on the
     plonk_api circuit -- lookup, instance column, six permutation sets, two instances: the oracle prover's 4 160 bytes."""
-    from tests import prover_replay as R
     c, P, vk, fixed, sigma, gens = setup
     inst = [[[2]], [[2]]]
     want = prove(setup, [witness(), witness()], inst, 777)

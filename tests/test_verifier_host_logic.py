@@ -123,7 +123,6 @@ def test_msm_arithmetic_host_logic(eng):
 @pytest.mark.parametrize("curve,k", [("pallas", 4), ("vesta", 1)])
 def test_opening_proof_host_logic(eng, curve, k):
     """`test_opening_proof` (poly/commitment.rs:304-379) with the oracle as the prover and halo2_b200.verifier as the verifier."""
-    from tests.test_verifier_oracle import _WriteT
     c = pasta.CURVES[curve]
     r = c.r
     n = 1 << k
@@ -134,7 +133,7 @@ def test_opening_proof_host_logic(eng, curve, k):
     s_poly = pasta.gen_scalars(c.scalar, SEED + 2, n)
     l_rand, r_rand = pasta.gen_scalars(c.scalar, SEED + 3, k), pasta.gen_scalars(c.scalar, SEED + 4, k)
     p_t = pasta.to_affine(c, pasta.best_multiexp(c, px + [blind], gt + [wt]))
-    W = _WriteT(r)
+    W = R._WriteT(r)
     W.write_point(p_t)
     x = W.squeeze_challenge()
     v = pasta.eval_polynomial_mod(r, px, x)

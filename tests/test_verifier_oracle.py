@@ -133,28 +133,6 @@ def test_msm_arithmetic_oracle():
         new().add_to_g_scalars(sc[:15])                        # assert_eq!(scalars.len(), params.n), msm.rs:100
 
 
-class _WriteT:
-    """The write-side transcript of tests/prover_replay.py on affine tuples (what the oracle speaks)."""
-
-    def __init__(self, modulus):
-        self.T = R.Blake2bTranscript(modulus)
-
-    def write_point(self, pt):
-        self.T.write_point(cref.affines_to_bytes([pt])[0])
-
-    def write_scalar(self, s):
-        self.T.write_scalar(s)
-
-    def common_point(self, pt):
-        self.T.common_point(cref.affines_to_bytes([pt])[0])
-
-    def common_scalar(self, s):
-        self.T.common_scalar(s)
-
-    def squeeze_challenge(self):
-        return self.T.squeeze_challenge()
-
-
 @pytest.mark.parametrize("curve,k", [("pallas", 4), ("vesta", 3)])
 def test_opening_proof_oracle(curve, k):
     """poly/commitment.rs:304-379 (`test_opening_proof`, K = 6 there) through the oracle: commit, create_proof, read the
@@ -169,7 +147,7 @@ def test_opening_proof_oracle(curve, k):
     s_poly = pasta.gen_scalars(c.scalar, SEED + 2, n)
     l_rand, r_rand = pasta.gen_scalars(c.scalar, SEED + 3, k), pasta.gen_scalars(c.scalar, SEED + 4, k)
     p = pasta.to_affine(c, pasta.best_multiexp(c, px + [blind], g + [w]))
-    W = _WriteT(r)
+    W = R._WriteT(r)
     W.write_point(p)
     x = W.squeeze_challenge()
     v = pasta.eval_polynomial_mod(r, px, x)

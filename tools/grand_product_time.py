@@ -23,7 +23,7 @@ import torch  # noqa: E402
 import halo2_b200 as h2  # noqa: E402
 from halo2_b200 import lib as L  # noqa: E402
 from oracle import cref, pasta  # noqa: E402
-from tests.test_gpu_grand_product_fused import composition_lookup, composition_permutation  # noqa: E402
+from tests.grand_product_cases import composition_lookup, composition_permutation  # noqa: E402
 
 M = pasta.P_MOD
 ZETA = pow(5, (M - 1) // 3, M)

@@ -156,9 +156,11 @@ def real_bench(k, lanes, reps):
     from tests import plonk_api_circuit as circ
     from tests import plonk_prover as PP
     from tests import plonk_verifier as PV
-    from tests.test_keygen_oracle import ZETA, bench_copies, delta_of, prover_pk_dict
+    from tests.bench_circuit import bench_copies
+    from tests.plonk_api_circuit import ZETA
+    from tests.plonk_prover import prover_pk_dict
     n, m = 1 << k, pasta.P_MOD
-    delta = delta_of(m)
+    delta = PV.scalar_delta(m)
     dev = L._inited_device or 0
     free = lambda: int(torch.cuda.mem_get_info(dev)[0])
     pts = cref.gen_points("vesta", 99, n + 2)

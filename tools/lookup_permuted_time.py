@@ -40,7 +40,7 @@ def timed(torch, fn):
 
 
 def run_single(h2, torch, reps, ks):
-    from tests.test_gpu_lookup_permuted import columns
+    from tests.lookup_permuted_cases import columns
     rows = []
     for k in ks:
         n = 1 << k
@@ -64,14 +64,14 @@ def run_single(h2, torch, reps, ks):
 
 def run_fused(h2, torch, reps, ks, counts):
     from oracle import pasta
-    from tests.test_gpu_grand_product_fused import _params
-    from tests.test_gpu_lookup_permuted import columns, composition
+    from tests.bench_circuit import _bench_params
+    from tests.lookup_permuted_cases import columns, composition
     from halo2_b200.products import _commit
     rows = []
     for k in ks:
         n = 1 << k
         u = n - BF - 1
-        prm = _params(h2, k)
+        prm = _bench_params(h2, k)
         D = h2.EvaluationDomain("fp", 3, k, pasta.zeta_candidates("fp")[0])
         for count in counts:
             for hot in (False, True):
