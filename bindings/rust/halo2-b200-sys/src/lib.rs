@@ -36,6 +36,10 @@ extern "C" {
     pub fn h2_poly_free(poly: u64) -> c_int;
     pub fn h2_poly_upload(poly: u64, src: *const c_void, len: usize, repr: c_int) -> c_int;
     pub fn h2_poly_download(poly: u64, dst: *mut c_void, len: usize, repr: c_int) -> c_int;
+    pub fn h2_poly_upload_dev(polys: *const u64, count: usize, d_src: *const *const c_void, lens: *const usize, repr: c_int,
+                              stream: *mut c_void) -> c_int;
+    pub fn h2_poly_download_dev(polys: *const u64, count: usize, d_dst: *const *mut c_void, lens: *const usize, repr: c_int,
+                                stream: *mut c_void) -> c_int;
     pub fn h2_poly_lagrange_to_coeff(dst: u64, src: u64, k: u32, omega_inv: *const c_void, divisor: *const c_void, repr: c_int) -> c_int;
     pub fn h2_poly_coeff_to_extended(dst: u64, src: u64, k: u32, ext_k: u32, zeta: *const c_void, ext_omega: *const c_void,
                                      repr: c_int) -> c_int;

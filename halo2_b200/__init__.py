@@ -10,7 +10,8 @@ from .arithmetic import (best_multiexp, small_multiexp, best_fft, best_fft_curve
                          eval_polynomial, compute_inner_product, kate_division)
 from .poly import (Params, EvaluationDomain, Blind, ResidentPoly, lagrange_generators, compress_points, decompress_points, hash_to_curve,  # noqa: F401
                    eval_polynomial_resident, inner_product_resident, kate_division_resident, batch_invert_resident,
-                   running_product_resident, permute_expression_pair_resident, share_resident, set_rows_resident)
+                   running_product_resident, permute_expression_pair_resident, share_resident, set_rows_resident,
+                   upload_tensors_resident, download_tensors_resident, upload_dev_resident, download_dev_resident)
 
 from .evaluator import Ast, AstLeaf, Evaluator  # noqa: F401
 from .verifier import MSM, Guard, VerifyError, verify_proof, compute_b  # noqa: F401
@@ -30,7 +31,8 @@ __all__ = ["Ast", "AstLeaf", "Evaluator", "Assembly", "CopyConstraints", "Provin
            "lagrange_generators", "compress_points", "decompress_points", "hash_to_curve",
            "eval_polynomial", "compute_inner_product", "kate_division", "eval_polynomial_resident", "inner_product_resident",
            "kate_division_resident", "batch_invert_resident", "running_product_resident", "permute_expression_pair_resident",
-           "share_resident", "permutation_commit", "lookup_commit_product", "permutation_product_resident", "lookup_product_resident",
+           "share_resident", "upload_tensors_resident", "download_tensors_resident", "upload_dev_resident", "download_dev_resident",
+           "permutation_commit", "lookup_commit_product", "permutation_product_resident", "lookup_product_resident",
            "lookup_commit_permuted", "lookup_permute_resident", "Permuted", "set_rows_resident", "instance_commit", "advice_commit",
            "InstanceSingle", "AdviceSingle", "InstanceTooLarge",
            "vanishing_commit", "vanishing_quotient_resident", "Committed", "Constructed", "Evaluated",

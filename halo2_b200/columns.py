@@ -13,7 +13,7 @@ from typing import List, NamedTuple, Sequence
 import numpy as np
 
 from . import lib as _l
-from .poly import EvaluationDomain, Params, ResidentPoly, set_rows_resident
+from .poly import EvaluationDomain, Params, ResidentPoly, _tensor_rows, is_device_tensor, set_rows_resident, upload_tensors_resident
 from .products import _commit
 
 
@@ -64,18 +64,23 @@ def _split(flat: list, sizes: Sequence[int]) -> List[list]:
 
 
 def instance_commit(params: Params, domain: EvaluationDomain, instances: Sequence[Sequence], blinding_factors: int) -> List[InstanceSingle]:
-    """The instance columns of every proof (plonk/prover.rs:79-124): `instances[p]` is proof p's list of columns (ints or
-    (len, 32) uint8 arrays).  Each column is zero-padded to n and committed with Blind::default(); raises InstanceTooLarge
-    when a column is longer than n - (blinding_factors + 1).  Returns one InstanceSingle per proof."""
+    """The instance columns of every proof (plonk/prover.rs:79-124): `instances[p]` is proof p's list of columns (ints,
+    (len, 32) uint8 arrays, or CUDA tensors as ResidentPoly.from_tensor takes them).  Each column is zero-padded to n and
+    committed with Blind::default(); raises InstanceTooLarge when a column is longer than n - (blinding_factors + 1).  The
+    tensor columns go up in one h2_poly_upload_dev on torch's current stream.  Returns one InstanceSingle per proof."""
     n, m = domain.n, domain.m
-    cols = [_column_bytes(col, m) for per in instances for col in per]
-    if any(c.shape[0] > n - (blinding_factors + 1) for c in cols):
+    cols = [col if is_device_tensor(col) else _column_bytes(col, m) for per in instances for col in per]
+    rows = [_tensor_rows(c, "an instance column") if is_device_tensor(c) else c.shape[0] for c in cols]
+    if any(r > n - (blinding_factors + 1) for r in rows):
         raise InstanceTooLarge("instance column longer than n - (blinding_factors + 1) (Error::InstanceTooLarge)")
     live: List[ResidentPoly] = []
     try:
-        for c in cols:
-            live.append(ResidentPoly(domain.field, n, c if c.shape[0] else None))   # allocated zero-filled: the padding
+        for c, r in zip(cols, rows):
+            host = r and not is_device_tensor(c)
+            live.append(ResidentPoly(domain.field, n, c if host else None))   # allocated zero-filled: the padding
         values = list(live)
+        dev = [(p, c) for p, c, r in zip(values, cols, rows) if r and is_device_tensor(c)]
+        upload_tensors_resident([p for p, _ in dev], [c for _, c in dev])
         cm = _commit(params, values, [1] * len(values))
         polys, cosets = _transforms(domain, values, live) if values else ([], [])
     except BaseException:
@@ -88,10 +93,11 @@ def instance_commit(params: Params, domain: EvaluationDomain, instances: Sequenc
 
 def advice_commit(params: Params, domain: EvaluationDomain, advice: Sequence[Sequence], rng, blinding_factors: int) -> List[AdviceSingle]:
     """The advice columns of every proof (plonk/prover.rs:269-335): `advice[p]` is proof p's list of n-row Lagrange columns,
-    host arrays (ints or (n, 32) uint8) or ResidentPolys, which receive their blinding rows in place.  `rng` (scalar() -> int)
-    is drawn in the reference's order: per proof, per column, the blinding_factors + 1 unusable rows in row order, then one
-    blind per column (:276-282, :294-304).  One h2_poly_set_rows writes every column's blinding rows, one commitment pass
-    commits them, and the transforms run one batched call each.  Returns one AdviceSingle per proof."""
+    host arrays (ints or (n, 32) uint8), CUDA tensors (as ResidentPoly.from_tensor takes them; all of them go up in one
+    h2_poly_upload_dev on torch's current stream) or ResidentPolys, which receive their blinding rows in place.  `rng`
+    (scalar() -> int) is drawn in the reference's order: per proof, per column, the blinding_factors + 1 unusable rows in row
+    order, then one blind per column (:276-282, :294-304).  One h2_poly_set_rows writes every column's blinding rows, one
+    commitment pass commits them, and the transforms run one batched call each.  Returns one AdviceSingle per proof."""
     n, m = domain.n, domain.m
     rows = blinding_factors + 1
     usable = n - rows
@@ -102,7 +108,7 @@ def advice_commit(params: Params, domain: EvaluationDomain, advice: Sequence[Seq
         blinds.append([rng.scalar() for _ in per])
     live: List[ResidentPoly] = []
     try:
-        values = []
+        values, dev = [], []
         for per in advice:
             for col in per:
                 if isinstance(col, ResidentPoly):
@@ -110,11 +116,19 @@ def advice_commit(params: Params, domain: EvaluationDomain, advice: Sequence[Seq
                         raise _l.H2Error("an advice column holds fewer than n rows")
                     values.append(col)
                     continue
+                if is_device_tensor(col):
+                    if _tensor_rows(col, "an advice column") != n:
+                        raise _l.H2Error("an advice column does not have n rows")
+                    live.append(ResidentPoly(domain.field, n))
+                    values.append(live[-1])
+                    dev.append((live[-1], col))
+                    continue
                 arr = _column_bytes(col, m)
                 if arr.shape[0] != n:
                     raise _l.H2Error("an advice column does not have n rows")
                 live.append(ResidentPoly(domain.field, n, arr))
                 values.append(live[-1])
+        upload_tensors_resident([p for p, _ in dev], [c for _, c in dev])   # before the blinding rows overwrite their tail
         flat_blinds = [b for per in blinds for b in per]
         set_rows_resident(values, usable, blinding)
         cm = _commit(params, values, flat_blinds)

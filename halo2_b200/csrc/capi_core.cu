@@ -122,6 +122,12 @@ int PolyArgs::find(bool out, const uint64_t *h, size_t n, const char *name, uint
         if (!(v[i] = find(out, h[i], name, (int64_t)i, off, len, len_name))) return 1;
     return 0;
 }
+int PolyArgs::find(bool out, const uint64_t *h, size_t n, const char *name, const size_t *lens, const char *len_name, std::vector<PolyBuf *> &v) {
+    v.resize(n);
+    for (size_t i = 0; i < n; i++)
+        if (!(v[i] = find(out, h[i], name, (int64_t)i, 0, lens[i], arg_label(len_name, (int64_t)i).c_str()))) return 1;
+    return 0;
+}
 // Batch slices and product columns run concurrently: an output written twice, or read as another one's input, would race.
 // The arguments are walked in lookup order, and the first one that clashes with an earlier one is reported.
 int PolyArgs::distinct(const char *in_place_out, const char *in_place_in) {

@@ -1,6 +1,9 @@
 // C ABI of the engine, part 3 of 5: the NTT pipeline (ntt.cuh), the domain transforms, device-resident polynomials.
 #include "util_kernels.cuh"
 #include "ntt.cuh"
+#include "columns_io.cuh"
+
+#include <algorithm>
 
 // ------------------------------------------------------------------------------------------------
 // NTT pipeline
@@ -355,6 +358,71 @@ extern "C" int h2_poly_download(uint64_t poly, void *dst, size_t len, int repr) 
     PolyBuf *b = g.in(poly, "poly", len, "len");
     if (!b) return 1;
     return h.down(b->field, dst, b->buf.as<fe>(), len, g_ctx.stream);
+}
+// h2_poly_upload_dev / h2_poly_download_dev (K25, columns_io.cuh): column i moves lens[i] elements between polys[i] and the
+// caller's device pointer ptrs[i], every column in one launch on the caller's stream.  Every check runs before the first
+// launch; the caller's pointers are checked where they are non-empty.
+static int poly_io_dev(const char *who, bool up, const uint64_t *polys, size_t count, const void *const *ptrs, const size_t *lens, int repr,
+                       void *stream) {
+    const char *pname = up ? "d_src" : "d_dst";
+    CtxLock lk;
+    const HostArgs h(who, repr);
+    if (require_ready() || h.check({{polys, "polys", count != 0}, {ptrs, pname, count != 0}, {lens, "lens", count != 0}})) return 1;
+    if (count == 0) return 0;
+    Context &X = g_ctx;
+    const std::string w(who);
+    auto bad = [&](size_t i, const std::string &why) { return fail(w + ": " + pname + "[" + std::to_string(i) + "]: " + why); };
+    PolyArgs g(who);
+    std::vector<PolyBuf *> ps;
+    if ((up ? g.out(polys, count, "polys", lens, "lens", ps) || g.distinct() : g.in(polys, count, "polys", lens, "lens", ps))) return 1;
+    uint64_t longest = 0;
+    std::vector<IoCol> io(count);
+    std::vector<std::pair<uintptr_t, size_t>> ranges;   // download: the caller's byte ranges, to refuse overlaps
+    for (size_t i = 0; i < count; i++) {
+        io[i] = {(uint64_t)(uintptr_t)ptrs[i], (uint64_t)lens[i]};
+        if (lens[i] == 0) continue;
+        if (!ptrs[i]) return bad(i, "null pointer");
+        cudaPointerAttributes a;
+        if (cudaPointerGetAttributes(&a, ptrs[i]) != cudaSuccess) { cudaGetLastError(); a.type = cudaMemoryTypeUnregistered; }
+        if (a.type != cudaMemoryTypeDevice && a.type != cudaMemoryTypeManaged)
+            return bad(i, std::string("not device memory (host columns go through ") + (up ? "h2_poly_upload)" : "h2_poly_download)"));
+        if (a.device != X.device)
+            return bad(i, "memory of device " + std::to_string(a.device) + ", not the calling context's device " + std::to_string(X.device));
+        if ((uintptr_t)ptrs[i] % 16) return bad(i, "not 16-byte aligned");
+        if (!up) ranges.push_back({(uintptr_t)ptrs[i], i});
+        if (lens[i] > longest) longest = lens[i];
+    }
+    if (!up) {
+        std::sort(ranges.begin(), ranges.end());
+        size_t reach = 0;   // of the ranges so far (by start address), the one that ends last
+        for (size_t j = 1; j < ranges.size(); j++) {
+            const size_t prev = ranges[reach].second, cur = ranges[j].second;
+            if (ranges[j].first < ranges[reach].first + lens[prev] * sizeof(fe))
+                return bad(std::max(prev, cur), "overlaps " + std::string(pname) + "[" + std::to_string(std::min(prev, cur)) + "]");
+            reach = j;   // no overlap: range j starts at or after every earlier end, so it ends last
+        }
+    }
+    if (longest == 0) return 0;
+    cudaStream_t s = (cudaStream_t)stream;
+    StreamSplice splice(s);   // the column table is the context's scratch
+    if (splice.failed) return 1;
+    ColTable t;
+    if (col_table(ps, io.data(), count * sizeof(IoCol), s, &t)) return 1;
+    return by_field(ps[0]->field, [&](auto p) {
+        using P = decltype(p);
+        for (size_t c0 = 0; c0 < count; c0 += 65535) {   // grid.y limit
+            const uint32_t cols = (uint32_t)std::min<size_t>(count - c0, 65535);
+            LAUNCH(columns_io_kernel<P>, dim3(blocks_for(longest, 256), cols), 256, 0, s, t.cols, reinterpret_cast<const IoCol *>(t.data), (uint32_t)c0,
+                   up ? 1 : 0, h.canon() ? 1 : 0);
+        }
+        return 0;
+    });
+}
+extern "C" int h2_poly_upload_dev(const uint64_t *polys, size_t count, const void *const *d_src, const size_t *lens, int repr, void *stream) {
+    return poly_io_dev("h2_poly_upload_dev", true, polys, count, d_src, lens, repr, stream);
+}
+extern "C" int h2_poly_download_dev(const uint64_t *polys, size_t count, void *const *d_dst, const size_t *lens, int repr, void *stream) {
+    return poly_io_dev("h2_poly_download_dev", false, polys, count, (const void *const *)d_dst, lens, repr, stream);
 }
 // mode as in ntt_host: 1 = inverse transform with divisor, 2 = coeff_to_extended, 3 = extended_to_coeff.  Column i goes from
 // src[i] to dst[i]; a batch reaches ntt_run through one table of its columns' pointers (the sources, then the destinations).

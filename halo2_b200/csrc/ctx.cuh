@@ -335,6 +335,9 @@ struct PolyArgs {
     int out(const uint64_t *h, size_t n, const char *name, uint64_t off, uint64_t len, const char *len_name, Polys &v) { return find(true, h, n, name, off, len, len_name, v); }
     int out(const uint64_t *h, size_t n, const char *name, uint64_t len, const char *len_name, Polys &v) { return find(true, h, n, name, 0, len, len_name, v); }
     int in(const uint64_t *h, size_t n, const char *name, uint64_t len, const char *len_name, Polys &v) { return find(false, h, n, name, 0, len, len_name, v); }
+    // element i holds at least lens[i] elements ("a polynomial holds fewer than <len_name>[i] elements")
+    int out(const uint64_t *h, size_t n, const char *name, const size_t *lens, const char *len_name, Polys &v) { return find(true, h, n, name, lens, len_name, v); }
+    int in(const uint64_t *h, size_t n, const char *name, const size_t *lens, const char *len_name, Polys &v) { return find(false, h, n, name, lens, len_name, v); }
     int distinct(const char *in_place_out = nullptr, const char *in_place_in = nullptr);
     PolyArgs(const PolyArgs &) = delete;
     PolyArgs &operator=(const PolyArgs &) = delete;
@@ -348,6 +351,7 @@ struct PolyArgs {
     std::vector<PolyBuf *> held;             // the shared polynomials this call is a user of
     PolyBuf *find(bool out, uint64_t h, const char *name, int64_t i, uint64_t off, uint64_t len, const char *len_name);
     int find(bool out, const uint64_t *h, size_t n, const char *name, uint64_t off, uint64_t len, const char *len_name, Polys &v);
+    int find(bool out, const uint64_t *h, size_t n, const char *name, const size_t *lens, const char *len_name, Polys &v);
 };
 // One upload of a kernel's column table into the context's table buffer (col_tab), on `s`: the device
 // pointers of `cols` in the order the kernel reads them (a null PolyBuf gives a null pointer), then `bytes` host bytes from

@@ -18,7 +18,7 @@ import numpy as np
 
 from . import lib as _l
 from .evaluator import AstLeaf, compile_ast
-from .poly import FIELDS, Blind, EvaluationDomain, Params, ResidentPoly, _handles, batch_invert_resident, share_resident
+from .poly import FIELDS, Blind, EvaluationDomain, Params, ResidentPoly, _handles, _tensor_rows, batch_invert_resident, is_device_tensor, share_resident
 
 
 class Assembly:
@@ -191,23 +191,32 @@ def _as_bytes(values, m: int) -> np.ndarray:
     return np.frombuffer(b"".join((int(v) % m).to_bytes(32, "little") for v in values), dtype=np.uint8).reshape(-1, 32)
 
 
+def _lagrange_column(domain: EvaluationDomain, values) -> ResidentPoly:
+    """n values (ints, an (n, 32) uint8 array, or a CUDA tensor as ResidentPoly.from_tensor takes it) as a resident column."""
+    if is_device_tensor(values):
+        assert _tensor_rows(values, "a fixed column") == domain.n, "a fixed column must have n values"
+        return ResidentPoly.from_tensor(domain.field, values)
+    vals = _as_bytes(values, domain.m)
+    assert vals.shape[0] == domain.n, "a fixed column must have n values"
+    return ResidentPoly(domain.field, domain.n, vals)
+
+
 def _fixed_values(domain: EvaluationDomain, fixed) -> List[ResidentPoly]:
-    """The fixed columns as resident Lagrange values.  A column is its values (ints or an (n, 32) uint8 array) or a
-    (numerators, denominators) pair of such, which goes through batch_invert_assigned_resident."""
+    """The fixed columns as resident Lagrange values.  A column is its values (ints, an (n, 32) uint8 array or a CUDA
+    tensor) or a (numerators, denominators) pair of such, which goes through batch_invert_assigned_resident."""
     out: List[ResidentPoly] = []
     try:
         for col in fixed:
             if isinstance(col, tuple):
-                num, den = (ResidentPoly(domain.field, domain.n, _as_bytes(v, domain.m)) for v in col)
+                num, den = (ResidentPoly.from_tensor(domain.field, v, length=domain.n) if is_device_tensor(v) else
+                            ResidentPoly(domain.field, domain.n, _as_bytes(v, domain.m)) for v in col)
                 try:
                     out.extend(batch_invert_assigned_resident([num], [den]))
                 finally:
                     num.close()
                     den.close()
             else:
-                vals = _as_bytes(col, domain.m)
-                assert vals.shape[0] == domain.n, "a fixed column must have n values"
-                out.append(ResidentPoly(domain.field, domain.n, vals))
+                out.append(_lagrange_column(domain, col))
     except BaseException:
         for p in out:
             p.close()

@@ -352,6 +352,32 @@ class ResidentPoly:
         _l.check(_l.init().h2_poly_download(self._h, _l.ptr(out), ctypes.c_size_t(n), _l.REPR_CANONICAL))
         return out
 
+    @classmethod
+    def from_tensor(cls, field: str, t, length: Optional[int] = None, repr: str = "canonical", stream=None) -> "ResidentPoly":
+        """A polynomial of `length` elements (default: the tensor's rows) filled from a CUDA tensor on the device, without
+        a trip through host memory (h2_poly_upload_dev).  `t`: contiguous torch.uint8 of shape (rows, 32), one element per
+        row in `repr` ("canonical" or "montgomery").  Asynchronous on `stream` (default: torch's current stream on t's
+        device), ordered before every later call of the calling thread's lane."""
+        rows = _tensor_rows(t, "t")
+        p = cls(field, rows if length is None else length)
+        try:
+            p.upload_tensor(t, repr=repr, stream=stream)
+        except BaseException:
+            p.close()
+            raise
+        return p
+
+    def upload_tensor(self, t, repr: str = "canonical", stream=None) -> None:
+        """Rows [0, t.shape[0]) <- a CUDA tensor (see from_tensor)."""
+        upload_tensors_resident([self], [t], repr=repr, stream=stream)
+
+    def to_tensor(self, length: Optional[int] = None, repr: str = "canonical", out=None, stream=None):
+        """The first `length` elements (default: out's rows, else the polynomial's length) as a (length, 32) torch.uint8
+        CUDA tensor in `repr`, into `out` when given.  Asynchronous on `stream` (default: torch's current stream), after
+        every earlier call of the calling thread's lane (h2_poly_download_dev)."""
+        return download_tensors_resident([self], None if length is None else [length], repr=repr, out=None if out is None else [out],
+                                         stream=stream)[0]
+
     def copy_from(self, src: "ResidentPoly", length: int, src_off: int = 0, dst_off: int = 0) -> "ResidentPoly":
         """self[dst_off : dst_off + length] = src[src_off : src_off + length] on the device (`h_poly.chunks_exact(n)`)."""
         _l.check(_l.init().h2_poly_copy(self._h, ctypes.c_size_t(int(dst_off)), src._h, ctypes.c_size_t(int(src_off)), ctypes.c_size_t(int(length))))
@@ -385,6 +411,111 @@ class ResidentPoly:
 
 def _handles(polys: Sequence["ResidentPoly"]):
     return (ctypes.c_uint64 * len(polys))(*[p._h.value for p in polys])
+
+
+_REPRS = {"canonical": _l.REPR_CANONICAL, "montgomery": _l.REPR_MONTGOMERY}
+
+
+def _repr_id(repr: str) -> int:
+    if repr not in _REPRS:
+        raise ValueError(f"repr must be 'canonical' or 'montgomery', not {repr!r}")
+    return _REPRS[repr]
+
+
+def is_device_tensor(x) -> bool:
+    """x is a CUDA torch tensor (told without importing torch: a package that never sees one never loads it)."""
+    return getattr(x, "is_cuda", False) is True and hasattr(x, "data_ptr")
+
+
+def _tensor_rows(t, name: str, limit: Optional[int] = None) -> int:
+    """The rows of a column tensor the device transfers take: contiguous, torch.uint8, shape (rows, 32), at most `limit`
+    rows, a CUDA tensor on the library's device.  Anything else is refused; nothing is reinterpreted."""
+    import torch
+    if not isinstance(t, torch.Tensor):
+        raise TypeError(f"{name}: expected a torch.Tensor, got {type(t).__name__}")
+    if t.dtype != torch.uint8:
+        raise ValueError(f"{name}: dtype {t.dtype}, expected torch.uint8 (32 bytes per element)")
+    if t.dim() != 2 or t.shape[1] != 32:
+        raise ValueError(f"{name}: shape {tuple(t.shape)}, expected (rows, 32)")
+    if not t.is_contiguous():
+        raise ValueError(f"{name}: not contiguous")
+    if limit is not None and t.shape[0] > limit:
+        raise ValueError(f"{name}: {t.shape[0]} rows, the polynomial holds {limit}")
+    if not t.is_cuda:
+        raise ValueError(f"{name}: a CPU tensor; host columns go through ResidentPoly(values) / upload()")
+    _l.init()
+    if t.device.index != _l._inited_device:
+        raise ValueError(f"{name}: on {t.device}, the library runs on cuda:{_l._inited_device}")
+    return int(t.shape[0])
+
+
+def _stream_handle(stream, device) -> int:
+    import torch
+    s = torch.cuda.current_stream(device) if stream is None else stream
+    return int(s.cuda_stream)
+
+
+def upload_dev_resident(polys: Sequence["ResidentPoly"], ptrs: Sequence[int], lens: Sequence[int], repr_id: int, stream: int) -> None:
+    """h2_poly_upload_dev: polys[i][0 .. lens[i]) <- the device address ptrs[i], one call for every column, on the CUDA stream
+    handle `stream` (0: the legacy default stream)."""
+    _dev_io("h2_poly_upload_dev", polys, ptrs, lens, repr_id, stream)
+
+
+def download_dev_resident(polys: Sequence["ResidentPoly"], ptrs: Sequence[int], lens: Sequence[int], repr_id: int, stream: int) -> None:
+    """h2_poly_download_dev: the device address ptrs[i] <- polys[i][0 .. lens[i]), one call for every column."""
+    _dev_io("h2_poly_download_dev", polys, ptrs, lens, repr_id, stream)
+
+
+def _dev_io(name, polys, ptrs, lens, repr_id, stream) -> None:
+    count = len(polys)
+    if len(ptrs) != count or len(lens) != count:
+        raise ValueError("one pointer and one length per polynomial")
+    fn = getattr(_l.init(), name)
+    _l.check(fn(_handles(polys), ctypes.c_size_t(count), (ctypes.c_void_p * count)(*[int(p) for p in ptrs]),
+                (ctypes.c_size_t * count)(*[int(n) for n in lens]), ctypes.c_int(int(repr_id)), ctypes.c_void_p(int(stream))))
+
+
+def upload_tensors_resident(polys: Sequence["ResidentPoly"], tensors: Sequence, repr: str = "canonical", stream=None) -> None:
+    """polys[i][0 .. rows_i) <- tensors[i] (CUDA tensors as ResidentPoly.from_tensor takes them), every column in one
+    h2_poly_upload_dev on `stream` (default: torch's current stream on the tensors' device)."""
+    if len(polys) != len(tensors):
+        raise ValueError("one tensor per polynomial")
+    if not polys:
+        return
+    rid = _repr_id(repr)
+    rows = [_tensor_rows(t, f"tensors[{i}]", p.len) for i, (p, t) in enumerate(zip(polys, tensors))]
+    upload_dev_resident(polys, [t.data_ptr() for t in tensors], rows, rid, _stream_handle(stream, tensors[0].device))
+
+
+def download_tensors_resident(polys: Sequence["ResidentPoly"], lengths: Optional[Sequence[int]] = None, repr: str = "canonical",
+                              out: Optional[Sequence] = None, stream=None) -> list:
+    """[the first lengths[i] elements of polys[i]] as (lengths[i], 32) torch.uint8 CUDA tensors, every column in one
+    h2_poly_download_dev on `stream` (default: torch's current stream).  lengths default to out's rows, else to the
+    polynomials' lengths; `out` (optional) are the destination tensors, which must not overlap."""
+    import torch
+    count = len(polys)
+    if (lengths is not None and len(lengths) != count) or (out is not None and len(out) != count):
+        raise ValueError("one length and one output tensor per polynomial")
+    rid = _repr_id(repr)
+    rows = [_tensor_rows(t, f"out[{i}]") for i, t in enumerate(out)] if out is not None else None
+    if lengths is None:
+        lengths = rows if rows is not None else [p.len for p in polys]
+    lengths = [int(n) for n in lengths]
+    for i, (p, n) in enumerate(zip(polys, lengths)):
+        if n < 0 or n > p.len:
+            raise ValueError(f"lengths[{i}] = {n}: the polynomial holds {p.len}")
+        if rows is not None and rows[i] < n:
+            raise ValueError(f"out[{i}]: {rows[i]} rows, fewer than the {n} requested")
+    if not polys:
+        return []
+    _l.init()
+    device = out[0].device if out is not None else torch.device("cuda", _l._inited_device)
+    if out is None:
+        s = torch.cuda.current_stream(device) if stream is None else stream
+        with torch.cuda.stream(s):                     # allocated for the stream that writes it
+            out = [torch.empty((n, 32), dtype=torch.uint8, device=device) for n in lengths]
+    download_dev_resident(polys, [t.data_ptr() for t in out], lengths, rid, _stream_handle(stream, device))
+    return list(out)
 
 
 def share_resident(polys: Sequence["ResidentPoly"]) -> None:

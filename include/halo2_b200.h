@@ -174,6 +174,17 @@ int h2_poly_free(uint64_t poly);
 int h2_poly_share(const uint64_t *polys, size_t n);
 int h2_poly_upload(uint64_t poly, const void *src, size_t len, int repr);
 int h2_poly_download(uint64_t poly, void *dst, size_t len, int repr);
+/* The same transfers from and to the caller's DEVICE memory, every column in one launch: column i moves the first lens[i]
+ * elements (32 B each, `repr`) between polys[i] and d_src[i] / d_dst[i], converting on the way.  The bytes equal those of
+ * h2_poly_upload / h2_poly_download of the same elements; like them there is no range check (values >= p are taken as
+ * they are).  Asynchronous on `stream`: the copy runs after the caller's earlier work on `stream` and after the calling
+ * context's earlier calls, and the context's later calls run after it; no host synchronisation.  Refused before anything
+ * is launched: an unknown handle or one of another field, lens[i] above the polynomial's length, for upload a shared or
+ * repeated destination (download reads shared polynomials, on every lane), a null, host (use h2_poly_upload /
+ * h2_poly_download), other-device or not 16-byte aligned pointer, and for download destination ranges that overlap.
+ * lens[i] == 0 moves nothing and its pointer is not checked; count == 0 does nothing. */
+int h2_poly_upload_dev(const uint64_t *polys, size_t count, const void *const *d_src, const size_t *lens, int repr, void *stream);
+int h2_poly_download_dev(const uint64_t *polys, size_t count, void *const *d_dst, const size_t *lens, int repr, void *stream);
 /* a[index] += delta on a resident polynomial: the one-coefficient corrections of the opening argument
  * (poly/commitment/prover.rs:51 `s_poly[0] -= s_at_x3`, :78 `p_prime_poly[0] -= v`). */
 int h2_poly_add_at(uint64_t poly, size_t index, const void *delta, int repr);
