@@ -1,165 +1,11 @@
-"""plonk::create_proof composed from package calls only, for the argument tests: instance_commit / advice_commit,
-lookup_commit_permuted, permutation_commit, lookup_commit_product, vanishing_commit, the gates' expressions with the
-permutation and lookup arguments' construct, vanishing construct, evaluate_columns and every argument's evaluate in the
-reference's write order, the opens, and multiopen.create_proof.  Also:
-
-- a proving key built from Lagrange columns with the same transforms create_proof_engine uses;
-- a circuit whose lookup is not linear in the columns (a selector-gated input and table over two rows) with a pinned key,
-  so that compressing on the coset and extending the compressed Lagrange column give different polynomials.
-"""
+"""For the argument tests: a circuit whose lookup is not linear in the columns (a selector-gated input and table over two
+rows) with a pinned key, so that compressing on the coset and extending the compressed Lagrange column give different
+polynomials, and an on_construct hook for tests/plonk_prover.create_proof_engine that records that difference."""
 from __future__ import annotations
 
 import numpy as np
 
 from oracle import cref, pasta
-from tests import plonk_prover as PP
-
-
-# ---- the proving key ---------------------------------------------------------------------------------------------------
-def proving_key(h2, D, fixed, sigma, blinding_factors: int):
-    """A halo2_b200.ProvingKey of the Lagrange columns `fixed` and `sigma` (ints or (n, 32) uint8), every form made the
-    way create_proof_engine makes its key, and l_0 / l_blind / l_last (keygen.rs:306-325)."""
-    from halo2_b200.keygen import PermutationProvingKey
-    n, bf = D.n, blinding_factors
-    live = []
-
-    def keep(p):
-        live.append(p)
-        return p
-
-    def lag(vals):
-        return keep(h2.ResidentPoly(D.field, n, vals if hasattr(vals, "dtype") else cref.ints_to_bytes([v % D.m for v in vals])))
-
-    try:
-        coeff = lambda p: D.lagrange_to_coeff_resident(p, out=keep(h2.ResidentPoly(D.field, n)))           # noqa: E731
-        ext = lambda p: D.coeff_to_extended_resident(p, out=keep(h2.ResidentPoly(D.field, D.extended_len())))  # noqa: E731
-        fv = [lag(f) for f in fixed]
-        fp = [coeff(p) for p in fv]
-        sv = [lag(s) for s in sigma]
-        sp = [coeff(p) for p in sv]
-        ls, tmp = [], []
-        for rows in ({0}, set(range(n - bf, n)), {n - bf - 1}):
-            co = coeff(lag([1 if r in rows else 0 for r in range(n)]))
-            tmp += live[-2:]
-            ls.append(ext(co))
-        pk = h2.ProvingKey(fv, fp, [ext(p) for p in fp], PermutationProvingKey(sv, sp, [ext(p) for p in sp]), *ls)
-    except BaseException:
-        for p in live:
-            p.close()
-        raise
-    for p in tmp:
-        p.close()
-    return pk
-
-
-# ---- the composition ---------------------------------------------------------------------------------------------------
-def create_proof_package(h2, params, D, pk, vk, advice, instances, rng, transcript, delta: int, on_construct=None) -> None:
-    """plonk::create_proof (prover.rs:43-727) from package calls.  `pk`: a halo2_b200.ProvingKey; `advice[p]`, `instances[p]`:
-    proof p's columns; `rng`: scalar() and poly(n); `transcript`: tests/prover_replay.Blake2bTranscript.  on_construct, if
-    given, is called as on_construct(extended evaluator, permuted, lookups per proof over it, theta) once every argument is
-    constructed, before anything is closed."""
-    bf = vk.blinding_factors()
-    chunk_len = vk.degree() - 2
-    proofs = len(advice)
-    owned = []                                                     # everything with a close(), freed at the end whatever happens
-
-    def lookups_over(fixed, adv, inst):
-        ast = lambda e: PP._to_ast(h2, e, fixed, adv, inst)       # noqa: E731
-        return [([ast(e) for e in inp], [ast(e) for e in tab]) for inp, tab in vk.lookups]
-
-    def columns_of(fixed, adv, inst):
-        return [{"Advice": adv, "Fixed": fixed, "Instance": inst}[kind][i] for kind, i in vk.permutation_columns]
-
-    try:
-        transcript.common_scalar(vk.transcript_repr())
-        inst = h2.instance_commit(params, D, instances, bf)
-        owned += [p for s in inst for p in s.values + s.polys + s.cosets]
-        for s in inst:
-            for cm in s.commitments:
-                transcript.common_point(cm)
-        adv = h2.advice_commit(params, D, advice, rng, bf)
-        owned += [p for s in adv for p in s.values + s.polys + s.cosets]
-        for s in adv:
-            for cm in s.commitments:
-                transcript.write_point(cm)
-        ev_l = h2.Evaluator(D, "lagrange")
-        FL = [ev_l.register_poly(p) for p in pk.fixed_values]
-        AL = [[ev_l.register_poly(p) for p in s.values] for s in adv]
-        IL = [[ev_l.register_poly(p) for p in s.values] for s in inst]
-        theta = transcript.squeeze_challenge()
-        permuted, cms = h2.lookup_commit_permuted(params, D, ev_l, [lookups_over(FL, AL[p], IL[p]) for p in range(proofs)], theta, bf, rng)
-        owned += [q for per in permuted for lk in per for q in lk[:8]]
-        for cm in cms:
-            transcript.write_point(cm)
-        beta = transcript.squeeze_challenge()
-        gamma = transcript.squeeze_challenge()
-        sets, cms = h2.permutation_commit(params, D, pk, [columns_of(pk.fixed_values, adv[p].values, inst[p].values) for p in range(proofs)],
-                                          beta, gamma, delta, chunk_len, bf, rng)
-        perm_committed = [h2.PermutationCommitted(per) for per in sets]
-        owned += perm_committed
-        for cm in cms:
-            transcript.write_point(cm)
-        products, cms = h2.lookup_commit_product(params, D, permuted, beta, gamma, bf, rng)
-        lookup_committed = [h2.LookupCommitted(per, prods) for per, prods in zip(permuted, products)]
-        owned += lookup_committed
-        for cm in cms:
-            transcript.write_point(cm)
-        vanishing, cm = h2.vanishing_commit(params, D, rng)
-        owned.append(vanishing)
-        transcript.write_point(cm)
-        y = transcript.squeeze_challenge()
-        ev_e = h2.Evaluator(D, "extended")
-        FC = [ev_e.register_poly(p) for p in pk.fixed_cosets]
-        L0, LB, LL = (ev_e.register_poly(p) for p in (pk.l0, pk.l_blind, pk.l_last))
-        exprs, perms, lookups, lookup_exprs = [], [], [], []
-        for p in range(proofs):                                    # prover.rs:460-564: per proof the gates, the permutation, the lookups
-            AC = [ev_e.register_poly(c) for c in adv[p].cosets]
-            IC = [ev_e.register_poly(c) for c in inst[p].cosets]
-            exprs += [PP._to_ast(h2, g, FC, AC, IC) for g in vk.gates]
-            constructed, es = perm_committed[p].construct(ev_e, pk, columns_of(FC, AC, IC), L0, LB, LL, beta, gamma, delta, chunk_len, bf)
-            perms.append(constructed)
-            exprs += es
-            lookup_exprs.append(lookups_over(FC, AC, IC))
-            constructed, es = lookup_committed[p].construct(ev_e, lookup_exprs[-1], theta, beta, gamma, L0, LB, LL)
-            owned.append(constructed)
-            lookups.append(constructed)
-            exprs += es
-        if on_construct is not None:
-            on_construct(ev_e, permuted, lookup_exprs, theta)
-        vanishing, cms = vanishing.construct(params, D, ev_e, exprs, y, rng)
-        owned.append(vanishing)
-        for cm in cms:
-            transcript.write_point(cm)
-        x = transcript.squeeze_challenge()
-        queries = ([s.polys for s in inst], [s.polys for s in adv], pk.fixed_polys, vk.instance_queries, vk.advice_queries, vk.fixed_queries)
-        ie, ae, fe = h2.evaluate_columns(D, x, *queries)
-        for e in [v for per in ie for v in per] + [v for per in ae for v in per] + fe:
-            transcript.write_scalar(e)
-        vanishing, random_eval = vanishing.evaluate(D, x)
-        owned.append(vanishing)
-        transcript.write_scalar(random_eval)
-        for e in h2.permutation_key_evaluate(pk, D, x):
-            transcript.write_scalar(e)
-        perm_ev, lookup_ev = [], []
-        for c in perms:
-            ev, es = c.evaluate(D, x)
-            perm_ev.append(ev)
-            for e in es:
-                transcript.write_scalar(e)
-        for c in lookups:
-            ev, es = c.evaluate(D, x)
-            lookup_ev.append(ev)
-            for e in es:
-                transcript.write_scalar(e)
-        iq, aq, fq = h2.open_columns(D, x, queries[0], queries[1], [s.blinds for s in adv], *queries[2:])
-        opened = []
-        for p in range(proofs):
-            opened += iq[p] + aq[p] + perm_ev[p].open(x) + lookup_ev[p].open(x)
-        opened += fq + h2.permutation_key_open(pk, x) + vanishing.open(x)
-        h2.multiopen.create_proof(params, rng, transcript, opened)
-    finally:
-        for o in owned:
-            o.close()
 
 
 # ---- a lookup that is not linear in the columns ------------------------------------------------------------------------
@@ -267,7 +113,7 @@ def nonlinear_case(h2, k: int, commit_lagrange, zeta: int, delta: int, base: int
 
 
 def coset_compression_differs(h2, D):
-    """An on_construct hook for create_proof_package that records, per proof and lookup, whether the input and table
+    """An on_construct hook for create_proof_engine that records, per proof and lookup, whether the input and table
     compressed on the coset differ from the compressed Lagrange columns extended (the route for linear lookups only)."""
     from halo2_b200.arguments import _compress
     seen = []

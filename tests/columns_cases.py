@@ -1,93 +1,62 @@
-"""The instance and advice phases of plonk::create_proof two ways, for the column tests: create_proof_engine's per-column
-composition (run up to its first challenge) and halo2_b200.instance_commit / advice_commit.  Both return the same record:
-the points in transcript order and the bytes of every column's values, coefficient form and coset."""
+"""The instance and advice phases of plonk::create_proof two ways, for the column tests: a composition of per-column calls
+and halo2_b200.instance_commit / advice_commit.  Both return the same record: the points in transcript order and the bytes
+of every column's values, coefficient form and coset."""
 from __future__ import annotations
 
 import numpy as np
 
-from oracle import cref, pasta
+from oracle import cref
 from tests import multiopen_cases as MC
-from tests import plonk_prover as PP
-from tests import prover_replay as R
 
 
-class _Stop(Exception):
-    pass
-
-
-class ShapeKey:
-    """What create_proof_engine reads from a key before its first challenge, for a circuit shape without a pinned key."""
-
-    def __init__(self, field: str, k: int, degree: int, blinding_factors: int, zeta: int):
-        self.scalar_modulus, self.k, self._deg, self._bf = pasta.FIELDS[field], k, degree, blinding_factors
-        d = pasta.EvaluationDomain(field, degree, k, zeta)
-        self.extended_k, self.omega = d.extended_k, d.omega
-
-    def blinding_factors(self) -> int:
-        return self._bf
-
-    def degree(self) -> int:
-        return self._deg
-
-    def transcript_repr(self) -> int:
-        return 0
-
-
-def _skip_key():
-    """A proving-key dict that makes create_proof_engine skip its keygen part (the phases here do not read it)."""
-    return {"fixed_l": [], "fixed_p": [], "fixed_c": [], "sigma_l": [], "sigma_p": [], "sigma_c": [], "l": [None, None, None]}
-
-
-def engine_phases(h2, prm, vk, advice, instances, seed: int, zeta: int) -> dict:
-    """create_proof_engine through its instance and advice phases, under SeededRng(seed)."""
-    field = {pasta.P_MOD: "fp", pasta.Q_MOD: "fq"}[vk.scalar_modulus]
+def composition_phases(h2, prm, D, bf: int, advice, instances, seed: int) -> dict:
+    """The instance and advice phases one column at a time under SeededRng(seed): each column uploaded (an advice column's
+    last n - usable rows overwritten with the rng's draws, prover.rs:276-282), the columns of a proof committed in one pass
+    (instances with Blind::default(), advice with one drawn blind per column), then lagrange_to_coeff and coeff_to_extended
+    per column.  Closes what it made."""
+    rng = MC.SeededRng(D.field, seed, True)
+    n, usable = D.n, D.n - (bf + 1)
     rec = {"common": [], "written": [], "values": [], "polys": [], "cosets": []}
+    live = []
 
-    class D(h2.EvaluationDomain):
-        def lagrange_to_coeff_resident(self, a, out=None):
-            rec["values"].append(a.download(self.n))
-            r = super().lagrange_to_coeff_resident(a, out)
-            rec["polys"].append(r.download(self.n))
-            return r
+    def resident(vals, length=n):
+        p = h2.ResidentPoly(D.field, length, None if vals is None else vals if hasattr(vals, "dtype") else cref.ints_to_bytes([v % D.m for v in vals]))
+        live.append(p)
+        return p
 
-        def coeff_to_extended_resident(self, a, out=None):
-            r = super().coeff_to_extended_resident(a, out)
-            rec["cosets"].append(r.download(self.extended_len()))
-            return r
+    def transform(vals):
+        polys = [D.lagrange_to_coeff_resident(v, out=resident(None)) for v in vals]
+        cosets = [D.coeff_to_extended_resident(p, out=resident(None, D.extended_len())) for p in polys]
+        rec["values"] += [v.download(n) for v in vals]
+        rec["polys"] += [p.download(n) for p in polys]
+        rec["cosets"] += [c.download(D.extended_len()) for c in cosets]
 
-    class Eng:
-        EvaluationDomain = D
-
-        def __getattr__(self, name):
-            return getattr(h2, name)
-
-    class T(R.Blake2bTranscript):
-        def common_point(self, xy):
-            rec["common"].append(np.array(xy, dtype=np.uint8).reshape(64))
-            super().common_point(xy)
-
-        def write_point(self, xy):
-            rec["written"].append(np.array(xy, dtype=np.uint8).reshape(64))
-            super().write_point(xy)
-
-        def squeeze_challenge(self):
-            raise _Stop()
+    def commit(vals, blinds):
+        return list(prm.commit_resident_affine(vals, [h2.Blind(b) for b in blinds], lagrange=True)) if vals else []
 
     try:
-        PP.create_proof_engine(Eng(), prm, vk, [], [], advice, instances, MC.SeededRng(field, seed, True), T(vk.scalar_modulus), zeta, 0,
-                               pk=_skip_key())
-    except _Stop:
-        pass
+        for inst in instances:
+            vals = [resident(list(col) + [0] * (n - len(col))) for col in inst]
+            rec["common"] += commit(vals, [1] * len(vals))
+            transform(vals)
+        for cols in advice:
+            vals = []
+            for col in cols:
+                v = resident(col)
+                v.copy_from(resident([rng.scalar() for _ in range(n - usable)], n - usable), n - usable, dst_off=usable)
+                vals.append(v)
+            rec["written"] += commit(vals, [rng.scalar() for _ in vals])
+            transform(vals)
+    finally:
+        for p in live:
+            p.close()
     return rec
 
 
-def batched_phases(h2, prm, vk, advice, instances, seed: int, zeta: int) -> dict:
+def batched_phases(h2, prm, D, bf: int, advice, instances, seed: int) -> dict:
     """instance_commit and advice_commit on the same inputs under SeededRng(seed); closes what they made."""
-    field = {pasta.P_MOD: "fp", pasta.Q_MOD: "fq"}[vk.scalar_modulus]
-    D = h2.EvaluationDomain(field, vk.degree(), vk.k, zeta)
-    bf = vk.blinding_factors()
     inst = h2.instance_commit(prm, D, instances, bf)
-    adv = h2.advice_commit(prm, D, advice, MC.SeededRng(field, seed, True), bf)
+    adv = h2.advice_commit(prm, D, advice, MC.SeededRng(D.field, seed, True), bf)
     rec = {"common": [c for s in inst for c in s.commitments], "written": [c for s in adv for c in s.commitments],
            "values": [], "polys": [], "cosets": []}
     for s in list(inst) + list(adv):

@@ -432,6 +432,8 @@ class FakeLib:
                   args("inputs", ins[:count], False) + args("tables", ins[count:], False))
         if c:
             return self._fail(f"h2_poly_lookup_permuted: {c}")
+        if count == 0:
+            return 0
         f = self.polys[ins[0]][0]
         col = lambda hs: np.ascontiguousarray(np.concatenate([self.polys[h][1][:n] for h in hs]))  # noqa: E731
         oa, ot = col(outs[:count]), col(outs[count:])

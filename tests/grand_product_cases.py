@@ -1,7 +1,6 @@
 """The product columns of the permutation and lookup arguments two more ways, for the product tests: the reference's loops
-restated with big integers (plonk/permutation/prover.rs:81-168, plonk/lookup/prover.rs:279-321), and the composition the
-engine-API prover uses (tests/plonk_prover.create_proof_engine's product steps: Ast programs, batch_invert,
-running_product, the host's last_z)."""
+restated with big integers (plonk/permutation/prover.rs:81-168, plonk/lookup/prover.rs:279-321), and a composition of
+finer calls (Ast programs, batch_invert, running_product, the host's last_z)."""
 from __future__ import annotations
 
 from oracle import cref, pasta
@@ -50,7 +49,7 @@ def oracle_lookup_product(a, s, a_perm, s_perm, beta, gamma, bf, blinding, m):
     return z[:n - bf] + list(blinding)                                                       # :319-321
 
 
-# ---- the engine-API prover's composition ------------------------------------------------------------------------------
+# ---- the composition of finer calls ------------------------------------------------------------------------------------
 def _close(*groups):
     for g in groups:
         for p in g:

@@ -1,5 +1,5 @@
 """Lookup columns for the batched lookup permutation's tests and timings: input / table pairs with a full-width or a hot
-input, and the per-lookup composition create_proof_engine uses (h2_poly_lookup_permute, then the blinding rows)."""
+input, and a per-lookup composition of finer calls (h2_poly_lookup_permute, then the blinding rows)."""
 from __future__ import annotations
 
 import numpy as np
@@ -21,8 +21,7 @@ def columns(field, n, u, seed, hot):
 
 
 def composition(eng, D, pairs, bf, blinding):
-    """What tests/plonk_prover.create_proof_engine does per lookup: h2_poly_lookup_permute over the usable rows, then the
-    blinding rows uploaded into rows [u, n)."""
+    """Per lookup: h2_poly_lookup_permute over the usable rows, then the blinding rows uploaded into rows [u, n)."""
     rows, n = bf + 1, D.n
     out = []
     for b, (a, t) in enumerate(pairs):

@@ -138,6 +138,16 @@ def plonk_api_key():
     return PV.PinnedKey(CASE["key_text"])
 
 
+def plonk_api_oracle_proof(g, w, u) -> bytes:
+    """The oracle prover's proof of what plonk_api_proof proves (two proofs, instance 2, seed 777) over the generators g, w
+    and u ((x, y) bytes rows)."""
+    from oracle import cref
+    c, A = pasta.VESTA, cref.bytes_to_affine
+    P = pasta.Params.from_generators(c, K, [A(x) for x in g], A(w[0]), A(u[0]))
+    vk = plonk_api_key()
+    return prove((c, P, vk, fixed_columns(M, ZETA), permutation_columns(M, vk.omega, DELTA), None), [witness(), witness()], [[[2]], [[2]]], 777)
+
+
 def plonk_api_proof(h2, prm):
     """create_proof_engine on the plonk_api circuit (k = 5, two proofs, seed 777) through `h2`, recording what the permuted
     and product commitments need.  Returns (proof bytes, record): record["theta"], the Lagrange columns registered by then
@@ -176,14 +186,14 @@ def plonk_api_proof(h2, prm):
 
 
 def plonk_api_lookups(h2, seen):
-    """The recorded Lagrange columns registered again in the prover's order (fixed, sigma, advice per proof, instance per
-    proof) on a new evaluator, and the key's lookup expressions over it: (domain, evaluator, lookups[proof])."""
+    """The recorded Lagrange columns registered again in the prover's order (fixed, advice per proof, instance per proof) on a
+    new evaluator, and the key's lookup expressions over it: (domain, evaluator, lookups[proof])."""
     vk = plonk_api_key()
     D = h2.EvaluationDomain("fp", vk.degree(), vk.k, ZETA)
     ev = h2.Evaluator(D, "lagrange")
     leaves = [ev.register_poly(h2.ResidentPoly("fp", D.n, c)) for c in seen["cols"]]
-    nf, ns, na = len(fixed_columns(M, ZETA)), len(vk.permutation_columns), 5
-    FL, AL = leaves[:nf], [leaves[nf + ns + p * na:nf + ns + (p + 1) * na] for p in range(2)]
-    IL = [leaves[nf + ns + 2 * na + p:nf + ns + 2 * na + p + 1] for p in range(2)]
+    nf, na = len(fixed_columns(M, ZETA)), 5
+    FL, AL = leaves[:nf], [leaves[nf + p * na:nf + (p + 1) * na] for p in range(2)]
+    IL = [leaves[nf + 2 * na + p:nf + 2 * na + p + 1] for p in range(2)]
     ast = lambda e, p: PP._to_ast(h2, e, FL, AL[p], IL[p])
     return D, ev, [[([ast(e, p) for e in inp], [ast(e, p) for e in tab]) for inp, tab in vk.lookups] for p in range(2)]

@@ -271,11 +271,12 @@ def create_proof(c: pasta.Curve, g, g_lagrange, w, u, vk: PV.PinnedKey, fixed: L
 
 
 # ------------------------------------------------------------------------------------------------------------------------
-# The same prover through the ENGINE's reference-facing API (halo2_b200: resident polynomials, device transforms, Ast programs,
-# batch_invert / running product, the lookup permutation, fixed-base commits, the multi-point opening) -- the composition a
-# patched plonk::create_proof would make.  With the same seeded randomness it writes THE SAME PROOF BYTES as the oracle version
-# above.  (tests/test_real_proof.py runs it over the ABI stand-in: transforms and group operations through the oracle, the
-# Ast evaluator / scans / lookup permutation through the host-emulated device bodies.)
+# The same prover composed from the engine's phase calls (halo2_b200: instance_commit / advice_commit, lookup_commit_permuted,
+# permutation_commit, lookup_commit_product, vanishing_commit, the arguments' construct / evaluate / open, evaluate_columns /
+# open_columns, multiopen.create_proof) -- the composition a patched plonk::create_proof would make, with each lookup
+# compressed on the extended coset as lookup/prover.rs:172-176 does.  With the same seeded randomness it writes THE SAME PROOF
+# BYTES as the oracle version above.  (tests/test_real_proof.py runs it over the ABI stand-in: transforms and group operations
+# through the oracle, the device bodies on the host emulation.)
 # ------------------------------------------------------------------------------------------------------------------------
 def _to_ast(eng, e, fixed_l, advice_l, instance_l):
     """Expression::evaluate (circuit.rs:514-611) with the prover's closures (prover.rs:481-516): queries become leaves with rotations."""
@@ -297,42 +298,14 @@ def _to_ast(eng, e, fixed_l, advice_l, instance_l):
     raise ValueError(name)
 
 
-# The Ast programs create_proof_engine evaluates, built from leaves alone so that a test can run exactly the prover's programs
-# over columns of its own.  Column arguments are lists of leaves; a permutation or lookup argument's leaves come in its order.
+# The Ast programs CrefProver evaluates, built from leaves alone so that a test can run exactly the prover's programs over
+# columns of its own.  Column arguments are lists of leaves; a permutation or lookup argument's leaves come in its order.
 def lookup_compression(eng, exprs, theta: int, fixed, advice, instance):
     """compress_expressions of lookup/prover.rs commit_permuted: a lookup's input or table expressions compressed by powers of theta (Lagrange basis)."""
     acc = eng.Ast.constant_term(0)
     for e in exprs:
         acc = acc * theta + _to_ast(eng, e, fixed, advice, instance)
     return acc
-
-
-def permutation_denominator(eng, cols, sigmas, beta: int, gamma: int):
-    """permutation/prover.rs commit, before batch_invert: prod_j (beta * sigma_j + gamma + column_j) over one chunk of columns (Lagrange basis)."""
-    den = None
-    for col, sl in zip(cols, sigmas):
-        term = sl * beta + eng.Ast.constant_term(gamma) + col
-        den = term if den is None else den * term
-    return den
-
-
-def permutation_numerator(eng, inv_den, cols, first: int, beta: int, gamma: int, delta: int, m: int):
-    """permutation/prover.rs commit, after batch_invert: 1 / den * prod_j (beta * delta^(first + j) * omega^row + gamma + column_j); `first` is the
-    chunk's first global column index (Lagrange basis)."""
-    num = inv_den
-    for j, col in enumerate(cols):
-        num = num * (eng.Ast.linear_term(pow(delta, first + j, m) * beta % m) + eng.Ast.constant_term(gamma) + col)
-    return num
-
-
-def lookup_product_denominator(eng, permuted_input, permuted_table, beta: int, gamma: int):
-    """lookup/prover.rs commit_product, before batch_invert: (A' + beta) (S' + gamma) (Lagrange basis)."""
-    return (permuted_input + eng.Ast.constant_term(beta)) * (permuted_table + eng.Ast.constant_term(gamma))
-
-
-def lookup_product_numerator(eng, inv_den, input_, table, beta: int, gamma: int):
-    """lookup/prover.rs commit_product, after batch_invert: 1 / den * (A + beta) (S + gamma), A and S the compressed columns (Lagrange basis)."""
-    return inv_den * (input_ + eng.Ast.constant_term(beta)) * (table + eng.Ast.constant_term(gamma))
 
 
 def vanishing_expressions(eng, vk: PV.PinnedKey, beta: int, gamma: int, delta: int, fixed, sigmas, lagrange, advice, instance, perm_z, lookups):
@@ -373,245 +346,177 @@ def vanishing_expressions(eng, vk: PV.PinnedKey, beta: int, gamma: int, delta: i
     return exprs
 
 
-def create_proof_engine(eng, params, vk: PV.PinnedKey, fixed, sigma, advice, instances, rng, transcript, zeta: int, delta: int, pk=None) -> None:
-    """plonk::create_proof (prover.rs:43-727) on the engine.  `params`: halo2_b200.Params with u; `rng`: scalar() -> int,
-    poly(n) -> (n, 32) bytes; `transcript`: tests/prover_replay.Blake2bTranscript (points as (64,) uint8).  Columns are lists of
-    ints or (n, 32) uint8 arrays.  `pk`: a dict that keeps the key-dependent resident polynomials (the ProvingKey's fixed /
-    permutation polynomials and cosets, l_0 / l_blind / l_last: keygen.rs:240-331) between proofs; the caller closes its values."""
-    Ast, Blind = eng.Ast, eng.Blind
-    field = {pasta.P_MOD: "fp", pasta.Q_MOD: "fq"}[vk.scalar_modulus]
-    m = vk.scalar_modulus
-    k, n = vk.k, 1 << vk.k
-    bf = vk.blinding_factors()
-    usable = n - (bf + 1)
-    cs_degree = vk.degree()
-    chunk_len = cs_degree - 2
-    D = eng.EvaluationDomain(field, cs_degree, k, zeta)
-    assert D.extended_k == vk.extended_k and D.omega == vk.omega
-    L = D.extended_len()
-    num_proofs = len(advice)
+def proving_key(eng, D, fixed, sigma, blinding_factors: int):
+    """A halo2_b200.ProvingKey of the Lagrange columns `fixed` and `sigma` (ints or (n, 32) uint8): every column, its
+    coefficients and its extended coset, and l_0 / l_blind / l_last (keygen.rs:240-331).  The one key builder of the tests."""
+    from halo2_b200.keygen import PermutationProvingKey
+    n, bf = D.n, blinding_factors
     live = []
 
-    def RP(vals, length=n, keep=False):
-        data = None if vals is None else (vals if hasattr(vals, "dtype") else PV._ints_to_bytes(vals))
-        p = eng.ResidentPoly(field, length, data)
-        if not keep:
-            live.append(p)
+    def keep(p):
+        live.append(p)
         return p
 
-    coeff = lambda lag: D.lagrange_to_coeff_resident(lag, out=RP(None))
-    ext = lambda co: D.coeff_to_extended_resident(co, out=RP(None, L))
-    commit = lambda polys, blinds, lagrange: params.commit_resident_affine(polys, [Blind(b) for b in blinds], lagrange=lagrange)
+    def lag(vals):
+        return keep(eng.ResidentPoly(D.field, n, vals if hasattr(vals, "dtype") else PV._ints_to_bytes([v % D.m for v in vals])))
 
-    def overwrite_rows(p, start, vals):                            # rows [start, start + len) <- vals, on the device (h2_poly_copy)
-        tmp = RP(vals, len(vals))
-        p.copy_from(tmp, len(vals), src_off=0, dst_off=start)
-
-    def element(p, idx):                                           # one element back to the host
-        one = RP(None, 1)
-        one.copy_from(p, 1, src_off=idx)
-        return int.from_bytes(one.download(1)[0].tobytes(), "little")
-
-    own_pk = pk is None
     try:
-        transcript.common_scalar(vk.transcript_repr())
-        # ---- instance and advice columns ----
-        inst_l, inst_p, inst_c = [], [], []
-        for inst in instances:
-            vals = [RP([v % m for v in col] + [0] * (n - len(col))) for col in inst]
-            if vals:
-                for cm in commit(vals, [1] * len(vals), True):
-                    transcript.common_point(cm)
-            polys = [coeff(v) for v in vals]
-            inst_l.append(vals), inst_p.append(polys), inst_c.append([ext(p) for p in polys])
-        adv_l, adv_p, adv_c, adv_b = [], [], [], []
-        for cols in advice:
-            vals = []
-            for col in cols:                                        # the blinding rows are the prover's (prover.rs:276-282)
-                v = RP(col if hasattr(col, "dtype") else [x % m for x in col])
-                overwrite_rows(v, usable, [rng.scalar() for _ in range(n - usable)])
-                vals.append(v)
-            blinds = [rng.scalar() for _ in vals]
-            for cm in commit(vals, blinds, True):                   # all columns of a proof in one pass (prover.rs:290-299)
-                transcript.write_point(cm)
-            polys = [coeff(v) for v in vals]
-            adv_l.append(vals), adv_p.append(polys), adv_c.append([ext(p) for p in polys]), adv_b.append(blinds)
-        own_pk = pk is None
-        pk = {} if pk is None else pk
-        if "fixed_l" not in pk:                                     # keygen_pk's part (keygen.rs:240-331), once per key
-            kcoeff = lambda lag: D.lagrange_to_coeff_resident(lag, out=RP(None, keep=True))
-            kext = lambda co: D.coeff_to_extended_resident(co, out=RP(None, L, keep=True))
-            pk["fixed_l"] = [RP(f, keep=True) for f in fixed]
-            pk["fixed_p"] = [kcoeff(f) for f in pk["fixed_l"]]
-            pk["fixed_c"] = [kext(p_) for p_ in pk["fixed_p"]]
-            pk["sigma_l"] = [RP(s_, keep=True) for s_ in sigma]
-            pk["sigma_p"] = [kcoeff(s_) for s_ in pk["sigma_l"]]
-            pk["sigma_c"] = [kext(p_) for p_ in pk["sigma_p"]]
-            pk["l"] = []
-            for rows in ({0}, set(range(n - bf, n)), {n - bf - 1}):
-                lag = RP([1 if r in rows else 0 for r in range(n)], keep=True)
-                co = kcoeff(lag)
-                pk["l"].append(kext(co))
-                pk.setdefault("tmp", []).extend([lag, co])
-        fixed_l, fixed_p, fixed_c = pk["fixed_l"], pk["fixed_p"], pk["fixed_c"]
-        sigma_l, sigma_p, sigma_c = pk["sigma_l"], pk["sigma_p"], pk["sigma_c"]
-        l0_c, l_blind_c, l_last_c = pk["l"]
-        # the Lagrange-basis evaluator (value_evaluator, prover.rs:331-365)
-        ev_l = eng.Evaluator(D, "lagrange")
-        FL = [ev_l.register_poly(p) for p in fixed_l]
-        SL = [ev_l.register_poly(p) for p in sigma_l]
-        AL = [[ev_l.register_poly(p) for p in cols] for cols in adv_l]
-        IL = [[ev_l.register_poly(p) for p in cols] for cols in inst_l]
-        theta = transcript.squeeze_challenge()
-        # ---- lookups: compressed and permuted columns ----
-        lookups = []
-        for pr in range(num_proofs):
-            per = []
-            for inp, tab in vk.lookups:
-                ci, ct = (ev_l.evaluate(lookup_compression(eng, exprs, theta, FL, AL[pr], IL[pr]), out=RP(None)) for exprs in (inp, tab))
-                pi, pt = eng.permute_expression_pair_resident(ci, ct, usable, RP(None), RP(None))
-                overwrite_rows(pi, usable, [rng.scalar() for _ in range(bf + 1)])
-                overwrite_rows(pt, usable, [rng.scalar() for _ in range(bf + 1)])
-                bi = rng.scalar()
-                bt = rng.scalar()
-                cmi, cmt = commit([pi, pt], [bi, bt], True)
-                transcript.write_point(cmi)
-                transcript.write_point(cmt)
-                per.append({"ci": ci, "ct": ct, "pi": pi, "pt": pt, "pi_poly": coeff(pi), "pt_poly": coeff(pt), "bi": bi, "bt": bt})
-            lookups.append(per)
-        beta = transcript.squeeze_challenge()
-        gamma = transcript.squeeze_challenge()
-        # ---- permutation products: denominators and numerators as Ast programs, batch_invert, the running product ----
-        col_leaf = lambda pr, col: {"Advice": AL[pr], "Fixed": FL, "Instance": IL[pr]}[col[0]][col[1]]
-        perms = []
-        for pr in range(num_proofs):
-            sets, last_z = [], 1
-            for ci_ in range(0, len(vk.permutation_columns), chunk_len):
-                cols = [col_leaf(pr, col) for col in vk.permutation_columns[ci_:ci_ + chunk_len]]
-                den = permutation_denominator(eng, cols, SL[ci_:ci_ + chunk_len], beta, gamma)
-                inv_den = eng.batch_invert_resident(ev_l.evaluate(den, out=RP(None)))
-                num = permutation_numerator(eng, ev_l.register_poly(inv_den), cols, ci_, beta, gamma, delta, m)
-                mv = ev_l.evaluate(num, out=RP(None))
-                z = eng.running_product_resident(mv, init=last_z, dst=RP(None))
-                overwrite_rows(z, n - bf, [rng.scalar() for _ in range(bf)])
-                last_z = element(z, n - (bf + 1))
-                blind = rng.scalar()
-                transcript.write_point(commit([z], [blind], True)[0])
-                zp = coeff(z)
-                sets.append({"poly": zp, "coset": ext(zp), "blind": blind})
-            perms.append(sets)
-        # ---- lookup products ----
-        for pr in range(num_proofs):
-            for lk in lookups[pr]:
-                PI, PT, CI, CT = (ev_l.register_poly(lk[kk]) for kk in ("pi", "pt", "ci", "ct"))
-                inv_den = eng.batch_invert_resident(ev_l.evaluate(lookup_product_denominator(eng, PI, PT, beta, gamma), out=RP(None)))
-                num = lookup_product_numerator(eng, ev_l.register_poly(inv_den), CI, CT, beta, gamma)
-                z = eng.running_product_resident(ev_l.evaluate(num, out=RP(None)), init=1, dst=RP(None))
-                overwrite_rows(z, n - bf, [rng.scalar() for _ in range(bf)])
-                lk["zb"] = rng.scalar()
-                transcript.write_point(commit([z], [lk["zb"]], True)[0])
-                lk["z_poly"] = coeff(z)
-        # ---- the vanishing argument's random polynomial ----
-        random_poly = rng.poly(n)
-        random_poly = random_poly if isinstance(random_poly, eng.ResidentPoly) else eng.ResidentPoly(field, n, random_poly)
-        live.append(random_poly)
-        random_blind = rng.scalar()
-        transcript.write_point(commit([random_poly], [random_blind], False)[0])
-        y = transcript.squeeze_challenge()
-        # ---- h(X): one Ast over the cosets, folded by y; / (X^n - 1); back to coefficients; pieces ----
-        ev_e = eng.Evaluator(D, "extended")
-        FC = [ev_e.register_poly(p) for p in fixed_c]
-        SC = [ev_e.register_poly(p) for p in sigma_c]
-        L0, LB, LL = (ev_e.register_poly(p) for p in (l0_c, l_blind_c, l_last_c))
-        exprs = []
-        for pr in range(num_proofs):
-            AC = [ev_e.register_poly(p) for p in adv_c[pr]]
-            IC = [ev_e.register_poly(p) for p in inst_c[pr]]
-            ZC = [ev_e.register_poly(s["coset"]) for s in perms[pr]]
-            LK = [tuple(ev_e.register_poly(ext(lk[kk])) for kk in ("z_poly", "pi_poly", "pt_poly"))
-                  + tuple(ev_e.register_poly(ext(coeff(lk[kk]))) for kk in ("ci", "ct")) for lk in lookups[pr]]
-            exprs += vanishing_expressions(eng, vk, beta, gamma, delta, FC, SC, (L0, LB, LL), AC, IC, ZC, LK)
-        last_rot = -(bf + 1)
-        h_ext = ev_e.evaluate(Ast.distribute_powers(exprs, y), out=RP(None, L))
-        D.divide_by_vanishing_poly_resident(h_ext)
-        h = D.extended_to_coeff_resident(h_ext, out=RP(None, n * (cs_degree - 1)))
-        h_pieces = [RP(None).copy_from(h, n, src_off=a * n) for a in range(cs_degree - 1)]
-        h_blinds = [rng.scalar() for _ in h_pieces]
-        for cm in commit(h_pieces, h_blinds, False):
-            transcript.write_point(cm)
-        x = transcript.squeeze_challenge()
-        xn = pow(x, n, m)
-        rotx = lambda r: D.rotate_omega(x, r)
-        # ---- every evaluation in ONE batched reduction, written in the reference's order ----
-        ev_list = []
-        for pr in range(num_proofs):
-            ev_list += [(inst_p[pr][col], rotx(r)) for col, r in vk.instance_queries]
-        for pr in range(num_proofs):
-            ev_list += [(adv_p[pr][col], rotx(r)) for col, r in vk.advice_queries]
-        ev_list += [(fixed_p[col], rotx(r)) for col, r in vk.fixed_queries]
-        ev_list.append((random_poly, x))
-        ev_list += [(sp, x) for sp in sigma_p]
-        for pr in range(num_proofs):
-            sets = perms[pr]
-            for a, st in enumerate(sets):
-                ev_list += [(st["poly"], x), (st["poly"], rotx(1))]
-                if a + 1 < len(sets):
-                    ev_list.append((st["poly"], rotx(last_rot)))
-        for pr in range(num_proofs):
-            for lk in lookups[pr]:
-                ev_list += [(lk["z_poly"], x), (lk["z_poly"], rotx(1)), (lk["pi_poly"], x), (lk["pi_poly"], rotx(-1)), (lk["pt_poly"], x)]
-        for e in eng.eval_polynomial_resident([p for p, _ in ev_list], [pt for _, pt in ev_list], n=n):
-            transcript.write_scalar(e)
-        # h_poly = sum_i piece_i * xn^i, one scale_add pass per piece (vanishing/prover.rs:128-138)
-        h_poly = RP(None).copy_from(h_pieces[-1], n)
-        h_blind = h_blinds[-1]
-        for piece, b in zip(reversed(h_pieces[:-1]), reversed(h_blinds[:-1])):
-            eng.opening._scale_add(h_poly, xn, piece, 1, n)
-            h_blind = (h_blind * xn + b) % m
-        # ---- the query list and the multi-point opening ----
-        Q = eng.multiopen.ProverQuery
-        one_b = Blind(1)
-        queries = []
-        for pr in range(num_proofs):
-            queries += [Q(rotx(r), inst_p[pr][col], one_b) for col, r in vk.instance_queries]
-            queries += [Q(rotx(r), adv_p[pr][col], Blind(adv_b[pr][col])) for col, r in vk.advice_queries]
-            sets = perms[pr]
-            for st in sets:
-                queries += [Q(x, st["poly"], Blind(st["blind"])), Q(rotx(1), st["poly"], Blind(st["blind"]))]
-            for st in list(reversed(sets))[1:]:
-                queries.append(Q(rotx(last_rot), st["poly"], Blind(st["blind"])))
-            for lk in lookups[pr]:
-                queries += [Q(x, lk["z_poly"], Blind(lk["zb"])), Q(x, lk["pi_poly"], Blind(lk["bi"])), Q(x, lk["pt_poly"], Blind(lk["bt"])),
-                            Q(rotx(-1), lk["pi_poly"], Blind(lk["bi"])), Q(rotx(1), lk["z_poly"], Blind(lk["zb"]))]
-        queries += [Q(rotx(r), fixed_p[col], one_b) for col, r in vk.fixed_queries]
-        queries += [Q(x, sp, one_b) for sp in sigma_p]
-        queries.append(Q(x, h_poly, Blind(h_blind)))
-        queries.append(Q(x, random_poly, Blind(random_blind)))
-        eng.multiopen.create_proof(params, rng, transcript, queries)
-    finally:
+        coeff = lambda p: D.lagrange_to_coeff_resident(p, out=keep(eng.ResidentPoly(D.field, n)))           # noqa: E731
+        ext = lambda p: D.coeff_to_extended_resident(p, out=keep(eng.ResidentPoly(D.field, D.extended_len())))  # noqa: E731
+        fv = [lag(f) for f in fixed]
+        fp = [coeff(p) for p in fv]
+        sv = [lag(s) for s in sigma]
+        sp = [coeff(p) for p in sv]
+        ls, tmp = [], []
+        for rows in ({0}, set(range(n - bf, n)), {n - bf - 1}):
+            co = coeff(lag([1 if r in rows else 0 for r in range(n)]))
+            tmp += live[-2:]
+            ls.append(ext(co))
+        pk = eng.ProvingKey(fv, fp, [ext(p) for p in fp], PermutationProvingKey(sv, sp, [ext(p) for p in sp]), *ls)
+    except BaseException:
         for p in live:
             p.close()
-        if own_pk and pk:
-            close_proving_key(pk)
+        raise
+    for p in tmp:
+        p.close()
+    return pk
 
 
-def prover_pk_dict(pk):
-    """A halo2_b200.ProvingKey in the shape create_proof_engine(pk=...) keeps it."""
-    P = pk.permutation
-    return {"fixed_l": pk.fixed_values, "fixed_p": pk.fixed_polys, "fixed_c": pk.fixed_cosets, "sigma_l": P.permutations,
-            "sigma_p": P.polys, "sigma_c": P.cosets, "l": [pk.l0, pk.l_blind, pk.l_last]}
+def close_proving_key(pk: dict) -> None:
+    """Closes the key create_proof_engine stored in the dict `pk`, if it stored one."""
+    key = pk.pop("key", None)
+    if key is not None:
+        key.close()
 
 
 def prover_pk_bytes(pk) -> list:
-    """The bytes of every polynomial of a halo2_b200.ProvingKey, in prover_pk_dict's order."""
-    d = prover_pk_dict(pk)
-    return [p.download().tobytes() for key in ("fixed_l", "fixed_p", "fixed_c", "sigma_l", "sigma_p", "sigma_c", "l") for p in d[key]]
+    """The bytes of every polynomial of a halo2_b200.ProvingKey: fixed values, coefficients and cosets, then the permutation's,
+    then l_0, l_blind and l_last."""
+    return [p.download().tobytes() for p in pk._all()]
 
 
-def close_proving_key(pk) -> None:
-    for key in ("fixed_l", "fixed_p", "fixed_c", "sigma_l", "sigma_p", "sigma_c", "l", "tmp"):
-        for p in pk.pop(key, []):
-            p.close()
+def create_proof_engine(eng, params, vk: PV.PinnedKey, fixed, sigma, advice, instances, rng, transcript, zeta: int, delta: int, pk=None,
+                        on_construct=None) -> None:
+    """plonk::create_proof (prover.rs:43-727) from the engine's phase calls.  `params`: halo2_b200.Params with u; `rng`:
+    scalar() -> int, poly(n) -> (n, 32) bytes; `transcript`: tests/prover_replay.Blake2bTranscript (points as (64,) uint8).
+    Columns are lists of ints or (n, 32) uint8 arrays; `advice[p]`, `instances[p]`: proof p's.
+
+    `pk`: a halo2_b200.ProvingKey, used as it is (the caller closes it); None, for a key built from `fixed` and `sigma` and
+    closed at the end; or a dict (see below).  `on_construct`, if given, is called as on_construct(extended evaluator,
+    permuted lookups per proof, lookup expressions per proof over that evaluator, theta) once every argument is constructed,
+    before anything is closed."""
+    field = {pasta.P_MOD: "fp", pasta.Q_MOD: "fq"}[vk.scalar_modulus]
+    bf = vk.blinding_factors()
+    chunk_len = vk.degree() - 2
+    D = eng.EvaluationDomain(field, vk.degree(), vk.k, zeta)
+    assert D.extended_k == vk.extended_k and D.omega == vk.omega
+    proofs = len(advice)
+    owned = []                                                     # everything with a close(), freed at the end whatever happens
+
+    def lookups_over(fixed_, adv_, inst_):
+        ast = lambda e: _to_ast(eng, e, fixed_, adv_, inst_)       # noqa: E731
+        return [([ast(e) for e in inp], [ast(e) for e in tab]) for inp, tab in vk.lookups]
+
+    def columns_of(fixed_, adv_, inst_):
+        return [{"Advice": adv_, "Fixed": fixed_, "Instance": inst_}[kind][i] for kind, i in vk.permutation_columns]
+
+    try:
+        if pk is None:
+            pk = proving_key(eng, D, fixed, sigma, bf)
+            owned.append(pk)
+        elif isinstance(pk, dict):                                 # only for bench.py: it keeps the key between proofs in a dict
+            if "key" not in pk:                                    # and frees it with close_proving_key
+                pk["key"] = proving_key(eng, D, fixed, sigma, bf)
+            pk = pk["key"]
+        transcript.common_scalar(vk.transcript_repr())
+        inst = eng.instance_commit(params, D, instances, bf)
+        owned += [p for s in inst for p in s.values + s.polys + s.cosets]
+        for s in inst:
+            for cm in s.commitments:
+                transcript.common_point(cm)
+        adv = eng.advice_commit(params, D, advice, rng, bf)
+        owned += [p for s in adv for p in s.values + s.polys + s.cosets]
+        for s in adv:
+            for cm in s.commitments:
+                transcript.write_point(cm)
+        ev_l = eng.Evaluator(D, "lagrange")
+        FL = [ev_l.register_poly(p) for p in pk.fixed_values]
+        AL = [[ev_l.register_poly(p) for p in s.values] for s in adv]
+        IL = [[ev_l.register_poly(p) for p in s.values] for s in inst]
+        theta = transcript.squeeze_challenge()
+        permuted, cms = eng.lookup_commit_permuted(params, D, ev_l, [lookups_over(FL, AL[p], IL[p]) for p in range(proofs)], theta, bf, rng)
+        owned += [q for per in permuted for lk in per for q in lk[:8]]
+        for cm in cms:
+            transcript.write_point(cm)
+        beta = transcript.squeeze_challenge()
+        gamma = transcript.squeeze_challenge()
+        sets, cms = eng.permutation_commit(params, D, pk, [columns_of(pk.fixed_values, adv[p].values, inst[p].values) for p in range(proofs)],
+                                           beta, gamma, delta, chunk_len, bf, rng)
+        perm_committed = [eng.PermutationCommitted(per) for per in sets]
+        owned += perm_committed
+        for cm in cms:
+            transcript.write_point(cm)
+        products, cms = eng.lookup_commit_product(params, D, permuted, beta, gamma, bf, rng)
+        lookup_committed = [eng.LookupCommitted(per, prods) for per, prods in zip(permuted, products)]
+        owned += lookup_committed
+        for cm in cms:
+            transcript.write_point(cm)
+        vanishing, cm = eng.vanishing_commit(params, D, rng)
+        owned.append(vanishing)
+        transcript.write_point(cm)
+        y = transcript.squeeze_challenge()
+        ev_e = eng.Evaluator(D, "extended")
+        FC = [ev_e.register_poly(p) for p in pk.fixed_cosets]
+        L0, LB, LL = (ev_e.register_poly(p) for p in (pk.l0, pk.l_blind, pk.l_last))
+        exprs, perms, lookups, lookup_exprs = [], [], [], []
+        for p in range(proofs):                                    # prover.rs:460-564: per proof the gates, the permutation, the lookups
+            AC = [ev_e.register_poly(c) for c in adv[p].cosets]
+            IC = [ev_e.register_poly(c) for c in inst[p].cosets]
+            exprs += [_to_ast(eng, g, FC, AC, IC) for g in vk.gates]
+            constructed, es = perm_committed[p].construct(ev_e, pk, columns_of(FC, AC, IC), L0, LB, LL, beta, gamma, delta, chunk_len, bf)
+            perms.append(constructed)
+            exprs += es
+            lookup_exprs.append(lookups_over(FC, AC, IC))
+            constructed, es = lookup_committed[p].construct(ev_e, lookup_exprs[-1], theta, beta, gamma, L0, LB, LL)
+            owned.append(constructed)
+            lookups.append(constructed)
+            exprs += es
+        if on_construct is not None:
+            on_construct(ev_e, permuted, lookup_exprs, theta)
+        vanishing, cms = vanishing.construct(params, D, ev_e, exprs, y, rng)
+        owned.append(vanishing)
+        for cm in cms:
+            transcript.write_point(cm)
+        x = transcript.squeeze_challenge()
+        queries = ([s.polys for s in inst], [s.polys for s in adv], pk.fixed_polys, vk.instance_queries, vk.advice_queries, vk.fixed_queries)
+        ie, ae, fe = eng.evaluate_columns(D, x, *queries)
+        for e in [v for per in ie for v in per] + [v for per in ae for v in per] + fe:
+            transcript.write_scalar(e)
+        vanishing, random_eval = vanishing.evaluate(D, x)
+        owned.append(vanishing)
+        transcript.write_scalar(random_eval)
+        for e in eng.permutation_key_evaluate(pk, D, x):
+            transcript.write_scalar(e)
+        perm_ev, lookup_ev = [], []
+        for c in perms:
+            ev, es = c.evaluate(D, x)
+            perm_ev.append(ev)
+            for e in es:
+                transcript.write_scalar(e)
+        for c in lookups:
+            ev, es = c.evaluate(D, x)
+            lookup_ev.append(ev)
+            for e in es:
+                transcript.write_scalar(e)
+        iq, aq, fq = eng.open_columns(D, x, queries[0], queries[1], [s.blinds for s in adv], *queries[2:])
+        opened = []
+        for p in range(proofs):
+            opened += iq[p] + aq[p] + perm_ev[p].open(x) + lookup_ev[p].open(x)
+        opened += fq + eng.permutation_key_open(pk, x) + vanishing.open(x)
+        eng.multiopen.create_proof(params, rng, transcript, opened)
+    finally:
+        for o in owned:
+            o.close()
 
 
 # ------------------------------------------------------------------------------------------------------------------------

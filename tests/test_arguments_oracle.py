@@ -1,11 +1,9 @@
 """The permutation and lookup arguments' construct / evaluate / open and the column evaluations (halo2_b200.arguments) over
 the ABI stand-in, without a GPU:
 
-- the plonk_api circuit (a linear lookup) proved with package calls only writes the oracle prover's and
-  create_proof_engine's 4160 bytes, which the golden-pinned verifier accepts;
 - a circuit with a selector-gated, two-row lookup (tests/arguments_cases.py) at k = 4 ... 6, two proofs and three
-  permutation sets: the package's proofs are accepted, a flipped byte or a wrong instance is rejected, and its compressed
-  input and table differ between the coset compression and the extended Lagrange column;
+  permutation sets: tests/plonk_prover.create_proof_engine's proofs are accepted, a flipped byte or a wrong instance is
+  rejected, and its compressed input and table differ between the coset compression and the extended Lagrange column;
 - every argument error raises before any launch, and every object frees what it allocated on every path."""
 import numpy as np
 import pytest
@@ -13,7 +11,6 @@ import pytest
 import halo2_b200
 from halo2_b200 import arguments as A
 from halo2_b200 import lib as L
-from oracle import cref, pasta
 from tests import arguments_cases as AC
 from tests import fake_engine
 from tests import multiopen_cases as MC
@@ -27,49 +24,15 @@ def _gens(prm_gens):
     return tuple(np.asarray(g) for g in prm_gens)
 
 
-def test_plonk_api_proof_from_package_calls_is_byte_identical():
-    """Under the golden key and one seeded rng, the package composition writes the oracle prover's proof and
-    create_proof_engine's, and frees every polynomial it made; the golden-pinned verifier accepts the proof."""
-    c = pasta.VESTA
-    P = pasta.Params.new(c, 5)
-    vk = PV.PinnedKey(circ.CASE["key_text"])
-    fixed, sigma = circ.fixed_columns(circ.M, circ.ZETA), circ.permutation_columns(circ.M, vk.omega, circ.DELTA)
-    gens = (cref.affines_to_bytes(P.g), cref.affines_to_bytes(P.g_lagrange), cref.affines_to_bytes([P.w]), cref.affines_to_bytes([P.u]))
-    inst = [[[2]], [[2]]]
-    oracle = circ.prove((c, P, vk, fixed, sigma, gens), [circ.witness(), circ.witness()], inst, 777)
-    with fake_engine.installed() as fake:
-        prm = halo2_b200.Params("vesta", 5, gens[0], gens[1], gens[2], u=gens[3])
-        D = halo2_b200.EvaluationDomain("fp", vk.degree(), vk.k, circ.ZETA)
-        T = R.Blake2bTranscript(circ.M)
-        PP.create_proof_engine(halo2_b200, prm, vk, fixed, sigma, [circ.witness(), circ.witness()], inst, MC.SeededRng("fp", 777, True), T, circ.ZETA, circ.DELTA)
-        engine = bytes(T.proof)
-        pk = AC.proving_key(halo2_b200, D, fixed, sigma, vk.blinding_factors())
-        held, calls = set(fake.polys), len(fake.calls)
-        T = R.Blake2bTranscript(circ.M)
-        AC.create_proof_package(halo2_b200, prm, D, pk, vk, [circ.witness(), circ.witness()], inst, MC.SeededRng("fp", 777, True), T, circ.DELTA)
-        got = bytes(T.proof)
-        assert set(fake.polys) == held                             # the composition freed everything it made
-        mine = fake.calls[calls:]
-        assert mine.count("h2_poly_coeff_to_extended_batch") == 2 + 2     # instance and advice columns; each proof's lookup products
-        assert "h2_poly_lookup_permute" not in mine and mine.count("h2_poly_lookup_permuted") == 1
-        pk.close()
-        prm.close()
-        assert not fake.polys
-    assert len(got) == 4160 and got == engine == oracle
-    assert PV.verify_proof(PV.OracleArm("vesta", 5, *gens), vk, got, inst, circ.DELTA)
-
-
 def _nonlinear_proof(k, seed=11, instance=None, hook=None):
     prm, commit, gens = AC.params_for(halo2_b200, k)
     vk, D, fixed, sigma, advice, inst = AC.nonlinear_case(halo2_b200, k, commit, circ.ZETA, circ.DELTA)
-    pk = AC.proving_key(halo2_b200, D, fixed, sigma, vk.blinding_factors())
     insts = [inst, inst] if instance is None else instance
     try:
         T = R.Blake2bTranscript(circ.M)
-        AC.create_proof_package(halo2_b200, prm, D, pk, vk, [advice, advice], insts, MC.SeededRng("fp", seed, True), T, circ.DELTA,
-                                on_construct=hook(D) if hook else None)
+        PP.create_proof_engine(halo2_b200, prm, vk, fixed, sigma, [advice, advice], insts, MC.SeededRng("fp", seed, True), T, circ.ZETA, circ.DELTA,
+                               on_construct=hook(D) if hook else None)
     finally:
-        pk.close()
         prm.close()
     return vk, bytes(T.proof), inst, gens
 

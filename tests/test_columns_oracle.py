@@ -1,7 +1,7 @@
 """CPU checks of the column-batched transforms and of instance_commit / advice_commit: the batched NTT pass bodies on the
 host emulation against the oracle's transforms, h2_poly_set_rows on the ABI stand-in (tests/fake_engine.py) against
 per-column copies, and the two phases over the stand-in against
-create_proof_engine's per-column composition on the plonk_api circuit."""
+a composition of per-column calls on the plonk_api circuit."""
 import ctypes
 
 import numpy as np
@@ -94,8 +94,8 @@ def test_set_rows_equals_per_column_copies():
 
 
 def test_phases_of_the_plonk_api_circuit():
-    """instance_commit and advice_commit over the stand-in equal create_proof_engine's instance and advice phases on the
-    plonk_api circuit (k = 5, 5 advice columns, two proofs) under the same rng: the commitments in transcript order and the
+    """instance_commit and advice_commit over the stand-in equal the per-column composition of the instance and advice phases
+    on the plonk_api circuit (k = 5, 5 advice columns, two proofs) under the same rng: the commitments in transcript order and the
     bytes of every column's values, polynomial and coset.  advice_commit makes one set_rows call, and the two phases one
     batched call per transform each."""
     import halo2_b200
@@ -104,9 +104,10 @@ def test_phases_of_the_plonk_api_circuit():
         g, gl, w, u = _gens()
         prm = halo2_b200.Params("vesta", 5, g, gl, w, u=u)
         advice, instances = [circ.witness(), circ.witness()], [[[2]], [[2]]]
-        want = CC.engine_phases(halo2_b200, prm, vk, advice, instances, 777, circ.ZETA)
+        D = halo2_b200.EvaluationDomain("fp", vk.degree(), vk.k, circ.ZETA)
+        want = CC.composition_phases(halo2_b200, prm, D, vk.blinding_factors(), advice, instances, 777)
         fake.calls.clear()
-        got = CC.batched_phases(halo2_b200, prm, vk, advice, instances, 777, circ.ZETA)
+        got = CC.batched_phases(halo2_b200, prm, D, vk.blinding_factors(), advice, instances, 777)
         for name in ("h2_poly_set_rows", "h2_poly_lagrange_to_coeff_batch", "h2_poly_coeff_to_extended_batch"):
             assert fake.calls.count(name) == (1 if name == "h2_poly_set_rows" else 2), name
         assert fake.calls.count("h2_msm_registered_polys_affine") == 2

@@ -1,15 +1,13 @@
-"""GPU checks of halo2_b200.arguments: proofs composed from package calls only (tests/arguments_cases.create_proof_package)
-against create_proof_engine on the plonk_api circuit and on the benchmark circuit at k = 14, the circuit with a selector-gated
-two-row lookup at k = 8 ... 18, the same proofs on a lane over a shared proving key, and cleanup when construct or evaluate
-fails."""
-import numpy as np
+"""GPU checks of halo2_b200.arguments: proofs composed from the phase calls (tests/plonk_prover.create_proof_engine) of the
+circuit with a selector-gated two-row lookup at k = 8 ... 18, the same proofs on a lane over a shared proving key, and cleanup
+when construct or evaluate fails.  tests/test_gpu_zz_real_proof.py checks the composition's bytes against the references."""
 import pytest
 
 import halo2_b200
 from halo2_b200 import arguments as A
 from halo2_b200 import lib as L
 from halo2_b200 import poly as P
-from oracle import cref, pasta
+from oracle import cref
 from tests import arguments_cases as AC
 from tests import multiopen_cases as MC
 from tests import plonk_api_circuit as circ
@@ -20,54 +18,11 @@ from tests import prover_replay as R
 pytestmark = pytest.mark.gpu
 
 
-def _engine_proof(prm, vk, fixed, sigma, advice, inst, seed, pk=None):
+def _proof(prm, vk, pk, advice, inst, seed, hook=None):
     T = R.Blake2bTranscript(circ.M)
-    PP.create_proof_engine(halo2_b200, prm, vk, fixed, sigma, advice, inst, MC.SeededRng("fp", seed, True), T, circ.ZETA, circ.DELTA, pk=pk)
+    PP.create_proof_engine(halo2_b200, prm, vk, None, None, advice, inst, MC.SeededRng("fp", seed, True), T, circ.ZETA, circ.DELTA, pk=pk,
+                           on_construct=hook)
     return bytes(T.proof)
-
-
-def _package_proof(prm, D, pk, vk, advice, inst, seed, hook=None):
-    T = R.Blake2bTranscript(circ.M)
-    AC.create_proof_package(halo2_b200, prm, D, pk, vk, advice, inst, MC.SeededRng("fp", seed, True), T, circ.DELTA, on_construct=hook)
-    return bytes(T.proof)
-
-
-def test_plonk_api_circuit_equals_create_proof_engine():
-    vk = PV.PinnedKey(circ.CASE["key_text"])
-    fixed, sigma = circ.fixed_columns(circ.M, circ.ZETA), circ.permutation_columns(circ.M, vk.omega, circ.DELTA)
-    inst = [[[2]], [[2]]]
-    prm = halo2_b200.Params.new("vesta", 5)
-    D = halo2_b200.EvaluationDomain("fp", vk.degree(), vk.k, circ.ZETA)
-    pk = AC.proving_key(halo2_b200, D, fixed, sigma, vk.blinding_factors())
-    try:
-        want = _engine_proof(prm, vk, fixed, sigma, [circ.witness(), circ.witness()], inst, 777)
-        got = _package_proof(prm, D, pk, vk, [circ.witness(), circ.witness()], inst, 777)
-        assert len(got) == 4160 and got == want
-        earm = PV.EngineArm(halo2_b200, "vesta", 5, params=prm)
-        assert PV.verify_proof(earm, vk, got, inst, circ.DELTA)
-        assert PV.verify_proof(PV.OracleArm("vesta", 5, prm.g, prm.g_lagrange, prm.w, prm.u), vk, got, inst, circ.DELTA)
-    finally:
-        pk.close()
-        prm.close()
-
-
-def test_benchmark_circuit_k14_equals_create_proof_engine():
-    from tests import bench_circuit as BC
-    k, m = 14, circ.M
-    prm = halo2_b200.Params.new("vesta", k)
-    D = halo2_b200.EvaluationDomain("fp", BC.DEGREE, k, circ.ZETA)
-    fixed, sigma, adv = BC.columns(k, m, D.omega, circ.DELTA, circ.A_SMALL * circ.ZETA % m)
-    fb, sb, ab = ([cref.ints_to_bytes(c_) for c_ in cols] for cols in (fixed, sigma, adv))
-    vk = PV.PinnedKey(BC.pinned_key_text(k, D.extended_k, pasta.Q_MOD, m, D.omega, [_commit(prm, c_) for c_ in fb], [_commit(prm, c_) for c_ in sb]))
-    pk = AC.proving_key(halo2_b200, D, fb, sb, vk.blinding_factors())
-    try:
-        want = _engine_proof(prm, vk, fb, sb, [ab], [[]], 5)
-        got = _package_proof(prm, D, pk, vk, [ab], [[]], 5)
-        assert got == want
-        assert PV.verify_proof(PV.EngineArm(halo2_b200, "vesta", k, params=prm), vk, got, [[]], circ.DELTA)
-    finally:
-        pk.close()
-        prm.close()
 
 
 def _commit(prm, values):
@@ -80,7 +35,7 @@ def _nonlinear(k):
     prm = halo2_b200.Params.new("vesta", k)
     vk, D, fixed, sigma, advice, inst = AC.nonlinear_case(halo2_b200, k, lambda c: _commit(prm, c), circ.ZETA, circ.DELTA)
     adv = [cref.ints_to_bytes(c) for c in advice]
-    return prm, vk, D, AC.proving_key(halo2_b200, D, fixed, sigma, vk.blinding_factors()), adv, inst
+    return prm, vk, D, PP.proving_key(halo2_b200, D, fixed, sigma, vk.blinding_factors()), adv, inst
 
 
 @pytest.mark.parametrize("k", [8, 12, 16, 18])
@@ -92,7 +47,7 @@ def test_nonlinear_lookup_circuit(k):
     try:
         assert len(vk.permutation_columns) == 10 and vk.degree() - 2 == 4
         seen, hook = AC.coset_compression_differs(halo2_b200, D)
-        proof = _package_proof(prm, D, pk, vk, [adv, adv], [inst, inst], 40 + k, hook=hook)
+        proof = _proof(prm, vk, pk, [adv, adv], [inst, inst], 40 + k, hook=hook)
         assert seen == [True] * 4
         arms = [PV.EngineArm(halo2_b200, "vesta", k, params=prm)]
         if k == 8:
@@ -113,9 +68,9 @@ def test_on_a_lane_with_a_shared_key():
     prm, vk, D, pk, adv, inst = _nonlinear(12)
     try:
         pk.share()
-        want = _package_proof(prm, D, pk, vk, [adv, adv], [inst, inst], 3)
+        want = _proof(prm, vk, pk, [adv, adv], [inst, inst], 3)
         with L.Lane():
-            got = _package_proof(prm, D, pk, vk, [adv, adv], [inst, inst], 3)
+            got = _proof(prm, vk, pk, [adv, adv], [inst, inst], 3)
         assert got == want
         assert PV.verify_proof(PV.EngineArm(halo2_b200, "vesta", 12, params=prm), vk, got, [inst, inst], circ.DELTA)
     finally:

@@ -26,7 +26,7 @@ from tests.abi_cases import _err, _lib, _run_parallel, _sigma_call  # noqa: E402
 from tests.bench_circuit import _bench_assembly, _bench_params, bench_copies  # noqa: E402
 from tests.keygen_cases import oracle_sigma  # noqa: E402
 from tests.plonk_api_circuit import ZETA, golden_columns, plonk_api_copies  # noqa: E402
-from tests.plonk_prover import prover_pk_bytes, prover_pk_dict  # noqa: E402
+from tests.plonk_prover import prover_pk_bytes  # noqa: E402
 from tests.plonk_verifier import scalar_delta  # noqa: E402
 
 SEED = 0x41534D42
@@ -251,7 +251,7 @@ def test_benchmark_circuit_proof_from_copies_k14(eng):
         for src in (cc, asm):
             keys.append(eng.keygen_pk(prm, D, fixed, src, delta, BC.BLINDING_FACTORS))
             T = R.Blake2bTranscript(m)
-            PP.create_proof_engine(eng, prm, vk, None, None, [ab], [[]], MC.SeededRng("fp", 5, True), T, ZETA, delta, pk=prover_pk_dict(keys[-1]))
+            PP.create_proof_engine(eng, prm, vk, None, None, [ab], [[]], MC.SeededRng("fp", 5, True), T, ZETA, delta, pk=keys[-1])
             proofs.append(bytes(T.proof))
         assert prover_pk_bytes(keys[0]) == prover_pk_bytes(keys[1])
         assert proofs[0] == proofs[1]

@@ -9,7 +9,8 @@ numerators and denominators (Lagrange basis), and the whole of h(X) over the ext
 
 The cases:
   - the golden programs: for every pinned key of tests/golden/golden_proofs.json.gz, the Lagrange-basis programs and h(X) of
-    two proofs, built by the prover's own builders (tests/plonk_prover.py), over seeded columns with rows of 0, 1 and m - 1;
+    two proofs, built by tests/plonk_prover.py's builders and the product programs below, over seeded columns with rows of
+    0, 1 and m - 1;
   - generated trees over every node kind and the rotations where wrapping goes wrong, at 1 to 1024 rows;
   - raw programs: NEG, the operand-stack and program-length limits, LinearTerm at n = 1 and 2, shifts of INT32_MIN and
     INT32_MAX, hundreds of leaf handles, thousands of constants, operands longer than 2^log_n;
@@ -213,8 +214,37 @@ class _Leaves:
         return [AstLeaf(self.count - k + i) for i in range(k)]
 
 
+# The product columns' programs (Lagrange basis) of the reference's loops; the batched product calls run them in one kernel.
+def permutation_denominator(eng, cols, sigmas, beta: int, gamma: int):
+    """permutation/prover.rs commit, before batch_invert: prod_j (beta * sigma_j + gamma + column_j) over one chunk of columns."""
+    den = None
+    for col, sl in zip(cols, sigmas):
+        term = sl * beta + eng.Ast.constant_term(gamma) + col
+        den = term if den is None else den * term
+    return den
+
+
+def permutation_numerator(eng, inv_den, cols, first: int, beta: int, gamma: int, delta: int, m: int):
+    """permutation/prover.rs commit, after batch_invert: 1 / den * prod_j (beta * delta^(first + j) * omega^row + gamma + column_j); `first` is the
+    chunk's first global column index."""
+    num = inv_den
+    for j, col in enumerate(cols):
+        num = num * (eng.Ast.linear_term(pow(delta, first + j, m) * beta % m) + eng.Ast.constant_term(gamma) + col)
+    return num
+
+
+def lookup_product_denominator(eng, permuted_input, permuted_table, beta: int, gamma: int):
+    """lookup/prover.rs commit_product, before batch_invert: (A' + beta) (S' + gamma)."""
+    return (permuted_input + eng.Ast.constant_term(beta)) * (permuted_table + eng.Ast.constant_term(gamma))
+
+
+def lookup_product_numerator(eng, inv_den, input_, table, beta: int, gamma: int):
+    """lookup/prover.rs commit_product, after batch_invert: 1 / den * (A + beta) (S + gamma), A and S the compressed columns."""
+    return inv_den * (input_ + eng.Ast.constant_term(beta)) * (table + eng.Ast.constant_term(gamma))
+
+
 def golden_programs(vk: PV.PinnedKey, m: int, num_proofs: int, seed: int):
-    """The prover's programs of `num_proofs` proofs under `vk`, built by tests/plonk_prover.py's builders with seeded
+    """The prover's programs of `num_proofs` proofs under `vk`, built by the builders above and tests/plonk_prover.py's with seeded
     challenges in the field of modulus m: ([(name, Lagrange-basis Ast)], Lagrange leaf count, h(X), extended leaf count,
     the gate part of h(X))."""
     Ast, _, _ = _ast()
@@ -236,12 +266,12 @@ def golden_programs(vk: PV.PinnedKey, m: int, num_proofs: int, seed: int):
         leaf = lambda col: {"Advice": AL[pr], "Fixed": FL, "Instance": IL[pr]}[col[0]][col[1]]
         for first in range(0, len(vk.permutation_columns), chunk_len):
             cols = [leaf(c) for c in vk.permutation_columns[first:first + chunk_len]]
-            progs += [(f"permutation {first} den", PP.permutation_denominator(E, cols, SL[first:first + chunk_len], beta, gamma)),
-                      (f"permutation {first} num", PP.permutation_numerator(E, lag.new(1)[0], cols, first, beta, gamma, delta, m))]
+            progs += [(f"permutation {first} den", permutation_denominator(E, cols, SL[first:first + chunk_len], beta, gamma)),
+                      (f"permutation {first} num", permutation_numerator(E, lag.new(1)[0], cols, first, beta, gamma, delta, m))]
         for li in range(len(vk.lookups)):
             PI, PT, CI, CT = lag.new(4)
-            progs += [(f"lookup {li} product den", PP.lookup_product_denominator(E, PI, PT, beta, gamma)),
-                      (f"lookup {li} product num", PP.lookup_product_numerator(E, lag.new(1)[0], CI, CT, beta, gamma))]
+            progs += [(f"lookup {li} product den", lookup_product_denominator(E, PI, PT, beta, gamma)),
+                      (f"lookup {li} product num", lookup_product_numerator(E, lag.new(1)[0], CI, CT, beta, gamma))]
     ext = _Leaves()
     FC, SC, LG = ext.new(vk.num_fixed_columns), ext.new(len(vk.permutation_columns)), ext.new(3)
     exprs, gates = [], None

@@ -1,5 +1,5 @@
 """GPU checks of the column-batched transforms (h2_poly_lagrange_to_coeff_batch / h2_poly_coeff_to_extended_batch),
-h2_poly_set_rows, and instance_commit / advice_commit against the per-column composition of create_proof_engine."""
+h2_poly_set_rows, and instance_commit / advice_commit against a composition of per-column calls."""
 import ctypes
 
 import numpy as np
@@ -196,8 +196,9 @@ def test_phases_of_the_plonk_api_circuit():
     vk = PV.PinnedKey(circ.CASE["key_text"])
     prm = _params("vesta", vk.k)
     advice, instances = [circ.witness(), circ.witness()], [[[2]], [[2]]]
-    want = CC.engine_phases(halo2_b200, prm, vk, advice, instances, 777, circ.ZETA)
-    CC.assert_same(want, CC.batched_phases(halo2_b200, prm, vk, advice, instances, 777, circ.ZETA))
+    D = halo2_b200.EvaluationDomain("fp", vk.degree(), vk.k, circ.ZETA)
+    bf = vk.blinding_factors()
+    CC.assert_same(CC.composition_phases(halo2_b200, prm, D, bf, advice, instances, 777), CC.batched_phases(halo2_b200, prm, D, bf, advice, instances, 777))
     prm.close()
 
 
@@ -213,7 +214,9 @@ def test_phases_of_a_golden_proof_shape():
     zeta = pasta.zeta_candidates(field)[0]
     advice = CC.random_columns(field, 5, 2, 10, 1 << 11)
     instances = [[[3, 4, 5]] * vk.num_instance_columns] * 2
-    CC.assert_same(CC.engine_phases(halo2_b200, prm, vk, advice, instances, 91, zeta), CC.batched_phases(halo2_b200, prm, vk, advice, instances, 91, zeta))
+    D = halo2_b200.EvaluationDomain(field, vk.degree(), 11, zeta)
+    bf = vk.blinding_factors()
+    CC.assert_same(CC.composition_phases(halo2_b200, prm, D, bf, advice, instances, 91), CC.batched_phases(halo2_b200, prm, D, bf, advice, instances, 91))
     prm.close()
 
 
@@ -221,9 +224,10 @@ def test_phases_of_the_benchmark_circuit_shape():
     """The benchmark circuit's shape (benches/plonk.rs) at k = 14: 5 advice columns, one instance column, two proofs per call."""
     from tests import bench_circuit as BC
     zeta = pasta.zeta_candidates("fp")[0]
-    vk = CC.ShapeKey("fp", 14, BC.DEGREE, BC.BLINDING_FACTORS, zeta)
+    D = halo2_b200.EvaluationDomain("fp", BC.DEGREE, 14, zeta)
     prm = _params("vesta", 14)
     advice = CC.random_columns("fp", 9, 2, 5, 1 << 14)
     instances = [[list(range(1, 40))], [[7] * 100]]
-    CC.assert_same(CC.engine_phases(halo2_b200, prm, vk, advice, instances, 5, zeta), CC.batched_phases(halo2_b200, prm, vk, advice, instances, 5, zeta))
+    bf = BC.BLINDING_FACTORS
+    CC.assert_same(CC.composition_phases(halo2_b200, prm, D, bf, advice, instances, 5), CC.batched_phases(halo2_b200, prm, D, bf, advice, instances, 5))
     prm.close()

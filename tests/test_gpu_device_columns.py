@@ -5,7 +5,7 @@ ResidentPoly.from_tensor / upload_tensor / to_tensor, upload_tensors_resident / 
   both fields, both reprs, 1, 3 and 17 columns of different lengths per call, random 256-bit inputs (most of them >= p);
 - the stream contract with no host synchronisation between the calls, on the primary context and on a lane;
 - instance_commit / advice_commit / keygen fed CUDA tensors give the host columns' commitments and keys, and proofs composed
-  from package calls the host columns' bytes, which the verifier accepts;
+  from the phase calls (tests/plonk_prover.create_proof_engine) the host columns' bytes, which the verifier accepts;
 - every refusal happens before anything is launched and leaves the destination alone;
 - a lane exports a shared key's polynomial."""
 import ctypes
@@ -19,6 +19,7 @@ from oracle import cref, pasta  # noqa: E402
 from tests import arguments_cases as AC  # noqa: E402
 from tests import multiopen_cases as MC  # noqa: E402
 from tests import plonk_api_circuit as circ  # noqa: E402
+from tests import plonk_prover as PP  # noqa: E402
 from tests import plonk_verifier as PV  # noqa: E402
 from tests import prover_replay as R  # noqa: E402
 
@@ -235,17 +236,17 @@ def _cuda(torch, cols):
     return [torch.from_numpy(np.ascontiguousarray(c)).cuda() for c in cols]
 
 
-def _proof(eng, prm, D, pk, vk, advice, inst, seed):
+def _proof(eng, prm, pk, vk, advice, inst, seed):
     T = R.Blake2bTranscript(circ.M)
-    AC.create_proof_package(eng, prm, D, pk, vk, advice, inst, MC.SeededRng("fp", seed, True), T, circ.DELTA)
+    PP.create_proof_engine(eng, prm, vk, None, None, advice, inst, MC.SeededRng("fp", seed, True), T, circ.ZETA, circ.DELTA, pk=pk)
     return bytes(T.proof)
 
 
-def _same_proof(eng, torch, prm, D, pk, vk, advice, inst, seed, k):
-    want = _proof(eng, prm, D, pk, vk, advice, inst, seed)
+def _same_proof(eng, torch, prm, pk, vk, advice, inst, seed, k):
+    want = _proof(eng, prm, pk, vk, advice, inst, seed)
     adv_t = [_cuda(torch, per) for per in advice]
     inst_t = [_cuda(torch, [cref.ints_to_bytes([v % circ.M for v in col]) for col in per]) for per in inst]
-    got = _proof(eng, prm, D, pk, vk, adv_t, inst_t, seed)
+    got = _proof(eng, prm, pk, vk, adv_t, inst_t, seed)
     assert got == want
     assert PV.verify_proof(PV.EngineArm(eng, "vesta", k, params=prm), vk, got, inst, circ.DELTA)
 
@@ -255,10 +256,10 @@ def test_proof_plonk_api_circuit(eng, torch):
     fixed, sigma = circ.fixed_columns(circ.M, circ.ZETA), circ.permutation_columns(circ.M, vk.omega, circ.DELTA)
     prm = eng.Params.new("vesta", 5)
     D = eng.EvaluationDomain("fp", vk.degree(), vk.k, circ.ZETA)
-    pk = AC.proving_key(eng, D, fixed, sigma, vk.blinding_factors())
+    pk = PP.proving_key(eng, D, fixed, sigma, vk.blinding_factors())
     try:
         adv = [[cref.ints_to_bytes([v % circ.M for v in col]) for col in circ.witness()] for _ in range(2)]
-        _same_proof(eng, torch, prm, D, pk, vk, adv, [[[2]], [[2]]], 777, 5)
+        _same_proof(eng, torch, prm, pk, vk, adv, [[[2]], [[2]]], 777, 5)
     finally:
         pk.close()
         prm.close()
@@ -273,9 +274,9 @@ def test_proof_benchmark_circuit_k14(eng, torch):
     fb, sb, ab = ([cref.ints_to_bytes(c_) for c_ in cols] for cols in (fixed, sigma, adv))
     commit = lambda v: cref.bytes_to_affine(eng.batch_normalize(prm.commit_lagrange(v, eng.Blind(1)).reshape(1, 96), "vesta")[0])  # noqa: E731
     vk = PV.PinnedKey(BC.pinned_key_text(k, D.extended_k, pasta.Q_MOD, m, D.omega, [commit(c) for c in fb], [commit(c) for c in sb]))
-    pk = AC.proving_key(eng, D, fb, sb, vk.blinding_factors())
+    pk = PP.proving_key(eng, D, fb, sb, vk.blinding_factors())
     try:
-        _same_proof(eng, torch, prm, D, pk, vk, [ab], [[]], 5, k)
+        _same_proof(eng, torch, prm, pk, vk, [ab], [[]], 5, k)
     finally:
         pk.close()
         prm.close()
@@ -286,10 +287,10 @@ def test_proof_nonlinear_circuit(eng, torch, k):
     prm = eng.Params.new("vesta", k)
     commit = lambda c: cref.bytes_to_affine(eng.batch_normalize(prm.commit_lagrange(cref.ints_to_bytes(c), eng.Blind(1)).reshape(1, 96), "vesta")[0])  # noqa: E731
     vk, D, fixed, sigma, advice, inst = AC.nonlinear_case(eng, k, commit, circ.ZETA, circ.DELTA)
-    pk = AC.proving_key(eng, D, fixed, sigma, vk.blinding_factors())
+    pk = PP.proving_key(eng, D, fixed, sigma, vk.blinding_factors())
     try:
         adv = [cref.ints_to_bytes(c) for c in advice]
-        _same_proof(eng, torch, prm, D, pk, vk, [adv, adv], [inst, inst], 40 + k, k)
+        _same_proof(eng, torch, prm, pk, vk, [adv, adv], [inst, inst], 40 + k, k)
     finally:
         pk.close()
         prm.close()

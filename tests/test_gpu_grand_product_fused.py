@@ -3,11 +3,10 @@ halo2_b200.permutation_commit / lookup_commit_product):
 
 - the products equal the reference's loops restated with big integers (tests/grand_product_cases.py) element for
   element, both fields, k = 1, 4, 8, 11, several proofs, sets and lookups per call;
-- at k = 14, 16, 18 and 20 the z columns and their commitments are byte-identical to the composition the engine-API prover
-  uses (Ast programs, batch_invert, running_product, the host's last_z);
+- at k = 14, 16, 18 and 20 the z columns and their commitments are byte-identical to a composition of finer calls (Ast
+  programs, batch_invert, running_product, the host's last_z);
 - a real proof of the benchmark circuit at k = 14 (tests/plonk_prover.create_proof_engine): permutation_commit, fed the
   challenges and draws the proof made, gives the permutation product commitments at their position in the proof bytes;
-- on the plonk_api circuit (k = 5, lookups and an instance column) the lookup z columns equal the prover's;
 - sigma from a shared keygen_pk key on a lane, the z handles unknown elsewhere;
 - every validation error, on the primary context and on a lane, fails with a message and leaves z_out untouched."""
 import ctypes
@@ -25,7 +24,6 @@ from tests.bench_circuit import _bench_params, bench_copies  # noqa: E402
 from tests.grand_product_cases import (_close, composition_lookup, composition_permutation, oracle_lookup_product,  # noqa: E402
                                        oracle_permutation_product)
 from tests.plonk_api_circuit import ZETA  # noqa: E402
-from tests.plonk_prover import prover_pk_dict  # noqa: E402
 from tests.plonk_verifier import scalar_delta  # noqa: E402
 
 SEED = 0x46555345
@@ -129,20 +127,14 @@ def test_same_bytes_as_the_composition(eng, k):
 
 # ---- 3. real proofs -----------------------------------------------------------------------------------------------------
 class RecordingTranscript:
-    """Passes every call through; records the challenges and, on every point written, calls on_point(index)."""
-    def __init__(self, inner, on_point=None):
-        self.inner, self.challenges, self.points, self.on_point = inner, [], 0, on_point
+    """Passes every call through; records the challenges."""
+    def __init__(self, inner):
+        self.inner, self.challenges = inner, []
 
     def squeeze_challenge(self):
         c = self.inner.squeeze_challenge()
         self.challenges.append(c)
         return c
-
-    def write_point(self, xy):
-        if self.on_point:
-            self.on_point(self.points)
-        self.points += 1
-        self.inner.write_point(xy)
 
     def __getattr__(self, name):
         return getattr(self.inner, name)
@@ -169,7 +161,7 @@ def test_benchmark_proof_k14_contains_the_permutation_commitments(eng):
         rng = MC.RecordingRng(MC.SeededRng("fp", 11, True))
         T = RecordingTranscript(R.Blake2bTranscript(m))
         ab = [cref.ints_to_bytes(c) for c in adv]
-        PP.create_proof_engine(eng, prm, vk, None, None, [ab], [[]], rng, T, ZETA, delta, pk=prover_pk_dict(pk))
+        PP.create_proof_engine(eng, prm, vk, None, None, [ab], [[]], rng, T, ZETA, delta, pk=pk)
         proof = bytes(T.proof)
         assert not vk.lookups
         bf, usable, nadv = vk.blinding_factors(), n - (vk.blinding_factors() + 1), len(adv)
@@ -187,58 +179,6 @@ def test_benchmark_proof_k14_contains_the_permutation_commitments(eng):
     finally:
         if pk is not None:
             pk.close()
-        prm.close()
-
-
-def test_plonk_api_lookup_products_equal_the_provers(eng):
-    from tests import multiopen_cases as MC
-    from tests import plonk_prover as PP
-    from tests import plonk_verifier as PV
-    from tests import prover_replay as R
-    vk = PV.PinnedKey(circ.CASE["key_text"])
-    k, n, M = 5, 32, circ.M
-    bf = vk.blinding_factors()
-    prm = eng.Params.new("vesta", k)
-    seen = {"perm": [], "z": []}
-    real = eng.permute_expression_pair_resident
-    real_rp = eng.running_product_resident
-
-    class Eng:                                                  # the package, recording the lookup columns and every running product
-        def __getattr__(self, name):
-            return getattr(eng, name)
-
-        def permute_expression_pair_resident(self, ci, ct, usable, oi, ot):
-            pi, pt = real(ci, ct, usable, oi, ot)
-            seen["perm"].append((ci, ct, pi, pt))
-            return pi, pt
-
-        def running_product_resident(self, src, init=1, dst=None, n=None):
-            z = real_rp(src, init=init, dst=dst, n=n)
-            seen["z"].append(z)
-            return z
-
-    snaps = []
-    rng = MC.RecordingRng(MC.SeededRng("fp", 777, True))
-    nsets = -(-len(vk.permutation_columns) // (vk.degree() - 2))
-
-    def on_point(i):                                            # a product column's commitment: snapshot it and its inputs
-        if len(seen["z"]) > 2 * nsets and len(snaps) < len(seen["z"]) - 2 * nsets:
-            b = len(snaps)
-            snaps.append((seen["z"][-1].download(), [p.download() for p in seen["perm"][b]], rng.draws[-(bf + 1):-1]))
-    T = RecordingTranscript(R.Blake2bTranscript(M), on_point)
-    try:
-        inst = [[[2]], [[2]]]
-        PP.create_proof_engine(Eng(), prm, vk, circ.fixed_columns(M, circ.ZETA), circ.permutation_columns(M, vk.omega, circ.DELTA),
-                               [circ.witness(), circ.witness()], inst, rng, T, circ.ZETA, circ.DELTA)
-        assert len(vk.lookups) >= 1 and len(snaps) == 2 * len(vk.lookups)
-        D = eng.EvaluationDomain("fp", vk.degree(), k, circ.ZETA)
-        beta, gamma = T.challenges[1], T.challenges[2]
-        cols = [tuple(eng.ResidentPoly("fp", n, c) for c in s[1]) for s in snaps]
-        z = eng.lookup_product_resident(D, [cols[:len(vk.lookups)], cols[len(vk.lookups):]], beta, gamma, bf, [x for s in snaps for x in s[2]])
-        for got, s in zip([q for per in z for q in per], snaps):
-            assert (got.download() == s[0]).all()
-        _close([p for c in cols for p in c], *z)
-    finally:
         prm.close()
 
 

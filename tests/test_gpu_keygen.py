@@ -24,7 +24,7 @@ from tests.abi_cases import _err, _lib, _run_parallel, _sigma_call  # noqa: E402
 from tests.bench_circuit import _bench_assembly, _bench_params  # noqa: E402
 from tests.keygen_cases import oracle_sigma, random_mapping  # noqa: E402
 from tests.plonk_api_circuit import ZETA, golden_columns, plonk_api_copies  # noqa: E402
-from tests.plonk_prover import prover_pk_bytes, prover_pk_dict  # noqa: E402
+from tests.plonk_prover import prover_pk_bytes  # noqa: E402
 from tests.plonk_verifier import scalar_delta  # noqa: E402
 
 SEED = 0x4B455947
@@ -200,7 +200,7 @@ def test_benchmark_circuit_key_and_proof_k14(eng):
         PP.create_proof_engine(eng, prm, vk, fb, sb, [ab], [[]], MC.SeededRng("fp", 5, True), T, ZETA, delta)
         want = bytes(T.proof)
         T = R.Blake2bTranscript(m)
-        PP.create_proof_engine(eng, prm, vk, None, None, [ab], [[]], MC.SeededRng("fp", 5, True), T, ZETA, delta, pk=prover_pk_dict(pk))
+        PP.create_proof_engine(eng, prm, vk, None, None, [ab], [[]], MC.SeededRng("fp", 5, True), T, ZETA, delta, pk=pk)
         got = bytes(T.proof)
         assert got == want
         arm = PV.EngineArm(eng, "vesta", k, params=prm)

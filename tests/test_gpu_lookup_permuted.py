@@ -78,9 +78,10 @@ def test_byte_identical_to_the_composition(eng, k):
 
 
 def test_plonk_api_proof(eng):
-    """The plonk_api circuit (k = 5, two proofs, lookups): lookup_commit_permuted, fed the recorded theta and draws, gives the
-    permuted commitments at their offsets in the proof bytes, and lookup_commit_product, given its result as it is and the
-    recorded beta, gamma and draws, gives the lookup product commitments."""
+    """The plonk_api circuit (k = 5, two proofs, lookups), proved by create_proof_engine with the oracle prover's bytes:
+    lookup_commit_permuted, fed the recorded theta and draws, gives the permuted commitments at their offsets in the oracle's
+    proof, and lookup_commit_product, given its result as it is and the recorded beta, gamma and draws, gives the lookup
+    product commitments."""
     from tests import bench_circuit as BC
     from tests import multiopen_cases as MC
     from tests import plonk_api_circuit as circ
@@ -90,6 +91,7 @@ def test_plonk_api_proof(eng):
     prm = BC._bench_params(eng, 5)
     try:
         proof, seen = circ.plonk_api_proof(eng, prm)
+        assert proof == circ.plonk_api_oracle_proof(prm.g, prm.w, prm.u)
         D, ev, lookups = circ.plonk_api_lookups(eng, seen)
         perm, cm = eng.lookup_commit_permuted(prm, D, ev, lookups, seen["theta"], bf, MC.ReplayRng(seen["draws"][seen["draws_at_theta"]:]))
         at = seen["points_at_theta"]

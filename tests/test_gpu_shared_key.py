@@ -24,7 +24,7 @@ from tests import plonk_api_circuit as circ  # noqa: E402
 from tests.abi_cases import _bind, _create, _destroy, _err, _lib, _run_parallel  # noqa: E402
 from tests.bench_circuit import bench_copies  # noqa: E402
 from tests.plonk_api_circuit import ZETA  # noqa: E402
-from tests.plonk_prover import prover_pk_bytes, prover_pk_dict  # noqa: E402
+from tests.plonk_prover import prover_pk_bytes  # noqa: E402
 from tests.plonk_verifier import scalar_delta  # noqa: E402
 
 SEED = 0x5348415245
@@ -396,7 +396,7 @@ def test_shared_key_proves_on_four_lanes_k14(eng):
 
     def prove(pk, seed):
         T = R.Blake2bTranscript(M)
-        PP.create_proof_engine(eng, prm14, vk, None, None, [ab], [[]], MC.SeededRng("fp", seed, True), T, ZETA, delta, pk=prover_pk_dict(pk))
+        PP.create_proof_engine(eng, prm14, vk, None, None, [ab], [[]], MC.SeededRng("fp", seed, True), T, ZETA, delta, pk=pk)
         return bytes(T.proof)
 
     def on_lanes(pk):

@@ -1,8 +1,8 @@
 """GPU test (runs last): a REAL PLONK proof of the reference's own test circuit (halo2_proofs/tests/plonk_api.rs:21-420, k = 5,
 two instances) is produced ON THE DEVICE by plonk::create_proof composed from the engine's reference-facing API
-(tests/plonk_prover.create_proof_engine: resident polynomials, device transforms, Ast programs in both bases, batch_invert and
-the running product, the lookup permutation, fixed-base commits, batched evaluations, the multi-point opening and the opening
-argument) under the reference's GOLDEN verifying key -- the same 4 160 bytes as the oracle's prover with the same randomness --
+(tests/plonk_prover.create_proof_engine: the instance and advice commitments, the lookups' permuted and product columns, the
+permutation products, the vanishing argument, the arguments' construct / evaluate / open, the multi-point opening and the
+opening argument) under the reference's GOLDEN verifying key -- the same 4 160 bytes as the oracle's prover with the same randomness --
 and is accepted by the engine's verifier and by the restated reference verifier that the reference's sixteen golden proofs pin.
 
 This composition was validated without a GPU (tests/test_real_proof.py: the same code over the ABI stand-in, device bodies on the
@@ -56,15 +56,25 @@ def test_real_proof_on_the_device():
 
 
 def test_benchmark_circuit_real_proof_on_the_device():
-    """The reference's benchmark circuit (benches/plonk.rs, tests/bench_circuit.py) at k = 8: key generated on the device, a real proof
-    through the engine-API prover with the proving key's polynomials resident between two proofs, THE SAME BYTES as the same prover
-    on the C restatement (tests/plonk_prover.CrefProver), accepted by the engine's verifier -- the workload of bench.py's
-    extra.create_proof_k14_real."""
+    """The reference's benchmark circuit (benches/plonk.rs, tests/bench_circuit.py) at k = 8: key generated on the device, a
+    real proof through the engine's phase calls with the proving key's polynomials resident between two proofs (in a dict, as
+    bench.py keeps them), THE SAME BYTES as the same prover on the C restatement (tests/plonk_prover.CrefProver), accepted by
+    the engine's verifier -- the workload of bench.py's extra.create_proof_k14_real."""
+    _benchmark_circuit_proofs(8)
+
+
+def test_benchmark_circuit_k14_real_proof_on_the_device():
+    """The same at bench.py's own k = 14."""
+    _benchmark_circuit_proofs(14)
+
+
+def _benchmark_circuit_proofs(k):
+    import os
+
     import halo2_b200 as h2
     from halo2_b200 import lib as L
     from tests import bench_circuit as BC
     L.init()
-    k = 8
     n = 1 << k
     m = circ.M
     pts = cref.gen_points("vesta", 99, n + 2)
@@ -83,7 +93,7 @@ def test_benchmark_circuit_real_proof_on_the_device():
             T = R.Blake2bTranscript(m)
             PP.create_proof_engine(h2, prm, vk, fb, sb, [ab], [[]], MC.SeededRng("fp", seed, True), T, circ.ZETA, circ.DELTA, pk=pk)
             proofs.append(bytes(T.proof))
-        cp = PP.CrefProver(cref, "vesta", "fp", g, gl, w, u, 8)
+        cp = PP.CrefProver(cref, "vesta", "fp", g, gl, w, u, os.cpu_count() or 1)
         Tc = R.Blake2bTranscript(m)
         cp.create_proof(vk, fb, sb, [ab], [[]], MC.SeededRng("fp", 6, True), Tc, circ.ZETA, circ.DELTA)
         assert proofs[1] == bytes(Tc.proof) and proofs[0] != proofs[1]

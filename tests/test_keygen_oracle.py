@@ -22,7 +22,6 @@ from tests.fake_engine import KEYGEN_CHUNK
 from tests.keygen_cases import oracle_assembly, oracle_copy, oracle_sigma, random_mapping
 from tests.kernel_emul import build as emul_build
 from tests.plonk_api_circuit import ZETA, plonk_api_copies
-from tests.plonk_prover import prover_pk_dict
 from tests.plonk_verifier import scalar_delta
 
 
@@ -154,8 +153,8 @@ def test_emul_sigma_rejects_out_of_range_entries(emu, field):
 
 # ---- 3. keygen.py over an ABI stand-in ---------------------------------------------------------------------------------
 def test_keygen_pk_reproduces_the_test_provers_key():
-    """keygen_pk's resident key at k = 5 holds exactly the values create_proof_engine's own keygen part computes, and a proof
-    made with it is the proof made with the host-built sigma."""
+    """keygen_pk's resident key at k = 5 holds exactly the values of the tests' key builder (tests/plonk_prover.proving_key)
+    over the host-built sigma, and a proof made with it is the proof made with that key."""
     import halo2_b200 as h2
     from tests import multiopen_cases as MC
     from tests import plonk_prover as PP
@@ -183,19 +182,16 @@ def test_keygen_pk_reproduces_the_test_provers_key():
         assert fake.calls.count("h2_poly_permutation_sigma") == 1
         assert fake.calls.count("h2_poly_lagrange_to_coeff") == fake.calls.count("h2_poly_coeff_to_extended") == 4 + 3 + 3
         adv_bytes = [cref.ints_to_bytes(col) for col in adv]
-        ref_pk = {}
+        ref_pk = PP.proving_key(h2, D, fixed, sigma, BC.BLINDING_FACTORS)
         T = R.Blake2bTranscript(m)
-        PP.create_proof_engine(h2, prm, vk, fixed, sigma, [adv_bytes], [[]], MC.SeededRng("fp", 5, True), T, ZETA, delta, pk=ref_pk)
+        PP.create_proof_engine(h2, prm, vk, None, None, [adv_bytes], [[]], MC.SeededRng("fp", 5, True), T, ZETA, delta, pk=ref_pk)
         want = bytes(T.proof)
-        mine = prover_pk_dict(pk)
-        for key in ("fixed_l", "fixed_p", "fixed_c", "sigma_l", "sigma_p", "sigma_c", "l"):
-            assert len(mine[key]) == len(ref_pk[key])
-            for a, b in zip(mine[key], ref_pk[key]):
-                assert a.len == b.len and (a.download() == b.download()).all(), key
+        assert [p.len for p in pk._all()] == [p.len for p in ref_pk._all()]
+        assert PP.prover_pk_bytes(pk) == PP.prover_pk_bytes(ref_pk)
         T = R.Blake2bTranscript(m)
-        PP.create_proof_engine(h2, prm, vk, None, None, [adv_bytes], [[]], MC.SeededRng("fp", 5, True), T, ZETA, delta, pk=mine)
+        PP.create_proof_engine(h2, prm, vk, None, None, [adv_bytes], [[]], MC.SeededRng("fp", 5, True), T, ZETA, delta, pk=pk)
         assert bytes(T.proof) == want
-        PP.close_proving_key(ref_pk)
+        ref_pk.close()
         pk.close()
         assert not fake.polys
         prm.close()

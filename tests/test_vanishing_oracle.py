@@ -7,7 +7,6 @@ import numpy as np
 import pytest
 
 from oracle import cref, pasta
-from tests import plonk_prover as PP
 from tests.kernel_emul import build as emul_build
 
 
@@ -89,44 +88,3 @@ def test_sizes_rejected_before_any_launch(emu, k, ext_k, count, t_len, reason):
 def test_sizes_accepted(emu, k, ext_k, count, t_len):
     assert emu.emu_vanishing_quotient_sizes(k, ext_k, ctypes.c_uint64(count), t_len) is None
 
-
-def test_a_whole_proof_with_the_module_over_the_stand_in():
-    """A proof whose vanishing argument comes from halo2_b200.vanishing (tests/arguments_cases.create_proof_package), over the
-    ABI stand-in with the fused bodies on the host emulation: the same points, scalars, h_poly / random_poly queries and proof
-    bytes as create_proof_engine on the plonk_api circuit under its golden key, one quotient call instead of the division,
-    transform and copies, and every polynomial released."""
-    import halo2_b200
-    from tests import arguments_cases as AC
-    from tests import fake_engine
-    from tests import multiopen_cases as MC
-    from tests import plonk_api_circuit as circ
-    from tests import plonk_verifier as PV
-    from tests import vanishing_cases as VC
-    vk = circ.plonk_api_key()
-    P = pasta.Params.new(pasta.VESTA, 5)
-    gens = (cref.affines_to_bytes(P.g), cref.affines_to_bytes(P.g_lagrange), cref.affines_to_bytes([P.w]), cref.affines_to_bytes([P.u]))
-    fixed, sigma = circ.fixed_columns(circ.M, circ.ZETA), circ.permutation_columns(circ.M, vk.omega, circ.DELTA)
-    inst = [[[2]], [[2]]]
-    adv = [circ.witness(), circ.witness()]
-    with fake_engine.installed() as fake:
-        prm = halo2_b200.Params("vesta", 5, *gens[:3], u=gens[3])
-        D = halo2_b200.EvaluationDomain("fp", vk.degree(), vk.k, circ.ZETA)
-        want = VC.record(halo2_b200, circ.M, lambda eng, t: PP.create_proof_engine(eng, prm, vk, fixed, sigma, adv, inst, MC.SeededRng("fp", 777, True),
-                                                                                  t, circ.ZETA, circ.DELTA))
-        pk = AC.proving_key(halo2_b200, D, fixed, sigma, vk.blinding_factors())
-        fake.calls.clear()
-        got = VC.record(halo2_b200, circ.M, lambda eng, t: AC.create_proof_package(eng, prm, D, pk, vk, adv, inst, MC.SeededRng("fp", 777, True), t,
-                                                                                  circ.DELTA))
-        assert fake.calls.count("h2_poly_vanishing_quotient") == 1
-        assert "h2_poly_divide_by_vanishing" not in fake.calls and "h2_poly_extended_to_coeff" not in fake.calls
-        assert len(got["points"]) == len(want["points"]) and all(np.array_equal(a, b) for a, b in zip(got["points"], want["points"]))
-        assert got["scalars"] == want["scalars"]
-        for (px, pa, pb), (wx, wa, wb) in zip(got["queries"], want["queries"]):
-            assert px == wx and pb == wb and np.array_equal(pa, wa)
-        assert got["proof"] == want["proof"] and len(got["proof"]) == 4160
-        pk.close()
-        assert not fake.polys
-        earm = PV.EngineArm(halo2_b200, "vesta", 5, *gens)
-        assert PV.verify_proof(earm, vk, got["proof"], inst, circ.DELTA)
-        earm.close()
-        prm.close()

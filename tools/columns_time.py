@@ -1,6 +1,6 @@
 """Time of the instance / advice columns' domain transforms on the GPU: lagrange_to_coeff then coeff_to_extended of `count`
-resident columns, one call per column per step (the composition of tests/plonk_prover.create_proof_engine) against one
-column-batched call per step (h2_poly_lagrange_to_coeff_batch / h2_poly_coeff_to_extended_batch).
+resident columns, one call per column per step (this tool's own per-column composition) against one column-batched call
+per step (h2_poly_lagrange_to_coeff_batch / h2_poly_coeff_to_extended_batch).
 
   python tools/columns_time.py [--cases 11x10,14x1,14x4,14x16,17x1,...] [--reps 7] [--out columns_time.json]
 

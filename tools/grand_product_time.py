@@ -1,7 +1,6 @@
 """Time of the permutation and lookup product columns on the GPU: one call per argument (h2_poly_permutation_product /
-h2_poly_lookup_product, csrc/grandproduct.cuh) against the composition the engine-API prover uses today
-(tests/plonk_prover.create_proof_engine: per column set two Ast programs, batch_invert, running_product, the blinding rows
-uploaded, last_z read back to the host).
+h2_poly_lookup_product, csrc/grandproduct.cuh) against a composition of finer calls (tests/grand_product_cases.py: per
+column set two Ast programs, batch_invert, running_product, the blinding rows uploaded, last_z read back to the host).
 
   python tools/grand_product_time.py [--ks 14,16,18,20] [--reps 5] [--out grand_product_time.json]
 

@@ -158,7 +158,6 @@ def real_bench(k, lanes, reps):
     from tests import plonk_verifier as PV
     from tests.bench_circuit import bench_copies
     from tests.plonk_api_circuit import ZETA
-    from tests.plonk_prover import prover_pk_dict
     n, m = 1 << k, pasta.P_MOD
     delta = PV.scalar_delta(m)
     dev = L._inited_device or 0
@@ -177,7 +176,7 @@ def real_bench(k, lanes, reps):
 
     def prove(pk, seed):
         T = R.Blake2bTranscript(m)
-        PP.create_proof_engine(h2, prm, vk, None, None, [ab], [[]], MC.SeededRng("fp", seed, True), T, ZETA, delta, pk=prover_pk_dict(pk))
+        PP.create_proof_engine(h2, prm, vk, None, None, [ab], [[]], MC.SeededRng("fp", seed, True), T, ZETA, delta, pk=pk)
         return bytes(T.proof)
     seeds = [3000 * k + i for i in range(max(lanes))]
     pk = keygen()

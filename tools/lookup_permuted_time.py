@@ -1,7 +1,7 @@
 """Time of the lookup argument's permuted columns on the GPU, from compressed columns to committed permuted columns: one call
-for every lookup (h2_poly_lookup_permuted + one batched commit, csrc/lookup.cuh) against the composition the engine-API
-prover uses today (tests/plonk_prover.create_proof_engine: per lookup h2_poly_lookup_permute, the blinding rows uploaded,
-one commit of its two columns).
+for every lookup (h2_poly_lookup_permuted + one batched commit, csrc/lookup.cuh) against a per-lookup composition
+(tests/lookup_permuted_cases.py: per lookup h2_poly_lookup_permute, the blinding rows uploaded, one commit of its two
+columns).
 
   python tools/lookup_permuted_time.py [--ks 14,16,18,20] [--counts 1,4,16] [--reps 5] [--out lookup_permuted_time.json]
   python tools/lookup_permuted_time.py --single [--pkg DIR]    # h2_poly_lookup_permute alone, one lookup

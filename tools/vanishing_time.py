@@ -1,7 +1,7 @@
 """Time of the vanishing argument's quotient on the GPU: h(X) on the extended domain -> its quotient_poly_degree pieces of n
 coefficients, the existing sequence (h2_poly_divide_by_vanishing in place, h2_poly_extended_to_coeff into a temporary of
-n (d - 1) coefficients, d - 1 h2_poly_copy calls; the composition of tests/plonk_prover.create_proof_engine) against one
-h2_poly_vanishing_quotient call.
+n (d - 1) coefficients, d - 1 h2_poly_copy calls; this tool's own composition) against one h2_poly_vanishing_quotient
+call.
 
   python tools/vanishing_time.py [--ks 11,14,17,20] [--degrees 3,5] [--reps 15] [--out vanishing_time.json]
 
