@@ -23,7 +23,7 @@ from typing import List, NamedTuple, Sequence, Tuple
 from . import lib as _l
 from .evaluator import Ast, AstLeaf
 from .multiopen import ProverQuery
-from .poly import Blind, EvaluationDomain, ResidentPoly, eval_polynomial_resident
+from .poly import Blind, EvaluationDomain, ResidentPoly, _split, eval_polynomial_resident, freed_on_failure
 from .products import Permuted
 
 
@@ -51,11 +51,6 @@ def _evaluate(pairs, n: int) -> List[int]:
     if not pairs:
         return []
     return eval_polynomial_resident([p for p, _ in pairs], [x for _, x in pairs], n=n)
-
-
-def _close(polys) -> None:
-    for p in polys:
-        p.close()
 
 
 # ---- the permutation argument ------------------------------------------------------------------------------------------
@@ -110,7 +105,9 @@ class PermutationCommitted(NamedTuple):
         return PermutationConstructed(self, blinding_factors), exprs
 
     def close(self) -> None:
-        _close([p for s in self.sets for p in s[:2]])
+        for s in self.sets:
+            s[0].close()
+            s[1].close()
 
 
 class PermutationConstructed(NamedTuple):
@@ -207,7 +204,8 @@ class LookupCommitted(NamedTuple):
         _check("permuted_input_coset", [p.permuted_input_coset for p in self.permuted], d.field, big)
         _check("permuted_table_coset", [p.permuted_table_coset for p in self.permuted], d.field, big)
         cosets = d.coeff_to_extended_batch_resident([z for z, _ in self.products]) if self.products else []
-        try:
+        with freed_on_failure() as fresh:
+            fresh.extend(cosets)
             one, beta_c, gamma_c = Ast.constant_term(1), Ast.constant_term(beta), Ast.constant_term(gamma)
             active = one - (l_last + l_blind)
             exprs: List[Ast] = []
@@ -220,13 +218,11 @@ class LookupCommitted(NamedTuple):
                           (left - right) * active,                                      # :426-447
                           (a - s) * l0,                                                 # :448-456
                           (a - s) * (a - a.with_rotation(-1)) * active]                 # :457-469
-        except BaseException:
-            _close(cosets)
-            raise
         return LookupConstructed(self, cosets), exprs
 
     def close(self) -> None:
-        _close([q for p in self.permuted for q in p[:8]] + [z for z, _ in self.products])
+        for q in [q for p in self.permuted for q in p[:8]] + [z for z, _ in self.products]:
+            q.close()
 
 
 class LookupConstructed(NamedTuple):
@@ -248,7 +244,8 @@ class LookupConstructed(NamedTuple):
         return LookupEvaluated(self, domain), _evaluate(pairs, domain.n)
 
     def close(self) -> None:
-        _close(self.product_cosets)
+        for p in self.product_cosets:
+            p.close()
         self.committed.close()
 
 
@@ -296,11 +293,7 @@ def evaluate_columns(domain: EvaluationDomain, x: int, instance_polys, advice_po
     holds the circuit's (column index, rotation) pairs.  Returns (instance evals per proof, advice evals per proof, fixed
     evals): the caller writes every proof's instance evals, then every proof's advice evals, then the fixed evals."""
     groups = _column_pairs(domain, x, instance_polys, advice_polys, fixed_polys, instance_queries, advice_queries, fixed_queries)
-    flat = _evaluate([pair for g in groups for pair in g], domain.n)
-    out, at = [], 0
-    for g in groups:
-        out.append(flat[at:at + len(g)])
-        at += len(g)
+    out = _split(_evaluate([pair for g in groups for pair in g], domain.n), [len(g) for g in groups])
     proofs = len(instance_polys)
     return out[:proofs], out[proofs:2 * proofs], out[-1]
 

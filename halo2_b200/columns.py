@@ -13,8 +13,8 @@ from typing import List, NamedTuple, Sequence
 import numpy as np
 
 from . import lib as _l
-from .poly import EvaluationDomain, Params, ResidentPoly, _tensor_rows, is_device_tensor, set_rows_resident, upload_tensors_resident
-from .products import _commit
+from .poly import (Blind, EvaluationDomain, Params, ResidentPoly, _split, _tensor_rows, freed_on_failure, is_device_tensor, set_rows_resident,
+                   upload_tensors_resident)
 
 
 class InstanceTooLarge(_l.H2Error):
@@ -38,29 +38,13 @@ class AdviceSingle(NamedTuple):
     cosets: List[ResidentPoly]             # extended domain
 
 
-def _column_bytes(col, m: int) -> np.ndarray:
-    if isinstance(col, np.ndarray):
-        return _l.as_u8(col, 32)
-    return np.frombuffer(b"".join((int(v) % m).to_bytes(32, "little") for v in col), dtype=np.uint8).reshape(-1, 32)
-
-
-def _transforms(domain: EvaluationDomain, values: List[ResidentPoly], live: List[ResidentPoly]):
-    """lagrange_to_coeff then coeff_to_extended of every column, one call each; new polynomials go to `live`."""
-    polys = [ResidentPoly(domain.field, domain.n) for _ in values]
-    live += polys
+def _transforms(domain: EvaluationDomain, values: List[ResidentPoly], fresh):
+    """lagrange_to_coeff then coeff_to_extended of every column, one call each, into new polynomials from `fresh`."""
+    polys = [fresh.keep(ResidentPoly(domain.field, domain.n)) for _ in values]
     domain.lagrange_to_coeff_batch_resident(values, out=polys)
-    cosets = [ResidentPoly(domain.field, domain.extended_len()) for _ in values]
-    live += cosets
+    cosets = [fresh.keep(ResidentPoly(domain.field, domain.extended_len())) for _ in values]
     domain.coeff_to_extended_batch_resident(polys, out=cosets)
     return polys, cosets
-
-
-def _split(flat: list, sizes: Sequence[int]) -> List[list]:
-    out, at = [], 0
-    for s in sizes:
-        out.append(flat[at:at + s])
-        at += s
-    return out
 
 
 def instance_commit(params: Params, domain: EvaluationDomain, instances: Sequence[Sequence], blinding_factors: int) -> List[InstanceSingle]:
@@ -69,24 +53,17 @@ def instance_commit(params: Params, domain: EvaluationDomain, instances: Sequenc
     committed with Blind::default(); raises InstanceTooLarge when a column is longer than n - (blinding_factors + 1).  The
     tensor columns go up in one h2_poly_upload_dev on torch's current stream.  Returns one InstanceSingle per proof."""
     n, m = domain.n, domain.m
-    cols = [col if is_device_tensor(col) else _column_bytes(col, m) for per in instances for col in per]
+    cols = [col if is_device_tensor(col) else _l.fe_array(col, m) for per in instances for col in per]
     rows = [_tensor_rows(c, "an instance column") if is_device_tensor(c) else c.shape[0] for c in cols]
     if any(r > n - (blinding_factors + 1) for r in rows):
         raise InstanceTooLarge("instance column longer than n - (blinding_factors + 1) (Error::InstanceTooLarge)")
-    live: List[ResidentPoly] = []
-    try:
-        for c, r in zip(cols, rows):
-            host = r and not is_device_tensor(c)
-            live.append(ResidentPoly(domain.field, n, c if host else None))   # allocated zero-filled: the padding
-        values = list(live)
+    with freed_on_failure() as fresh:
+        values = [fresh.keep(ResidentPoly(domain.field, n, c if r and not is_device_tensor(c) else None))   # allocated zero-filled: the padding
+                  for c, r in zip(cols, rows)]
         dev = [(p, c) for p, c, r in zip(values, cols, rows) if r and is_device_tensor(c)]
         upload_tensors_resident([p for p, _ in dev], [c for _, c in dev])
-        cm = _commit(params, values, [1] * len(values))
-        polys, cosets = _transforms(domain, values, live) if values else ([], [])
-    except BaseException:
-        for p in live:
-            p.close()
-        raise
+        cm = params.commit_resident_affine(values, [Blind() for _ in values], lagrange=True)
+        polys, cosets = _transforms(domain, values, fresh) if values else ([], [])
     sizes = [len(per) for per in instances]
     return [InstanceSingle(c, v, p, e) for c, v, p, e in zip(_split(cm, sizes), _split(values, sizes), _split(polys, sizes), _split(cosets, sizes))]
 
@@ -106,8 +83,7 @@ def advice_commit(params: Params, domain: EvaluationDomain, advice: Sequence[Seq
         for _ in per:
             blinding.append([rng.scalar() for _ in range(rows)])
         blinds.append([rng.scalar() for _ in per])
-    live: List[ResidentPoly] = []
-    try:
+    with freed_on_failure() as fresh:
         values, dev = [], []
         for per in advice:
             for col in per:
@@ -119,24 +95,17 @@ def advice_commit(params: Params, domain: EvaluationDomain, advice: Sequence[Seq
                 if is_device_tensor(col):
                     if _tensor_rows(col, "an advice column") != n:
                         raise _l.H2Error("an advice column does not have n rows")
-                    live.append(ResidentPoly(domain.field, n))
-                    values.append(live[-1])
-                    dev.append((live[-1], col))
+                    values.append(fresh.keep(ResidentPoly(domain.field, n)))
+                    dev.append((values[-1], col))
                     continue
-                arr = _column_bytes(col, m)
+                arr = _l.fe_array(col, m)
                 if arr.shape[0] != n:
                     raise _l.H2Error("an advice column does not have n rows")
-                live.append(ResidentPoly(domain.field, n, arr))
-                values.append(live[-1])
+                values.append(fresh.keep(ResidentPoly(domain.field, n, arr)))
         upload_tensors_resident([p for p, _ in dev], [c for _, c in dev])   # before the blinding rows overwrite their tail
-        flat_blinds = [b for per in blinds for b in per]
         set_rows_resident(values, usable, blinding)
-        cm = _commit(params, values, flat_blinds)
-        polys, cosets = _transforms(domain, values, live) if values else ([], [])
-    except BaseException:
-        for p in live:
-            p.close()
-        raise
+        cm = params.commit_resident_affine(values, [Blind(b) for per in blinds for b in per], lagrange=True)
+        polys, cosets = _transforms(domain, values, fresh) if values else ([], [])
     sizes = [len(per) for per in advice]
     return [AdviceSingle(c, b, v, p, e)
             for c, b, v, p, e in zip(_split(cm, sizes), blinds, _split(values, sizes), _split(polys, sizes), _split(cosets, sizes))]

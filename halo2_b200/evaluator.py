@@ -14,7 +14,7 @@ from typing import List, Optional, Sequence
 import numpy as np
 
 from . import lib as _l
-from .poly import EvaluationDomain, ResidentPoly
+from .poly import EvaluationDomain, ResidentPoly, freed_on_failure
 
 OP_POLY, OP_CONST, OP_LINEAR, OP_ADD, OP_MUL, OP_SCALE, OP_NEG = range(7)
 
@@ -132,14 +132,15 @@ class Evaluator:
         """evaluator.rs:129-228."""
         d = self.domain
         code, consts = compile_ast(ast, d.m, self.stride)
-        out = ResidentPoly(d.field, 1 << self.log_n) if out is None else out
-        cs = np.ascontiguousarray(np.stack([_l.fe_bytes(c) for c in consts])) if consts else np.zeros((0, 32), dtype=np.uint8)
+        cs = _l.fe_array(consts, d.m)
         omega = d.omega if self.basis == "lagrange" else d.extended_omega
         lin = 1 if self.basis == "lagrange" else d.g_coset
         hs = (ctypes.c_uint64 * max(len(self.polys), 1))(*[p._h.value for p in self.polys])
-        _l.check(_l.init().h2_poly_eval_ast(out._h, hs, ctypes.c_size_t(len(self.polys)), ctypes.c_uint32(self.log_n),
-                                            code.ctypes.data_as(ctypes.c_void_p), ctypes.c_size_t(code.shape[0]), _l.ptr(cs),
-                                            ctypes.c_size_t(len(consts)), _l.ptr(_l.fe_bytes(omega)), _l.ptr(_l.fe_bytes(lin)), _l.REPR_CANONICAL))
+        with freed_on_failure() as fresh:
+            out = fresh.keep(ResidentPoly(d.field, 1 << self.log_n)) if out is None else out
+            _l.check(_l.init().h2_poly_eval_ast(out._h, hs, ctypes.c_size_t(len(self.polys)), ctypes.c_uint32(self.log_n),
+                                                code.ctypes.data_as(ctypes.c_void_p), ctypes.c_size_t(code.shape[0]), _l.ptr(cs),
+                                                ctypes.c_size_t(len(consts)), _l.ptr(_l.fe_bytes(omega)), _l.ptr(_l.fe_bytes(lin)), _l.REPR_CANONICAL))
         return out
 
     def close(self) -> None:

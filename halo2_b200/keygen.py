@@ -18,7 +18,8 @@ import numpy as np
 
 from . import lib as _l
 from .evaluator import AstLeaf, compile_ast
-from .poly import FIELDS, Blind, EvaluationDomain, Params, ResidentPoly, _handles, _tensor_rows, batch_invert_resident, is_device_tensor, share_resident
+from .poly import (FIELDS, Blind, EvaluationDomain, Params, ResidentPoly, _handles, _tensor_rows, batch_invert_resident, freed_on_failure, is_device_tensor,
+                   share_resident)
 
 
 class Assembly:
@@ -133,11 +134,11 @@ def build_permutation_polys(domain: EvaluationDomain, assembly: Union[Assembly, 
     if assembly.n != domain.n:
         raise _l.H2Error(f"the assembly has {assembly.n} rows, the domain {domain.n}")
     cols = assembly.num_columns
-    polys = [ResidentPoly(domain.field, domain.n) for _ in range(cols)]
     if not cols:
-        return polys
+        return []
     omega, dl = _l.ptr(_l.fe_bytes(domain.omega)), _l.ptr(_l.fe_bytes(int(delta) % domain.m))
-    try:
+    with freed_on_failure() as fresh:
+        polys = [fresh.keep(ResidentPoly(domain.field, domain.n)) for _ in range(cols)]
         if isinstance(assembly, CopyConstraints):
             copies = np.ascontiguousarray(assembly.copies, dtype=np.uint32)
             _l.check(_l.init().h2_poly_permutation_sigma_copies(_handles(polys), ctypes.c_size_t(cols), ctypes.c_uint32(domain.k),
@@ -147,10 +148,6 @@ def build_permutation_polys(domain: EvaluationDomain, assembly: Union[Assembly, 
             mapping = np.ascontiguousarray(assembly.mapping)
             _l.check(_l.init().h2_poly_permutation_sigma(_handles(polys), ctypes.c_size_t(cols), ctypes.c_uint32(domain.k),
                                                          mapping.ctypes.data_as(ctypes.c_void_p), omega, dl, _l.REPR_CANONICAL))
-    except BaseException:
-        for p in polys:
-            p.close()
-        raise
     return polys
 
 
@@ -160,35 +157,23 @@ def batch_invert_assigned_resident(numerators: Sequence[ResidentPoly], denominat
     is 0, as ff::BatchInvert leaves zeros alone.  Returns new polynomials; the inputs are not changed."""
     assert len(numerators) == len(denominators)
     lib = _l.init()
-    out = []
-    for num, den in zip(numerators, denominators):
-        n = num.len
-        assert n & (n - 1) == 0 and den.len >= n and den.field == num.field, "columns of 2^k elements in one field"
-        code, consts = compile_ast(AstLeaf(0) * AstLeaf(1), FIELDS[num.field], 1)
-        inv = ResidentPoly(num.field, n)
-        res = ResidentPoly(num.field, n)
-        try:
-            inv.copy_from(den, n)
-            batch_invert_resident(inv, n)
-            one = _l.ptr(_l.fe_bytes(1))
-            _l.check(lib.h2_poly_eval_ast(res._h, _handles([num, inv]), ctypes.c_size_t(2), ctypes.c_uint32(n.bit_length() - 1),
-                                          code.ctypes.data_as(ctypes.c_void_p), ctypes.c_size_t(code.shape[0]), None, ctypes.c_size_t(len(consts)),
-                                          one, one, _l.REPR_CANONICAL))
-        except BaseException:
-            res.close()
-            for p in out:
-                p.close()
-            raise
-        finally:
-            inv.close()
-        out.append(res)
-    return out
-
-
-def _as_bytes(values, m: int) -> np.ndarray:
-    if hasattr(values, "dtype"):
-        return _l.as_u8(values, 32)
-    return np.frombuffer(b"".join((int(v) % m).to_bytes(32, "little") for v in values), dtype=np.uint8).reshape(-1, 32)
+    with freed_on_failure() as out:
+        for num, den in zip(numerators, denominators):
+            n = num.len
+            assert n & (n - 1) == 0 and den.len >= n and den.field == num.field, "columns of 2^k elements in one field"
+            code, consts = compile_ast(AstLeaf(0) * AstLeaf(1), FIELDS[num.field], 1)
+            inv = ResidentPoly(num.field, n)
+            res = out.keep(ResidentPoly(num.field, n))
+            try:
+                inv.copy_from(den, n)
+                batch_invert_resident(inv, n)
+                one = _l.ptr(_l.fe_bytes(1))
+                _l.check(lib.h2_poly_eval_ast(res._h, _handles([num, inv]), ctypes.c_size_t(2), ctypes.c_uint32(n.bit_length() - 1),
+                                              code.ctypes.data_as(ctypes.c_void_p), ctypes.c_size_t(code.shape[0]), None, ctypes.c_size_t(len(consts)),
+                                              one, one, _l.REPR_CANONICAL))
+            finally:
+                inv.close()
+    return list(out)
 
 
 def _lagrange_column(domain: EvaluationDomain, values) -> ResidentPoly:
@@ -196,7 +181,7 @@ def _lagrange_column(domain: EvaluationDomain, values) -> ResidentPoly:
     if is_device_tensor(values):
         assert _tensor_rows(values, "a fixed column") == domain.n, "a fixed column must have n values"
         return ResidentPoly.from_tensor(domain.field, values)
-    vals = _as_bytes(values, domain.m)
+    vals = _l.fe_array(values, domain.m)
     assert vals.shape[0] == domain.n, "a fixed column must have n values"
     return ResidentPoly(domain.field, domain.n, vals)
 
@@ -204,12 +189,11 @@ def _lagrange_column(domain: EvaluationDomain, values) -> ResidentPoly:
 def _fixed_values(domain: EvaluationDomain, fixed) -> List[ResidentPoly]:
     """The fixed columns as resident Lagrange values.  A column is its values (ints, an (n, 32) uint8 array or a CUDA
     tensor) or a (numerators, denominators) pair of such, which goes through batch_invert_assigned_resident."""
-    out: List[ResidentPoly] = []
-    try:
+    with freed_on_failure() as out:
         for col in fixed:
             if isinstance(col, tuple):
                 num, den = (ResidentPoly.from_tensor(domain.field, v, length=domain.n) if is_device_tensor(v) else
-                            ResidentPoly(domain.field, domain.n, _as_bytes(v, domain.m)) for v in col)
+                            ResidentPoly(domain.field, domain.n, _l.fe_array(v, domain.m)) for v in col)
                 try:
                     out.extend(batch_invert_assigned_resident([num], [den]))
                 finally:
@@ -217,11 +201,7 @@ def _fixed_values(domain: EvaluationDomain, fixed) -> List[ResidentPoly]:
                     den.close()
             else:
                 out.append(_lagrange_column(domain, col))
-    except BaseException:
-        for p in out:
-            p.close()
-        raise
-    return out
+    return list(out)
 
 
 def keygen_vk(params: Params, domain: EvaluationDomain, fixed, assembly: Union[Assembly, CopyConstraints], delta: int):
@@ -233,8 +213,6 @@ def keygen_vk(params: Params, domain: EvaluationDomain, fixed, assembly: Union[A
     nf = len(polys)
     try:
         polys += build_permutation_polys(domain, assembly, delta)
-        if not polys:
-            return np.zeros((0, 64), dtype=np.uint8), np.zeros((0, 64), dtype=np.uint8)
         cm = params.commit_resident_affine(polys, [Blind() for _ in polys], lagrange=True)
         return cm[:nf], cm[nf:]
     finally:
@@ -284,23 +262,17 @@ def keygen_pk(params: Params, domain: EvaluationDomain, fixed, assembly: Union[A
     assert params.n == domain.n
     n = domain.n
     assert 0 <= blinding_factors < n - 1
-    live: List[ResidentPoly] = []
+    with freed_on_failure() as fresh:
+        def coeff(lag):
+            return domain.lagrange_to_coeff_resident(lag, out=fresh.keep(ResidentPoly(domain.field, n)))
 
-    def coeff(lag):
-        return domain.lagrange_to_coeff_resident(lag, out=keep(ResidentPoly(domain.field, n)))
+        def ext(co):
+            return fresh.keep(domain.coeff_to_extended_resident(co))
 
-    def ext(co):
-        return keep(domain.coeff_to_extended_resident(co))
-
-    def keep(p):
-        live.append(p)
-        return p
-
-    try:
-        fixed_values = [keep(p) for p in _fixed_values(domain, fixed)]
+        fixed_values = [fresh.keep(p) for p in _fixed_values(domain, fixed)]
         fixed_polys = [coeff(v) for v in fixed_values]
         fixed_cosets = [ext(p) for p in fixed_polys]
-        perms = [keep(p) for p in build_permutation_polys(domain, assembly, delta)]
+        perms = [fresh.keep(p) for p in build_permutation_polys(domain, assembly, delta)]
         perm_polys = [coeff(v) for v in perms]
         perm = PermutationProvingKey(perms, perm_polys, [ext(p) for p in perm_polys])
         ls = []
@@ -313,8 +285,4 @@ def keygen_pk(params: Params, domain: EvaluationDomain, fixed, assembly: Union[A
                 ls.append(ext(lag))
             finally:
                 lag.close()
-        return ProvingKey(fixed_values, fixed_polys, fixed_cosets, perm, *ls)
-    except BaseException:
-        for p in live:
-            p.close()
-        raise
+    return ProvingKey(fixed_values, fixed_polys, fixed_cosets, perm, *ls)

@@ -147,3 +147,11 @@ def fe_bytes(x) -> np.ndarray:
     if arr.size != 32:
         raise ValueError("field element must be 32 bytes")
     return arr
+
+
+def fe_array(values, modulus: int) -> np.ndarray:
+    """Field elements -> contiguous (n, 32) uint8: an (n, 32) uint8 array as it is (as_u8), or ints reduced mod `modulus`,
+    32 bytes little-endian each."""
+    if hasattr(values, "dtype"):
+        return as_u8(values, 32)
+    return np.frombuffer(b"".join((int(v) % modulus).to_bytes(32, "little") for v in values), dtype=np.uint8).reshape(-1, 32)

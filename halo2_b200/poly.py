@@ -8,8 +8,9 @@ field elements); the transforms run on the GPU.
 """
 from __future__ import annotations
 
+import contextlib
 import ctypes
-from typing import Optional, Sequence
+from typing import List, Optional, Sequence
 
 import numpy as np
 
@@ -20,6 +21,7 @@ FIELDS = {
     "fq": 0x40000000000000000000000000000000224698FC0994A8DD8C46EB2100000001,
 }
 S = 32  # two-adicity of both fields
+_MSM_BATCH = 64  # the most polynomials one h2_msm_registered_batch* / h2_msm_registered_polys* call takes (csrc/capi_msm.cu)
 DIRECT_DEFAULT: Optional[bool] = None  # None: window tables (Params(direct=True) opts into digit-multiples tables; tests flip this)
 
 
@@ -185,87 +187,67 @@ class Params:
         """<poly, g_lagrange> + r * w   (commitment.rs:135-150)."""
         return self._commit(self._h_gl, poly, r)
 
-    def _commit_many(self, handle, polys, blinds: Sequence[Blind]) -> np.ndarray:
-        batch = len(polys)
-        assert batch == len(blinds) and batch >= 1
-        stack = np.ascontiguousarray(np.stack([_l.as_u8(p, 32) for p in polys]))
-        assert stack.shape[1] == self.n, "polynomial length != params.n"
-        bl = np.ascontiguousarray(np.stack([_l.fe_bytes(b.value) for b in blinds]))
-        out = np.zeros((batch, 96), dtype=np.uint8)
-        _l.check(_l.init().h2_msm_registered_batch(handle, _l.ptr(stack), ctypes.c_size_t(self.n), _l.ptr(bl), ctypes.c_size_t(batch),
-                                                    _l.REPR_CANONICAL, _l.ptr(out)))
+    def _commit_batched(self, polys, blinds: Sequence[Blind], lagrange: bool, affine: bool, resident: bool) -> np.ndarray:
+        """Every batched commit: the blinds encoded once, then one MSM pass per _MSM_BATCH polynomials (host arrays, or
+        ResidentPolys with resident=True).  Returns (batch, 64) affine or (batch, 96) Jacobian points."""
+        assert len(polys) == len(blinds)
+        lib, handle, n = _l.init(), self._h_gl if lagrange else self._h_g, ctypes.c_size_t(self.n)
+        bl = _l.fe_array([b.value for b in blinds], FIELDS[_l.SCALAR_FIELD[self.curve]])
+        out = np.zeros((len(polys), 64 if affine else 96), dtype=np.uint8)
+        for lo in range(0, len(polys), _MSM_BATCH):
+            part = polys[lo:lo + _MSM_BATCH]
+            count, b, o = ctypes.c_size_t(len(part)), _l.ptr(bl[lo:lo + _MSM_BATCH]), _l.ptr(out[lo:lo + _MSM_BATCH])
+            if resident:
+                fn = lib.h2_msm_registered_polys_affine if affine else lib.h2_msm_registered_polys
+                _l.check(fn(handle, _handles(part), count, n, b, _l.REPR_CANONICAL, o))
+            else:
+                stack = np.ascontiguousarray(np.stack([_l.as_u8(p, 32) for p in part]))
+                assert stack.shape[1] == self.n, "polynomial length != params.n"
+                fn = lib.h2_msm_registered_batch_affine if affine else lib.h2_msm_registered_batch
+                _l.check(fn(handle, _l.ptr(stack), n, b, count, _l.REPR_CANONICAL, o))
         return out
 
     def commit_many_affine(self, polys, blinds: Sequence[Blind], lagrange: bool = False) -> np.ndarray:
         """commit_many / commit_lagrange_many followed by C::Curve::batch_normalize on the device: the affine points
         the prover writes to the transcript (plonk/prover.rs:305-316), (batch, 64) uint8."""
-        batch = len(polys)
-        assert batch == len(blinds) and batch >= 1
-        stack = np.ascontiguousarray(np.stack([_l.as_u8(p, 32) for p in polys]))
-        assert stack.shape[1] == self.n, "polynomial length != params.n"
-        bl = np.ascontiguousarray(np.stack([_l.fe_bytes(b.value) for b in blinds]))
-        out = np.zeros((batch, 64), dtype=np.uint8)
-        _l.check(_l.init().h2_msm_registered_batch_affine(self._h_gl if lagrange else self._h_g, _l.ptr(stack), ctypes.c_size_t(self.n),
-                                                           _l.ptr(bl), ctypes.c_size_t(batch), _l.REPR_CANONICAL, _l.ptr(out)))
-        return out
+        return self._commit_batched(polys, blinds, lagrange, affine=True, resident=False)
 
     def commit_many(self, polys, blinds: Sequence[Blind]) -> np.ndarray:
         """[commit(p, r) for p, r in zip(polys, blinds)] in one pass over the resident table -- the shape
         of the prover's per-column loops (plonk/prover.rs:305-309, vanishing/prover.rs:102-106)."""
-        return self._commit_many(self._h_g, polys, blinds)
+        return self._commit_batched(polys, blinds, lagrange=False, affine=False, resident=False)
 
     def commit_lagrange_many(self, polys, blinds: Sequence[Blind]) -> np.ndarray:
-        return self._commit_many(self._h_gl, polys, blinds)
+        return self._commit_batched(polys, blinds, lagrange=True, affine=False, resident=False)
 
     def commit_resident(self, polys: Sequence["ResidentPoly"], blinds: Sequence[Blind], lagrange: bool = False) -> np.ndarray:
         """[commit(p, r)] (or commit_lagrange with lagrange=True) for device-resident polynomials: nothing but the
         blinds goes up, nothing but the points comes back."""
-        batch = len(polys)
-        assert batch == len(blinds) and batch >= 1
-        hs = (ctypes.c_uint64 * batch)(*[p._h.value for p in polys])
-        bl = np.ascontiguousarray(np.stack([_l.fe_bytes(b.value) for b in blinds]))
-        out = np.zeros((batch, 96), dtype=np.uint8)
-        _l.check(_l.init().h2_msm_registered_polys(self._h_gl if lagrange else self._h_g, hs, ctypes.c_size_t(batch), ctypes.c_size_t(self.n),
-                                                    _l.ptr(bl), _l.REPR_CANONICAL, _l.ptr(out)))
-        return out
+        return self._commit_batched(polys, blinds, lagrange, affine=False, resident=True)
 
     def commit_resident_affine(self, polys: Sequence["ResidentPoly"], blinds: Sequence[Blind], lagrange: bool = False) -> np.ndarray:
         """commit_resident + C::Curve::batch_normalize on the device: (batch, 64) affine points, ready for write_point."""
-        batch = len(polys)
-        assert batch == len(blinds) and batch >= 1
-        hs = (ctypes.c_uint64 * batch)(*[p._h.value for p in polys])
-        bl = np.ascontiguousarray(np.stack([_l.fe_bytes(b.value) for b in blinds]))
-        out = np.zeros((batch, 64), dtype=np.uint8)
-        _l.check(_l.init().h2_msm_registered_polys_affine(self._h_gl if lagrange else self._h_g, hs, ctypes.c_size_t(batch), ctypes.c_size_t(self.n),
-                                                           _l.ptr(bl), _l.REPR_CANONICAL, _l.ptr(out)))
-        return out
+        return self._commit_batched(polys, blinds, lagrange, affine=True, resident=True)
 
-    def ipa_rounds_transcript(self, p_prime, x3: int, z: int, challenge, l_rand: Sequence[int], r_rand: Sequence[int]):
-        """ipa_rounds for a transcript-driven caller: `p_prime` may be a ResidentPoly (nothing is uploaded), L_j / R_j come back
-        as the AFFINE points the reference writes to the transcript (prover.rs:120-125), and `challenge(j, l_xy, r_xy) -> u_j`.
-        Returns (L (k, 64), R (k, 64), c)."""
+    def _ipa_rounds(self, begin, width: int, x3: int, z: int, challenge, l_rand: Sequence[int], r_rand: Sequence[int]):
+        """The round loop of ipa_rounds / ipa_rounds_transcript: `begin(lib, x3, session)` opens the session on p', and the
+        rounds return L_j / R_j as Jacobian (width 96) or affine (width 64) points."""
         if self.u is None or not self._has_table:
             raise _l.H2Error("ipa_rounds needs Params(u=..., precompute=True)")
-        m = FIELDS[{"pallas": "fq", "vesta": "fp"}[self.curve]]
+        m = FIELDS[_l.SCALAR_FIELD[self.curve]]
         lib = _l.init()
         assert len(l_rand) == self.k and len(r_rand) == self.k
         sess = ctypes.c_uint64(0)
-        if isinstance(p_prime, ResidentPoly):
-            _l.check(lib.h2_ipa_begin_poly(self._h_g, ctypes.c_uint32(self.k), p_prime._h, _l.ptr(_l.fe_bytes(x3 % m)), _l.REPR_CANONICAL,
-                                           ctypes.byref(sess)))
-        else:
-            pp = _l.as_u8(p_prime, 32)
-            assert pp.shape[0] == self.n
-            _l.check(lib.h2_ipa_begin(self._h_g, ctypes.c_uint32(self.k), _l.ptr(pp), _l.ptr(_l.fe_bytes(x3 % m)), _l.REPR_CANONICAL,
-                                      ctypes.byref(sess)))
-        ls = np.zeros((self.k, 64), dtype=np.uint8)
-        rs = np.zeros((self.k, 64), dtype=np.uint8)
-        lr = np.zeros((2, 64), dtype=np.uint8)
+        _l.check(begin(lib, _l.ptr(_l.fe_bytes(x3 % m)), ctypes.byref(sess)))
+        round_call = lib.h2_ipa_round_affine if width == 64 else lib.h2_ipa_round
+        ls = np.zeros((self.k, width), dtype=np.uint8)
+        rs = np.zeros((self.k, width), dtype=np.uint8)
+        lr = np.zeros((2, width), dtype=np.uint8)
         zb = _l.fe_bytes(z % m)
         try:
             for j in range(self.k):
-                _l.check(lib.h2_ipa_round_affine(sess, _l.ptr(zb), _l.ptr(_l.fe_bytes(l_rand[j] % m)), _l.ptr(_l.fe_bytes(r_rand[j] % m)),
-                                                 _l.REPR_CANONICAL, _l.ptr(lr)))
+                _l.check(round_call(sess, _l.ptr(zb), _l.ptr(_l.fe_bytes(l_rand[j] % m)), _l.ptr(_l.fe_bytes(r_rand[j] % m)),
+                                    _l.REPR_CANONICAL, _l.ptr(lr)))
                 ls[j], rs[j] = lr[0], lr[1]
                 u_j = int(challenge(j, ls[j], rs[j])) % m
                 _l.check(lib.h2_ipa_fold(sess, _l.ptr(_l.fe_bytes(u_j)), _l.ptr(_l.fe_bytes(pow(u_j, -1, m))), _l.REPR_CANONICAL))
@@ -276,39 +258,31 @@ class Params:
             if sess.value:
                 lib.h2_ipa_finish(sess, _l.REPR_CANONICAL, None)
         return ls, rs, int.from_bytes(cb[0].tobytes(), "little")
+
+    def _begin_host(self, p_prime):
+        def begin(lib, x3, sess):
+            pp = _l.as_u8(p_prime, 32)
+            assert pp.shape[0] == self.n
+            return lib.h2_ipa_begin(self._h_g, ctypes.c_uint32(self.k), _l.ptr(pp), x3, _l.REPR_CANONICAL, sess)
+        return begin
+
+    def ipa_rounds_transcript(self, p_prime, x3: int, z: int, challenge, l_rand: Sequence[int], r_rand: Sequence[int]):
+        """ipa_rounds for a transcript-driven caller: `p_prime` may be a ResidentPoly (nothing is uploaded), L_j / R_j come back
+        as the AFFINE points the reference writes to the transcript (prover.rs:120-125), and `challenge(j, l_xy, r_xy) -> u_j`.
+        Returns (L (k, 64), R (k, 64), c)."""
+        if isinstance(p_prime, ResidentPoly):
+            def begin(lib, x3, sess):
+                return lib.h2_ipa_begin_poly(self._h_g, ctypes.c_uint32(self.k), p_prime._h, x3, _l.REPR_CANONICAL, sess)
+        else:
+            begin = self._begin_host(p_prime)
+        return self._ipa_rounds(begin, 64, x3, z, challenge, l_rand, r_rand)
 
     def ipa_rounds(self, p_prime, x3: int, z: int, challenge, l_rand: Sequence[int], r_rand: Sequence[int]):
         """The round loop of commitment::create_proof (poly/commitment/prover.rs:100-142) on the device.
         `p_prime` (:80) is the blinded polynomial with P(x3) removed; `challenge(j, L_j, R_j) -> u_j` is the
         caller's transcript (write L_j, R_j; squeeze u_j); l_rand / r_rand are the per-round blinds (:112-113).
         Returns (L (k, 96), R (k, 96), c) -- c is what :147 writes to the transcript."""
-        if self.u is None or not self._has_table:
-            raise _l.H2Error("ipa_rounds needs Params(u=..., precompute=True)")
-        m = FIELDS[{"pallas": "fq", "vesta": "fp"}[self.curve]]
-        lib = _l.init()
-        pp = _l.as_u8(p_prime, 32)
-        assert pp.shape[0] == self.n and len(l_rand) == self.k and len(r_rand) == self.k
-        sess = ctypes.c_uint64(0)
-        _l.check(lib.h2_ipa_begin(self._h_g, ctypes.c_uint32(self.k), _l.ptr(pp), _l.ptr(_l.fe_bytes(x3 % m)), _l.REPR_CANONICAL,
-                                  ctypes.byref(sess)))
-        ls = np.zeros((self.k, 96), dtype=np.uint8)
-        rs = np.zeros((self.k, 96), dtype=np.uint8)
-        lr = np.zeros((2, 96), dtype=np.uint8)
-        zb = _l.fe_bytes(z % m)
-        try:
-            for j in range(self.k):
-                _l.check(lib.h2_ipa_round(sess, _l.ptr(zb), _l.ptr(_l.fe_bytes(l_rand[j] % m)), _l.ptr(_l.fe_bytes(r_rand[j] % m)),
-                                          _l.REPR_CANONICAL, _l.ptr(lr)))
-                ls[j], rs[j] = lr[0], lr[1]
-                u_j = int(challenge(j, ls[j], rs[j])) % m
-                _l.check(lib.h2_ipa_fold(sess, _l.ptr(_l.fe_bytes(u_j)), _l.ptr(_l.fe_bytes(pow(u_j, -1, m))), _l.REPR_CANONICAL))
-            cb = np.zeros((2, 32), dtype=np.uint8)
-            _l.check(lib.h2_ipa_finish(sess, _l.REPR_CANONICAL, _l.ptr(cb)))
-            sess.value = 0
-        finally:
-            if sess.value:
-                lib.h2_ipa_finish(sess, _l.REPR_CANONICAL, None)
-        return ls, rs, int.from_bytes(cb[0].tobytes(), "little")
+        return self._ipa_rounds(self._begin_host(p_prime), 96, x3, z, challenge, l_rand, r_rand)
 
     def close(self) -> None:
         lib = _l.load()
@@ -359,12 +333,9 @@ class ResidentPoly:
         row in `repr` ("canonical" or "montgomery").  Asynchronous on `stream` (default: torch's current stream on t's
         device), ordered before every later call of the calling thread's lane."""
         rows = _tensor_rows(t, "t")
-        p = cls(field, rows if length is None else length)
-        try:
+        with freed_on_failure() as fresh:
+            p = fresh.keep(cls(field, rows if length is None else length))
             p.upload_tensor(t, repr=repr, stream=stream)
-        except BaseException:
-            p.close()
-            raise
         return p
 
     def upload_tensor(self, t, repr: str = "canonical", stream=None) -> None:
@@ -407,6 +378,36 @@ class ResidentPoly:
             self.close()
         except Exception:
             pass
+
+
+class _Fresh(list):
+    """The resident polynomials a call makes for its result (see freed_on_failure)."""
+
+    def keep(self, poly: ResidentPoly) -> ResidentPoly:
+        self.append(poly)
+        return poly
+
+
+@contextlib.contextmanager
+def freed_on_failure():
+    """`with freed_on_failure() as fresh:` -- the polynomials handed to fresh.keep(poly) (which returns poly) are closed if the
+    block raises and kept if it returns, so a call that fails leaves none of its outputs allocated."""
+    fresh = _Fresh()
+    try:
+        yield fresh
+    except BaseException:
+        for p in fresh:
+            p.close()
+        raise
+
+
+def _split(flat: list, sizes: Sequence[int]) -> List[list]:
+    """flat cut into consecutive lists of sizes[0], sizes[1], ... items: one list per proof."""
+    out, at = [], 0
+    for s in sizes:
+        out.append(flat[at:at + s])
+        at += s
+    return out
 
 
 def _handles(polys: Sequence["ResidentPoly"]):
@@ -534,8 +535,7 @@ def set_rows_resident(polys: Sequence["ResidentPoly"], start: int, values) -> No
     if isinstance(values, np.ndarray):
         arr = np.ascontiguousarray(values, dtype=np.uint8)
     else:
-        m = FIELDS[polys[0].field]
-        arr = np.frombuffer(b"".join((int(v) % m).to_bytes(32, "little") for col in values for v in col), dtype=np.uint8)
+        arr = _l.fe_array((v for col in values for v in col), FIELDS[polys[0].field])
     arr = arr.reshape(count, -1, 32) if arr.size else np.zeros((count, 0, 32), dtype=np.uint8)
     _l.check(_l.init().h2_poly_set_rows(_handles(polys), ctypes.c_size_t(count), ctypes.c_size_t(int(start)), ctypes.c_size_t(arr.shape[1]),
                                         _l.ptr(arr) if arr.size else None, _l.REPR_CANONICAL))
@@ -546,8 +546,7 @@ def eval_polynomial_resident(polys: Sequence["ResidentPoly"], points: Sequence[i
     batch = len(polys)
     assert batch == len(points) and batch >= 1
     n = polys[0].len if n is None else int(n)
-    m = FIELDS[polys[0].field]
-    pts = np.ascontiguousarray(np.stack([_l.fe_bytes(int(x) % m) for x in points]))
+    pts = _l.fe_array(points, FIELDS[polys[0].field])
     out = np.zeros((batch, 32), dtype=np.uint8)
     _l.check(_l.init().h2_poly_eval(_handles(polys), ctypes.c_size_t(batch), ctypes.c_size_t(n), _l.ptr(pts), _l.REPR_CANONICAL, _l.ptr(out)))
     return [int.from_bytes(r.tobytes(), "little") for r in out]
@@ -571,11 +570,11 @@ def kate_division_resident(src: Sequence["ResidentPoly"], points: Sequence[int],
     batch = len(src)
     assert batch == len(points) and batch >= 1
     n = src[0].len if n is None else int(n)
-    m = FIELDS[src[0].field]
-    if dst is None:
-        dst = [ResidentPoly(src[0].field, max(n - 1, 1)) for _ in range(batch)]
-    pts = np.ascontiguousarray(np.stack([_l.fe_bytes(int(x) % m) for x in points]))
-    _l.check(_l.init().h2_poly_kate_division(_handles(dst), _handles(src), ctypes.c_size_t(batch), ctypes.c_size_t(n), _l.ptr(pts), _l.REPR_CANONICAL))
+    pts = _l.fe_array(points, FIELDS[src[0].field])
+    with freed_on_failure() as fresh:
+        if dst is None:
+            dst = [fresh.keep(ResidentPoly(src[0].field, max(n - 1, 1))) for _ in range(batch)]
+        _l.check(_l.init().h2_poly_kate_division(_handles(dst), _handles(src), ctypes.c_size_t(batch), ctypes.c_size_t(n), _l.ptr(pts), _l.REPR_CANONICAL))
     return list(dst)
 
 
@@ -588,8 +587,9 @@ def batch_invert_resident(a: "ResidentPoly", n: Optional[int] = None) -> "Reside
 def running_product_resident(src: "ResidentPoly", init: int = 1, dst: Optional["ResidentPoly"] = None, n: Optional[int] = None) -> "ResidentPoly":
     """z[0] = init, z[i] = z[i-1] * src[i-1] (plonk/permutation/prover.rs:150-156), left on the device."""
     n = src.len if n is None else int(n)
-    dst = ResidentPoly(src.field, n) if dst is None else dst
-    _l.check(_l.init().h2_poly_running_product(dst._h, src._h, ctypes.c_size_t(n), _l.ptr(_l.fe_bytes(int(init) % FIELDS[src.field])), _l.REPR_CANONICAL))
+    with freed_on_failure() as fresh:
+        dst = fresh.keep(ResidentPoly(src.field, n)) if dst is None else dst
+        _l.check(_l.init().h2_poly_running_product(dst._h, src._h, ctypes.c_size_t(n), _l.ptr(_l.fe_bytes(int(init) % FIELDS[src.field])), _l.REPR_CANONICAL))
     return dst
 
 
@@ -600,9 +600,10 @@ def permute_expression_pair_resident(input_expression: "ResidentPoly", table_exp
     row of every run of equal inputs.  The blinding rows from `usable_rows` on (:625-627) are the caller's: write them with
     `upload_at`-style calls or `add_at`.  An input value missing from the table raises H2Error (the reference returns
     Error::ConstraintSystemFailure, :605-608)."""
-    out_input = ResidentPoly(input_expression.field, input_expression.len) if out_input is None else out_input
-    out_table = ResidentPoly(input_expression.field, input_expression.len) if out_table is None else out_table
-    _l.check(_l.init().h2_poly_lookup_permute(input_expression._h, table_expression._h, ctypes.c_size_t(int(usable_rows)), out_input._h, out_table._h))
+    with freed_on_failure() as fresh:
+        out_input = fresh.keep(ResidentPoly(input_expression.field, input_expression.len)) if out_input is None else out_input
+        out_table = fresh.keep(ResidentPoly(input_expression.field, input_expression.len)) if out_table is None else out_table
+        _l.check(_l.init().h2_poly_lookup_permute(input_expression._h, table_expression._h, ctypes.c_size_t(int(usable_rows)), out_input._h, out_table._h))
     return out_input, out_table
 
 
@@ -710,7 +711,7 @@ class EvaluationDomain:
         """In place on a resident extended-domain polynomial (the step between the AST evaluation and extended_to_coeff,
         plonk/vanishing/prover.rs:81-88)."""
         assert a.len >= self.extended_len()
-        t = np.ascontiguousarray(np.stack([_l.fe_bytes(x) for x in self.t_evaluations]))
+        t = _l.fe_array(self.t_evaluations, self.m)
         _l.check(_l.init().h2_poly_divide_by_vanishing(a._h, ctypes.c_uint32(self.extended_k), _l.ptr(t), ctypes.c_uint32(len(self.t_evaluations)),
                                                        _l.REPR_CANONICAL))
         return a
@@ -723,19 +724,21 @@ class EvaluationDomain:
         return out
 
     def coeff_to_extended_resident(self, a: "ResidentPoly", out: Optional["ResidentPoly"] = None) -> "ResidentPoly":
-        out = ResidentPoly(self.field, self.extended_len()) if out is None else out
-        _l.check(_l.init().h2_poly_coeff_to_extended(out._h, a._h, ctypes.c_uint32(self.k), ctypes.c_uint32(self.extended_k),
-                                                     _l.ptr(_l.fe_bytes(self.g_coset)), _l.ptr(_l.fe_bytes(self.extended_omega)),
-                                                     _l.REPR_CANONICAL))
+        with freed_on_failure() as fresh:
+            out = fresh.keep(ResidentPoly(self.field, self.extended_len())) if out is None else out
+            _l.check(_l.init().h2_poly_coeff_to_extended(out._h, a._h, ctypes.c_uint32(self.k), ctypes.c_uint32(self.extended_k),
+                                                         _l.ptr(_l.fe_bytes(self.g_coset)), _l.ptr(_l.fe_bytes(self.extended_omega)),
+                                                         _l.REPR_CANONICAL))
         return out
 
     def extended_to_coeff_resident(self, a: "ResidentPoly", out: Optional["ResidentPoly"] = None) -> "ResidentPoly":
         out_len = self.n * self.quotient_poly_degree
-        out = ResidentPoly(self.field, out_len) if out is None else out
-        _l.check(_l.init().h2_poly_extended_to_coeff(out._h, a._h, ctypes.c_uint32(self.extended_k),
-                                                     _l.ptr(_l.fe_bytes(self.extended_omega_inv)),
-                                                     _l.ptr(_l.fe_bytes(self.extended_ifft_divisor)), _l.ptr(_l.fe_bytes(self.g_coset)),
-                                                     ctypes.c_size_t(out_len), _l.REPR_CANONICAL))
+        with freed_on_failure() as fresh:
+            out = fresh.keep(ResidentPoly(self.field, out_len)) if out is None else out
+            _l.check(_l.init().h2_poly_extended_to_coeff(out._h, a._h, ctypes.c_uint32(self.extended_k),
+                                                         _l.ptr(_l.fe_bytes(self.extended_omega_inv)),
+                                                         _l.ptr(_l.fe_bytes(self.extended_ifft_divisor)), _l.ptr(_l.fe_bytes(self.g_coset)),
+                                                         ctypes.c_size_t(out_len), _l.REPR_CANONICAL))
         return out
 
     def lagrange_to_coeff_batch_resident(self, polys: Sequence["ResidentPoly"], out: Optional[Sequence["ResidentPoly"]] = None) -> list:
@@ -750,16 +753,10 @@ class EvaluationDomain:
 
     def coeff_to_extended_batch_resident(self, polys: Sequence["ResidentPoly"], out: Optional[Sequence["ResidentPoly"]] = None) -> list:
         """coeff_to_extended of every column in one call (h2_poly_coeff_to_extended_batch).  out=None allocates the cosets."""
-        fresh = out is None
-        out = [ResidentPoly(self.field, self.extended_len()) for _ in polys] if fresh else list(out)
-        assert len(out) == len(polys)
-        try:
+        with freed_on_failure() as fresh:
+            out = [fresh.keep(ResidentPoly(self.field, self.extended_len())) for _ in polys] if out is None else list(out)
+            assert len(out) == len(polys)
             _l.check(_l.init().h2_poly_coeff_to_extended_batch(_handles(out), _handles(polys), ctypes.c_size_t(len(polys)), ctypes.c_uint32(self.k),
                                                                ctypes.c_uint32(self.extended_k), _l.ptr(_l.fe_bytes(self.g_coset)),
                                                                _l.ptr(_l.fe_bytes(self.extended_omega)), _l.REPR_CANONICAL))
-        except BaseException:
-            if fresh:
-                for p in out:
-                    p.close()
-            raise
         return out

@@ -11,28 +11,9 @@ from __future__ import annotations
 import ctypes
 from typing import List, NamedTuple, Sequence, Tuple
 
-import numpy as np
-
 from . import lib as _l
 from .evaluator import Ast
-from .poly import Blind, EvaluationDomain, Params, ResidentPoly, _handles
-
-_MAX_COMMIT_BATCH = 64   # h2_msm_registered_polys_affine takes at most this many polynomials per pass
-
-
-def _scalars(values, m: int) -> np.ndarray:
-    if not values:
-        return None
-    return np.frombuffer(b"".join((int(v) % m).to_bytes(32, "little") for v in values), dtype=np.uint8).reshape(-1, 32)
-
-
-def _alloc(field: str, n: int, count: int) -> List[ResidentPoly]:
-    return [ResidentPoly(field, n) for _ in range(count)]
-
-
-def _close(polys) -> None:
-    for p in polys:
-        p.close()
+from .poly import Blind, EvaluationDomain, Params, ResidentPoly, _handles, _split, freed_on_failure
 
 
 def permutation_product_resident(domain: EvaluationDomain, columns: Sequence[Sequence[ResidentPoly]], sigmas: Sequence[ResidentPoly], beta: int,
@@ -49,16 +30,14 @@ def permutation_product_resident(domain: EvaluationDomain, columns: Sequence[Seq
     sets = -(-cols // chunk_len)
     if len(blinding) != proofs * sets * blinding_factors:
         raise _l.H2Error(f"expected {proofs * sets * blinding_factors} blinding values, got {len(blinding)}")
-    z = _alloc(domain.field, n, proofs * sets)
-    try:
+    bl = _l.fe_array(blinding, m) if blinding else None                       # no blinding rows: a null pointer
+    with freed_on_failure() as fresh:
+        z = [fresh.keep(ResidentPoly(domain.field, n)) for _ in range(proofs * sets)]
         _l.check(_l.init().h2_poly_permutation_product(
             _handles(z), ctypes.c_size_t(proofs), _handles([c for per in columns for c in per]), _handles(sigmas), ctypes.c_size_t(cols),
             ctypes.c_uint32(chunk_len), ctypes.c_uint32(domain.k), _l.ptr(_l.fe_bytes(beta % m)), _l.ptr(_l.fe_bytes(gamma % m)),
-            _l.ptr(_l.fe_bytes(domain.omega)), _l.ptr(_l.fe_bytes(delta % m)), _l.ptr(_scalars(blinding, m)), ctypes.c_uint32(blinding_factors),
+            _l.ptr(_l.fe_bytes(domain.omega)), _l.ptr(_l.fe_bytes(delta % m)), _l.ptr(bl), ctypes.c_uint32(blinding_factors),
             _l.REPR_CANONICAL))
-    except BaseException:
-        _close(z)
-        raise
     return [z[p * sets:(p + 1) * sets] for p in range(proofs)]
 
 
@@ -71,27 +50,14 @@ def lookup_product_resident(domain: EvaluationDomain, lookups: Sequence[Sequence
     flat = [lk for per in lookups for lk in per]
     if len(blinding) != len(flat) * blinding_factors:
         raise _l.H2Error(f"expected {len(flat) * blinding_factors} blinding values, got {len(blinding)}")
-    z = _alloc(domain.field, n, len(flat))
-    try:
+    bl = _l.fe_array(blinding, m) if blinding else None
+    with freed_on_failure() as fresh:
+        z = [fresh.keep(ResidentPoly(domain.field, n)) for _ in flat]
         parts = [_handles([lk[j] for lk in flat]) for j in range(4)]
         _l.check(_l.init().h2_poly_lookup_product(_handles(z), ctypes.c_size_t(len(flat)), *parts, ctypes.c_uint32(domain.k),
-                                                   _l.ptr(_l.fe_bytes(beta % m)), _l.ptr(_l.fe_bytes(gamma % m)), _l.ptr(_scalars(blinding, m)),
+                                                   _l.ptr(_l.fe_bytes(beta % m)), _l.ptr(_l.fe_bytes(gamma % m)), _l.ptr(bl),
                                                    ctypes.c_uint32(blinding_factors), _l.REPR_CANONICAL))
-    except BaseException:
-        _close(z)
-        raise
-    out, at = [], 0
-    for per in lookups:
-        out.append(z[at:at + len(per)])
-        at += len(per)
-    return out
-
-
-def _commit(params: Params, polys: List[ResidentPoly], blinds: List[int]) -> np.ndarray:
-    if not polys:
-        return np.zeros((0, 64), dtype=np.uint8)
-    return np.concatenate([params.commit_resident_affine(polys[i:i + _MAX_COMMIT_BATCH], [Blind(b) for b in blinds[i:i + _MAX_COMMIT_BATCH]],
-                                                         lagrange=True) for i in range(0, len(polys), _MAX_COMMIT_BATCH)])
+    return _split(z, [len(per) for per in lookups])
 
 
 def permutation_commit(params: Params, domain: EvaluationDomain, pk, columns: Sequence[Sequence[ResidentPoly]], beta: int, gamma: int, delta: int,
@@ -109,15 +75,13 @@ def permutation_commit(params: Params, domain: EvaluationDomain, pk, columns: Se
         blinding += [rng.scalar() for _ in range(blinding_factors)]
         blinds.append(rng.scalar())
     z = [p for per in permutation_product_resident(domain, columns, sigmas, beta, gamma, delta, chunk_len, blinding_factors, blinding) for p in per]
-    cosets: List[ResidentPoly] = []
-    try:
-        cm = _commit(params, z, blinds)
+    with freed_on_failure() as fresh:
+        fresh.extend(z)
+        cm = params.commit_resident_affine(z, [Blind(b) for b in blinds], lagrange=True)
+        cosets = []
         for p in z:
             domain.lagrange_to_coeff_resident(p)                                  # in place: z becomes permutation_product_poly
-            cosets.append(domain.coeff_to_extended_resident(p))
-    except BaseException:
-        _close(z + cosets)
-        raise
+            cosets.append(fresh.keep(domain.coeff_to_extended_resident(p)))
     return [list(zip(z, cosets, blinds))[p * sets:(p + 1) * sets] for p in range(proofs)], cm
 
 
@@ -133,18 +97,12 @@ def lookup_commit_product(params: Params, domain: EvaluationDomain, lookups, bet
         blinds.append(rng.scalar())
     z = lookup_product_resident(domain, lookups, beta, gamma, blinding_factors, blinding)
     flat = [p for per in z for p in per]
-    try:
-        cm = _commit(params, flat, blinds)
+    with freed_on_failure() as fresh:
+        fresh.extend(flat)
+        cm = params.commit_resident_affine(flat, [Blind(b) for b in blinds], lagrange=True)
         for p in flat:
             domain.lagrange_to_coeff_resident(p)
-    except BaseException:
-        _close(flat)
-        raise
-    out, at = [], 0
-    for per in z:
-        out.append(list(zip(per, blinds[at:at + len(per)])))
-        at += len(per)
-    return out, cm
+    return [list(zip(per, bl)) for per, bl in zip(z, _split(blinds, [len(per) for per in z]))], cm
 
 
 def lookup_permute_resident(domain: EvaluationDomain, pairs: Sequence[Tuple[ResidentPoly, ResidentPoly]], blinding_factors: int,
@@ -156,14 +114,12 @@ def lookup_permute_resident(domain: EvaluationDomain, pairs: Sequence[Tuple[Resi
     m, n, rows = domain.m, domain.n, blinding_factors + 1
     if len(blinding) != len(pairs) * 2 * rows:
         raise _l.H2Error(f"expected {len(pairs) * 2 * rows} blinding values, got {len(blinding)}")
-    out = _alloc(domain.field, n, 2 * len(pairs))
-    try:
+    bl = _l.fe_array(blinding, m) if blinding else None
+    with freed_on_failure() as fresh:
+        out = [fresh.keep(ResidentPoly(domain.field, n)) for _ in range(2 * len(pairs))]
         _l.check(_l.init().h2_poly_lookup_permuted(_handles(out[0::2]), _handles(out[1::2]), ctypes.c_size_t(len(pairs)),
                                                     _handles([p[0] for p in pairs]), _handles([p[1] for p in pairs]), ctypes.c_uint32(domain.k),
-                                                    _l.ptr(_scalars(blinding, m)), ctypes.c_uint32(blinding_factors), _l.REPR_CANONICAL))
-    except BaseException:
-        _close(out)
-        raise
+                                                    _l.ptr(bl), ctypes.c_uint32(blinding_factors), _l.REPR_CANONICAL))
     return list(zip(out[0::2], out[1::2]))
 
 
@@ -202,29 +158,15 @@ def lookup_commit_permuted(params: Params, domain: EvaluationDomain, evaluator, 
             acc = acc * theta + e
         return evaluator.evaluate(acc)
 
-    compressed: List[ResidentPoly] = []
-    permuted: List[ResidentPoly] = []
-    extra: List[ResidentPoly] = []
-    try:
-        for per in lookups:
-            for inp, tab in per:
-                compressed += [compress(inp), compress(tab)]
-        permuted = [q for pair in lookup_permute_resident(domain, list(zip(compressed[0::2], compressed[1::2])), blinding_factors, blinding)
+    with freed_on_failure() as fresh:
+        compressed = [fresh.keep(compress(e)) for per in lookups for inp, tab in per for e in (inp, tab)]
+        permuted = [fresh.keep(q) for pair in lookup_permute_resident(domain, list(zip(compressed[0::2], compressed[1::2])), blinding_factors, blinding)
                     for q in pair]
-        cm = _commit(params, permuted, blinds)
+        cm = params.commit_resident_affine(permuted, [Blind(b) for b in blinds], lagrange=True)
+        extra = []
         for q in permuted:
-            co = domain.lagrange_to_coeff_resident(q, out=ResidentPoly(domain.field, domain.n))
-            extra.append(co)
-            extra.append(domain.coeff_to_extended_resident(co))
-    except BaseException:
-        _close(compressed + permuted + extra)
-        raise
-    out, at = [], 0
-    for per in lookups:
-        mine = []
-        for _ in per:
-            c, q, e, b = compressed[at:at + 2], permuted[at:at + 2], extra[2 * at:2 * at + 4], blinds[at:at + 2]
-            mine.append(Permuted(c[0], c[1], q[0], q[1], e[0], e[2], e[1], e[3], b[0], b[1]))
-            at += 2
-        out.append(mine)
-    return out, cm
+            co = domain.lagrange_to_coeff_resident(q, out=fresh.keep(ResidentPoly(domain.field, domain.n)))
+            extra += [co, fresh.keep(domain.coeff_to_extended_resident(co))]
+    flat = [Permuted(compressed[i], compressed[i + 1], permuted[i], permuted[i + 1], extra[2 * i], extra[2 * i + 2], extra[2 * i + 1],
+                     extra[2 * i + 3], blinds[i], blinds[i + 1]) for i in range(0, len(permuted), 2)]
+    return _split(flat, [len(per) for per in lookups]), cm

@@ -20,35 +20,21 @@ from . import lib as _l
 from .evaluator import Ast
 from .multiopen import ProverQuery
 from .opening import _scale_add
-from .poly import Blind, EvaluationDomain, Params, ResidentPoly, _handles, eval_polynomial_resident
-
-_MAX_COMMIT_BATCH = 64   # h2_msm_registered_polys_affine takes at most this many polynomials per pass
+from .poly import Blind, EvaluationDomain, Params, ResidentPoly, _handles, eval_polynomial_resident, freed_on_failure
 
 
 def vanishing_quotient_resident(domain: EvaluationDomain, h_ext: ResidentPoly, out: Optional[List[ResidentPoly]] = None) -> List[ResidentPoly]:
     """`divide_by_vanishing_poly`, `extended_to_coeff` and `chunks_exact(n)` (vanishing/prover.rs:84-100) of the extended-domain
     evaluations `h_ext` in one device call (h2_poly_vanishing_quotient): the quotient_poly_degree pieces of n coefficients.
     `h_ext` is only read.  out=None allocates the pieces (and frees them again if the call fails)."""
-    fresh = out is None
-    pieces = [ResidentPoly(domain.field, domain.n) for _ in range(domain.quotient_poly_degree)] if fresh else list(out)
-    t = np.ascontiguousarray(np.stack([_l.fe_bytes(v) for v in domain.t_evaluations]))
-    try:
+    with freed_on_failure() as fresh:
+        pieces = [fresh.keep(ResidentPoly(domain.field, domain.n)) for _ in range(domain.quotient_poly_degree)] if out is None else list(out)
+        t = _l.fe_array(domain.t_evaluations, domain.m)
         _l.check(_l.init().h2_poly_vanishing_quotient(
             _handles(pieces), ctypes.c_size_t(len(pieces)), h_ext._h, ctypes.c_uint32(domain.k), ctypes.c_uint32(domain.extended_k),
             _l.ptr(_l.fe_bytes(domain.extended_omega_inv)), _l.ptr(_l.fe_bytes(domain.extended_ifft_divisor)),
             _l.ptr(_l.fe_bytes(domain.g_coset)), _l.ptr(t), ctypes.c_uint32(len(domain.t_evaluations)), _l.REPR_CANONICAL))
-    except BaseException:
-        if fresh:
-            for p in pieces:
-                p.close()
-        raise
     return pieces
-
-
-def _commit(params: Params, polys: List[ResidentPoly], blinds: List[int]) -> np.ndarray:
-    """params.commit (over g, not g_lagrange) of every polynomial, affine, at most _MAX_COMMIT_BATCH per pass."""
-    return np.concatenate([params.commit_resident_affine(polys[i:i + _MAX_COMMIT_BATCH], [Blind(b) for b in blinds[i:i + _MAX_COMMIT_BATCH]])
-                           for i in range(0, len(polys), _MAX_COMMIT_BATCH)])
 
 
 class Committed(NamedTuple):
@@ -68,13 +54,10 @@ class Committed(NamedTuple):
             pieces = vanishing_quotient_resident(domain, h_ext)
         finally:
             h_ext.close()
-        try:
+        with freed_on_failure() as fresh:
+            fresh.extend(pieces)
             blinds = [rng.scalar() for _ in pieces]
-            cm = _commit(params, pieces, blinds)
-        except BaseException:
-            for p in pieces:
-                p.close()
-            raise
+            cm = params.commit_resident_affine(pieces, [Blind(b) for b in blinds])
         return Constructed(pieces, blinds, self), cm
 
     def close(self) -> None:
@@ -93,15 +76,12 @@ class Constructed(NamedTuple):
         (:144-145).  Returns (Evaluated, random_eval)."""
         n, m = domain.n, domain.m
         xn = pow(int(x), n, m)
-        h_poly = ResidentPoly(domain.field, n)
-        try:
+        with freed_on_failure() as fresh:
+            h_poly = fresh.keep(ResidentPoly(domain.field, n))
             h_poly.copy_from(self.h_pieces[-1], n)
             for piece in reversed(self.h_pieces[:-1]):
                 _scale_add(h_poly, xn, piece, 1, n)
             random_eval = eval_polynomial_resident([self.committed.random_poly], [int(x) % m], n=n)[0]
-        except BaseException:
-            h_poly.close()
-            raise
         h_blind = 0
         for b in reversed(self.h_blinds):
             h_blind = (h_blind * xn + b) % m
@@ -134,12 +114,8 @@ def vanishing_commit(params: Params, domain: EvaluationDomain, rng) -> Tuple[Com
     commitment over g (params.commit, :53).  Returns (Committed, the (64,) affine commitment the caller writes)."""
     n = domain.n
     rp = rng.poly(n)
-    if not isinstance(rp, ResidentPoly):
-        rp = ResidentPoly(domain.field, n, rp)
-    try:
+    with freed_on_failure() as fresh:
+        rp = fresh.keep(rp if isinstance(rp, ResidentPoly) else ResidentPoly(domain.field, n, rp))
         blind = rng.scalar()
-        cm = _commit(params, [rp], [blind])[0]
-    except BaseException:
-        rp.close()
-        raise
+        cm = params.commit_resident_affine([rp], [Blind(blind)])[0]
     return Committed(rp, blind), cm

@@ -153,7 +153,7 @@ class MSM:
         k = len(u)
         assert k > 0 and (1 << k) == self.params.n, "compute_s: u.len() != params.k"
         accumulate = 0 if self.g_scalars is None else 1
-        ub = np.ascontiguousarray(np.stack([_l.fe_bytes(int(x) % self.r) for x in u]))
+        ub = _l.fe_array(u, self.r)
         _l.check(_l.init().h2_poly_compute_s(self._g()._h, _l.ptr(ub), ctypes.c_uint32(k), _l.ptr(_l.fe_bytes(int(init) % self.r)), accumulate,
                                              _l.REPR_CANONICAL))
 
@@ -211,7 +211,7 @@ class MSM:
             scalars.append(self.w_scalar)
             bases.append(P.w.reshape(64))
         if scalars:
-            sc = np.ascontiguousarray(np.stack([_l.fe_bytes(s) for s in scalars]))
+            sc = _l.fe_array(scalars, self.r)
             parts.append(best_multiexp(sc, np.ascontiguousarray(np.stack(bases)), curve=P.curve))
         if not parts:
             return np.zeros(96, dtype=np.uint8)                  # the empty multiexp: the identity

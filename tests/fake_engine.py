@@ -206,11 +206,15 @@ class FakeLib:
 
     def h2_msm_registered_polys(self, handle, polys, batch, n, extra, repr_, out):
         self._log("h2_msm_registered_polys")
+        if _v(batch) > 64:
+            return self._fail("h2_msm_registered_polys: batch > 64")
         _wr(out, self._registered(handle, polys, batch, n, extra, False))
         return 0
 
     def h2_msm_registered_polys_affine(self, handle, polys, batch, n, extra, repr_, out):
         self._log("h2_msm_registered_polys_affine")
+        if _v(batch) > 64:
+            return self._fail("h2_msm_registered_polys: batch > 64")
         _wr(out, self._registered(handle, polys, batch, n, extra, True))
         return 0
 

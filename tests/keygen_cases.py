@@ -62,3 +62,21 @@ def random_mapping(rng, cols: int, n: int) -> np.ndarray:
     mp[cols - 1, n - 1] = (0, 0)
     mp[:, 0, 0] = np.arange(cols)
     return mp
+
+
+def wide_keygen_vk(h2, prm, D, delta: int, fixed_cols: int = 40, perm_cols: int = 30, seed: int = 5):
+    """keygen_vk over `prm` of more fixed and permutation columns together than one MSM pass takes (64 polynomials), and the
+    same columns committed one at a time with commit_lagrange.  Returns (keygen_vk's (fixed, permutation) commitments, the
+    one-at-a-time ones), each an (m, 64) affine array."""
+    import random
+    from oracle import cref, pasta
+    n, m = D.n, D.m
+    fixed = [pasta.gen_scalars(D.field, seed + i, n) for i in range(fixed_cols)]
+    asm = h2.Assembly(n, perm_cols)
+    rnd = random.Random(seed)
+    for _ in range(2 * perm_cols):
+        asm.copy(rnd.randrange(perm_cols), rnd.randrange(n), rnd.randrange(perm_cols), rnd.randrange(n))
+    got = h2.keygen_vk(prm, D, fixed, asm, delta)
+    one = lambda col: h2.batch_normalize(prm.commit_lagrange(cref.ints_to_bytes(col), h2.Blind()).reshape(1, 96), prm.curve)[0]  # noqa: E731
+    sigma = oracle_sigma(asm.mapping, n, D.omega, delta, m)
+    return got, (np.stack([one(c) for c in fixed]), np.stack([one(s) for s in sigma]))

@@ -22,7 +22,7 @@ from tests import bench_circuit as BC  # noqa: E402
 from tests import plonk_api_circuit as circ  # noqa: E402
 from tests.abi_cases import _err, _lib, _run_parallel, _sigma_call  # noqa: E402
 from tests.bench_circuit import _bench_assembly, _bench_params  # noqa: E402
-from tests.keygen_cases import oracle_sigma, random_mapping  # noqa: E402
+from tests.keygen_cases import oracle_sigma, random_mapping, wide_keygen_vk  # noqa: E402
 from tests.plonk_api_circuit import ZETA, golden_columns, plonk_api_copies  # noqa: E402
 from tests.plonk_prover import prover_pk_bytes  # noqa: E402
 from tests.plonk_verifier import scalar_delta  # noqa: E402
@@ -214,6 +214,22 @@ def test_benchmark_circuit_key_and_proof_k14(eng):
     finally:
         if pk is not None:
             pk.close()
+        prm.close()
+
+
+def test_keygen_vk_commits_more_columns_than_one_msm_pass(eng):
+    """keygen_vk of 40 fixed and 30 permutation columns, more than the 64 polynomials one h2_msm_registered_polys_affine
+    call takes, commits every column as commit_lagrange does alone."""
+    k = 4
+    n = 1 << k
+    pts = cref.gen_points("vesta", SEED, n + 2)
+    prm = eng.Params("vesta", k, pts[:n], pts[:n], pts[n:n + 1], u=pts[n + 1:])
+    try:
+        D = eng.EvaluationDomain("fp", 3, k, ZETA)
+        (fc, pc), (want_fc, want_pc) = wide_keygen_vk(eng, prm, D, scalar_delta(pasta.P_MOD))
+        assert fc.shape == (40, 64) and pc.shape == (30, 64)
+        assert (fc == want_fc).all() and (pc == want_pc).all()
+    finally:
         prm.close()
 
 

@@ -19,7 +19,7 @@ from tests import fake_engine
 from tests import plonk_api_circuit as circ
 from tests.bench_circuit import _bench_setup, bench_copies
 from tests.fake_engine import KEYGEN_CHUNK
-from tests.keygen_cases import oracle_assembly, oracle_copy, oracle_sigma, random_mapping
+from tests.keygen_cases import oracle_assembly, oracle_copy, oracle_sigma, random_mapping, wide_keygen_vk
 from tests.kernel_emul import build as emul_build
 from tests.plonk_api_circuit import ZETA, plonk_api_copies
 from tests.plonk_verifier import scalar_delta
@@ -225,6 +225,24 @@ def test_keygen_accepts_assigned_fixed_columns():
             co.close()
         assert l_vals == [[1] + [0] * 7, [0] * 6 + [1, 1], [0] * 5 + [1, 0, 0]]
         pk.close()
+        prm.close()
+        assert not fake.polys
+
+
+def test_keygen_vk_commits_more_columns_than_one_msm_pass():
+    """keygen_vk of 40 fixed and 30 permutation columns, more than the 64 polynomials one h2_msm_registered_polys_affine
+    call takes, commits every column as commit_lagrange does alone, in two passes."""
+    import halo2_b200 as h2
+    k = 3
+    n = 1 << k
+    pts = cref.gen_points("vesta", 8, n + 2)
+    with fake_engine.installed() as fake:
+        prm = h2.Params("vesta", k, pts[:n], pts[:n], pts[n:n + 1], u=pts[n + 1:])
+        D = h2.EvaluationDomain("fp", 3, k, ZETA)
+        (fc, pc), (want_fc, want_pc) = wide_keygen_vk(h2, prm, D, scalar_delta(pasta.P_MOD))
+        assert fake.calls.count("h2_msm_registered_polys_affine") == 2
+        assert fc.shape == (40, 64) and pc.shape == (30, 64)
+        assert (fc == want_fc).all() and (pc == want_pc).all()
         prm.close()
         assert not fake.polys
 

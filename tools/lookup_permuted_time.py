@@ -66,7 +66,6 @@ def run_fused(h2, torch, reps, ks, counts):
     from oracle import pasta
     from tests.bench_circuit import _bench_params
     from tests.lookup_permuted_cases import columns, composition
-    from halo2_b200.products import _commit
     rows = []
     for k in ks:
         n = 1 << k
@@ -81,14 +80,14 @@ def run_fused(h2, torch, reps, ks, counts):
 
                 def new():
                     out = [q for pr in h2.lookup_permute_resident(D, pairs, BF, blinding) for q in pr]
-                    return out, _commit(prm, out, blinds)
+                    return out, prm.commit_resident_affine(out, [h2.Blind(b) for b in blinds], lagrange=True)
 
                 def old_path():
                     out, cms = [], []
                     for b in range(count):
                         pi, pt = composition(h2, D, [pairs[b]], BF, blinding[2 * (BF + 1) * b:2 * (BF + 1) * (b + 1)])[0]
                         out += [pi, pt]
-                        cms.append(_commit(prm, [pi, pt], blinds[2 * b:2 * b + 2]))
+                        cms.append(prm.commit_resident_affine([pi, pt], [h2.Blind(x) for x in blinds[2 * b:2 * b + 2]], lagrange=True))
                     return out, cms
 
                 t_new, t_old = [], []
