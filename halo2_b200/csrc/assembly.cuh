@@ -168,6 +168,53 @@ struct AssemblyOps {
     }
 };
 
+// After r Borůvka rounds a component with a live copy has >= 2^r cells, so F takes at most floor(log2 cells) rounds.
+inline uint32_t as_round_limit(uint64_t cells) {
+    uint32_t r = 0;
+    while ((2ull << r) <= cells) r++;
+    return r;
+}
+// The per-copy scratch (as_edge) of m copies, in u32 words: the error word (u64), `changed` (the pointer-jumping flag, in
+// a u64 slot), the copies (4 words each), ea, eb, flag (m + 1 words: the scan's total), the two live lists, ra, rb, keep
+// (m + 1) and F.
+struct AsEdgeLayout {
+    uint64_t err, changed, copies, ea, eb, flag, live[2], ra, rb, keep, fl, end;
+};
+inline AsEdgeLayout as_edge_layout(uint64_t m) {
+    AsEdgeLayout A{};
+    auto take = [&](uint64_t words) { const uint64_t at = A.end; A.end += words; return at; };
+    A.err = take(2);
+    A.changed = take(2);
+    A.copies = take(4 * m);
+    A.ea = take(m);
+    A.eb = take(m);
+    A.flag = take(m + 1);
+    A.live[0] = take(m);
+    A.live[1] = take(m);
+    A.ra = take(m);
+    A.rb = take(m);
+    A.keep = take(m + 1);
+    A.fl = take(m);
+    return A;
+}
+// The per-slot scratch (as_slot) of S slots, in u32 words: the slots' cells, order and nxt (two buffers each) and the
+// radix sort's digit counts, H2_AS_TILE per tile and the scan's total.
+struct AsSlotLayout {
+    uint64_t ntiles, scell, order[2], nxt[2], counts, end;
+};
+inline AsSlotLayout as_slot_layout(uint64_t S) {
+    AsSlotLayout A{};
+    auto take = [&](uint64_t words) { const uint64_t at = A.end; A.end += words; return at; };
+    A.ntiles = (S + H2_AS_TILE - 1) / H2_AS_TILE;
+    A.scell = take(S);
+    A.order[0] = take(S);
+    A.order[1] = take(S);
+    A.nxt[0] = take(S);
+    A.nxt[1] = take(S);
+    A.counts = take(H2_AS_TILE * A.ntiles + 1);
+    return A;
+}
+
 #if defined(__CUDACC__)
 #define H2_AS_TID ((uint64_t)blockIdx.x * blockDim.x + threadIdx.x)
 __global__ void __launch_bounds__(256) as_encode_kernel(const uint32_t *copies, uint32_t m, uint32_t cols, uint32_t k, uint32_t *ea, uint32_t *eb,

@@ -20,18 +20,16 @@ static int polyops_run(int mode, const std::vector<PolyBuf *> &a, const std::vec
     Context &X = g_ctx;
     cudaStream_t s = X.stream;
     const uint32_t batch = (uint32_t)a.size();
-    // level sizes: m[0] = n, m[l + 1] = ceil(m[l] / CHUNK), down to 1
-    std::vector<uint64_t> m{(uint64_t)n}, off{0};
-    while (m.back() > 1) { off.push_back(off.back() + (m.size() > 1 ? m.back() * batch : 0)); m.push_back((m.back() + H2_POLY_CHUNK - 1) / H2_POLY_CHUNK); }
-    if (mode == 1 && m.size() == 1) { off.push_back(0); m.push_back(1); }   // a length-1 inner product still needs its product level
-    const size_t L = m.size() - 1;                               // levels above the polynomial itself
-    const uint64_t lvl_total = off.back() + m.back() * batch + batch;
-    if (X.po_lvl.ensure(lvl_total * sizeof(fe)) || X.po_q.ensure(lvl_total * sizeof(fe)) || X.po_pts.ensure((L + 2) * batch * sizeof(fe)) ||
+    GpTree T;
+    if (const char *e = gp_reduce_plan(n, batch, mode == 1, &T)) return fail(std::string(h.who) + ": " + e);
+    const uint64_t *m = T.m;
+    const size_t L = T.L;                                        // levels above the polynomial itself
+    if (X.po_lvl.ensure(T.total * sizeof(fe)) || X.po_q.ensure(T.total * sizeof(fe)) || X.po_pts.ensure((L + 2) * batch * sizeof(fe)) ||
         X.misc.ensure(batch * sizeof(fe) + 64))
         return 1;
     fe *lvl = X.po_lvl.as<fe>(), *qarr = X.po_q.as<fe>(), *pts = X.po_pts.as<fe>();
-    auto level = [&](size_t l) { return lvl + off[l]; };         // values of level l >= 1: [batch][m[l]]
-    auto qlevel = [&](size_t l) { return qarr + off[l]; };
+    auto level = [&](size_t l) { return lvl + T.off[l]; };       // values of level l >= 1: [batch][m[l]]
+    auto qlevel = [&](size_t l) { return qarr + T.off[l]; };
     std::vector<PolyBuf *> cols(a);                              // a, then c (null pointers without it)
     cols.insert(cols.end(), c.begin(), c.end());
     cols.resize(2 * batch);
@@ -186,12 +184,11 @@ extern "C" int h2_poly_batch_invert(uint64_t poly, size_t n) {
 template <class P> static int grand_product_run(PolyBuf *d, PolyBuf *a, size_t n, const void *init, const HostArgs &h) {
     Context &X = g_ctx;
     cudaStream_t s = X.stream;
-    std::vector<uint64_t> m{(uint64_t)n}, off{0};
-    while (m.back() > H2_POLY_CHUNK) { off.push_back(off.back() + (m.size() > 1 ? m.back() : 0)); m.push_back((m.back() + H2_POLY_CHUNK - 1) / H2_POLY_CHUNK); }
-    const size_t L = m.size() - 1;
-    uint64_t total = 1;
-    for (size_t l = 1; l <= L; l++) total += m[l];
-    if (X.po_lvl.ensure(total * sizeof(fe)) || X.po_q.ensure(total * sizeof(fe))) return 1;
+    GpTree T;
+    if (const char *e = gp_scan_plan(n, 1, false, &T)) return fail(std::string(h.who) + ": " + e);
+    const uint64_t *m = T.m, *off = T.off;
+    const size_t L = T.L;
+    if (X.po_lvl.ensure(T.total * sizeof(fe)) || X.po_q.ensure(T.total * sizeof(fe))) return 1;
     fe *lvl = X.po_lvl.as<fe>(), *ex = X.po_q.as<fe>();
     const fe *src = a->buf.as<fe>();
     const fe in0 = h.elem<P>(init);
@@ -284,9 +281,8 @@ template <class P> static int lk_sort(fe *keys, uint64_t N, uint32_t count, cuda
     return 0;
 }
 // The permuted columns of `count` lookups of u usable rows (lookup.cuh), and with `blinding` (count x 2 rows values) the
-// blinding rows [u, u + rows) of every output.  Scratch from the lane's pools, per lookup (N = the power of two >= u, >= 2):
-//   lk_keys  32 N bytes (the sorted table)          lk_u32  4 (3 u + 2) bytes (cnt | unconsumed, scanned in one pass; leftovers)
-//   col_tab  32 bytes of pointers + 64 rows bytes of blinding values;  plus 4 bytes per 8192 scanned words and the error word.
+// blinding rows [u, u + rows) of every output.  Scratch from the lane's pools: lk_keys and lk_u32 as lk_plan lays them out,
+// col_tab 32 bytes of pointers + 64 rows bytes of blinding values per lookup, 4 bytes per 8192 scanned words.
 // `h`: the encoding of the blinding values (nullptr without them).  One synchronisation; *bad = the lowest lookup with an input value
 // its table lacks, H2_LK_NONE when none -- and then every output is as it was (the one writing kernel runs after the miss is known and
 // checks for it first).
@@ -296,14 +292,13 @@ static int lookup_permuted_run(const std::vector<PolyBuf *> &out_in, const std::
     Context &X = g_ctx;
     cudaStream_t s = X.stream;
     const uint32_t count = (uint32_t)in.size();
-    uint64_t N = 2;
-    while (N < u) N <<= 1;
-    const uint64_t w = u + 1, nblind = blinding ? (uint64_t)count * 2 * rows : 0;
+    const LkPlan plan = lk_plan(u, count);
+    const uint64_t N = plan.N, w = plan.w, nblind = blinding ? (uint64_t)count * 2 * rows : 0;
     std::vector<PolyBuf *> cols(in);                             // LkCols: in, tab, out_in, out_tab
     for (auto *v : {&tab, &out_in, &out_tab}) cols.insert(cols.end(), v->begin(), v->end());
-    if (X.lk_keys.ensure(count * N * sizeof(fe)) || X.lk_u32.ensure(((2 * w + u) * count + 4) * sizeof(uint32_t))) return 1;
-    fe *keys = X.lk_keys.as<fe>();
-    uint32_t *sc = X.lk_u32.as<uint32_t>(), *left = sc + 2 * w * count, *err = left + u * count;
+    if (X.lk_keys.ensure(plan.keys_end * sizeof(fe)) || X.lk_u32.ensure(plan.u32_end * sizeof(uint32_t))) return 1;
+    fe *keys = X.lk_keys.as<fe>() + plan.keys;
+    uint32_t *u32 = X.lk_u32.as<uint32_t>(), *sc = u32 + plan.sc, *left = u32 + plan.left, *err = u32 + plan.err;
     ColTable t;
     if (col_table(cols, blinding, nblind * sizeof(fe), s, &t)) return 1;
     LkCols c;
@@ -492,19 +487,19 @@ static int as_read_u32(uint32_t *h, const uint32_t *d, cudaStream_t s) {     // 
     return 0;
 }
 // The copy-cycle mapping of m copies (4 uint32 each, synthesis order) over cols * 2^k cells into X.kg_map as (column,
-// row) pairs; *bad = 2 i (column) / 2 i + 1 (row) of the first bad copy i, or ~0.  Scratch in the lane's pools:
-//   as_edge  u32: copies 4m | ea m | eb m | flag m + 1 | live 2 x m | ra m | rb m | keep m + 1 | F m | changed, error word
-//   as_cell  u32: comp N | best N          as_slot  u32: scell S | order 2 x S | nxt 2 x S | digit counts 256 ntiles + 1
+// row) pairs; *bad = 2 i (column) / 2 i + 1 (row) of the first bad copy i, or ~0.  Scratch in the lane's pools: as_edge
+// and as_slot as assembly.cuh lays them out, as_cell u32: comp N | best N.
 static int assembly_run(uint32_t cols, uint32_t k, const uint32_t *copies, uint64_t m, unsigned long long *bad) {
     Context &X = g_ctx;
     cudaStream_t s = X.stream;
     const uint64_t N = (uint64_t)cols << k;
-    if (X.kg_map.ensure(N * sizeof(uint2)) || X.as_edge.ensure((14 * m + 8) * sizeof(uint32_t))) return 1;
+    const AsEdgeLayout E = as_edge_layout(m);
+    if (X.kg_map.ensure(N * sizeof(uint2)) || X.as_edge.ensure(E.end * sizeof(uint32_t))) return 1;
     uint2 *map = X.kg_map.as<uint2>();
-    unsigned long long *err = X.as_edge.as<unsigned long long>();
-    uint32_t *changed = X.as_edge.as<uint32_t>() + 2;
-    uint32_t *cp = changed + 2, *ea = cp + 4 * m, *eb = ea + m, *flag = eb + m, *live[2] = {flag + m + 1, flag + 2 * m + 1};
-    uint32_t *ra = live[1] + m, *rb = ra + m, *keep = rb + m, *fl = keep + m + 1;
+    uint32_t *edge = X.as_edge.as<uint32_t>();
+    unsigned long long *err = reinterpret_cast<unsigned long long *>(edge + E.err);
+    uint32_t *changed = edge + E.changed, *cp = edge + E.copies, *ea = edge + E.ea, *eb = edge + E.eb, *flag = edge + E.flag;
+    uint32_t *live[2] = {edge + E.live[0], edge + E.live[1]}, *ra = edge + E.ra, *rb = edge + E.rb, *keep = edge + E.keep, *fl = edge + E.fl;
     CU(cudaMemsetAsync(err, 0xFF, sizeof *err, s));
     if (m) {
         if (upload_async(cp, copies, m * 4 * sizeof(uint32_t), s)) return 1;
@@ -524,8 +519,7 @@ static int assembly_run(uint32_t cols, uint32_t k, const uint32_t *copies, uint6
         if (X.as_cell.ensure(2 * N * sizeof(uint32_t))) return 1;
         uint32_t *comp = X.as_cell.as<uint32_t>(), *best = comp + N;
         LAUNCH(as_iota_kernel, blocks_for(N, 256), 256, 0, s, comp, N);
-        uint32_t limit = 0;                                     // after r rounds a component with a live copy has >= 2^r cells
-        while ((2ull << limit) <= N) limit++;
+        const uint32_t limit = as_round_limit(N);
         for (uint32_t round = 0, cur = 0; L; round++, cur ^= 1) {
             if (round == limit) return fail("h2_poly_permutation_sigma_copies: internal error: the spanning forest needs more than log2(cells) rounds");
             const uint32_t *lv = live[cur];
@@ -549,10 +543,11 @@ static int assembly_run(uint32_t cols, uint32_t k, const uint32_t *copies, uint6
     // 3. slots, stably sorted by cell
     const uint64_t S = 2ull * q;
     if (S >= (1ull << 32)) return fail("h2_poly_permutation_sigma_copies: the spanning forest has 2^31 copies or more");
-    const uint64_t ntiles = (S + H2_AS_TILE - 1) / H2_AS_TILE;
-    if (X.as_slot.ensure((5 * S + H2_AS_TILE * ntiles + 1) * sizeof(uint32_t))) return 1;
-    uint32_t *scell = X.as_slot.as<uint32_t>(), *order[2] = {scell + S, scell + 2 * S}, *nxt[2] = {scell + 3 * S, scell + 4 * S};
-    uint32_t *counts = scell + 5 * S;
+    const AsSlotLayout Q = as_slot_layout(S);
+    const uint64_t ntiles = Q.ntiles;
+    if (X.as_slot.ensure(Q.end * sizeof(uint32_t))) return 1;
+    uint32_t *slot = X.as_slot.as<uint32_t>(), *scell = slot + Q.scell, *order[2] = {slot + Q.order[0], slot + Q.order[1]};
+    uint32_t *nxt[2] = {slot + Q.nxt[0], slot + Q.nxt[1]}, *counts = slot + Q.counts;
     LAUNCH(as_slots_kernel, blocks_for(S, 256), 256, 0, s, (const uint32_t *)fl, S, (const uint32_t *)ea, (const uint32_t *)eb, scell, order[0]);
     uint32_t o = 0;
     for (uint32_t shift = 0; shift == 0 || ((N - 1) >> shift); shift += H2_AS_DIGIT_BITS, o ^= 1) {
@@ -620,14 +615,12 @@ static int product_run(bool perm, const std::vector<PolyBuf *> &z, const std::ve
     Context &X = g_ctx;
     cudaStream_t s = X.stream;
     const uint64_t n = 1ull << k, count = z.size();
-    GpLevels G{};
-    G.m[0] = n; G.m[1] = (n + H2_POLY_CHUNK - 1) / H2_POLY_CHUNK; G.L = 1;
-    while (G.m[G.L] > H2_POLY_CHUNK) { G.off[G.L + 1] = G.off[G.L] + G.m[G.L] * count; G.m[G.L + 1] = (G.m[G.L] + H2_POLY_CHUNK - 1) / H2_POLY_CHUNK; G.L++; }
-    const uint64_t total = G.off[G.L] + G.m[G.L] * count;
+    GpTree G;
+    if (const char *e = gp_scan_plan(n, count, true, &G)) return fail(std::string(h.who) + ": " + e);
     const uint64_t tlen = perm ? KeygenOps<P>::table_len(k, ncols) : 0, nblind = count * bf;
     std::vector<PolyBuf *> cols(z);
     cols.insert(cols.end(), ins.begin(), ins.end());
-    if (X.gp_val.ensure(count * n * sizeof(fe)) || X.po_lvl.ensure(total * sizeof(fe)) || X.po_q.ensure(total * sizeof(fe)) ||
+    if (X.gp_val.ensure(count * n * sizeof(fe)) || X.po_lvl.ensure(G.total * sizeof(fe)) || X.po_q.ensure(G.total * sizeof(fe)) ||
         X.gp_aux.ensure((tlen + count) * sizeof(fe)))
         return 1;
     fe *val = X.gp_val.as<fe>(), *lvl = X.po_lvl.as<fe>(), *ex = X.po_q.as<fe>(), *tab = X.gp_aux.as<fe>(), *init = tab + tlen;
@@ -647,7 +640,7 @@ static int product_run(bool perm, const std::vector<PolyBuf *> &z, const std::ve
     LAUNCH(gp_mv_up_kernel<P>, dim3(blocks_for(G.m[1], 128), (uint32_t)count), 128, 0, s, (const fe *const *)zp, val, n, lvl, G.m[1]);
     for (uint32_t l = 1; l < G.L; l++)
         LAUNCH(gp_up_kernel<P>, dim3(blocks_for(G.m[l + 1], 128), (uint32_t)count), 128, 0, s, (const fe *)(lvl + G.off[l]), G.m[l], lvl + G.off[l + 1], G.m[l + 1]);
-    LAUNCH(gp_carry_kernel<P>, blocks_for(count / sets, 64), 64, 0, s, (const fe *)val, (const fe *)lvl, G, n - bf - 1, sets, init, (uint32_t)(count / sets));
+    LAUNCH(gp_carry_kernel<P>, blocks_for(count / sets, 64), 64, 0, s, (const fe *)val, (const fe *)lvl, (const GpLevels &)G, n - bf - 1, sets, init, (uint32_t)(count / sets));
     for (uint32_t l = G.L + 1; l-- > 0;) {
         const uint64_t chunks = (G.m[l] + H2_POLY_CHUNK - 1) / H2_POLY_CHUNK;
         LAUNCH(gp_down_kernel<P>, dim3(blocks_for(chunks, 128), (uint32_t)count), 128, 0, s, l == 0 ? (const fe *)val : (const fe *)(lvl + G.off[l]), G.m[l],

@@ -26,14 +26,8 @@
 
 namespace h2 {
 
-#define H2_GP_MAX_LEVELS 8   // n <= 2^30: level sizes 2^30, 2^25, ..., 2^10, 32
-
-// The running product's chunk tree over `batch` columns of n values: level 0 is the flat [batch][n] scratch, level l >= 1
-// lives at lvl + off[l] as [batch][m[l]], m[l + 1] = ceil(m[l] / CHUNK), down to m[L] <= CHUNK.
-struct GpLevels {
-    uint64_t m[H2_GP_MAX_LEVELS], off[H2_GP_MAX_LEVELS];
-    uint32_t L;
-};
+// The product columns' chunk tree is gp_scan_plan's with level 1 always present (polyops.cuh); its level 0 is the flat
+// [batch][n] scratch of step 3.
 
 template <class P> struct ProductArgs {
     // permutation factors of row i of column b = (proof, set) = (b / sets, b % sets); cols: proofs x ncols column pointers

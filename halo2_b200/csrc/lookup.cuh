@@ -40,6 +40,26 @@ H2_HD bool fe_canon_lt(const fe &a, const fe &b) {
 //   left  u32 [b u, (b + 1) u)             table ranks of the leftover values, ascending
 // The scan runs once over all 2 count w words; a lookup's values are differences from its segment's first word (exact in
 // u32 arithmetic, every segment sums to at most u < 2^31).
+// The plan of one call: N and w, the element offsets of keys (in lk_keys), of sc, left and the error word (in lk_u32), and
+// where each pool's part ends.
+struct LkPlan {
+    uint64_t N, w;
+    uint64_t keys, keys_end;                   // fe
+    uint64_t sc, left, err, u32_end;           // u32
+};
+inline LkPlan lk_plan(uint64_t u, uint64_t count) {
+    LkPlan P{};
+    P.N = 2;
+    while (P.N < u) P.N <<= 1;
+    P.w = u + 1;
+    P.keys = 0;
+    P.keys_end = count * P.N;
+    auto take = [&](uint64_t words) { const uint64_t at = P.u32_end; P.u32_end += words; return at; };
+    P.sc = take(2 * P.w * count);
+    P.left = take(u * count);
+    P.err = take(1);
+    return P;
+}
 // unc[r] = 1 when table rank r < u is consumed by no input row (cnt[r] == 0); unc[u] = 0 closes the segment
 H2_HD void lk_unconsumed_body(const uint32_t *cnt, uint64_t u, uint32_t *unc, uint64_t r) {
     if (r <= u) unc[r] = (r < u && cnt[r] == 0) ? 1u : 0u;

@@ -19,6 +19,48 @@ namespace h2 {
 
 #define H2_POLY_CHUNK 32
 
+// The levels of a chunk tree over `batch` columns of n values: level 0 is the caller's data, level l = 1 ... L lives in
+// scratch at off[l] as [batch][m[l]], m[l + 1] = ceil(m[l] / CHUNK).  Kernels that walk the levels themselves take the
+// GpLevels part by value (gp_carry_kernel).  A reduction of n < 2^32 values takes all 8 entries: 2^32 - 1, 2^27, ..., 4, 1.
+#define H2_GP_MAX_LEVELS 8
+struct GpLevels {
+    uint64_t m[H2_GP_MAX_LEVELS], off[H2_GP_MAX_LEVELS];
+    uint32_t L;
+};
+// The plan of one call: its levels and the elements they take in each level array (po_lvl, po_q).  The plans below return
+// nullptr, or the reason n is refused.
+struct GpTree : GpLevels {
+    uint64_t total;
+};
+constexpr const char *gp_push_level(GpTree *T, uint64_t batch) {
+    if (T->L + 1 >= H2_GP_MAX_LEVELS) return "n needs more chunk-tree levels than H2_GP_MAX_LEVELS";
+    T->off[T->L + 1] = T->L ? T->off[T->L] + T->m[T->L] * batch : 0;
+    T->m[T->L + 1] = (T->m[T->L] + H2_POLY_CHUNK - 1) / H2_POLY_CHUNK;
+    T->L++;
+    T->total = T->off[T->L] + T->m[T->L] * batch;
+    return nullptr;
+}
+// The reduction to one value (eval, inner product, kate division).  `inner`: a length-1 inner product still gets its
+// product level.
+constexpr const char *gp_reduce_plan(uint64_t n, uint64_t batch, bool inner, GpTree *T) {
+    *T = GpTree{};
+    T->m[0] = n;
+    while (T->m[T->L] > 1)
+        if (const char *e = gp_push_level(T, batch)) return e;
+    if (inner && T->L == 0) { T->m[1] = 1; T->L = 1; T->total = batch; }
+    return nullptr;
+}
+// The scan down to <= CHUNK values (the running product, K21's product columns).  `level1`: level 1 even when n <= CHUNK.
+constexpr const char *gp_scan_plan(uint64_t n, uint64_t batch, bool level1, GpTree *T) {
+    *T = GpTree{};
+    T->m[0] = n;
+    while (T->m[T->L] > H2_POLY_CHUNK || (level1 && T->L == 0))
+        if (const char *e = gp_push_level(T, batch)) return e;
+    return nullptr;
+}
+static_assert([] { GpTree T{}; return !gp_reduce_plan(0xFFFFFFFFull, 1, false, &T) && T.L + 1 == H2_GP_MAX_LEVELS; }(),
+              "a reduction of n < 2^32 values fits GpLevels");
+
 template <class P> struct PolyOps {
     // level of eval_polynomial: out[b][t] = sum_{i < CHUNK} in_b[t CHUNK + i] x_b^i   (Horner from the top of the chunk)
     // in_ptrs != nullptr: level 0 reads polynomial b from in_ptrs[b]; else from in_flat + b * m

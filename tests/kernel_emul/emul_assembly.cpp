@@ -1,5 +1,7 @@
 // TEST-ONLY serial execution of the copy-cycle kernels (assembly.cuh) in the order and with the launch shapes of
-// capi_poly.cu's assembly_run; the scans are plain exclusive scans, as the scan kernels of msm.cuh compute them.
+// capi_poly.cu's assembly_run, with its round limit (as_round_limit) but separate vectors where the device carves
+// as_edge_layout and as_slot_layout; the scans are plain exclusive scans, as the scan kernels of msm.cuh compute them.
+#include <algorithm>
 #include <vector>
 #include "assembly.cuh"
 using namespace h2;
@@ -33,8 +35,7 @@ extern "C" int emu_assembly(const uint32_t *copies, uint64_t m, uint32_t cols, u
     if (L) {
         std::vector<uint32_t> comp(N), best(N);
         grid(N, 256, [&](uint64_t v) { AssemblyOps::iota_body(comp.data(), N, v); });
-        uint32_t limit = 0;
-        while ((2ull << limit) <= N) limit++;
+        const uint32_t limit = as_round_limit(N);
         uint32_t *live[2] = {live0.data(), live1.data()};
         for (uint32_t round = 0, cur = 0; L; round++, cur ^= 1) {
             if (round == limit) return 2;
@@ -58,7 +59,7 @@ extern "C" int emu_assembly(const uint32_t *copies, uint64_t m, uint32_t cols, u
     *forest_out = q;
     if (q == 0) return 0;
     grid(m, 256, [&](uint64_t i) { AssemblyOps::compact_body(keep.data(), (uint32_t)m, nullptr, fl.data(), i); });
-    const uint64_t S = 2ull * q, ntiles = (S + H2_AS_TILE - 1) / H2_AS_TILE;
+    const uint64_t S = 2ull * q, ntiles = as_slot_layout(S).ntiles;
     std::vector<uint32_t> scell(S), order0(S), order1(S), nxt0(S), nxt1(S), counts(H2_AS_TILE * ntiles + 1);
     uint32_t *order[2] = {order0.data(), order1.data()}, *nxt[2] = {nxt0.data(), nxt1.data()};
     grid(S, 256, [&](uint64_t s) { AssemblyOps::slots_body(fl.data(), S, ea.data(), eb.data(), scell.data(), order[0], s); });
@@ -86,4 +87,14 @@ extern "C" int emu_assembly(const uint32_t *copies, uint64_t m, uint32_t cols, u
         grid(S, 256, [&](uint64_t s) { AssemblyOps::jump_slots_body(nxt[t], nxt[t ^ 1], S, s); });
     grid(S, 256, [&](uint64_t p) { AssemblyOps::final_body(order[o], S, scell.data(), nxt[t], k, map, p); });
     return 0;
+}
+
+// The scratch layouts' fields in declaration order: as_edge_layout(m) into edge (13 values), as_slot_layout(S) into slot (8)
+extern "C" void emu_assembly_layouts(uint64_t m, uint64_t S, uint64_t *edge, uint64_t *slot) {
+    const AsEdgeLayout E = as_edge_layout(m);
+    const uint64_t e[] = {E.err, E.changed, E.copies, E.ea, E.eb, E.flag, E.live[0], E.live[1], E.ra, E.rb, E.keep, E.fl, E.end};
+    const AsSlotLayout Q = as_slot_layout(S);
+    const uint64_t q[] = {Q.ntiles, Q.scell, Q.order[0], Q.order[1], Q.nxt[0], Q.nxt[1], Q.counts, Q.end};
+    std::copy(e, e + 13, edge);
+    std::copy(q, q + 8, slot);
 }

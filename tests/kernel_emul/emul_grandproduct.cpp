@@ -1,5 +1,6 @@
 // TEST-ONLY serial execution of the product-column kernels (grandproduct.cuh) with the launch schedule of capi_poly.cu's
-// product_run: power tables, factors, batch inversion over the flat scratch, the batched chunk tree, carries, blinding rows.
+// product_run: power tables, factors, batch inversion over the flat scratch, the batched chunk tree of gp_scan_plan,
+// carries, blinding rows.
 #include <cstring>
 #include <vector>
 #include "grandproduct.cuh"
@@ -23,11 +24,9 @@ static void run(bool perm, const uint8_t *ins_in, uint64_t n_ins, uint32_t ncols
         ip[c] = ins[c].data();
     }
     for (uint64_t b = 0; b < count; b++) zp[b] = z[b].data();
-    GpLevels G{};
-    G.m[0] = n; G.m[1] = (n + H2_POLY_CHUNK - 1) / H2_POLY_CHUNK; G.L = 1;
-    while (G.m[G.L] > H2_POLY_CHUNK) { G.off[G.L + 1] = G.off[G.L] + G.m[G.L] * count; G.m[G.L + 1] = (G.m[G.L] + H2_POLY_CHUNK - 1) / H2_POLY_CHUNK; G.L++; }
-    const uint64_t total = G.off[G.L] + G.m[G.L] * count;
-    std::vector<fe> val(count * n), lvl(total), ex(total), init(count), blind(count * bf);
+    GpTree G;
+    gp_scan_plan(n, count, true, &G);                            // k <= 30 fits
+    std::vector<fe> val(count * n), lvl(G.total), ex(G.total), init(count), blind(count * bf);
     for (uint64_t j = 0; j < count * bf; j++) blind[j] = load_mont<P>(blinding + 32 * j);
     const fe b_m = load_mont<P>(beta), g_m = load_mont<P>(gamma);
     if (perm) {

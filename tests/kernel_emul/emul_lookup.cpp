@@ -1,6 +1,7 @@
-// TEST-ONLY serial execution of the lookup-permutation kernel bodies (lookup.cuh): load, the bitonic network stage by stage
-// (the global-stage body for every stride -- the shared-memory kernel runs the same compare-exchanges), run starts + lower
-// bounds, the two scans, leftover scatter, fill.  Never loaded by the halo2_b200 package; see tests/kernel_emul/README.md.
+// TEST-ONLY serial execution of the lookup-permutation kernel bodies (lookup.cuh) on lk_plan's N and w: load, the bitonic
+// network stage by stage (the global-stage body for every stride -- the shared-memory kernel runs the same
+// compare-exchanges), run starts + lower bounds, the two scans, leftover scatter, fill.  Never loaded by the halo2_b200
+// package; see tests/kernel_emul/README.md.
 #include <cstring>
 #include <vector>
 #include "lookup.cuh"
@@ -16,15 +17,15 @@ template <class P> static int run_lookup(const uint8_t *input, const uint8_t *ta
         memcpy(x.v, out_tab + 32 * i, 32); ot[i] = fe_to_mont<P>(x);
     }
     if (u) {
-        uint64_t N = 2;
-        while (N < u) N <<= 1;
-        std::vector<fe> ka(N), kt(N), left(u + 1);
+        const LkPlan plan = lk_plan(u, 1);
+        const uint64_t N = plan.N, w = plan.w;
+        std::vector<fe> ka(N), kt(N), left(w);
         for (uint64_t i = 0; i < N; i++) { K::load_body(a.data(), u, ka.data(), N, i); K::load_body(t.data(), u, kt.data(), N, i); }
         for (auto *keys : {ka.data(), kt.data()})
             for (uint64_t size = 2; size <= N; size <<= 1)
                 for (uint64_t stride = size / 2; stride >= 1; stride >>= 1)
                     for (uint64_t th = 0; th < N / 2; th++) K::global_stage_body(keys, N, size, stride, th);
-        std::vector<uint32_t> first(u + 1, 0), unc(u + 1, 0), fs(u + 1), us(u + 1);
+        std::vector<uint32_t> first(w, 0), unc(w, 0), fs(w), us(w);
         for (size_t i = 0; i < u; i++) unc[i] = 1;
         uint32_t err = 0;
         for (uint64_t r = 0; r < u; r++) K::first_body(ka.data(), kt.data(), u, first.data(), unc.data(), &err, oa.data(), ot.data(), r);

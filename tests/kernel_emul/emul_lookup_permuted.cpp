@@ -1,5 +1,5 @@
 // TEST-ONLY serial execution of the batched lookup-permutation bodies (lookup.cuh) in capi_poly.cu's launch schedule
-// (lookup_permuted_run): load every table, the bitonic network stage by stage (the global-stage body for every stride --
+// (lookup_permuted_run), on the scratch of lk_plan: load every table, the bitonic network stage by stage (the global-stage body for every stride --
 // the shared-memory kernel runs the same compare-exchanges), ranks + histogram, unconsumed flags, ONE exclusive scan over
 // the whole call's concatenated segments, leftovers, then -- only when no lookup missed -- the fill and blinding rows.
 // Never loaded by the halo2_b200 package; see tests/kernel_emul/README.md.
@@ -23,11 +23,10 @@ static uint32_t run_permuted(const uint8_t *inputs, const uint8_t *tables, uint3
     std::vector<fe> blind = blinding ? load(blinding, count * 2 * rows) : std::vector<fe>();
     uint32_t err = H2_LK_NONE;
     if (u) {
-        uint64_t N = 2;
-        while (N < u) N <<= 1;
-        const uint64_t w = u + 1;
-        std::vector<fe> keys(count * N);
-        std::vector<uint32_t> sc(2 * w * count, 0), left(u * count, 0);
+        const LkPlan plan = lk_plan(u, count);
+        const uint64_t N = plan.N, w = plan.w;
+        std::vector<fe> keys(plan.keys_end);
+        std::vector<uint32_t> sc(plan.left - plan.sc, 0), left(plan.err - plan.left, 0);
         for (uint32_t b = 0; b < count; b++) {
             fe *kt = keys.data() + b * N;
             for (uint64_t i = 0; i < N; i++) K::load_body(tab.data() + b * n, u, kt, N, i);
@@ -60,6 +59,12 @@ static uint32_t run_permuted(const uint8_t *inputs, const uint8_t *tables, uint3
         x = fe_from_mont<P>(ot[i]); memcpy(out_tab + 32 * i, x.v, 32);
     }
     return err;
+}
+// lk_plan's fields in declaration order
+extern "C" void emu_lookup_plan(uint64_t u, uint64_t count, uint64_t *out) {
+    const LkPlan P = lk_plan(u, count);
+    const uint64_t f[] = {P.N, P.w, P.keys, P.keys_end, P.sc, P.left, P.err, P.u32_end};
+    memcpy(out, f, sizeof f);
 }
 // h2_poly_lookup_permuted: n = 2^k rows per lookup, u = n - rows usable ones, blinding = count x 2 rows values
 extern "C" uint32_t emu_lookup_permuted(int field, const uint8_t *inputs, const uint8_t *tables, uint32_t count, size_t n, size_t u, const uint8_t *blinding,

@@ -1,4 +1,5 @@
-// TEST-ONLY serial execution of the polynomial reductions (polyops.cuh) with the level schedule of capi.cu's polyops_run.
+// TEST-ONLY serial execution of the polynomial reductions (polyops.cuh) on the chunk trees of gp_reduce_plan and
+// gp_scan_plan, as capi_poly.cu's polyops_run and grand_product_run run them.
 #include <cstring>
 #include <vector>
 #include "polyops.cuh"
@@ -17,12 +18,11 @@ template <class P> static int run_polyops(int mode, const uint8_t *a_in, const u
         }
         ap[b] = a[b].data(); cp[b] = c[b].data(); qp[b] = c[b].data();
     }
-    std::vector<uint64_t> m{n}, off{0};
-    while (m.back() > 1) { off.push_back(off.back() + (m.size() > 1 ? m.back() * batch : 0)); m.push_back((m.back() + H2_POLY_CHUNK - 1) / H2_POLY_CHUNK); }
-    if (mode == 1 && m.size() == 1) { off.push_back(0); m.push_back(1); }
-    const size_t L = m.size() - 1;
-    const uint64_t total = off.back() + m.back() * batch + batch;
-    std::vector<fe> lvl(total), qarr(total), pts((L + 2) * batch);
+    GpTree T;
+    if (gp_reduce_plan(n, batch, mode == 1, &T)) return -1;
+    const uint64_t *m = T.m, *off = T.off;
+    const size_t L = T.L;
+    std::vector<fe> lvl(T.total), qarr(T.total), pts((L + 2) * batch);
     for (uint32_t b = 0; b < batch; b++) {
         if (mode == 1) pts[b] = fe_one<P>();
         else { memcpy(pts[b].v, points + 32 * b, 32); pts[b] = fe_to_mont<P>(pts[b]); }
@@ -63,7 +63,7 @@ extern "C" int emu_polyops(int field, int mode, const uint8_t *a, const uint8_t 
 }
 
 // batch_invert in place (mode 0) / exclusive running product with `init` (mode 1: out[0] = init, out[i] = out[i-1] * a[i-1]), with
-// the level schedule of capi.cu's grand_product_run.  a: n canonical elements.
+// the chunk tree of gp_scan_plan.  a: n canonical elements.
 template <class P> static int run_grand(int mode, const uint8_t *a_in, uint64_t n, const uint8_t *init, uint8_t *out) {
     std::vector<fe> a(n);
     for (uint64_t i = 0; i < n; i++) { memcpy(a[i].v, a_in + 32 * i, 32); a[i] = fe_to_mont<P>(a[i]); }
@@ -73,12 +73,11 @@ template <class P> static int run_grand(int mode, const uint8_t *a_in, uint64_t 
         return 0;
     }
     fe in0; memcpy(in0.v, init, 32); in0 = fe_to_mont<P>(in0);
-    std::vector<uint64_t> m{n}, off{0};
-    while (m.back() > H2_POLY_CHUNK) { off.push_back(off.back() + (m.size() > 1 ? m.back() : 0)); m.push_back((m.back() + H2_POLY_CHUNK - 1) / H2_POLY_CHUNK); }
-    const size_t L = m.size() - 1;
-    uint64_t total = 1;
-    for (size_t l = 1; l <= L; l++) total += m[l];
-    std::vector<fe> lvl(total), ex(total), o(n);
+    GpTree T;
+    if (gp_scan_plan(n, 1, false, &T)) return -1;
+    const uint64_t *m = T.m, *off = T.off;
+    const size_t L = T.L;
+    std::vector<fe> lvl(T.total), ex(T.total), o(n);
     for (size_t l = 0; l < L; l++)
         for (uint64_t t = 0; t < m[l + 1]; t++) GrandProduct<P>::up_body(l == 0 ? a.data() : lvl.data() + off[l], m[l], lvl.data() + off[l + 1], m[l + 1], t);
     for (size_t l = L + 1; l-- > 0;) {
@@ -92,4 +91,16 @@ template <class P> static int run_grand(int mode, const uint8_t *a_in, uint64_t 
 }
 extern "C" int emu_grand_product(int field, int mode, const uint8_t *a, uint64_t n, const uint8_t *init, uint8_t *out) {
     return field == 0 ? run_grand<FpParams>(mode, a, n, init, out) : run_grand<FqParams>(mode, a, n, init, out);
+}
+
+// The chunk-tree plans themselves.  rule 0: gp_reduce_plan, 1: the same for an inner product, 2: gp_scan_plan, 3: the same
+// with level 1.  m, off: H2_GP_MAX_LEVELS values each.  Returns 1 when the plan refuses n.
+extern "C" int emu_chunk_tree(int rule, uint64_t n, uint64_t batch, uint64_t *m, uint64_t *off, uint32_t *L, uint64_t *total) {
+    GpTree T;
+    if (rule < 2 ? gp_reduce_plan(n, batch, rule == 1, &T) : gp_scan_plan(n, batch, rule == 3, &T)) return 1;
+    memcpy(m, T.m, sizeof T.m);
+    memcpy(off, T.off, sizeof T.off);
+    *L = T.L;
+    *total = T.total;
+    return 0;
 }
