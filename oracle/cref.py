@@ -35,7 +35,8 @@ def lib() -> ctypes.CDLL:
         for name in ("orc_best_multiexp", "orc_naive_msm", "orc_best_fft", "orc_ifft", "orc_coeff_to_extended",
                      "orc_extended_to_coeff", "orc_field_op", "orc_scalar_mul", "orc_point_add",
                      "orc_jac_to_affine", "orc_on_curve", "orc_gen_scalars", "orc_gen_points", "orc_ec_fft",
-                     "orc_batch_normalize", "orc_params_lagrange", "orc_ipa_rounds", "orc_eval_polynomial", "orc_kate_division", "orc_ast_eval", "orc_compute_s"):
+                     "orc_batch_normalize", "orc_params_lagrange", "orc_ipa_rounds", "orc_eval_polynomial", "orc_kate_division", "orc_ast_eval", "orc_compute_s",
+                     "orc_permutation_product", "orc_lookup_product", "orc_divide_by_vanishing_poly"):
             getattr(_lib, name).restype = ctypes.c_int
     return _lib
 
@@ -174,6 +175,48 @@ def kate_division(field: str, a: np.ndarray, b) -> np.ndarray:
     p = np.ascontiguousarray(a, dtype=np.uint8).reshape(-1, 32)
     out = np.zeros((max(p.shape[0] - 1, 0), 32), dtype=np.uint8)
     lib().orc_kate_division(FIELD_ID[field], _p(p), ctypes.c_size_t(p.shape[0]), _p(_fe(b)), _p(out))
+    return out
+
+
+def permutation_product(field: str, columns: np.ndarray, sigmas: np.ndarray, chunk_len: int, beta, gamma, omega, delta, blinding: np.ndarray,
+                        bf: int) -> np.ndarray:
+    """plonk/permutation/prover.rs:81-168 for every proof: columns (proofs, cols, n, 32), sigmas (cols, n, 32), blinding
+    (proofs x sets x bf, 32) in the rng's order.  Returns z (proofs, sets, n, 32)."""
+    c = np.ascontiguousarray(columns, dtype=np.uint8)
+    s = np.ascontiguousarray(sigmas, dtype=np.uint8)
+    proofs, cols, n = c.shape[0], c.shape[1], c.shape[2]
+    assert s.shape == (cols, n, 32) and n & (n - 1) == 0
+    sets = -(-cols // chunk_len)
+    bl = np.ascontiguousarray(blinding, dtype=np.uint8).reshape(-1, 32)
+    assert bl.shape[0] == proofs * sets * bf
+    out = np.zeros((proofs, sets, n, 32), dtype=np.uint8)
+    rc = lib().orc_permutation_product(FIELD_ID[field], _p(c), _p(s), ctypes.c_size_t(proofs), ctypes.c_size_t(cols), ctypes.c_size_t(chunk_len),
+                                       ctypes.c_uint32(n.bit_length() - 1), _p(_fe(beta)), _p(_fe(gamma)), _p(_fe(omega)), _p(_fe(delta)),
+                                       _p(bl) if bf else None, ctypes.c_uint32(bf), _p(out))
+    assert rc == 0
+    return out
+
+
+def lookup_product(field: str, a: np.ndarray, s: np.ndarray, a_perm: np.ndarray, s_perm: np.ndarray, beta, gamma, blinding: np.ndarray,
+                   bf: int) -> np.ndarray:
+    """plonk/lookup/prover.rs:279-321 for one lookup: (n, 32) compressed input / table and permuted columns, bf blinding values."""
+    cols = [np.ascontiguousarray(x, dtype=np.uint8).reshape(-1, 32) for x in (a, s, a_perm, s_perm)]
+    n = cols[0].shape[0]
+    assert all(x.shape[0] == n for x in cols) and n & (n - 1) == 0
+    bl = np.ascontiguousarray(blinding, dtype=np.uint8).reshape(-1, 32)
+    assert bl.shape[0] == bf
+    out = np.zeros((n, 32), dtype=np.uint8)
+    rc = lib().orc_lookup_product(FIELD_ID[field], *(_p(x) for x in cols), ctypes.c_uint32(n.bit_length() - 1), _p(_fe(beta)), _p(_fe(gamma)),
+                                  _p(bl) if bf else None, ctypes.c_uint32(bf), _p(out))
+    assert rc == 0
+    return out
+
+
+def divide_by_vanishing_poly(field: str, a: np.ndarray, t_evaluations) -> np.ndarray:
+    """poly/domain.rs:329-348: a[i] * t_evaluations[i % len(t_evaluations)].  Returns a new array."""
+    out = np.ascontiguousarray(a, dtype=np.uint8).reshape(-1, 32).copy()
+    t = ints_to_bytes(t_evaluations)
+    assert lib().orc_divide_by_vanishing_poly(FIELD_ID[field], _p(out), ctypes.c_size_t(out.shape[0]), _p(t), ctypes.c_size_t(t.shape[0])) == 0
     return out
 
 

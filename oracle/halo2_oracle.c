@@ -19,6 +19,8 @@
  *   best_fft (G = curve point), batch_normalize, g -> g_lagrange
  *                      arithmetic.rs:192-295 at G = C::Curve; poly/commitment.rs:74-101 (Params::new from the generators on).
  *   permute_expression_pair  plonk/lookup/prover.rs:563-647 (sort + ordered map restated as sorted table + taken marks; serial).
+ *   product columns    plonk/permutation/prover.rs:81-168, plonk/lookup/prover.rs:279-321, with ff::BatchInvert; serial.
+ *   divide_by_vanishing_poly  poly/domain.rs:329-348; serial.
  *   eval_polynomial, kate_division, Evaluator::evaluate (postfix form): see each section (hash_to_curve is restated in pasta.py only).
  *   IPA round loop     poly/commitment/prover.rs:100-142 with parallel_generator_collapse :154-166 and
  *                      compute_inner_product arithmetic.rs:308-319; the transcript is factored out (challenges and
@@ -706,6 +708,122 @@ int orc_compute_s(int field, const uint8_t *u, uint32_t k, const uint8_t *init, 
     }
     store_vec(F, out, v, n);
     free(v);
+    return 0;
+}
+
+/* ---------------------------------------------------------------- the product columns and divide_by_vanishing_poly
+ * Serial restatements for the tests at production sizes, where the big-integer loops of tests/grand_product_cases.py take
+ * minutes.  batch_invert is ff::BatchInvert: one running product of the nonzero elements, one inversion, a backward sweep;
+ * zeros stay zero.  Returns 1 when its scratch cannot be allocated. */
+static int batch_invert(const field_t *F, fe *a, size_t n) {
+    fe *pre = (fe *)malloc((n ? n : 1) * sizeof(fe)), acc, t;
+    if (!pre) return 1;
+    fe_from_bytes(F, &acc, (const uint8_t[32]){1});
+    for (size_t i = 0; i < n; i++) {
+        pre[i] = acc;
+        if (!fe_is_zero(&a[i])) fe_mul(F, &acc, &acc, &a[i]);
+    }
+    fe_inv(F, &acc, &acc);
+    for (size_t i = n; i-- > 0;) {
+        if (fe_is_zero(&a[i])) continue;
+        fe_mul(F, &t, &acc, &pre[i]);                   /* a[i]^-1 = (a[0..i] product)^-1 * (a[0..i-1] product) */
+        fe_mul(F, &acc, &acc, &a[i]);
+        a[i] = t;
+    }
+    free(pre);
+    return 0;
+}
+/* permutation::Argument::commit, plonk/permutation/prover.rs:81-168, for `proofs` proofs of the same sigmas.  columns:
+ * proofs x cols x n, sigmas: cols x n, blinding: proofs x sets x bf values in the rng's order, out: proofs x sets x n. */
+int orc_permutation_product(int field, const uint8_t *columns, const uint8_t *sigmas, size_t proofs, size_t cols, size_t chunk_len, uint32_t k,
+                            const uint8_t *beta, const uint8_t *gamma, const uint8_t *omega, const uint8_t *delta, const uint8_t *blinding,
+                            uint32_t bf, uint8_t *out) {
+    ensure_init(); const field_t *F = &FLD[field];
+    const size_t n = (size_t)1 << k;
+    if (chunk_len == 0 || (size_t)bf + 1 >= n) return 1;
+    fe b, g, w, d, one, x, y;
+    fe_from_bytes(F, &b, beta); fe_from_bytes(F, &g, gamma); fe_from_bytes(F, &w, omega); fe_from_bytes(F, &d, delta);
+    fe_from_bytes(F, &one, (const uint8_t[32]){1});
+    fe *mv = (fe *)malloc(n * sizeof(fe));
+    if (!mv) return 1;
+    size_t set_at = 0;
+    for (size_t p = 0; p < proofs; p++) {
+        fe last_z = one, deltaomega = one;
+        for (size_t c0 = 0; c0 < cols; c0 += chunk_len, set_at++) {
+            const size_t c1 = c0 + chunk_len < cols ? c0 + chunk_len : cols;
+            for (size_t i = 0; i < n; i++) mv[i] = one;
+            for (size_t c = c0; c < c1; c++) {                                  /* :101-116, v + beta sigma + gamma */
+                const uint8_t *v = columns + 32 * n * (p * cols + c), *s = sigmas + 32 * n * c;
+                for (size_t i = 0; i < n; i++) {
+                    fe_from_bytes(F, &x, s + 32 * i); fe_mul(F, &x, &x, &b); fe_add(F, &x, &x, &g);
+                    fe_from_bytes(F, &y, v + 32 * i); fe_add(F, &x, &x, &y);
+                    fe_mul(F, &mv[i], &mv[i], &x);
+                }
+            }
+            if (batch_invert(F, mv, n)) { free(mv); return 1; }                 /* :120 */
+            for (size_t c = c0; c < c1; c++) {                                  /* :124-143, v + delta^j omega^i beta + gamma */
+                const uint8_t *v = columns + 32 * n * (p * cols + c);
+                fe cur = deltaomega;
+                for (size_t i = 0; i < n; i++) {
+                    fe_mul(F, &x, &cur, &b); fe_add(F, &x, &x, &g);
+                    fe_from_bytes(F, &y, v + 32 * i); fe_add(F, &x, &x, &y);
+                    fe_mul(F, &mv[i], &mv[i], &x);
+                    fe_mul(F, &cur, &cur, &w);
+                }
+                fe_mul(F, &deltaomega, &deltaomega, &d);
+            }
+            uint8_t *z = out + 32 * n * set_at;                                 /* :150-156, z[0] = last_z */
+            fe acc = last_z;
+            for (size_t i = 0; i < n; i++) {
+                if (i == n - bf - 1) last_z = acc;                              /* :163 */
+                fe_to_bytes(F, z + 32 * i, &acc);
+                fe_mul(F, &acc, &acc, &mv[i]);
+            }
+            if (bf) memcpy(z + 32 * (n - bf), blinding + 32 * (size_t)bf * set_at, 32 * (size_t)bf);   /* :158-161 */
+        }
+    }
+    free(mv);
+    return 0;
+}
+/* lookup::Permuted::commit_product, plonk/lookup/prover.rs:279-321, for one lookup: the compressed input and table a, s, the
+ * permuted a', s' (n each), bf blinding values; out: n. */
+int orc_lookup_product(int field, const uint8_t *a, const uint8_t *s, const uint8_t *a_perm, const uint8_t *s_perm, uint32_t k, const uint8_t *beta,
+                       const uint8_t *gamma, const uint8_t *blinding, uint32_t bf, uint8_t *out) {
+    ensure_init(); const field_t *F = &FLD[field];
+    const size_t n = (size_t)1 << k;
+    if ((size_t)bf + 1 >= n) return 1;
+    fe b, g, x, y;
+    fe_from_bytes(F, &b, beta); fe_from_bytes(F, &g, gamma);
+    fe *lp = (fe *)malloc(n * sizeof(fe));
+    if (!lp) return 1;
+    for (size_t i = 0; i < n; i++) {                                           /* :281-291 */
+        fe_from_bytes(F, &x, a_perm + 32 * i); fe_add(F, &x, &x, &b);
+        fe_from_bytes(F, &y, s_perm + 32 * i); fe_add(F, &y, &y, &g);
+        fe_mul(F, &lp[i], &x, &y);
+    }
+    if (batch_invert(F, lp, n)) { free(lp); return 1; }                        /* :295 */
+    for (size_t i = 0; i < n; i++) {                                           /* :299-309 */
+        fe_from_bytes(F, &x, a + 32 * i); fe_add(F, &x, &x, &b); fe_mul(F, &lp[i], &lp[i], &x);
+        fe_from_bytes(F, &y, s + 32 * i); fe_add(F, &y, &y, &g); fe_mul(F, &lp[i], &lp[i], &y);
+    }
+    fe acc; fe_from_bytes(F, &acc, (const uint8_t[32]){1});                    /* :311-318, z[0] = ONE */
+    for (size_t i = 0; i < n - bf; i++) {
+        fe_to_bytes(F, out + 32 * i, &acc);
+        fe_mul(F, &acc, &acc, &lp[i]);
+    }
+    if (bf) memcpy(out + 32 * (n - bf), blinding, 32 * (size_t)bf);            /* :319-321 */
+    free(lp);
+    return 0;
+}
+/* divide_by_vanishing_poly, poly/domain.rs:329-348: a[i] *= t_evaluations[i % t_len], in place on len canonical elements */
+int orc_divide_by_vanishing_poly(int field, uint8_t *a, size_t len, const uint8_t *t_evals, size_t t_len) {
+    ensure_init(); const field_t *F = &FLD[field];
+    if (t_len == 0) return 1;
+    fe x, t;
+    for (size_t i = 0; i < len; i++) {
+        fe_from_bytes(F, &x, a + 32 * i); fe_from_bytes(F, &t, t_evals + 32 * (i % t_len));
+        fe_mul(F, &x, &x, &t); fe_to_bytes(F, a + 32 * i, &x);
+    }
     return 0;
 }
 

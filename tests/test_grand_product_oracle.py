@@ -127,3 +127,49 @@ def test_emul_lookup_product(emu, field, k, count, bf):
     got = emu_lookup_product(emu, field, lookups, beta, gamma, k, bf, blinding)
     assert got == want
     assert all(z[0] == 1 for z in got)
+
+
+# ---- the C restatement the large-k GPU tests compare against -----------------------------------------------------------
+@pytest.mark.parametrize("field", ["fp", "fq"])
+@pytest.mark.parametrize("k,proofs,cols,chunk_len,bf", PERM_SHAPES)
+def test_c_permutation_product_equals_the_big_integer_loops(field, k, proofs, cols, chunk_len, bf):
+    """cref.permutation_product (oracle/halo2_oracle.c) is the restatement tests/test_gpu_phases_large.py checks the device
+    against at k = 15 ... 20: the same z as the big-integer loops, zero denominators in the first and the last row included."""
+    n = 1 << k
+    seed = SEED + 9000 + 1000 * k + 10 * cols + chunk_len
+    zero_rows = [(proofs - 1, cols - 1, n // 2), (0, 0, 0), (0, cols - 1, n - 1)] if n > 2 else []
+    m, beta, gamma, sigmas, columns = permutation_case(field, k, proofs, cols, bf, seed, zero_rows)
+    omega, delta = pasta.omega_for_k(field, k), scalar_delta(m)
+    sets = -(-cols // chunk_len)
+    blinding = pasta.gen_scalars(field, seed + 7, proofs * sets * bf) if bf else []
+    want = oracle_permutation_product(columns, sigmas, beta, gamma, omega, delta, chunk_len, bf, blinding, m)
+    c = np.stack([np.stack([cref.ints_to_bytes(col) for col in per]) for per in columns])
+    s = np.stack([cref.ints_to_bytes(col) for col in sigmas])
+    got = cref.permutation_product(field, c, s, chunk_len, beta, gamma, omega, delta, cref.ints_to_bytes(blinding) if bf else np.zeros((0, 32), np.uint8), bf)
+    assert [[cref.bytes_to_ints(z) for z in per] for per in got] == want
+
+
+@pytest.mark.parametrize("field", ["fp", "fq"])
+@pytest.mark.parametrize("k,count,bf", LOOKUP_SHAPES)
+def test_c_lookup_product_equals_the_big_integer_loops(field, k, count, bf):
+    m, n = pasta.FIELDS[field], 1 << k
+    seed = SEED + 9500 + 100 * k + count
+    beta, gamma = pasta.gen_scalars(field, seed, 2)
+    lookups = [[pasta.gen_scalars(field, seed + 10 * b + j + 1, n) for j in range(4)] for b in range(count)]
+    if n > 2:
+        lookups[-1][2][0] = (-beta) % m                               # zero denominators in the first and the last row
+        lookups[0][3][n - 1] = (-gamma) % m
+    blinding = pasta.gen_scalars(field, seed + 9, count * bf) if bf else []
+    for b, lk in enumerate(lookups):
+        bl = blinding[b * bf:(b + 1) * bf]
+        want = oracle_lookup_product(*lk, beta, gamma, bf, bl, m)
+        got = cref.lookup_product(field, *(cref.ints_to_bytes(c) for c in lk), beta, gamma, cref.ints_to_bytes(bl) if bf else np.zeros((0, 32), np.uint8), bf)
+        assert cref.bytes_to_ints(got) == want
+
+
+@pytest.mark.parametrize("field", ["fp", "fq"])
+def test_c_divide_by_vanishing_poly_equals_the_domains(field):
+    for j, k in ((3, 4), (5, 6), (9, 5), (4, 9)):
+        D = pasta.EvaluationDomain(field, j, k)
+        h = cref.gen_scalars(field, SEED + 17 * k + j, D.extended_len())
+        assert cref.bytes_to_ints(cref.divide_by_vanishing_poly(field, h, D.t_evaluations)) == D.divide_by_vanishing_poly(cref.bytes_to_ints(h))
