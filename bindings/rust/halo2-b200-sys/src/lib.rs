@@ -128,6 +128,8 @@ extern "C" {
     pub fn h2_poly_coeff_to_extended_batch(dst: *const u64, src: *const u64, count: usize, k: u32, ext_k: u32, zeta: *const c_void,
                                            ext_omega: *const c_void, repr: c_int) -> c_int;
     pub fn h2_poly_set_rows(polys: *const u64, count: usize, start: usize, rows: usize, values: *const c_void, repr: c_int) -> c_int;
+    pub fn h2_poly_random(polys: *const u64, count: usize, lens: *const usize, seed32: *const c_void, stream: u64, block: u64, word: u32)
+                          -> c_int;
 }
 
 fn check(rc: c_int) {

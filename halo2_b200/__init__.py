@@ -23,6 +23,7 @@ from .columns import instance_commit, advice_commit, InstanceSingle, AdviceSingl
 from .vanishing import vanishing_commit, vanishing_quotient_resident, Committed, Constructed, Evaluated  # noqa: F401
 from .arguments import (PermutationCommitted, PermutationConstructed, PermutationEvaluated, permutation_key_evaluate,  # noqa: F401
                         permutation_key_open, LookupCommitted, LookupConstructed, LookupEvaluated, evaluate_columns, open_columns)
+from .rng import ChaCha20Rng, random_resident  # noqa: F401
 from . import multiopen, opening  # noqa: F401
 
 __all__ = ["Ast", "AstLeaf", "Evaluator", "Assembly", "CopyConstraints", "ProvingKey", "build_permutation_polys", "keygen_vk", "keygen_pk",
@@ -37,4 +38,4 @@ __all__ = ["Ast", "AstLeaf", "Evaluator", "Assembly", "CopyConstraints", "Provin
            "InstanceSingle", "AdviceSingle", "InstanceTooLarge",
            "vanishing_commit", "vanishing_quotient_resident", "Committed", "Constructed", "Evaluated",
            "PermutationCommitted", "PermutationConstructed", "PermutationEvaluated", "permutation_key_evaluate", "permutation_key_open",
-           "LookupCommitted", "LookupConstructed", "LookupEvaluated", "evaluate_columns", "open_columns"]
+           "LookupCommitted", "LookupConstructed", "LookupEvaluated", "evaluate_columns", "open_columns", "ChaCha20Rng", "random_resident"]

@@ -9,6 +9,7 @@
 #include "keygen.cuh"
 #include "assembly.cuh"
 #include "grandproduct.cuh"
+#include "chacha.cuh"
 
 // ------------------------------------------------------------------------------------------------
 // eval_polynomial / compute_inner_product / kate_division on resident polynomials (polyops.cuh)
@@ -599,6 +600,48 @@ extern "C" int h2_poly_permutation_sigma_copies(const uint64_t *dst, size_t cols
     std::vector<PolyBuf *> d;
     if (g.out(dst, cols, "dst", (size_t)1 << k, "2^k", d) || g.distinct()) return 1;
     return by_field(d[0]->field, [&](auto p) { return permutation_sigma_copies_run<decltype(p)>(d, k, copies, m, omega, delta, h); });
+}
+
+
+// ------------------------------------------------------------------------------------------------
+// the prover's random polynomials: ChaCha20Rng draws of Field::random (chacha.cuh)
+// ------------------------------------------------------------------------------------------------
+extern "C" int h2_poly_random(const uint64_t *polys, size_t count, const size_t *lens, const void *seed32, uint64_t stream, uint64_t block,
+                              uint32_t word) {
+    static const char *who = "h2_poly_random";
+    CtxLock lk;
+    if (require_ready()) return 1;
+    if (count == 0) return fail(std::string(who) + ": count == 0");
+    if (!polys || !lens) return fail(std::string(who) + ": null argument");
+    if (!seed32) return fail(std::string(who) + ": null seed32");
+    if (word >= 16) return fail(std::string(who) + ": word >= 16");
+    PolyArgs g(who);
+    std::vector<PolyBuf *> ps;
+    if (g.out(polys, count, "polys", lens, "lens", ps) || g.distinct()) return 1;
+    // draw j of the call reads blocks block + j and, with word != 0, block + j + 1: the last one must not pass 2^64 - 1
+    std::vector<RandCol> cols(count);
+    uint64_t total = 0, longest = 0;
+    for (size_t i = 0; i < count; i++) {            // each lens[i] fits its polynomial, so the sum cannot wrap
+        cols[i] = {total, (uint64_t)lens[i]};
+        total += lens[i];
+        longest = std::max<uint64_t>(longest, lens[i]);
+    }
+    if (total == 0) return 0;
+    if (total - 1 + (word != 0) > ~0ull - block) return fail(std::string(who) + ": the draws run past keystream block 2^64 - 1");
+    ChaChaKey key;
+    memcpy(key.k, seed32, sizeof key.k);
+    cudaStream_t s = g_ctx.stream;
+    ColTable t;
+    if (col_table(ps, cols.data(), count * sizeof(RandCol), s, &t)) return 1;
+    return by_field(ps[0]->field, [&](auto p) {
+        using P = decltype(p);
+        for (size_t c0 = 0; c0 < count; c0 += 65535) {   // grid.y limit
+            const uint32_t n = (uint32_t)std::min<size_t>(count - c0, 65535);
+            LAUNCH(chacha_random_kernel<P>, dim3(blocks_for(longest, 256), n), 256, 0, s, t.cols, reinterpret_cast<const RandCol *>(t.data), (uint32_t)c0,
+                   key, stream, block, word);
+        }
+        return 0;
+    });
 }
 
 

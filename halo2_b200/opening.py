@@ -8,7 +8,8 @@ and their inverses and the running blind f are a handful of scalars and stay wit
 
 Randomness: the reference draws s_poly (n scalars), its blind and two scalars per round from `rng` in that order
 (prover.rs:46-54, :112-113).  Here `rng` is any object with `poly(n)` -> a ResidentPoly or (n, 32) uint8 array the callee may
-keep, and `scalar()` -> int; drawing 2^k scalars is the caller's business (a patched prover would hand over its Vec).
+keep, and `scalar()` -> int.  halo2_b200.ChaCha20Rng draws s_poly on the device, the scalars a ChaCha20Rng with the same seed
+and position gives (h2_poly_random); any other rng hands over its own draws.
 """
 from __future__ import annotations
 

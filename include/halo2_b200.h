@@ -212,6 +212,17 @@ int h2_poly_coeff_to_extended_batch(const uint64_t *dst, const uint64_t *src, si
  * The polynomials must be the calling context's own and pairwise distinct, each with at least start + rows elements; every
  * check runs first and a failed call changes nothing.  count == 0 or rows == 0 does nothing.  Asynchronous. */
 int h2_poly_set_rows(const uint64_t *polys, size_t count, size_t start, size_t rows, const void *values, int repr);
+/* The prover's random polynomials (vanishing::Argument::commit's random_poly, commitment::create_proof's s_poly) drawn on
+ * the device, every polynomial in one launch: polys[i][0 .. lens[i]) <- consecutive Field::random draws of a rand_chacha
+ * 0.3.1 ChaCha20Rng with seed `seed32` (32 bytes), stream id `stream` and word position 16 * block + word (word < 16);
+ * polynomial i starts where polynomial i - 1 ended.  Draw j takes the 16 keystream words from 16 * (block + j) + word on,
+ * as eight next_u64, and is (lo + 2^256 hi) mod p of them (pasta_curves 0.5.1's from_u512), the element h2_poly_upload
+ * stores for that canonical value.  A caller that holds such an rng gets the scalars its own draws would give and then
+ * moves it on by 16 * sum(lens) words (set_word_pos).  Refused before anything is launched, writing nothing: count == 0, a
+ * null argument or seed, word >= 16, an unknown, shared or repeated polynomial, polynomials of two fields, lens[i] above a
+ * polynomial's length, and draws that would run past keystream block 2^64 - 1 (where the rng's counter wraps).  Elements
+ * past lens[i] are left as they are.  Asynchronous on the calling context's stream. */
+int h2_poly_random(const uint64_t *polys, size_t count, const size_t *lens, const void *seed32, uint64_t stream, uint64_t block, uint32_t word);
 int h2_msm_registered_polys(uint64_t bases_handle, const uint64_t *polys, size_t batch, size_t n, const void *extra_scalars, int repr,
                             void *out_xyz);
 /* The same pass followed by batch_normalize on the device: `batch` affine points (64 B each) -- what the prover writes to
